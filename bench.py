@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — correspondences/sec per ICP iteration on the BASELINE.json C3 workload.
 
-    python bench.py --gpus 1 --steps 20 --warmup 3                 # B200 arm
+    python bench.py --gpus 1 --steps 20 --warmup 3                 # GPU arm
     python bench.py --impl reference --steps 20 --warmup 3          # CPU arm (oracle port)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W       # weak scaling
@@ -26,6 +26,10 @@ N > 1      = independent pairs, one per GPU (weak scaling); the only collective 
              all-gather of the per-pair result records after the last registration.
 c4 / c5    = BASELINE configs[3] and [4] measured through their public entry points
              (tile_slabs + register per slab; simpleicp_batch), spread over the N ranks.
+--dump-outputs DIR  writes, on rank 0, what the last timed e2e registration returned as
+             DIR/<name>.npy (float64): H, the transformed movable cloud, the residuals and the
+             per-iteration records.  Inputs are seeded, so two builds can be compared output for
+             output.
 """
 from __future__ import annotations
 
@@ -193,7 +197,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def bind_to_gpu_numa_node(local: int):
     """Pinned buffers are first-touched by this process: run it on the GPU's own NUMA node."""
@@ -278,6 +282,34 @@ def run_c5(sb, rank, world, local, dist, pairs_per_gpu, n_pts):
             "failed": int((table[:, 16] < 0).sum()), "mean_iterations": float(table[table[:, 16] > 0, 16].mean()),
             "max_H_frobenius_vs_H_true": max(errs) if errs else None,
             "api": "simpleicp_b200.simpleicp_batch(pairs, engine='batched') on pinned host arrays, records all-gathered"}
+
+
+DUMP_BYTES = 64_000_000
+
+
+def dump_outputs(out_dir, res, seed: int = 0) -> None:
+    """What one registration returned, as float64 .npy files of at most DUMP_BYTES in all.  An
+    array too large for its share is replaced by a fixed seeded sample of its rows, stored with
+    the sampled row numbers (<name>_rows)."""
+    recs = res.records[:res.iterations]
+    arrays = {
+        "H": np.asarray(res.H, dtype=np.float64),
+        "iteration_records": np.array([[r["n_kept"], r["mean_res"], r["std_res"], *r["x"]] for r in recs],
+                                      dtype=np.float64).reshape(len(recs), 9),
+        "residuals": np.asarray(res.residuals, dtype=np.float64),
+        "X_mov_transformed": np.asarray(res.X_mov_transformed, dtype=np.float64),
+    }
+    # bytes each array may take, sampled row numbers included; H and the records take a few KB
+    share = {"H": 1 << 20, "iteration_records": 1 << 20, "residuals": 12 << 20, "X_mov_transformed": 40 << 20}
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        row_bytes = a.nbytes // max(len(a), 1)
+        if a.nbytes > share[name]:
+            rows = np.sort(np.random.default_rng(seed).choice(len(a), share[name] // (row_bytes + 8), replace=False))
+            np.save(out / f"{name}_rows.npy", rows.astype(np.float64))
+            a = a[rows]
+        np.save(out / f"{name}.npy", a)
 
 
 def _trace(msg):
@@ -398,6 +430,8 @@ def run_b200(args):
     torch.cuda.synchronize()
     e2e_s = time.perf_counter() - t0
     tm = eng.timings()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res)
     # the one collective of the multi-GPU run: the result records, gathered once after the last
     # registration (inside the reported time)
     if world > 1:
@@ -510,8 +544,8 @@ def run_b200(args):
         peaks = json.loads((REPO / "MEASURED_PEAKS.json").read_text())
     except (OSError, ValueError):
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
     rs_name = {2.0: "k_rs_fused", 1.0: "k_reject_solve", 0.0: "k_reject_solve"}.get(path, "k_reject_solve")
     if st["match_grid"] >= st["reject_solve"]:
         dom, dom_ms, dom_bytes = "k_match_grid_coop", st["match_grid"], b_match
@@ -607,6 +641,7 @@ def main():
     ap.add_argument("--no-c4c5", action="store_true")
     ap.add_argument("--c5-pairs-per-gpu", type=int, default=64)
     ap.add_argument("--c5-points", type=int, default=100_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3 if args.impl == "b200" else 0)
     if args.impl == "reference":

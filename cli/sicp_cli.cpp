@@ -20,7 +20,7 @@
 #include "sicp_b200.h"
 
 static void usage() {
-  puts("A simple version of the ICP algorithm (B200 build).\nUsage:\n  sicp_cli [OPTION...]\n\n"
+  puts("A simple version of the ICP algorithm (H100 build).\nUsage:\n  sicp_cli [OPTION...]\n\n"
        "  -f, --fixed arg                 Path to fixed point cloud\n"
        "  -m, --movable arg               Path to movable point cloud\n"
        "  -c, --correspondences arg       Number of initially selected correspondences (default: 1000)\n"

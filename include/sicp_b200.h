@@ -1,5 +1,5 @@
 /*
- * sicp_b200.h — C ABI of libsicp_b200.so: the B200 (sm_100a) ICP inner loop behind the
+ * sicp_b200.h — C ABI of libsicp_b200.so: the H100 (sm_90a) ICP inner loop behind the
  * simpleICP Python API.
  *
  * The reference (pglira/simpleICP) has no FFI/plugin layer (SURVEY.md §0.9); its boundary is the

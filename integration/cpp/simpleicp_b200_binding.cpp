@@ -8,7 +8,7 @@
 // exactly as /root/reference/c++/src/simpleicp.h:11-18 declares it, on top of the C ABI of
 // libsicp_b200.so (include/sicp_b200.h) and nothing else.  It REPLACES c++/src/simpleicp.cpp,
 // pointcloud.cpp and corrpts.cpp in the reference's build: linked with the reference's own,
-// unmodified c++/src/simpleicp-cli.cpp it gives the reference CLI running on the B200
+// unmodified c++/src/simpleicp-cli.cpp it gives the reference CLI running on the H100
 // (built by the recipe that also builds the CPU reference for the tests, oracle/Makefile target
 // _ref/simpleicp_cpp_b200; tests/test_gpu_linearized.py runs it).
 // Same arguments and defaults, same screen output (simpleicp.cpp:17-127), same exception for

@@ -66,8 +66,8 @@ def build():
     return OUT / "simpleicp_cpp", OUT / "simpleicp_cpp_driver"
 
 
-def run_cli(cli, fix, mov, flags):
-    cmd = [str(cli), "--fixed", str(REF / "data" / fix), "--movable", str(REF / "data" / mov)]
+def run_cli(cli, fix, mov, flags, data=REF / "data"):
+    cmd = [str(cli), "--fixed", str(Path(data) / fix), "--movable", str(Path(data) / mov)]
     for k, v in flags.items():
         cmd += [f"--{k}", repr(v) if isinstance(v, float) else str(v)]
     out = subprocess.run(cmd, capture_output=True, text=True, check=True).stdout

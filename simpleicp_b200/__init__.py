@@ -1,4 +1,4 @@
-"""simpleicp_b200 — B200-native (sm_100a) point-to-plane ICP with the simpleICP Python API.
+"""simpleicp_b200 — H100-native (sm_90a) point-to-plane ICP with the simpleICP Python API.
 
 Drop-in names of the reference package (python/simpleicp/__init__.py:12-14):
 ``SimpleICP``, ``PointCloud``, ``RigidBodyParameters``; plus the functional form

@@ -1,4 +1,4 @@
-"""Build libsicp_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libsicp_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m simpleicp_b200._build [--force] [--verbose]
 
@@ -23,7 +23,7 @@ LIB = PKG / "libsicp_b200.so"
 SOURCES = ["capi.cu", "batch.cu", "grid.cu", "nn.cu", "normals.cu", "reject_solve.cu", "transform.cu", "upload.cu", "io.cpp"]
 CLI_SRC = PKG.parent / "cli" / "sicp_cli.cpp"
 CLI_BIN = PKG / "sicp_cli"
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xptxas", "-v"]
 

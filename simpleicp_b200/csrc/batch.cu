@@ -2,8 +2,8 @@
 // independent pairs with ONE set of launches per stage and per iteration (BASELINE.json
 // configs[4]: 512 pairs of 100 000 points, 64 per GPU; SURVEY.md section 8e).
 //
-// A registration of a 100 000-point pair with 1000 correspondences is far too small to fill a
-// B200: one match launch has 16 000 threads, one reject/solve launch one block, and the host
+// A registration of a 100 000-point pair with 1000 correspondences is far too small to fill an
+// H100: one match launch has 16 000 threads, one reject/solve launch one block, and the host
 // drives ~30 launches per iteration-loop through a Python thread.  Here every kernel carries a
 // pair dimension instead:
 //   upload        one cudaMemcpyAsync per cloud straight from the caller's (pinned) arrays; the

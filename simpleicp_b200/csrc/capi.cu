@@ -255,8 +255,8 @@ int32_t sicp_create(int32_t device, void* cuda_stream, sicp_ctx** out) {
     SICP_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     SICP_CUDA(cudaGetDeviceProperties(&prop, device));
-    SICP_REQUIRE(prop.major >= 10, SICP_ERR_CUDA,
-                 std::string("libsicp_b200 is built for sm_100a only; device is sm_") +
+    SICP_REQUIRE(prop.major == 9 && prop.minor == 0, SICP_ERR_CUDA,
+                 std::string("libsicp_b200 is built for sm_90a only; device is sm_") +
                      std::to_string(prop.major) + std::to_string(prop.minor));
     c.num_sms = prop.multiProcessorCount;
     c.stream = reinterpret_cast<cudaStream_t>(cuda_stream);

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for libsicp_b200 (sm_100a only).
+// common.cuh — shared device/host helpers for libsicp_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -63,7 +63,7 @@ struct DevBuf {
 // ------------------------------------------------------------------------------------------
 // Geometry types
 // ------------------------------------------------------------------------------------------
-// One point of a cell-sorted cloud: 32 bytes = one L2 sector, fetched with a single LDG.E.256.
+// One point of a cell-sorted cloud: 32 bytes = one L2 sector.
 struct __align__(32) Rec {
   double x, y, z;
   long long idx;  // index in the caller's (unsorted) cloud

@@ -53,7 +53,7 @@ struct Batch;
 struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
-  int num_sms = 148;
+  int num_sms = 132;
   std::string err;
 
   // options

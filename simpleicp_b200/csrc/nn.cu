@@ -286,7 +286,7 @@ __device__ __forceinline__ void match_coop_body(
   // the safe side (a row is only skipped / narrowed when it certainly holds nothing nearer than
   // `best`); the distances themselves stay float64.  (Per-row float64 bounds, a float64 sqrt, two
   // float64 floor conversions and an integer division were half of the first iteration's
-  // instructions, profiles/r2_README.md.)
+  // instructions.)
   const float fqx = (float)((qx - g.ox) * g.inv_h), fqy = (float)((qy - g.oy) * g.inv_h),
               fqz = (float)((qz - g.oz) * g.inv_h);
   // float32 error of a cell coordinate (a query may lie far outside the grid) + cell faces vs the
@@ -363,7 +363,7 @@ __device__ __forceinline__ void match_coop_body(
       // (Requesting every cell-table entry step 2 might need before step 1's records — to shorten
       // the chain of dependent round trips — was measured 10 % SLOWER: the kernel is bound by
       // issue slots as much as by latency, and 8 extra loads per lane cost more than the round
-      // trip they save; profiles/README.md.)
+      // trip they save.)
       constexpr int NR = (8 + MG - 1) / MG;  // rows per lane in step 2
       // distances from the query to the faces of its own cell (>= 0 up to rounding)
       const double fxl = fmax(qx - (g.ox + cx * g.h), 0.0), fxh = fmax((g.ox + (cx + 1) * g.h) - qx, 0.0);

@@ -496,10 +496,9 @@ void estimate_normals_launch(Ctx& c, int k) {
   // All k-NN kernels hand record positions to k_pca_from_knn.  knn_coop: 1 = cooperative lanes
   // (k <= 16), 0 = one thread per query with the list in local memory, 2 = one thread per query
   // with the list in registers (k <= 16), -1 (default) = cooperative while the search is
-  // latency-bound (few queries: 80 us vs 200 us at K = 1000), one thread per query with the
-  // local-memory list once the queries fill the machine (K = 100 000, k = 10: 310 us; register
-  // list 425 us, cooperative 506 us — the fixed-length insertion network costs more than the
-  // early-exit loop saves in memory traffic; profiles/README.md).
+  // latency-bound (few queries), one thread per query with the local-memory list once the queries
+  // fill the machine (K = 100 000, k = 10: faster than a register list or cooperative lanes — the
+  // fixed-length insertion network costs more than the early-exit loop saves in memory traffic).
   const bool coop = (k <= 16) && (c.knn_coop == 1 || (c.knn_coop < 0 && c.K <= 16384));
   const bool reg = (k <= 16) && c.knn_coop == 2;
   c.knn_pos.reserve((size_t)c.K * k);

@@ -1331,7 +1331,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 // k_rs_fused — the same five steps WITHOUT grid barriers and without a cooperative launch.
 //
 // The cooperative kernel above spends half its time in four grid barriers and in serial sections
-// that 147 SMs wait for (profiles/r1_phase_timeline.md).  Here every dependency is resolved by
+// that all the other SMs wait for.  Here every dependency is resolved by
 // construction instead of by waiting:
 //   select     every block derives median and MAD ITSELF from the predictor histogram the match
 //              kernel filled and the per-bin index store it filled with the same atomic (slot =

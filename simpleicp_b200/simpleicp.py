@@ -1,5 +1,5 @@
 """SimpleICP facade: the reference's driver API (python/simpleicp/simpleicp.py:41-380) on top of
-the B200 library, plus the functional form ``simpleicp(X_fix, X_mov, **kwargs)`` (shape of
+the H100 library, plus the functional form ``simpleicp(X_fix, X_mov, **kwargs)`` (shape of
 julia/simpleicp.jl:216-222 and python/simpleicp/tests/test_simpleicp.py:18-32).
 
 What runs where

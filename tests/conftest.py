@@ -8,14 +8,13 @@ import pytest
 REPO = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(REPO))
 GOLD = REPO / "tests" / "golden"
-REFERENCE = Path("/root/reference")
 
 TRAVEL = ("dragon", "bunny", "multisensor", "webots")
 ALIAS = {"dragon_observed": "dragon", "dragon_movnormals": "dragon"}
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def decode_cloud(blob, n, scale):

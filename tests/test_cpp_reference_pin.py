@@ -19,7 +19,6 @@ The stand-alone restatement (its own eigenvector signs) is compared loosely: the
 flips the sign of that correspondence's distance, which moves the median the rejection is
 centred on (documented in the oracle's header).
 """
-import shutil
 import subprocess
 import sys
 from pathlib import Path
@@ -144,19 +143,22 @@ def test_standalone_restatement_reaches_the_same_registration():
         assert np.abs(r.T - T).max() < tol
 
 
-@pytest.mark.skipif(not Path("/root/reference/c++/src/simpleicp.cpp").exists() or shutil.which("g++") is None,
-                    reason="needs the reference tree and g++ (build container only)")
+@pytest.mark.skipif(not (ROOT / "oracle" / "_ref" / "simpleicp_cpp_driver").exists(),
+                    reason="oracle/_ref not built (build() makes it where the reference's C++ sources are readable)")
 def test_fixture_is_reproduced_by_the_recipe(tmp_path):
-    """Re-run the recipe: build oracle/_ref from the sources under /root/reference and compare the
-    dragon fixture field by field -- the committed numbers are the compiled reference's."""
+    """Re-run the recipe with the reference binaries build() compiled into oracle/_ref and compare
+    the dragon fixture field by field -- the committed numbers are the compiled reference's."""
     sys.path.insert(0, str(ROOT / "oracle"))
     import make_golden_cpp as mg
 
-    cli, driver = mg.build()
+    cli, driver = mg.OUT / "simpleicp_cpp", mg.OUT / "simpleicp_cpp_driver"
     fix, mov, flags = mg.CONFIGS["dragon"]
     X_fix, X_mov = load_pair("dragon")
+    # the .xyz files the recipe reads, rewritten from the lossless fixture (4 decimals, as stored)
+    np.savetxt(tmp_path / fix, X_fix, fmt="%.4f")
+    np.savetxt(tmp_path / mov, X_mov, fmt="%.4f")
     j, screen = mg.run_driver(driver, X_fix, X_mov, flags)
-    assert screen == mg.run_cli(cli, fix, mov, flags)
+    assert screen == mg.run_cli(cli, fix, mov, flags, data=tmp_path)
     fresh = mg.pack(j, screen, screen, dict(mg.DEFAULTS))
     g = dict(np.load(GOLD / "cppref_dragon.npz"))
     for key in ("H_api", "idx_fix", "normals", "planarity", "idx_mov_all", "dists_all", "idx_fix_kept", "n_kept",
@@ -166,6 +168,6 @@ def test_fixture_is_reproduced_by_the_recipe(tmp_path):
     # the reference CLI's own error path (simpleicp.cpp:26-36 -> simpleicp-cli.cpp:60-64)
     far = tmp_path / "far.xyz"
     np.savetxt(far, X_mov[:2000] + 1e4, fmt="%.4f")
-    r = subprocess.run([str(cli), "--fixed", "/root/reference/data/dragon1.xyz", "--movable", str(far),
+    r = subprocess.run([str(cli), "--fixed", str(tmp_path / fix), "--movable", str(far),
                         "--max_overlap_distance", "1"], capture_output=True, text=True)
     assert r.returncode == 1 and "Point clouds do not overlap within max_overlap_distance" in r.stderr

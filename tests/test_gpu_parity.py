@@ -838,7 +838,7 @@ def test_batched_engine_per_pair_status_and_front_end(gpu):
 
 
 def test_barrier_free_kernel_many_tiles_per_block(gpu):
-    """K = 300 000 > 148 x 768: every block of k_rs_fused streams several TMA-staged tiles and the
+    """K = 300 000 > 132 x 768: every block of k_rs_fused streams several TMA-staged tiles and the
     per-bin store runs at its larger capacity; results against the cooperative kernel."""
     X_fix, X_mov, H_true = O.c3_pair(400_000)
     with _capi.Engine() as e:

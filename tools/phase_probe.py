@@ -45,7 +45,7 @@ def probe(n, K, rings=(4, 8, 12, 16)):
                    f"mad[lv={t[25]:.0f} cand={t[27]:.0f}: levels={t[14]:.1f} gather={t[15]:.1f} sort={t[16]:.1f}]")
             print("  phases(us): " + seq + f" | D: red1={t[20]:.1f} reduce={t[17]:.1f} assemble={t[18]:.1f} eval0={t[21]:.1f} chol0={t[22]:.1f} lm={t[19]:.1f} lm_it={rec_lm} fastsel={t[28]:.0f} cand={t[26]:.0f}/{t[27]:.0f}")
             print("  " + sel)
-        for gb in (148, 74, 37, 18):
+        for gb in (132, 66, 33, 16):
             e.set_option("rs_blocks", gb)
             sw = e.time_stages(p, 20, False)
             t = e.phase_times()
