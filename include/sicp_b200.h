@@ -304,11 +304,24 @@ int32_t sicp_time_stages(sicp_ctx* ctx, const sicp_run_params* p, int32_t reps, 
  * relative to kernel entry.  [1] median done, [2] MAD done, [3] moments accumulated, [4] grid
  * barrier passed, [5] LM solve done, [6] barrier, [7] residual pass, [8] barrier, [9] exit;
  * [10..12] / [14..16] radix levels done / gather barrier / sort done for the median / MAD;
- * [24],[25] radix levels used, [26],[27] candidates sorted (raw counts, not times); [28] path:
+ * [24],[25] radix levels used, [26],[27] candidates sorted (raw counts, not times; 0 when a
+ * predictor select failed and no radix select followed); [28] path:
  * 0 radix select, 1 predictor histogram (cooperative kernel), 2 barrier-free kernel (there
  * [2] = select done, [3] = accumulation done in block 0, [4] = last block starts, [17] partials
- * reduced, [18] M assembled, [19] solve done, [9] exit).                                        */
+ * reduced, [18] M assembled, [19] solve done, [9] exit).
+ * Selection diagnostics (codes, not times; csrc/reject_solve.cuh: SelectPath, SelectOutcome):
+ * [29] the selection that produced the last record's median and MAD: 0 radix, 1 predictor gather
+ * of the cooperative kernel, 2 per-bin key store of the barrier-free kernel (not written by a
+ * barrier-free launch that missed its prediction: the general kernel repeats that iteration);
+ * [30] outcome of the predictor select of the last barrier-free launch, [31] of the last
+ * cooperative-kernel launch: 0 used, > 0 the first check that failed.                          */
 int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32] /*[h]*/);
+
+/* Test-only: overwrite the order-statistic predictor (median, MAD and the planarity bound of
+ * their population) that the next match bins the distances with, without resetting the loop.
+ * The predictor only accelerates the selection: any finite med and mad > 0 must give the same
+ * median and MAD, which is what tests use this for.                                            */
+int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double min_planarity);
 
 /* ---- .xyz text I/O (host only; SURVEY.md section 8f: file parsing dominates end-to-end time on
  * the lidar sets).  Contract of the reference readers (c++/src/simpleicp-cli.cpp:72-128,

@@ -21,6 +21,20 @@ ABI_VERSION = 2  # include/sicp_b200.h: SICP_ABI_VERSION
 NN_AUTO, NN_GRID, NN_BRUTE = 0, 1, 2
 SIGN_DGEEV, SIGN_CANONICAL = 0, 1
 
+# selection diagnostics of Engine.phase_times() (csrc/reject_solve.cuh: SelectPath, SelectOutcome)
+SLOT_SEL_PATH, SLOT_SEL_FUSED, SLOT_SEL_COOP = 29, 30, 31
+SEL_PATH_RADIX, SEL_PATH_PREDICT, SEL_PATH_BINSTORE = 0, 1, 2
+SEL_OK, SEL_NO_PREDICTION, SEL_NOT_ATTEMPTED, SEL_MEDIAN_OUTSIDE, SEL_MEDIAN_NO_BIN = 0, 1, 2, 3, 4
+SEL_MEDIAN_GAP, SEL_MEDIAN_CANDIDATES, SEL_MAD_BRACKET, SEL_MAD_WINDOW = 5, 6, 7, 8
+SEL_MAD_CANDIDATES, SEL_BIN_CAP = 9, 10
+SEL_OUTCOMES = {
+    "SEL_OK": SEL_OK, "SEL_NO_PREDICTION": SEL_NO_PREDICTION, "SEL_NOT_ATTEMPTED": SEL_NOT_ATTEMPTED,
+    "SEL_MEDIAN_OUTSIDE": SEL_MEDIAN_OUTSIDE, "SEL_MEDIAN_NO_BIN": SEL_MEDIAN_NO_BIN,
+    "SEL_MEDIAN_GAP": SEL_MEDIAN_GAP, "SEL_MEDIAN_CANDIDATES": SEL_MEDIAN_CANDIDATES,
+    "SEL_MAD_BRACKET": SEL_MAD_BRACKET, "SEL_MAD_WINDOW": SEL_MAD_WINDOW,
+    "SEL_MAD_CANDIDATES": SEL_MAD_CANDIDATES, "SEL_BIN_CAP": SEL_BIN_CAP,
+}
+
 # every symbol include/sicp_b200.h declares (tests check the library exports all of them)
 SYMBOLS = (
     "sicp_abi_version", "sicp_create", "sicp_destroy", "sicp_last_error", "sicp_set_option",
@@ -29,6 +43,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_debug_seed_predictor",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
 
@@ -150,6 +165,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
+        "sicp_debug_seed_predictor": [vp, dbl, dbl, dbl],
     }
     for name, args in sigs.items():
         fn = getattr(lib, name)
@@ -513,6 +529,18 @@ class Engine:
         us = (C.c_double * 32)()
         self._check(self._lib.sicp_get_phase_times(self._h, us))
         return list(us)
+
+    def selection(self) -> dict:
+        """Selection diagnostics of the last reject/solve launches (phase_times slots 29..31):
+        which path produced the last record's median/MAD, and the outcome codes of the last
+        predictor attempt of the barrier-free and of the cooperative kernel."""
+        us = self.phase_times()
+        return {"path": int(us[SLOT_SEL_PATH]), "fused": int(us[SLOT_SEL_FUSED]),
+                "coop": int(us[SLOT_SEL_COOP]), "cnt_med": int(us[26]), "cnt_edge": int(us[27])}
+
+    def seed_predictor(self, med: float, mad: float, min_planarity: float):
+        """Test-only (sicp_debug_seed_predictor): the predictor the next match bins with."""
+        self._check(self._lib.sicp_debug_seed_predictor(self._h, float(med), float(mad), float(min_planarity)))
 
     def timings(self) -> dict:
         t = Timings()

@@ -1085,6 +1085,24 @@ int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32]) {
   API_END
 }
 
+int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double min_planarity) {
+  API_BEGIN(ctx)
+  SICP_REQUIRE(std::isfinite(med) && std::isfinite(mad) && mad > 0.0, SICP_ERR_BAD_ARG,
+               "the predictor needs a finite median and a finite MAD > 0");
+  // read-modify-write of the device state like init_state(..., reset_loop = false): the loop
+  // (transform, parameters, stop flag, weights) is left as it is
+  DevState h;
+  SICP_CUDA(cudaMemcpyAsync(&h, c.dev_state.p, sizeof(h), cudaMemcpyDeviceToHost, c.stream));
+  sync(c);
+  h.pred_med = med;
+  h.pred_mad = mad;
+  h.pred_minpl = min_planarity;
+  h.pred_valid = 1;
+  SICP_CUDA(cudaMemcpyAsync(c.dev_state.p, &h, sizeof(h), cudaMemcpyHostToDevice, c.stream));
+  sync(c);
+  API_END
+}
+
 int32_t sicp_get_timings(sicp_ctx* ctx, sicp_timings* t) {
   API_BEGIN(ctx)
   SICP_REQUIRE(t != nullptr, SICP_ERR_BAD_ARG, "t is NULL");

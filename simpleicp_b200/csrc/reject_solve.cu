@@ -873,11 +873,12 @@ __device__ void uncertainties(Shared& s, const RSArgs& a, const double* An, doub
 //     everything farther than t_hi + g + 1 bins certainly above; the bins in between are the
 //     MAD candidates.
 // One gather pass + one grid barrier then yields both order statistics exactly (same values as
-// the radix path).  Returns false — before touching global state — when the prediction does not
-// bracket the ranks (first iteration, large change, too many candidates): the caller falls back.
+// the radix path).  Returns SEL_OK, or — before touching global state — the SelectOutcome of the
+// first check that failed when the prediction does not bracket the ranks (first iteration, large
+// change, too many candidates): the caller falls back.
 template <bool MULTI>
-__device__ bool predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, const DevState* st,
-                                     unsigned int& n1_out, double& median, double& mad) {
+__device__ int predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, const DevState* st,
+                                    unsigned int& n1_out, double& median, double& mad) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const double pm = st->pred_med, pd = st->pred_mad;
   constexpr int PER = (LH_BINS + RS_THREADS - 1) / RS_THREADS;
@@ -920,11 +921,11 @@ __device__ bool predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, cons
   const unsigned int under = wk.lin_hist[LH_BINS], over = wk.lin_hist[LH_BINS + 1];
   const unsigned int n1 = under + total_in + over;
   n1_out = n1;
-  if (n1 == 0) return true;
+  if (n1 == 0) return SEL_OK;
   const unsigned int k = (n1 - 1) >> 1;
   const bool even = ((n1 & 1u) == 0u);
   const unsigned int k2 = k + (even ? 1u : 0u);
-  if (k < under || k2 >= under + total_in) return false;
+  if (k < under || k2 >= under + total_in) return SEL_MEDIAN_OUTSIDE;
   const unsigned int r = k - under, r2 = k2 - under;
   // bins of the two middle ranks: first b with P[b] > r
 #pragma unroll
@@ -938,12 +939,12 @@ __device__ bool predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, cons
   }
   __syncthreads();
   const int bm = s.lh_i[0], bm2 = s.lh_i[1];
-  if (bm < 0 || bm2 < bm) return false;
+  if (bm < 0 || bm2 < bm) return SEL_MEDIAN_NO_BIN;
   const int g = bm2 - bm;
-  if (g > 4) return false;
+  if (g > 4) return SEL_MEDIAN_GAP;
   const unsigned int below_m = (bm > 0) ? P[bm - 1] : 0u;
   const unsigned int cnt_med = P[bm2] - below_m;
-  if (cnt_med > (unsigned int)(RS_CAP - 2)) return false;
+  if (cnt_med > (unsigned int)(RS_CAP - 2)) return SEL_MEDIAN_CANDIDATES;
   const unsigned int kA = r - below_m;
   auto Nin = [&](int t) -> unsigned int {
     const int hi = min(bm2 + t, LH_BINS - 1), lo = bm - t - 1;
@@ -965,12 +966,12 @@ __device__ bool predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, cons
   }
   __syncthreads();
   const int t_hi = s.lh_i[2], t_lo = s.lh_i[3];
-  if (t_hi > LH_BINS) return false;
+  if (t_hi > LH_BINS) return SEL_MAD_BRACKET;
   const int e_lo = max(t_lo - g, 0), e_hi = t_hi + g + 1;
-  if (bm - e_hi < 0 || bm2 + e_hi > LH_BINS - 1) return false;  // candidates must be regular bins
+  if (bm - e_hi < 0 || bm2 + e_hi > LH_BINS - 1) return SEL_MAD_WINDOW;  // candidates must be regular bins
   const unsigned int n_inner = (t_lo - g - 1 >= 0) ? Nin(t_lo - g - 1) : 0u;
   const unsigned int cnt_edge = Nin(e_hi) - n_inner;
-  if (cnt_edge > (unsigned int)(RS_CAP - 2) || k < n_inner || k2 - n_inner >= cnt_edge) return false;
+  if (cnt_edge > (unsigned int)(RS_CAP - 2) || k < n_inner || k2 - n_inner >= cnt_edge) return SEL_MAD_CANDIDATES;
   const unsigned int kM = k - n_inner;
   __syncthreads();
 
@@ -1009,7 +1010,7 @@ __device__ bool predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, cons
   block_select(s, s.sortbuf, (int)cnt_edge, kM, 64, ~0ull, klo, khi);
   mad = even ? (a.variant ? key_to_f64(khi) : 0.5 * (key_to_f64(klo) + key_to_f64(khi))) : key_to_f64(klo);
   __syncthreads();
-  return true;
+  return SEL_OK;
 }
 
 template <bool MULTI>
@@ -1040,9 +1041,15 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
   // ---- A + B: median and MAD of the planarity survivors
   unsigned int n1 = 0;
   double median = 0.0, mad = 0.0;
-  bool fast = false;
+  int sel = SEL_NOT_ATTEMPTED;
   if (a.hist_expected && st->pred_valid && st->pred_minpl == a.stat_minpl && st->pred_mad > 0.0)
-    fast = predicted_median_mad<MULTI>(s, a, wk, st, n1, median, mad);
+    sel = predicted_median_mad<MULTI>(s, a, wk, st, n1, median, mad);
+  const bool fast = sel == SEL_OK;
+  if (blockIdx.x == 0 && tid == 0) {
+    wk.phase_t[29] = fast ? SEL_PATH_PREDICT : SEL_PATH_RADIX;
+    wk.phase_t[31] = sel;
+    if (!fast) wk.phase_t[26] = wk.phase_t[27] = 0;  // the radix select writes its own counts
+  }
   sicp_iter_record* rec = a.rec;
   if (!fast) {
     __syncthreads();
@@ -1465,7 +1472,6 @@ struct SharedF {
   int is_last;
 };
 
-// Plan + gather + selection; true on success (median, mad, n1 set; n1 == 0 is a success).
 // k-th smallest (0-based) and its successor among n <= RS_THREADS keys in shared memory by direct
 // ranking — three block barriers instead of the eight radix passes block_select() needs when the
 // keys share their leading bytes (they always do here: the candidates come from a handful of
@@ -1501,8 +1507,10 @@ __device__ __forceinline__ void rank_select(Shared& s, const unsigned long long*
 }
 
 #define RSF_STAMP(i) do { if (bid == 0 && tid == 0) wk.phase_t[i] = global_timer_ns(); } while (0)
-__device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevState* st,
-                             unsigned int& n1_out, double& median, double& mad, const int G, const int bid) {
+// Plan + gather + selection; SEL_OK on success (median, mad, n1 set; n1 == 0 is a success), else
+// the SelectOutcome of the first check that failed.
+__device__ int fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevState* st,
+                            unsigned int& n1_out, double& median, double& mad, const int G, const int bid) {
   Shared& s = sf.s;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int PER = (LH_BINS + RS_THREADS - 1) / RS_THREADS;
@@ -1540,11 +1548,11 @@ __device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevS
   const unsigned int* P = s.hist;
   const unsigned int n1 = under + total_in + over;
   n1_out = n1;
-  if (n1 == 0) return true;
+  if (n1 == 0) return SEL_OK;
   const unsigned int k = (n1 - 1) >> 1;
   const bool even = ((n1 & 1u) == 0u);
   const unsigned int k2 = k + (even ? 1u : 0u);
-  if (k < under || k2 >= under + total_in) return false;
+  if (k < under || k2 >= under + total_in) return SEL_MEDIAN_OUTSIDE;
   const unsigned int r = k - under, r2 = k2 - under;
   // The plan searches monotone sequences in every thread (uniform shared-memory addresses, no
   // barrier): the prefix sums P, and the symmetric counts N_in(t) below, both non-decreasing.
@@ -1559,10 +1567,10 @@ __device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevS
   // bins of the two middle ranks (r2 < total_in = P[LH_BINS - 1])
   const int bm = first_above(r, 0, LH_BINS - 1), bm2 = first_above(r2, bm, LH_BINS - 1);
   const int g = bm2 - bm;
-  if (g > 4) return false;
+  if (g > 4) return SEL_MEDIAN_GAP;
   const unsigned int below_m = (bm > 0) ? P[bm - 1] : 0u;
   const unsigned int cnt_med = P[bm2] - below_m;
-  if (cnt_med > (unsigned int)(RS_CAP - 2)) return false;
+  if (cnt_med > (unsigned int)(RS_CAP - 2)) return SEL_MEDIAN_CANDIDATES;
   const unsigned int kA = r - below_m;
   auto Nin = [&](int t) -> unsigned int {
     const int hi = min(bm2 + t, LH_BINS - 1), lo = bm - t - 1;
@@ -1579,12 +1587,12 @@ __device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevS
   };
   const int t_hi = first_nin_above(k2);     // smallest t with N_in(t) >= k2 + 1
   const int t_lo = first_nin_above(k) - 1;  // largest t with N_in(t) <= k (-1: none)
-  if (t_hi > LH_BINS) return false;
+  if (t_hi > LH_BINS) return SEL_MAD_BRACKET;
   const int e_lo = max(t_lo - g, 0), e_hi = t_hi + g + 1;
-  if (bm - e_hi < 0 || bm2 + e_hi > LH_BINS - 1) return false;
+  if (bm - e_hi < 0 || bm2 + e_hi > LH_BINS - 1) return SEL_MAD_WINDOW;
   const unsigned int n_inner = (t_lo - g - 1 >= 0) ? Nin(t_lo - g - 1) : 0u;
   const unsigned int cnt_edge = Nin(e_hi) - n_inner;
-  if (cnt_edge > (unsigned int)(RS_CAP - 2) || k < n_inner || k2 - n_inner >= cnt_edge) return false;
+  if (cnt_edge > (unsigned int)(RS_CAP - 2) || k < n_inner || k2 - n_inner >= cnt_edge) return SEL_MAD_CANDIDATES;
   const unsigned int kM = k - n_inner;
   RSF_STAMP(10);
 
@@ -1623,7 +1631,7 @@ __device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevS
                                   : member(edge_hi_start + (u - c_low), bm2 + el, hi_b);
     }
   }
-  if (__syncthreads_or(over_cap)) return false;
+  if (__syncthreads_or(over_cap)) return SEL_BIN_CAP;
   RSF_STAMP(11);
   unsigned long long klo, khi;
   if (cnt_med <= (unsigned int)RS_THREADS) rank_select(s, s.sortbuf, (int)cnt_med, kA, klo, khi);
@@ -1641,7 +1649,7 @@ __device__ bool fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevS
     wk.phase_t[26] = cnt_med;
     wk.phase_t[27] = cnt_edge;
   }
-  return true;
+  return SEL_OK;
 }
 
 __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int bid, SharedF& sf) {
@@ -1679,8 +1687,15 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
   // ---- select (every block, identical result)
   unsigned int n1 = 0;
   double median = 0.0, mad = 0.0;
-  bool ok = a.hist_expected && st->pred_valid && st->pred_minpl == a.stat_minpl && st->pred_mad > 0.0;
-  if (ok) ok = fused_select(sf, a, wk, st, n1, median, mad, G, bid);
+  int sel = SEL_NO_PREDICTION;
+  if (a.hist_expected && st->pred_valid && st->pred_minpl == a.stat_minpl && st->pred_mad > 0.0)
+    sel = fused_select(sf, a, wk, st, n1, median, mad, G, bid);
+  bool ok = sel == SEL_OK;
+  if (bid == 0 && tid == 0) {
+    wk.phase_t[30] = sel;
+    if (ok || G == 1) wk.phase_t[29] = ok ? SEL_PATH_BINSTORE : SEL_PATH_RADIX;
+    if (!ok) wk.phase_t[26] = wk.phase_t[27] = 0;  // the radix fallback writes its own counts
+  }
   if (!ok && G == 1) {
     // a single block owns the whole problem (K <= 4096, or one pair of a batch): no prediction —
     // first iteration, large change — simply means the radix selection, here and now

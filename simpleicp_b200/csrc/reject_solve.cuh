@@ -53,6 +53,30 @@ __host__ __device__ inline int lh_bin(double d, double med, double mad) {
   return (int)t;
 }
 
+// Diagnostics written by block 0, thread 0 of the reject/solve kernels (sicp_get_phase_times).
+// Slot 29: which selection produced the record's median and MAD.
+enum SelectPath : int {
+  SEL_PATH_RADIX = 0,    // radix_median: iteration 0, the stage API, every fallback
+  SEL_PATH_PREDICT = 1,  // predicted_median_mad: gather pass of the cooperative kernel
+  SEL_PATH_BINSTORE = 2, // fused_select: per-bin key store of k_rs_fused / k_rs_batch
+};
+// Slot 30 (last k_rs_fused / k_rs_batch launch) and slot 31 (last k_reject_solve launch): outcome
+// of the attempt to select from the predictor histogram.  0 = used, else the first check that
+// failed.  _capi.py mirrors these values.
+enum SelectOutcome : int {
+  SEL_OK = 0,
+  SEL_NO_PREDICTION = 1,      // k_rs_fused: no histogram, no valid predictor, or one for another planarity bound
+  SEL_NOT_ATTEMPTED = 2,      // k_reject_solve: the same conditions; the radix select ran directly
+  SEL_MEDIAN_OUTSIDE = 3,     // a middle rank lies in the under- or overflow counter
+  SEL_MEDIAN_NO_BIN = 4,      // predicted_median_mad: no bin holds a middle rank (guard; the prefix sums rule it out)
+  SEL_MEDIAN_GAP = 5,         // the bins of the two middle ranks are more than 4 bins apart
+  SEL_MEDIAN_CANDIDATES = 6,  // the median bins hold more than RS_CAP - 2 members
+  SEL_MAD_BRACKET = 7,        // the regular bins hold fewer than k2 + 1 members: no MAD bracket
+  SEL_MAD_WINDOW = 8,         // the MAD candidate window runs past the regular bins
+  SEL_MAD_CANDIDATES = 9,     // the MAD window holds more than RS_CAP - 2 members
+  SEL_BIN_CAP = 10,           // fused_select: a candidate bin has more members than the key store holds
+};
+
 struct RSArgs {
   long long K;
   const double* dist;
