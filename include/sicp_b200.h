@@ -94,6 +94,8 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value);
  *        query in the grid search: 0 = by K, 1, 4, 8, 16), "rs_blocks" (blocks of the cooperative
  *        reject/solve kernel, 0 = one per SM), "fused" (1: iterations after the first run their
  *        reject + solve in the barrier-free kernel, 0: always the cooperative kernel),
+ *        "split_solve" (1: the serial part of the barrier-free kernel runs in a one-block kernel
+ *        launched behind it, 0: in the kernel's last block; the results are the same bit for bit),
  *        "warm_start" (1: the grid search of an iteration starts from the previous iteration's
  *        neighbour as upper bound), "keep_knn" (see sicp_get_knn), "knn_coop" (k-NN search: 1 cooperative
  *        lanes per query (k <= 16), 0 one thread per query, -1 (default) by the number of queries),

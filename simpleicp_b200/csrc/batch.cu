@@ -115,14 +115,12 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   b.lin_hist.reserve((size_t)n_pairs * (LH_BINS + 2));
   b.rec.reserve((size_t)n_pairs * (size_t)p.max_iterations);
   b.partials.reserve((size_t)n_pairs * 96 + 16);
-  b.ticket.reserve(n_pairs);
   b.phase_t.reserve((size_t)n_pairs * 32);
   b.flags.reserve(2 * (size_t)n_pairs);
   b.results.reserve(n_pairs);
   pinned_reserve(b.flags_host, b.flags_cap, 2 * (size_t)n_pairs);
   pinned_reserve(b.results_host, b.results_cap, (size_t)n_pairs);
   SICP_CUDA(cudaMemsetAsync(b.lin_hist.p, 0, sizeof(unsigned int) * (size_t)n_pairs * (LH_BINS + 2), st));
-  SICP_CUDA(cudaMemsetAsync(b.ticket.p, 0, sizeof(unsigned int) * (size_t)n_pairs, st));
   SICP_CUDA(cudaMemsetAsync(b.rec.p, 0, sizeof(sicp_iter_record) * (size_t)n_pairs * (size_t)p.max_iterations, st));
   SICP_CUDA(cudaMemsetAsync(b.nn_pos.p, 0xff, sizeof(uint32_t) * nq, st));
   SICP_CUDA(cudaMemsetAsync(b.keep.p, 0, nq, st));

@@ -319,6 +319,7 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.upload_threads = d.upload_threads;
     c.up.chunk = d.up.chunk;
     c.fused = d.fused;
+    c.split_solve = d.split_solve;
     c.warm_start = d.warm_start;
     c.sphere_scan = d.sphere_scan;
     c.pdl = d.pdl;
@@ -353,6 +354,8 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.warm_start = (value != 0) ? 1 : 0;
   } else if (k == "fused") {
     c.fused = (value != 0) ? 1 : 0;
+  } else if (k == "split_solve") {
+    c.split_solve = (value != 0) ? 1 : 0;
   } else if (k == "rs_blocks") {
     SICP_REQUIRE(value >= 0 && value <= 256, SICP_ERR_BAD_ARG, "rs_blocks out of range");
     c.rs_blocks = (int)value;
@@ -1077,10 +1080,11 @@ int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32]) {
   unsigned long long t[32];
   SICP_CUDA(cudaMemcpyAsync(t, c.phase_t.p, sizeof(t), cudaMemcpyDeviceToHost, c.stream));
   sync(c);
-  // slot 23 (kernel entry, before the dependent-launch wait) precedes stamp 0: signed offset
+  // slot 23 (kernel entry, before the dependent-launch wait) precedes stamp 0, and so may k_rs_solve's
+  // slots 1, 5 and 6 (entry, end of the rehearsal, wait released): signed offsets
   for (int i = 0; i < 32; ++i)
     us[i] = (i >= 24) ? (double)t[i]
-            : (i == 23) ? (double)(long long)(t[23] - t[0]) * 1e-3
+            : (i == 23 || (t[28] == 2 && (i == 1 || i == 5 || i == 6))) ? (double)(long long)(t[i] - t[0]) * 1e-3
                         : ((t[i] >= t[0]) ? (double)(t[i] - t[0]) * 1e-3 : -1.0);
   API_END
 }

@@ -138,6 +138,9 @@ struct Ctx {
   bool rsb_attr_set = false;
   bool rsf_attr_set = false;              // k_rs_fused's dynamic shared memory limit raised on this device
   DevBuf<unsigned int> rsf_ticket;        // blocks-finished counter of the barrier-free reject/solve kernel
+  int split_solve = 1;                    // option "split_solve": 1 = its serial tail in k_rs_solve, 0 = in its last block
+  DevBuf<RsSelect> rs_sel;                // k_rs_fused -> k_rs_solve
+  DevBuf<RsScratch> rs_scratch;           // stores of k_rs_solve's rehearsal
   int n_fused_last = 0, n_rerun_last = 0; // last run: iterations through k_rs_fused / repeated after a missed prediction
   int fused = 1;                          // option "fused": 0 = always the cooperative kernel
   bool bf_attr_set = false;               // k_bf_nn's dynamic shared memory limit raised on this device
@@ -214,7 +217,6 @@ struct Batch {
   DevBuf<unsigned int> lin_hist;       // n_pairs x (LH_BINS + 2)
   DevBuf<sicp_iter_record> rec;        // n_pairs x max_iterations
   DevBuf<double> partials;             // n_pairs x RSF_NPART (+ slack)
-  DevBuf<unsigned int> ticket;         // n_pairs
   DevBuf<unsigned long long> phase_t;  // 32 (diagnostics of pair 0)
   DevBuf<int> flags;                   // n_pairs x 2: {stop, iterations_done}
   DevBuf<sicp_pair_result> results;

@@ -1437,8 +1437,10 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 //   accumulate each block streams its share of (normal, distance, matched point, fixed point) —
 //              the match kernel stored the matched point, so there is no index chase — and
 //              writes keep flags and per-block partial sums.
-//   solve      the block that takes the LAST ticket reduces the partials in a fixed order and runs
-//              the Gauss-Newton loop; everybody else has already left the SM.
+//   solve      rs_tail reduces the partials in a fixed order and runs the Gauss-Newton loop: for
+//              more than one block in k_rs_solve, a one-block kernel launched behind this one
+//              (option split_solve 0: in the block that takes the LAST ticket; everybody else
+//              has already left the SM).
 //   statistics mean and standard deviation of the residuals at the solution come from the moment
 //              sums themselves (sum r = theta . sum phi, sum r^2 = theta^T M theta): no residual pass
 //              and no barrier in the loop.  The residual VECTOR of the final iteration is evaluated
@@ -1452,12 +1454,25 @@ constexpr int RSF_NACC = 30;             // accumulators per role
 constexpr int RSF_NPART = 3 * RSF_NACC;  // partial sums per block
 
 constexpr int RSF_TILE = 768;  // correspondences per TMA-staged tile of the moment pass
-// Grid cap of the fused kernel (H100: 132 SMs).  The last block keeps 32 x NB partial loads in
-// flight per value, NB = RSF_MAX_BLOCKS / 32 doubles per lane and value.
+// Grid cap of the fused kernel (H100: 132 SMs; the launch also leaves one SM to k_rs_solve).  The
+// serial tail keeps 32 x NB partial loads in flight per value, NB = RSF_MAX_BLOCKS / 32 doubles per
+// lane and value.
 constexpr int RSF_MAX_BLOCKS = 160;
+constexpr size_t RSF_PARTIALS = (size_t)RSF_NPART * RSF_MAX_BLOCKS;  // one half of ws.partials
 
-struct SharedF {
+// k_rs_fused variants.  SINGLE: one block owns the whole problem (K <= 4096, and k_rs_batch) and
+// runs the serial tail itself.  TICKET: many blocks, the last one to finish runs the tail (option
+// split_solve = 0).  SPLIT: many blocks that only select and accumulate; k_rs_solve runs the tail.
+enum FusedMode : int { RSF_SINGLE = 0, RSF_TICKET = 1, RSF_SPLIT = 2 };
+
+// what the serial tail uses of the shared memory
+struct SharedTail {
   Shared s;
+  double totf[RSF_NPART];
+  double m1[13];  // sum phi
+};
+
+struct SharedF : SharedTail {
   // the block's share of (normal, distance, matched point), staged by 1-D TMA bulk copies that are
   // issued at kernel entry: the moment pass does not depend on the select, only the keep test
   // does, so the data crosses L2/HBM while the block works out median and MAD
@@ -1467,8 +1482,6 @@ struct SharedF {
   unsigned long long edgebuf[RS_CAP];  // MAD candidates (the median candidates go to s.sortbuf)
   alignas(8) uint64_t t_bar;
   double redf[RS_WARPS][RSF_NACC];
-  double totf[RSF_NPART];
-  double m1[13];  // sum phi
   int is_last;
 };
 
@@ -1652,9 +1665,18 @@ __device__ int fused_select(SharedF& sf, const RSArgs& a, RSWork wk, const DevSt
   return SEL_OK;
 }
 
-__device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int bid, SharedF& sf) {
+__device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, const RSWork& wk,
+                                             const double* partials, const int G, const bool ok,
+                                             const unsigned int n1, const double median, const double mad,
+                                             const bool live);
+__device__ __noinline__ void rs_tail(SharedTail& sf, const RSArgs& a, const RSWork& wk, const double* partials,
+                                     const int G, const bool ok, const unsigned int n1, const double median,
+                                     const double mad, const bool live);
+
+template <int MODE>
+__device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, const int bid, SharedF& sf) {
   Shared& s = sf.s;
-  DevState* st = a.state;
+  const DevState* st = a.state;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const long long K = a.K;
   RSF_STAMP(23);            // kernel entry, before the wait (negative offset from stamp 0)
@@ -1693,23 +1715,25 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
   bool ok = sel == SEL_OK;
   if (bid == 0 && tid == 0) {
     wk.phase_t[30] = sel;
-    if (ok || G == 1) wk.phase_t[29] = ok ? SEL_PATH_BINSTORE : SEL_PATH_RADIX;
+    if (ok || MODE == RSF_SINGLE) wk.phase_t[29] = ok ? SEL_PATH_BINSTORE : SEL_PATH_RADIX;
     if (!ok) wk.phase_t[26] = wk.phase_t[27] = 0;  // the radix fallback writes its own counts
   }
-  if (!ok && G == 1) {
-    // a single block owns the whole problem (K <= 4096, or one pair of a batch): no prediction —
-    // first iteration, large change — simply means the radix selection, here and now
-    __syncthreads();
-    radix_median<false, 0>(s, a, wk, 0.0, n1, 0, 1);
-    if (n1 != 0) {
-      median = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
+  if constexpr (MODE == RSF_SINGLE) {
+    if (!ok) {
+      // a single block owns the whole problem (K <= 4096, or one pair of a batch): no prediction —
+      // first iteration, large change — simply means the radix selection, here and now
       __syncthreads();
-      unsigned int n1b = 0;
-      radix_median<false, 1>(s, a, wk, median, n1b, 0, 1);
-      mad = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
+      radix_median<false, 0>(s, a, wk, 0.0, n1, 0, 1);
+      if (n1 != 0) {
+        median = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
+        __syncthreads();
+        unsigned int n1b = 0;
+        radix_median<false, 1>(s, a, wk, median, n1b, 0, 1);
+        mad = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
+      }
+      __syncthreads();
+      ok = true;
     }
-    __syncthreads();
-    ok = true;
   }
   const double lim = a.variant ? 3.0 * (1.4826 * mad) : 3.0 * mad;
   RSF_STAMP(2);
@@ -1800,37 +1824,85 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
   }
   RSF_STAMP(3);
 
-  // ---- ticket: the last block to arrive owns the serial part
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) {
-    const unsigned int t = atomicAdd(wk.ticket, 1u);
-    sf.is_last = (t == (unsigned int)G - 1u) ? 1 : 0;
+  if constexpr (MODE == RSF_SPLIT) {
+    // every block reached the same outcome: block 0 hands it to k_rs_solve
+    if (bid == 0 && tid == 0) *wk.sel = RsSelect{median, mad, n1, ok ? 1 : 0};
+    return;
   }
-  __syncthreads();
-  if (!sf.is_last) return;
   __threadfence();
+  __syncthreads();
+  if constexpr (MODE == RSF_TICKET) {
+    // ---- ticket: the last block to arrive owns the serial part
+    if (tid == 0) {
+      const unsigned int t = atomicAdd(wk.ticket, 1u);
+      sf.is_last = (t == (unsigned int)G - 1u) ? 1 : 0;
+    }
+    __syncthreads();
+    if (!sf.is_last) return;
+    __threadfence();
+    if (tid == 0) *wk.ticket = 0u;
+#ifdef SICP_RS_REHEARSE_PROBE
+    // diagnostics build (tools/build_variants.py): the last block runs the tail twice, first as
+    // the rehearsal (stamps 1 and 5), to time a warm pass (stamps 4 to 9) against a cold one
+    if (tid == 0) wk.phase_t[1] = global_timer_ns();
+    rs_tail(sf, a, wk, wk.partials, G, ok, n1, median, mad, false);
+    __syncthreads();
+    if (tid == 0) wk.phase_t[5] = global_timer_ns();
+#endif
+  }
+  // one block (K <= 4096, k_rs_batch): inlined, the arguments stay where the kernel has them
+  if constexpr (MODE == RSF_SINGLE) rs_tail_body(sf, a, wk, wk.partials, G, ok, n1, median, mad, true);
+  else rs_tail(sf, a, wk, wk.partials, G, ok, n1, median, mad, true);
+}
+
+// Not inlined, so that k_rs_solve's rehearsal and its real pass run the same code.
+__device__ __noinline__ void rs_tail(SharedTail& sf, const RSArgs& a, const RSWork& wk, const double* partials,
+                                     const int G, const bool ok, const unsigned int n1, const double median,
+                                     const double mad, const bool live) {
+  rs_tail_body(sf, a, wk, partials, G, ok, n1, median, mad, live);
+}
+
+// The serial part of k_rs_fused, run by a whole block: fixed-order reduction of the per-block
+// partials, M, the solve, the statistics and the stores.  live == false is k_rs_solve's
+// rehearsal: the same instructions on whatever `partials` holds, with every store sent to
+// wk.scratch.  It reads the loop state and writes nothing a run can see; what it leaves behind
+// is this SM's instruction and constant caches filled with the tail's code, which the real pass
+// would otherwise fetch on its critical path.
+__device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, const RSWork& wk,
+                                             const double* partials, const int G, const bool ok,
+                                             const unsigned int n1, const double median, const double mad,
+                                             const bool live) {
+  Shared& s = sf.s;
+  const DevState* st = a.state;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long K = a.K;
+  DevState* sto = live ? a.state : &wk.scratch->st;
+  sicp_iter_record* rec = live ? a.rec : &wk.scratch->rec;
+  unsigned long long* pt = live ? wk.phase_t : wk.scratch->phase_t;
+  unsigned int* lin_hist = live ? wk.lin_hist : wk.scratch->lin_hist;
   // state the serial tail needs: requested now, so that the round trips overlap the partial sums
   const double prev_mean = __ldcg(&st->prev_mean), prev_std = __ldcg(&st->prev_std), w_state = __ldcg(&st->w);
   const unsigned int n_bf = a.unresolved ? __ldcg(&a.unresolved[K]) : 0u;
   if (tid == 0) {
-    *wk.ticket = 0u;
-    if (a.unresolved) a.unresolved[K] = 0u;  // read above (n_bf): the next match starts from a clean counter
-    wk.phase_t[4] = global_timer_ns();
-    wk.phase_t[28] = 2;  // fused path
+    // read above (n_bf): the next match starts from a clean counter
+    if (a.unresolved) *(live ? &a.unresolved[K] : &wk.scratch->unresolved) = 0u;
+    pt[4] = global_timer_ns();
+    pt[28] = 2;  // fused path
   }
   // the predictor histogram has been consumed by every block: leave it zeroed for the next match
-  for (int i = tid; i < LH_BINS + 2; i += RS_THREADS) wk.lin_hist[i] = 0;
-  sicp_iter_record* rec = a.rec;
+  for (int i = tid; i < LH_BINS + 2; i += RS_THREADS) lin_hist[i] = 0;
   if (!ok) {
-    if (tid == 0) st->stop = 3;  // re-run this iteration with the general kernel (host)
+    if (tid == 0) sto->stop = 3;  // re-run this iteration with the general kernel (host)
     return;
   }
+  const Rigid Tin = st->T;
+  double cm[3] = {a.cm[0], a.cm[1], a.cm[2]}, cf[3];
+  rigid_apply(Tin, cm[0], cm[1], cm[2], cf[0], cf[1], cf[2]);
   if (n1 == 0) {
     if (tid == 0) {
       rec->n_kept = 0;
       rec->median = rec->mad = nan("");
-      st->n_kept = 0;
+      sto->n_kept = 0;
     }
     return;
   }
@@ -1845,7 +1917,7 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
 #pragma unroll
       for (int u = 0; u < NB; ++u) {
         const int b = lane + 32 * u;
-        r[q][u] = (o < RSF_NPART && b < G) ? __ldcg(&wk.partials[(size_t)o * G + b]) : 0.0;
+        r[q][u] = (o < RSF_NPART && b < G) ? __ldcg(&partials[(size_t)o * G + b]) : 0.0;
       }
     }
 #pragma unroll
@@ -1859,7 +1931,7 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
     }
   }
   __syncthreads();
-  if (tid == 0) wk.phase_t[17] = global_timer_ns();
+  if (tid == 0) pt[17] = global_timer_ns();
   for (int e = tid; e < 169 + 13; e += RS_THREADS) {
     if (e >= 169) {
       const int o = e - 169;
@@ -1884,7 +1956,7 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
     s.M[r][c] = vv;
   }
   __syncthreads();
-  if (tid == 0) wk.phase_t[18] = global_timer_ns();
+  if (tid == 0) pt[18] = global_timer_ns();
   if (warp != 0) return;
   if (lane < 13) s.th_in[lane] = (lane == 12) ? 0.0 : theta_entry(Tin, cm, cf, lane);
   __syncwarp();
@@ -1915,25 +1987,25 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
     lm_solve(s, a, w, st->x, cm, cf, lo, lane);
   }
   if (lane == 0) {
-    wk.phase_t[19] = global_timer_ns();
-    wk.phase_t[21] = s.stamp[0];
-    wk.phase_t[22] = s.stamp[1];
+    pt[19] = global_timer_ns();
+    pt[21] = s.stamp[0];
+    pt[22] = s.stamp[1];
     rec->n_kept = n_kept;
     rec->median = median;
     rec->mad = mad;
-    st->pred_med = median;
-    st->pred_mad = mad;
-    st->pred_minpl = a.stat_minpl;
-    st->pred_valid = (mad > 0.0 && isfinite(mad) && isfinite(median)) ? 1 : 0;
+    sto->pred_med = median;
+    sto->pred_mad = mad;
+    sto->pred_minpl = a.stat_minpl;
+    sto->pred_valid = (mad > 0.0 && isfinite(mad) && isfinite(median)) ? 1 : 0;
     rec->mean_dist = mean_d;
     rec->std_dist = sqrt(a.variant ? var_d1 : var_d);
     rec->distance_weight = w;
     rec->lm_iterations = lo.iters;
     rec->n_bruteforce = (int)n_bf;
-    st->n_kept = n_kept;
-    st->skip = skip;
-    st->w = w;
-    if (n_kept < 6 && a.do_solve && a.arm_stop) st->stop = 2;
+    sto->n_kept = n_kept;
+    sto->skip = skip;
+    sto->w = w;
+    if (n_kept < 6 && a.do_solve && a.arm_stop) sto->stop = 2;
   }
   if (skip) return;
   // new transform(s)
@@ -1975,56 +2047,83 @@ __device__ void rs_fused_body(const RSArgs& a, RSWork wk, const int G, const int
   }
   if (a.variant) {
     if (lane < 6) {
-      st->sigma[lane] = nan("");
+      sto->sigma[lane] = nan("");
       rec->x[lane] = pick(lo.x, lane);
     }
   } else {
     if ((stop && a.arm_stop) || a.want_sigma) {
-      if (lane < 36) st->An[lane] = s.Ak[lane];
-      if (lane + 32 < 36) st->An[lane + 32] = s.Ak[lane + 32];
+      if (lane < 36) sto->An[lane] = s.Ak[lane];
+      if (lane + 32 < 36) sto->An[lane + 32] = s.Ak[lane + 32];
       __syncwarp();
-      uncertainties(s, a, s.Ak, w, lo.x, sum_r2, n_kept, lane, st->sigma);
+      uncertainties(s, a, s.Ak, w, lo.x, sum_r2, n_kept, lane, sto->sigma);
     }
     if (lane < 6) {
       const double xl = pick(lo.x, lane);
       rec->x[lane] = xl;
-      st->x[lane] = xl;
-      st->x_new[lane] = xl;
+      sto->x[lane] = xl;
+      sto->x_new[lane] = xl;
     }
   }
   if (lane == 0) {
     if (a.variant) {
-      for (int j = 0; j < 6; ++j) st->x_new[j] = lo.x[j];
+      for (int j = 0; j < 6; ++j) sto->x_new[j] = lo.x[j];
       const Rigid Hr = st->H_rep;
-      st->H_rep = (a.variant == SICP_VARIANT_LINEARIZED_CPP) ? rigid_compose(Hr, dH) : rigid_compose(dH, Hr);
+      sto->H_rep = (a.variant == SICP_VARIANT_LINEARIZED_CPP) ? rigid_compose(Hr, dH) : rigid_compose(dH, Hr);
     } else {
-      st->H_rep = T_new;
+      sto->H_rep = T_new;
     }
-    st->lm_ok = lo.ok;
-    st->T_new = T_new;
-    st->T_res = T_res;
-    st->T = T_new;
-    st->Tinv = rigid_inverse(T_new);
+    sto->lm_ok = lo.ok;
+    sto->T_new = T_new;
+    sto->T_res = T_res;
+    sto->T = T_new;
+    sto->Tinv = rigid_inverse(T_new);
     rec->mean_res = mean;
     rec->std_res = sd;
     // predictor of the next iteration from the residuals at the new transform (see k_reject_solve)
     if (sd > 0.0 && isfinite(sd) && isfinite(mean)) {
-      st->pred_med = mean;
-      st->pred_mad = 0.8 * sd;
-      st->pred_valid = 1;
+      sto->pred_med = mean;
+      sto->pred_mad = 0.8 * sd;
+      sto->pred_valid = 1;
     }
-    st->prev_mean = mean;
-    st->prev_std = sd;
-    st->iterations_done = a.it + 1;
-    if (stop && a.arm_stop) st->stop = 1;
-    st->converged = stop;
-    wk.phase_t[9] = global_timer_ns();
+    sto->prev_mean = mean;
+    sto->prev_std = sd;
+    sto->iterations_done = a.it + 1;
+    if (stop && a.arm_stop) sto->stop = 1;
+    sto->converged = stop;
+    pt[9] = global_timer_ns();
   }
 }
 
-__global__ void __launch_bounds__(RS_THREADS, 1) k_rs_fused(RSArgs a, RSWork wk) {
+template <int MODE>
+// (__grid_constant__: rs_tail takes the arguments by reference, straight from the parameter space)
+__global__ void __launch_bounds__(RS_THREADS, 1) k_rs_fused(const __grid_constant__ RSArgs a,
+                                                            const __grid_constant__ RSWork wk) {
   extern __shared__ __align__(16) unsigned char rsf_smem[];
-  rs_fused_body(a, wk, gridDim.x, blockIdx.x, *reinterpret_cast<SharedF*>(rsf_smem));
+  rs_fused_body<MODE>(a, wk, gridDim.x, blockIdx.x, *reinterpret_cast<SharedF*>(rsf_smem));
+}
+
+// The serial tail of k_rs_fused<RSF_SPLIT>, one block launched right behind it with PDL.  The
+// select/accumulate grid leaves one SM free (rs_fused_launch), so this block is resident while
+// those blocks still run.  It rehearses the tail on the previous iteration's partials (the other
+// half of ws.partials: complete, and of the same shape, so the rehearsal walks the branches of a
+// real iteration), then waits for the grid in griddepcontrol.wait and runs the tail for real.
+__global__ void __launch_bounds__(RS_THREADS, 1) k_rs_solve(const __grid_constant__ RSArgs a,
+                                                            const __grid_constant__ RSWork wk, int G, int rehearse) {
+  extern __shared__ __align__(16) unsigned char rss_smem[];
+  SharedTail& sh = *reinterpret_cast<SharedTail*>(rss_smem);
+  const int tid = threadIdx.x;
+  pdl_launch_dependents();  // the next match may take the SMs the select blocks leave
+  if (tid == 0) wk.phase_t[1] = global_timer_ns();
+  if (rehearse) {
+    rs_tail(sh, a, wk, wk.partials_prev, G, true, 1u, 0.0, 0.0, false);
+    __syncthreads();
+  }
+  if (tid == 0) wk.phase_t[5] = global_timer_ns();
+  pdl_wait();
+  if (tid == 0) wk.phase_t[6] = global_timer_ns();
+  if (a.state->stop) return;
+  const RsSelect sel = *wk.sel;
+  rs_tail(sh, a, wk, wk.partials, G, sel.ok != 0, sel.n1, sel.median, sel.mad, true);
 }
 
 // Batched form: one block per pair, every per-query pointer offset by the pair's q_off.
@@ -2036,7 +2135,6 @@ struct BatchRsArgs {
   int rec_stride;
   unsigned int* lin_hist;
   double* partials;
-  unsigned int* ticket;
   unsigned long long* phase_t;
 };
 __global__ void __launch_bounds__(RS_THREADS, 1) k_rs_batch(BatchRsArgs b) {
@@ -2060,9 +2158,8 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_rs_batch(BatchRsArgs b) {
   RSWork wk{};
   wk.lin_hist = b.lin_hist + (size_t)pair * (LH_BINS + 2);
   wk.partials = b.partials + (size_t)pair * RSF_NPART;
-  wk.ticket = b.ticket + pair;
   wk.phase_t = b.phase_t + (size_t)pair * 32;
-  rs_fused_body(a, wk, 1, 0, *reinterpret_cast<SharedF*>(rsf_smem));
+  rs_fused_body<RSF_SINGLE>(a, wk, 1, 0, *reinterpret_cast<SharedF*>(rsf_smem));
 }
 
 // End of a batched run, one block per pair: residuals of the kept correspondences at the final
@@ -2359,16 +2456,30 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
 void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, int rec_slot,
                      bool want_sigma) {
   const long long K = c.K;
-  // K <= 4096: a single block (it never needs the host's re-run protocol, see rs_fused_body)
+  // K <= 4096: a single block (it never needs the host's re-run protocol, see rs_fused_body).
+  // Otherwise at most one block per SM but one: k_rs_solve's block takes the SM left free while
+  // the select blocks run (both forms use the same grid, so their sums are the same bit for bit).
   const int G = (K <= 4096) ? 1
-                            : (int)std::min<long long>(std::min(c.num_sms, RSF_MAX_BLOCKS),
+                            : (int)std::min<long long>(std::min(c.num_sms - 1, RSF_MAX_BLOCKS),
                                                        std::max<long long>(1, (K + 767) / 768));
+  const bool split = G > 1 && c.split_solve;
   if (!c.rsf_attr_set) {
-    SICP_CUDA(cudaFuncSetAttribute(k_rs_fused, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)sizeof(SharedF)));
+    SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_TICKET>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)sizeof(SharedF)));
+    SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)sizeof(SharedF)));
+    SICP_CUDA(cudaFuncSetAttribute(k_rs_solve, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)sizeof(SharedTail)));
     c.rsf_attr_set = true;
   }
-  c.ws.partials.reserve((size_t)c.num_sms * (RSF_NPART + 2) + 16);
+  // two halves, by iteration parity: the select blocks write one while k_rs_solve rehearses on the
+  // other.  Zeroed when allocated, so that the first rehearsal never reads uninitialised memory.
+  if (c.ws.partials.cap < 2 * RSF_PARTIALS) {
+    c.ws.partials.reserve(2 * RSF_PARTIALS);
+    SICP_CUDA(cudaMemsetAsync(c.ws.partials.p, 0, 2 * RSF_PARTIALS * sizeof(double), c.stream));
+  }
   c.keep.reserve(K);
   c.resid.reserve(K);
   c.phase_t.reserve(32);
@@ -2376,6 +2487,8 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
     c.rsf_ticket.reserve(4);
     SICP_CUDA(cudaMemsetAsync(c.rsf_ticket.p, 0, 4 * sizeof(unsigned int), c.stream));
   }
+  c.rs_sel.reserve(1);
+  c.rs_scratch.reserve(1);
   RSArgs a;
   a.K = K;
   a.dist = c.dist.p;
@@ -2409,11 +2522,27 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   a.m_xyz = c.m_xyz.p;
   a.want_sigma = want_sigma ? 1 : 0;
   RSWork wk{};
-  wk.partials = c.ws.partials.p;
+  wk.partials = c.ws.partials.p + (size_t)(it & 1) * RSF_PARTIALS;
+  wk.partials_prev = c.ws.partials.p + (size_t)((it & 1) ^ 1) * RSF_PARTIALS;
   wk.phase_t = c.phase_t.p;
   wk.lin_hist = c.lin_hist.p;
   wk.ticket = c.rsf_ticket.p;
-  launch_kernel(k_rs_fused, dim3(G), dim3(RS_THREADS), sizeof(SharedF), c.stream, c.pdl != 0, a, wk);
+  wk.sel = c.rs_sel.p;
+  wk.scratch = c.rs_scratch.p;
+  const bool pdl = c.pdl != 0;
+  if (G == 1) {
+    launch_kernel(k_rs_fused<RSF_SINGLE>, dim3(1), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
+  } else if (!split) {
+    launch_kernel(k_rs_fused<RSF_TICKET>, dim3(G), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
+  } else {
+    launch_kernel(k_rs_fused<RSF_SPLIT>, dim3(G), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
+    SICP_CUDA(cudaGetLastError());
+    c.tm.kernel_launches += 1;
+    // without PDL the solve block starts after the select grid has finished: a rehearsal would
+    // only lengthen the iteration
+    launch_kernel(k_rs_solve, dim3(1), dim3(RS_THREADS), sizeof(SharedTail), c.stream, pdl, a, wk, G,
+                  pdl ? 1 : 0);
+  }
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
@@ -2454,7 +2583,6 @@ void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool wa
   ba.rec_stride = p.max_iterations;
   ba.lin_hist = b.lin_hist.p;
   ba.partials = b.partials.p;
-  ba.ticket = b.ticket.p;
   ba.phase_t = b.phase_t.p;
   launch_kernel(k_rs_batch, dim3(b.n_pairs), dim3(RS_THREADS), sizeof(SharedF), c.stream, c.pdl != 0, ba);
   SICP_CUDA(cudaGetLastError());

@@ -117,6 +117,22 @@ __device__ __forceinline__ bool pl_keep(float w, double min_planarity, int pl_si
   return (double)w >= min_planarity;
 }
 
+// Outcome of the select every block of k_rs_fused (split form) computes; block 0 hands it to k_rs_solve.
+struct RsSelect {
+  double median, mad;
+  unsigned int n1;  // planarity survivors
+  int ok;           // 0: the prediction did not bracket the order statistics
+};
+
+// Where the rehearsal of k_rs_solve sends every store of the serial tail.
+struct RsScratch {
+  DevState st;
+  sicp_iter_record rec;
+  unsigned long long phase_t[32];
+  unsigned int lin_hist[LH_BINS + 2];
+  unsigned int unresolved;
+};
+
 struct RSWork {
   unsigned int* hist;
   unsigned int* hist_other;
@@ -129,7 +145,12 @@ struct RSWork {
   unsigned long long* phase_t;  // 32 x %globaltimer stamps of block 0 (diagnostics)
   unsigned int* barrier;        // {arrival count, generation} of the grid barrier
   unsigned int* lin_hist;       // LH_BINS + 2 counters filled by the match kernels
-  unsigned int* ticket;         // fused kernel: blocks finished so far (the last one solves)
+  unsigned int* ticket;         // fused kernel (split_solve 0): blocks finished so far (the last one solves)
+  // fused kernel, split form: the other half of the double-buffered partials (the previous
+  // iteration's), the select outcome and the rehearsal's store target
+  const double* partials_prev;
+  RsSelect* sel;
+  RsScratch* scratch;
 };
 
 #ifdef __CUDACC__
