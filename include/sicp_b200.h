@@ -325,6 +325,14 @@ int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32] /*[h]*/);
  * median and MAD, which is what tests use this for.                                            */
 int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double min_planarity);
 
+/* Test-only: the uniform grid the searches run on.  side 0 = the fixed cloud's grid (k-NN of the
+ * normals; built by sicp_estimate_normals), 1 = the movable cloud's grid (correspondences; built
+ * by sicp_set_clouds).  o = origin (the cloud's bounding-box minimum), h = cell size, dims = cells
+ * per axis; a point v lies in cell floor((v - o) / h) of each axis.  Tests use it to place points
+ * relative to the real cell faces.  SICP_ERR_STATE if that grid has not been built.            */
+int32_t sicp_debug_grid_params(sicp_ctx* ctx, int32_t side, double o[3] /*[h]*/, double* h /*[h]*/,
+                               int32_t dims[3] /*[h]*/);
+
 /* ---- .xyz text I/O (host only; SURVEY.md section 8f: file parsing dominates end-to-end time on
  * the lidar sets).  Contract of the reference readers (c++/src/simpleicp-cli.cpp:72-128,
  * rust/src/io.rs:9-37, np.genfromtxt in python/simpleicp/tests/test_simpleicp.py:102-103):

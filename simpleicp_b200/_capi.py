@@ -43,7 +43,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
-    "sicp_debug_seed_predictor",
+    "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
 
@@ -166,6 +166,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
         "sicp_debug_seed_predictor": [vp, dbl, dbl, dbl],
+        "sicp_debug_grid_params": [vp, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(i32)],
     }
     for name, args in sigs.items():
         fn = getattr(lib, name)
@@ -541,6 +542,15 @@ class Engine:
     def seed_predictor(self, med: float, mad: float, min_planarity: float):
         """Test-only (sicp_debug_seed_predictor): the predictor the next match bins with."""
         self._check(self._lib.sicp_debug_seed_predictor(self._h, float(med), float(mad), float(min_planarity)))
+
+    def grid_params(self, side: str = "mov"):
+        """Test-only (sicp_debug_grid_params): (origin, cell size, dims) of the movable ("mov") or
+        the fixed ("fix") cloud's grid."""
+        o = (C.c_double * 3)()
+        h = C.c_double(0)
+        dims = (C.c_int32 * 3)()
+        self._check(self._lib.sicp_debug_grid_params(self._h, {"fix": 0, "mov": 1}[side], o, C.byref(h), dims))
+        return np.array(o), float(h.value), tuple(int(d) for d in dims)
 
     def timings(self) -> dict:
         t = Timings()

@@ -1107,6 +1107,20 @@ int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double 
   API_END
 }
 
+int32_t sicp_debug_grid_params(sicp_ctx* ctx, int32_t side, double o[3], double* h, int32_t dims[3]) {
+  API_BEGIN(ctx)
+  SICP_REQUIRE(side == 0 || side == 1, SICP_ERR_BAD_ARG, "side must be 0 (fixed) or 1 (movable)");
+  SICP_REQUIRE(o && h && dims, SICP_ERR_BAD_ARG, "NULL argument");
+  const Grid& g = (side == 0) ? c.gfix : c.gmov;
+  SICP_REQUIRE(g.built, SICP_ERR_STATE, "that grid has not been built");
+  for (int a = 0; a < 3; ++a) {
+    o[a] = g.o[a];
+    dims[a] = g.dims[a];
+  }
+  *h = g.h;
+  API_END
+}
+
 int32_t sicp_get_timings(sicp_ctx* ctx, sicp_timings* t) {
   API_BEGIN(ctx)
   SICP_REQUIRE(t != nullptr, SICP_ERR_BAD_ARG, "t is NULL");
