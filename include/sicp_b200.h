@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SICP_ABI_VERSION 2
+#define SICP_ABI_VERSION 3
 
 typedef enum {
   SICP_OK = 0,
@@ -253,15 +253,22 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, 
                       int64_t* n_selected /*[h] or NULL*/);
 
 /* ---- many independent pairs in one call (BASELINE.json configs[4]; SURVEY.md section 8e) --------
- * SimpleICP.run (simpleicp.py:75-324, defaults: no overlap filter) for n_pairs independent
- * (fixed, movable) pairs on ONE GPU with ONE set of kernel launches per stage and per iteration
- * for the whole batch: the grids of all 2 n_pairs clouds are built in one segmented counting
- * sort, the searches of all pairs run in one launch, reject + solve run one block per pair, every
- * pair has its own stop flag.  Results per pair equal those of sicp_register on that pair.
+ * SimpleICP.run (simpleicp.py:75-324) for n_pairs independent (fixed, movable) pairs on ONE GPU
+ * with ONE set of kernel launches per stage and per iteration for the whole batch: the grids of
+ * all 2 n_pairs clouds are built in one segmented counting sort, the searches of all pairs run in
+ * one launch, reject + solve run one block per pair, every pair has its own stop flag.  Results
+ * per pair equal those of sicp_register on that pair.
  * fix_xyz[i] / mov_xyz[i] point to the i-th pair's clouds (host, ideally pinned, or device);
- * correspondences must be <= 4096 (one block per pair) and max_overlap_distance must be unused.
- * out[i].status is the sicp_status of pair i (a pair without enough correspondences fails alone);
- * the call itself fails only on bad arguments or CUDA errors.                                   */
+ * correspondences must be <= 4096 (one block per pair).
+ * max_overlap_distance finite and > 0: PointCloud.select_in_range on every fixed point of pair i
+ * under that pair's initial transform, then the subsample over the survivors, as sicp_register
+ * does.  A pair without a survivor gets SICP_ERR_NO_OVERLAP and takes no part in the loop.
+ * observed (n_pairs x 6, radians, or NULL): row i replaces both run.lsq.x0 and run.lsq.observed
+ * for pair i (rbp_observed_values per pair; in the linearised variants only the initial
+ * transform); every other parameter is common to the batch.
+ * n_selected (or NULL) receives the selected fixed points of each pair (sicp_register's value).
+ * out[i].status is the sicp_status of pair i (a pair without overlap or without enough
+ * correspondences fails alone); the call itself fails only on bad arguments or CUDA errors.     */
 typedef struct {
   int32_t status;
   int32_t iterations;
@@ -276,7 +283,9 @@ typedef struct {
 int32_t sicp_register_batch(sicp_ctx* ctx, int32_t n_pairs, const double* const* fix_xyz /*[h|d]*/,
                             const int64_t* n_fix, const double* const* mov_xyz /*[h|d]*/,
                             const int64_t* n_mov, const sicp_register_params* p,
-                            sicp_pair_result* out /*[h] n_pairs*/);
+                            const double* observed /*[h] n_pairs x 6, radians, or NULL*/,
+                            sicp_pair_result* out /*[h] n_pairs*/,
+                            int64_t* n_selected /*[h] n_pairs or NULL*/);
 
 /* ---- PointCloud.transform_by_H (pointcloud.py:205-217), final application simpleicp.py:316 -- */
 int32_t sicp_transform(sicp_ctx* ctx, const double H[16], double* mov_xyz_out /*[h|d] n_mov x 3*/);

@@ -17,7 +17,7 @@ LIB_PATH = PKG / "libsicp_b200.so"
 
 SICP_OK, SICP_ERR_BAD_ARG, SICP_ERR_NO_OVERLAP, SICP_ERR_TOO_FEW_CORR = 0, 1, 2, 3
 SICP_ERR_CUDA, SICP_ERR_SINGULAR, SICP_ERR_STATE = 4, 5, 6
-ABI_VERSION = 2  # include/sicp_b200.h: SICP_ABI_VERSION
+ABI_VERSION = 3  # include/sicp_b200.h: SICP_ABI_VERSION
 NN_AUTO, NN_GRID, NN_BRUTE = 0, 1, 2
 SIGN_DGEEV, SIGN_CANONICAL = 0, 1
 
@@ -161,7 +161,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_register": [vp, vp, i64, vp, i64, C.POINTER(RegisterParams), C.POINTER(RunResult),
                           C.POINTER(IterRecord), vp, C.POINTER(i64)],
         "sicp_register_batch": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(vp), C.POINTER(i64),
-                                C.POINTER(RegisterParams), C.POINTER(PairResult)],
+                                C.POINTER(RegisterParams), vp, C.POINTER(PairResult), vp],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -477,24 +477,37 @@ class Engine:
         self._check(self._lib.sicp_get_residuals(self._h, _ptr(res), res.size, C.byref(n)))
         return out, [log[i] for i in range(out.iterations)], res, transform_out
 
-    def register_batch(self, pairs, correspondences, neighbors, params: RunParams):
+    def register_batch(self, pairs, correspondences, neighbors, params: RunParams,
+                       max_overlap_distance: float = -1.0, observed=None):
         """sicp_register_batch: SimpleICP.run for every (X_fix, X_mov) of `pairs` with one set of
         kernel launches per stage for the whole batch.  Clouds are NumPy arrays (pinned ones
-        upload at link speed) or CUDA tensors; nothing is copied on the host.  Returns the
-        ctypes array of PairResult (status per pair)."""
+        upload at link speed) or CUDA tensors; nothing is copied on the host.
+
+        `max_overlap_distance` finite and > 0 runs the overlap filter per pair; `observed`, an
+        (n_pairs, 6) array in radians, gives each pair its own x0 = observed values (None: those
+        of `params`).  Returns the ctypes array of PairResult (status per pair); its attribute
+        `n_selected` holds the selected fixed points of each pair (int64)."""
         n = len(pairs)
         keep = [(_as_f64_xyz(a), _as_f64_xyz(b)) for a, b in pairs]  # keeps converted copies alive
         fp = (C.c_void_p * n)(*[_ptr(a) for a, _ in keep])
         mp = (C.c_void_p * n)(*[_ptr(b) for _, b in keep])
         nf = (C.c_int64 * n)(*[int(a.shape[0]) for a, _ in keep])
         nm = (C.c_int64 * n)(*[int(b.shape[0]) for _, b in keep])
+        if observed is not None:
+            observed = np.ascontiguousarray(observed, dtype=np.float64)
+            if observed.shape != (n, 6):
+                raise ValueError(f"observed must have shape ({n}, 6), got {observed.shape}")
         rp = RegisterParams()
         rp.correspondences = int(correspondences)
         rp.neighbors = int(neighbors)
-        rp.max_overlap_distance = -1.0
+        rp.max_overlap_distance = float(max_overlap_distance)
         rp.run = params
         out = (PairResult * n)()
-        self._check(self._lib.sicp_register_batch(self._h, n, fp, nf, mp, nm, C.byref(rp), out))
+        n_selected = np.zeros(n, dtype=np.int64)
+        self._check(self._lib.sicp_register_batch(self._h, n, fp, nf, mp, nm, C.byref(rp),
+                                                  None if observed is None else _ptr(observed), out,
+                                                  _ptr(n_selected)))
+        out.n_selected = n_selected
         return out
 
     def get_transform(self) -> np.ndarray:

@@ -126,8 +126,13 @@ def simpleicp_batch(
     `engine="batched"` (default) hands the rank's share to the library's batched engine in chunks
     of `batch_size` pairs (sicp_register_batch: one set of kernel launches per stage and per
     iteration for the whole chunk, a block per pair for reject + solve, per-pair stop flags);
-    pairs it does not cover (overlap filter, more than 4096 correspondences, debug output) and
-    `engine="pool"` use the concurrent per-pair engines described above.
+    pairs it does not cover (more than 4096 correspondences, debug output) and `engine="pool"`
+    use the concurrent per-pair engines described above.
+
+    `rbp_observed_values` is either the common 6-tuple or an array of shape (n_pairs, 6) indexed
+    by pair number, one prior per pair (e.g. a GNSS/INS or odometry pose; angles in degrees):
+    each pair starts from its own row, which is also the transform its overlap filter runs under.
+    Every row is checked before any registration starts.
 
     A pair that cannot be registered (no overlap, fewer than 6 correspondences: ordinary
     data-dependent outcomes) gets a NaN record whose `iterations` field is minus the library's
@@ -140,6 +145,10 @@ def simpleicp_batch(
     get = pairs if callable(pairs) else (lambda i: pairs[i])  # type: ignore[index]
     mine = shard_pairs(n_pairs, world_size, rank)
     local = np.zeros((len(mine), RECORD_LEN))
+    rows = _per_pair_observed(run_kwargs, n_pairs)
+
+    def kw_of(i):
+        return run_kwargs if rows is None else {**run_kwargs, "rbp_observed_values": rows[i]}
 
     def record(res):
         last = res.records[res.iterations - 1]
@@ -160,9 +169,9 @@ def simpleicp_batch(
     if register_fn is not None:
         for j, i in enumerate(mine):
             Xf, Xm = get(i)
-            local[j] = guarded(register_fn, Xf, Xm, **run_kwargs)
+            local[j] = guarded(register_fn, Xf, Xm, **kw_of(i))
     elif engine == "batched" and _batchable(run_kwargs):
-        _run_batched(get, mine, local, device, batch_size, run_kwargs, messages)
+        _run_batched(get, mine, local, device, batch_size, run_kwargs, messages, rows)
     else:
         import threading
 
@@ -186,7 +195,7 @@ def simpleicp_batch(
                         if j is None:
                             break
                         Xf, Xm = get(mine[j])
-                        local[j] = guarded(register, Xf, Xm, engine=eng, **run_kwargs)
+                        local[j] = guarded(register, Xf, Xm, engine=eng, **kw_of(mine[j]))
             except Exception as e:  # surfaced after the join
                 errors.append(e)
 
@@ -218,28 +227,53 @@ _BATCH_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "m
 
 def _batchable(kw) -> bool:
     """Can the batched engine serve these run() arguments?  (One block per pair: at most 4096
-    correspondences; no overlap filter; nothing that needs per-pair host interaction.)"""
+    correspondences; nothing that needs per-pair host interaction.)"""
     if set(kw) - _BATCH_KEYS:
         return False
-    if np.isfinite(kw.get("max_overlap_distance", np.inf)):
-        return False
     return int(kw.get("correspondences", 1000)) <= 4096 and not kw.get("want_normals", False)
+
+
+def _per_pair_observed(kw, n_pairs: int):
+    """rbp_observed_values given per pair: the (n_pairs, 6) rows as float64 (degrees), each
+    checked as run() checks the common tuple.  None when the common 6-tuple (or nothing) is given."""
+    from .simpleicp import SimpleICPException, _check_arguments
+
+    if "rbp_observed_values" not in kw:
+        return None
+    try:
+        v = np.asarray(kw["rbp_observed_values"], dtype=np.float64)
+    except (TypeError, ValueError):
+        v = None
+    if v is not None and v.ndim == 1:
+        return None  # the common tuple: checked where it is used, as before
+    if v is None or v.shape != (n_pairs, 6):
+        raise SimpleICPException(
+            f"rbp_observed_values must have exactly 6 elements, or shape ({n_pairs}, 6) for one row per pair.")
+    for row in v:
+        _check_arguments(kw.get("distance_weights", 1), row, kw.get("rbp_observation_weights", (0.0,) * 6))
+    if not np.isfinite(v).all():
+        raise SimpleICPException("Every row of rbp_observed_values must be finite.")
+    return v
 
 
 _BATCH_ENGINES: dict = {}
 
 
-def _run_batched(get, mine, local, device, batch_size, kw, messages):
+def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
     import torch
 
     from . import _capi
     from .simpleicp import _check_arguments, _observed_in_radians
 
     dw = kw.get("distance_weights", 1)
-    obs_v = kw.get("rbp_observed_values", (0.0,) * 6)
     obs_w = kw.get("rbp_observation_weights", (0.0,) * 6)
-    _check_arguments(dw, obs_v, obs_w)
-    obs = _observed_in_radians(obs_v)
+    if rows is None:
+        obs_v = kw.get("rbp_observed_values", (0.0,) * 6)
+        _check_arguments(dw, obs_v, obs_w)
+        obs = _observed_in_radians(obs_v)
+    else:
+        obs = np.zeros(6)  # every pair's x0 and observed values come from its row
+    mod = float(kw.get("max_overlap_distance", np.inf))
     with torch.cuda.device(device):
         eng = _BATCH_ENGINES.get(int(device))
         if eng is None or not eng.alive:
@@ -250,7 +284,9 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages):
         for lo in range(0, len(mine), max(1, int(batch_size))):
             ids = range(lo, min(lo + max(1, int(batch_size)), len(mine)))
             pairs = [get(mine[j]) for j in ids]
-            res = eng.register_batch(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params)
+            observed = None if rows is None else np.array([_observed_in_radians(rows[mine[j]]) for j in ids])
+            res = eng.register_batch(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params,
+                                     mod if np.isfinite(mod) else -1.0, observed)
             for j, r in zip(ids, res):
                 if r.status == 0:
                     local[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)

@@ -176,6 +176,9 @@ struct PairDev {
   long long K;                 // selected fixed points (<= Kmax)
   long long q_off;             // first entry of this pair in the per-query arrays
   double cm[3];                // centre of the movable grid's box (moment centring)
+  // overlap filter: this pair's survivors are Batch::ovl_list[list_off, list_off + list_len)
+  long long list_off, list_len;
+  double obs[6];               // rbp_observed_values of this pair (radians)
 };
 
 // One cloud of a batched grid build (filled by the host from the bounding boxes).
@@ -212,6 +215,10 @@ struct Batch {
   int bin_cap = 0;
   DevBuf<uint32_t> nn_pos;
   DevBuf<uint8_t> keep;
+  // overlap filter, one entry per fixed point of the batch: keep flag, its exclusive prefix sum
+  // (total_fix + 1), the in-cloud indices of the survivors in ascending order per pair
+  DevBuf<uint32_t> ovl_flag, ovl_scan, ovl_list, ovl_sums;
+  DevBuf<uint32_t> ovl_bounds;  // n_pairs + 1 prefix values at the pair offsets
   // per-pair state
   DevBuf<DevState> state;
   DevBuf<unsigned int> lin_hist;       // n_pairs x (LH_BINS + 2)
@@ -235,6 +242,10 @@ struct Batch {
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
 void grid_build(Ctx& c, Grid& g, const double* xyz_dev, long long n);
 void make_float4_copy(Ctx& c);
+// Exclusive prefix sum of n uint32 values (four launches): out[0 .. n], out[n] = the total.
+// block_sums is scratch; n_nonzero (device) is incremented by the number of non-zero inputs.
+void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums,
+              unsigned int* n_nonzero);
 
 // 1-NN of K transformed queries into the movable cloud; fused point-to-plane distance.
 // If out_d2 != nullptr the squared NN distance is written instead of the plane distance epilogue
@@ -282,9 +293,13 @@ struct BatchHostCloud {
 };
 void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHostCloud>& clouds,
                       std::vector<GridView>& views, std::vector<double>& centres /* 3 per cloud */);
-void batch_select_gather_launch(Ctx& c, Batch& b, long long correspondences, int round_away);
+// with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud
+void batch_select_gather_launch(Ctx& c, Batch& b, bool with_list, int round_away);
 void batch_normals_launch(Ctx& c, Batch& b, int k);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
+// PointCloud.select_in_range of every fixed point of the batch under its pair's DevState
+// transform: Batch::ovl_flag[i] = (squared distance to the nearest movable point < r2)
+void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2);
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 

@@ -265,6 +265,19 @@ __global__ void __launch_bounds__(256) k_float4_copy(const double* __restrict__ 
 
 }  // namespace
 
+void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums,
+              unsigned int* n_nonzero) {
+  cudaStream_t st = c.stream;
+  const long long nsb = (n + kScanItems - 1) / kScanItems;
+  block_sums.reserve(nsb + 1);
+  k_scan_reduce<<<(unsigned)nsb, 256, 0, st>>>(in, n, block_sums.p, n_nonzero);
+  k_scan_blocksums<<<1, 1024, 0, st>>>(block_sums.p, (int)nsb);
+  k_scan_down<<<(unsigned)nsb, 256, 0, st>>>(in, n, block_sums.p, out);
+  k_scan_total<<<1, 32, 0, st>>>(in, n, out);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 4;
+}
+
 void grid_build(Ctx& c, Grid& g, const double* xyz, long long n) {
   cudaStream_t st = c.stream;
   g.built = false;
@@ -321,17 +334,12 @@ void grid_build(Ctx& c, Grid& g, const double* xyz, long long n) {
     g.cell_start.reserve(g.n_cells + 1);
     g.fill.reserve(g.n_cells);
     g.cid.reserve(n);
-    long long nsb = (g.n_cells + kScanItems - 1) / kScanItems;
-    g.block_sums.reserve(nsb + 1);
     SICP_CUDA(cudaMemsetAsync(g.fill.p, 0, g.n_cells * sizeof(uint32_t), st));
     SICP_CUDA(cudaMemsetAsync(c.misc_counters.p, 0, 64 * sizeof(unsigned int), st));
     GridParams gp{g.o[0], g.o[1], g.o[2], 1.0 / h, g.dims[0], g.dims[1], g.dims[2]};
     k_cell_count<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(xyz, n, gp, g.cid.p, g.fill.p);
-    k_scan_reduce<<<(unsigned)nsb, 256, 0, st>>>(g.fill.p, g.n_cells, g.block_sums.p, c.misc_counters.p);
-    k_scan_blocksums<<<1, 1024, 0, st>>>(g.block_sums.p, (int)nsb);
-    k_scan_down<<<(unsigned)nsb, 256, 0, st>>>(g.fill.p, g.n_cells, g.block_sums.p, g.cell_start.p);
-    k_scan_total<<<1, 32, 0, st>>>(g.fill.p, g.n_cells, g.cell_start.p);
-    c.tm.kernel_launches += 5;
+    scan_u32(c, g.fill.p, g.n_cells, g.cell_start.p, g.block_sums, c.misc_counters.p);
+    c.tm.kernel_launches += 1;
     unsigned int* nocc_host = reinterpret_cast<unsigned int*>(c.scal_host + 16);
     SICP_CUDA(cudaMemcpyAsync(nocc_host, c.misc_counters.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
     tr("count queued");
@@ -577,18 +585,13 @@ void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHo
     if (!again) break;
   }
   // exclusive scan of the concatenated counters -> global record positions
-  const long long nsb = (total_cells + kScanItems - 1) / kScanItems;
-  bg.block_sums.reserve(nsb + 1);
   c.misc_counters.reserve(64);
-  SICP_CUDA(cudaMemsetAsync(c.misc_counters.p + 16, 0, sizeof(unsigned int), st));  // the kernel's (unused here) occupancy counter
-  k_scan_reduce<<<(unsigned)nsb, 256, 0, st>>>(bg.fill.p, total_cells, bg.block_sums.p, c.misc_counters.p + 16);
-  k_scan_blocksums<<<1, 1024, 0, st>>>(bg.block_sums.p, (int)nsb);
-  k_scan_down<<<(unsigned)nsb, 256, 0, st>>>(bg.fill.p, total_cells, bg.block_sums.p, bg.cell_table.p);
-  k_scan_total<<<1, 32, 0, st>>>(bg.fill.p, total_cells, bg.cell_table.p);
+  SICP_CUDA(cudaMemsetAsync(c.misc_counters.p + 16, 0, sizeof(unsigned int), st));  // the scan's (unused here) occupancy counter
+  scan_u32(c, bg.fill.p, total_cells, bg.cell_table.p, bg.block_sums, c.misc_counters.p + 16);
   SICP_CUDA(cudaMemsetAsync(bg.fill.p, 0, (size_t)total_cells * sizeof(uint32_t), st));
   k_scatter_batch<<<dim3((unsigned)((max_n + 255) / 256), nc), 256, 0, st>>>(b.plans.p, bg.cid.p, bg.cell_table.p, bg.fill.p, bg.recs.p);
   SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 5;
+  c.tm.kernel_launches += 1;
   views.resize((size_t)nc);
   centres.resize((size_t)nc * 3);
   for (int i = 0; i < nc; ++i) {

@@ -239,13 +239,15 @@ __global__ void __launch_bounds__(128)
 // 16-lane group.  Later rings deal their (2r+1)^2 rows round-robin over the lanes.  The search is
 // latency-bound (a handful of 32-byte L2 sectors per query), so what counts is how many of
 // those loads are in flight — with one thread per query a K = 1000 search took 27 us.
-template <int MG>
+// KEEP (overlap filter of a batch, with_distance = 0, unlimited rings): instead of nn_idx and the
+// squared distance, keep[qi] = (d2 < cap2), the comparison of k_range_keep (capi.cu).
+template <int MG, bool KEEP = false>
 __device__ __forceinline__ void match_coop_body(
     const GridView& g, const DevState* __restrict__ st, const double* __restrict__ q_xyz,
     const float4* __restrict__ q_nrm, const double* __restrict__ mov_xyz, long long K, int rmax,
     int with_distance, long long* __restrict__ nn_idx, double* __restrict__ out,
     unsigned int* __restrict__ unresolved, unsigned int* __restrict__ lin_hist, double cap2,
-    const CorrOut& co, const long long gt) {
+    const CorrOut& co, const long long gt, uint32_t* __restrict__ keep = nullptr) {
   const long long qi = gt / MG;
   const int sub = threadIdx.x & (MG - 1);
   pdl_launch_dependents();
@@ -523,6 +525,12 @@ __device__ __forceinline__ void match_coop_body(
     if (r >= rmax) break;
   }
   if (sub != 0) return;
+  if constexpr (KEEP) {
+    // with cap2 the search stops once the side of the bound is decided (see grid_nn), so `best`
+    // is then an upper bound below cap2 or a value at or above it: the comparison is exact
+    keep[qi] = (best < cap2) ? 1u : 0u;  // strict: cKDTree distance_upper_bound semantics
+    return;
+  }
   if (co.nn_pos) co.nn_pos[qi] = resolved ? bpos : 0xffffffffu;
   if (!resolved) {
     const unsigned int slot = atomicAdd(&unresolved[K], 1u);
@@ -583,6 +591,24 @@ __global__ void __launch_bounds__(128) k_match_batch(BatchMatchArgs a) {
   match_coop_body<MG>(pd.gmov, a.state + blockIdx.y, a.q_xyz + 3 * q, a.q_nrm + q, nullptr, pd.K, 1 << 30, 1,
                       a.nn_idx + q, a.dist + q, nullptr, a.lin_hist + (size_t)blockIdx.y * (LH_BINS + 2), -1.0,
                       co, gt);
+}
+
+// Overlap filter of a batch (PointCloud.select_in_range, simpleicp.py:158-170): blockIdx.y is the
+// pair, the queries are ALL its fixed points, read in place from the concatenated clouds, and the
+// transform is the pair's DevState (its prior).  Bounded search with unlimited rings, one keep
+// flag per fixed point of the batch.
+template <int MG>
+__global__ void __launch_bounds__(128)
+    k_overlap_batch(const PairDev* __restrict__ pairs, const DevState* __restrict__ state,
+                    const double* __restrict__ fix_xyz, double r2, uint32_t* __restrict__ keep) {
+  const PairDev& pd = pairs[blockIdx.y];
+  const long long n = pd.n_fix;
+  const long long gt = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (gt / MG >= n) return;
+  const long long f = pd.fix_off;
+  const CorrOut co{nullptr, 0, nullptr, nullptr, 0, 0, nullptr, nullptr, -1.0};
+  match_coop_body<MG, true>(pd.gmov, state + blockIdx.y, fix_xyz + 3 * f, nullptr, nullptr, n, 1 << 30, 0,
+                            nullptr, nullptr, nullptr, nullptr, r2, co, gt, keep + f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -902,21 +928,25 @@ static void bf_launch(Ctx& c, bool with_distance, double* out, bool whole_set) {
 }
 
 namespace {
-// per pair: sel[i] = rint(linspace(0, n_fix - 1, K)) (PointCloud.select_n_points, k_select_n in
-// capi.cu) and the gather of the selected fixed points, in one launch for the whole batch
+// per pair: sel[i] = src[rint(linspace(0, m - 1, K))] (PointCloud.select_n_points, k_select_n in
+// capi.cu) and the gather of the selected fixed points, in one launch for the whole batch.  src is
+// the pair's survivor list of the overlap filter (m = its length) or, without a list, the whole
+// cloud (m = n_fix, src = identity).
 __global__ void __launch_bounds__(256)
-    k_select_gather_batch(const PairDev* __restrict__ pairs, const double* __restrict__ fix_xyz, int away,
-                          long long* __restrict__ sel, double* __restrict__ q_xyz) {
+    k_select_gather_batch(const PairDev* __restrict__ pairs, const double* __restrict__ fix_xyz,
+                          const uint32_t* __restrict__ list, int away, long long* __restrict__ sel,
+                          double* __restrict__ q_xyz) {
   const PairDev pd = pairs[blockIdx.y];
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= pd.K) return;
-  const long long m = pd.n_fix, n = pd.K;
+  const long long m = list ? pd.list_len : pd.n_fix, n = pd.K;
   long long j = i;
   if (n < m) {
     const double step = (n > 1) ? (double)(m - 1) / (double)(n - 1) : 0.0;
     const double y = (i == n - 1 && n > 1) ? (double)(m - 1) : (double)i * step;
     j = (long long)(away ? round(y) : rint(y));
   }
+  if (list) j = list[pd.list_off + j];
   sel[pd.q_off + i] = j;
   const double* __restrict__ src = fix_xyz + 3 * (pd.fix_off + j);
   double* __restrict__ dst = q_xyz + 3 * (pd.q_off + i);
@@ -926,10 +956,24 @@ __global__ void __launch_bounds__(256)
 }
 }  // namespace
 
-void batch_select_gather_launch(Ctx& c, Batch& b, long long correspondences, int round_away) {
-  (void)correspondences;
+void batch_select_gather_launch(Ctx& c, Batch& b, bool with_list, int round_away) {
   k_select_gather_batch<<<dim3((unsigned)((b.Kmax + 255) / 256), b.n_pairs), 256, 0, c.stream>>>(
-      b.pairs.p, b.fix_xyz.p, round_away, b.sel_idx.p, b.q_xyz.p);
+      b.pairs.p, b.fix_xyz.p, with_list ? b.ovl_list.p : nullptr, round_away, b.sel_idx.p, b.q_xyz.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2) {
+  // lanes per query by the number of queries in flight, as in batch_match_launch; the result does
+  // not depend on it, and the 2-lane form (which spills) is served by 4 lanes
+  const long long total = b.total_fix;
+  int mg = c.match_group;
+  if (mg == 0 || mg == 1) mg = (total <= 16384) ? 16 : ((total <= 65536) ? 8 : 4);
+  const dim3 grid((unsigned)((max_n_fix * std::max(mg, 4) + 127) / 128), b.n_pairs);
+  uint32_t* keep = b.ovl_flag.p;
+  if (mg <= 4) k_overlap_batch<4><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
+  else if (mg == 8) k_overlap_batch<8><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
+  else k_overlap_batch<16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

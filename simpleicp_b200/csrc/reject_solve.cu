@@ -2155,6 +2155,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_rs_batch(BatchRsArgs b) {
   a.cm[0] = pd.cm[0];
   a.cm[1] = pd.cm[1];
   a.cm[2] = pd.cm[2];
+  for (int j = 0; j < 6; ++j) a.obs[j] = pd.obs[j];
   RSWork wk{};
   wk.lin_hist = b.lin_hist + (size_t)pair * (LH_BINS + 2);
   wk.partials = b.partials + (size_t)pair * RSF_NPART;
@@ -2568,10 +2569,7 @@ void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool wa
   a.stat_minpl = c.variant ? -kInf : p.min_planarity;
   a.min_change = p.min_change;
   a.w_param = p.lsq.distance_weight;
-  for (int j = 0; j < 6; ++j) {
-    a.obs[j] = p.lsq.observed[j];
-    a.wobs[j] = p.lsq.obs_weight[j];
-  }
+  for (int j = 0; j < 6; ++j) a.wobs[j] = p.lsq.obs_weight[j];  // a.obs: per pair, PairDev::obs
   a.it = it;
   a.do_solve = 1;
   a.arm_stop = 1;

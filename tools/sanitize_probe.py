@@ -49,5 +49,10 @@ with _capi.Engine() as e:
 pairs = [sb.synthetic.c5_pair(i, 20_000) for i in range(4)]
 tab = sb.simpleicp_batch([(p[0], p[1]) for p in pairs], engine="batched", correspondences=500)
 assert np.isfinite(tab).all()
+# overlap filter + a prior per pair in the batch, one pair without any overlap
+ov = [(p[0][p[0][:, 0] < 20], p[1][p[1][:, 0] > 10]) for p in pairs] + [(pairs[0][0], pairs[0][1] + 1e4)]
+tab_o = sb.simpleicp_batch(ov, engine="batched", correspondences=500, max_overlap_distance=0.5,
+                           rbp_observed_values=np.zeros((len(ov), 6)), on_error="nan")
+assert np.isfinite(tab_o[:-1]).all() and tab_o[-1, 16] == -_capi.SICP_ERR_NO_OVERLAP
 print("ok", a.iterations, m.iterations, int(tab[:, 16].sum()), c.iterations, d.iterations, f.iterations, g.iterations, l.iterations,
       float(np.linalg.norm(c.H - H_true)), float(np.linalg.norm(l.T - H_true)))
