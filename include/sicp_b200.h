@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SICP_ABI_VERSION 3
+#define SICP_ABI_VERSION 4
 
 typedef enum {
   SICP_OK = 0,
@@ -102,8 +102,10 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value);
  *        "upload_threads" (worker threads that stage a cloud given in PAGEABLE host memory --
  *        e.g. a NumPy array -- through pinned buffers, default 2; 0: plain cudaMemcpyAsync, which
  *        the driver stages on the calling thread; pinned and device sources never use them),
- *        "upload_chunk_kb" (slice size of that staging, default 2048), "defaults" (any value:
- *        every option back to its default)                              */
+ *        "upload_chunk_kb" (slice size of that staging, default 2048), "normals_scratch_mb"
+ *        (bound of the movable-normals estimate's neighbour scratch, default 64: it runs in
+ *        launches of 2^20 x normals_scratch_mb / (4 k) queries), "defaults" (any value: every option back to its
+ *        default)                                                       */
 
 /* ---- clouds: SimpleICP.add_point_clouds (simpleicp.py:58-73) + PointCloud.X ---------------- */
 int32_t sicp_set_clouds(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, int64_t n_fix,
@@ -139,8 +141,9 @@ int32_t sicp_set_normals(sicp_ctx* ctx, const float* nx, const float* ny, const 
  *    and leaves `raise NotImplementedError` (corrpts.py:190-193).  Here: a correspondence that
  *    survived both rejections is dropped when acos|n_fix . (R n_mov)| > max_angle_rad, R the
  *    rotation of the iteration's transform.  Negative: no angle test.
- * Both act in sicp_match/sicp_reject/sicp_solve, sicp_iterate and sicp_run; sicp_register and
- * sicp_register_batch take their clouds themselves and always run without them.               */
+ * Both act in sicp_match/sicp_reject/sicp_solve, sicp_iterate and sicp_run.  sicp_register and
+ * sicp_register_batch take their clouds themselves and clear them; they estimate the movable
+ * attributes on the device instead when sicp_register_params.mov_neighbors > 0.               */
 int32_t sicp_set_mov_normals(sicp_ctx* ctx, const float* nx, const float* ny, const float* nz,
                              const float* planarity /*[h|d] n_mov each*/, double max_angle_rad);
 /* neighbour indices of the last sicp_estimate_normals (test/inspection hook), K x neighbors; they
@@ -237,13 +240,22 @@ int32_t sicp_select_n_points(sicp_ctx* ctx, int64_t n, int64_t* idx_out /*[h|d] 
  * overlaps the fixed-side work (grid, subsample, normals).  Equivalent to sicp_set_clouds,
  * sicp_set_selected(NULL), [sicp_select_in_range], sicp_select_n_points, sicp_estimate_normals,
  * sicp_run, sicp_transform in sequence; every stage-by-stage call remains valid afterwards
- * (sicp_get_residuals, sicp_get_knn, sicp_match ...).                                            */
+ * (sicp_get_residuals, sicp_get_knn, sicp_match ...).
+ * mov_neighbors = k > 0 adds pc_mov.estimate_normals(k) before the run (pointcloud.py:173-203):
+ * every movable point gets a normal and a planarity from its k nearest movable neighbours (itself
+ * included), estimated on the device right after the movable grid is built, and the loop runs
+ * as after sicp_set_mov_normals(those arrays, max_angle_rad).  k must be in [2, 64] and at most
+ * the number of movable points; the linearised variants have no movable-side branch
+ * (c++/src/corrpts.cpp:27-30) and refuse k > 0.  Violations are SICP_ERR_BAD_ARG before any
+ * device work.  A zero-initialised struct is the run without movable attributes.               */
 typedef struct {
   int64_t correspondences;       /* simpleicp.py:78 (default 1000)                                */
   int32_t neighbors;             /* simpleicp.py:79 (default 10)                                  */
-  int32_t reserved;
+  int32_t mov_neighbors;         /* 0: no movable attributes; k: estimate them (see above)        */
   double max_overlap_distance;   /* <= 0 or +inf: clouds fully overlap (simpleicp.py:81)          */
   sicp_run_params run;
+  double max_angle_rad;          /* read only when mov_neighbors > 0: as sicp_set_mov_normals'
+                                    (negative: no angle test, else <= pi/2)                       */
 } sicp_register_params;
 int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, int64_t n_fix,
                       const double* mov_xyz /*[h|d] n_mov x 3*/, int64_t n_mov,
@@ -266,6 +278,9 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, 
  * observed (n_pairs x 6, radians, or NULL): row i replaces both run.lsq.x0 and run.lsq.observed
  * for pair i (rbp_observed_values per pair; in the linearised variants only the initial
  * transform); every other parameter is common to the batch.
+ * mov_neighbors > 0: every pair's movable cloud gets its normals and planarities on the device
+ * (as sicp_register does; k must not exceed any pair's movable point count), max_angle_rad as
+ * there.
  * n_selected (or NULL) receives the selected fixed points of each pair (sicp_register's value).
  * out[i].status is the sicp_status of pair i (a pair without overlap or without enough
  * correspondences fails alone); the call itself fails only on bad arguments or CUDA errors.     */
@@ -299,6 +314,8 @@ typedef struct {
                                in the barrier-free kernel (all but the first, normally)          */
   int64_t rerun_iterations; /* ... iterations repeated through the general kernel because the
                                order-statistic prediction of the barrier-free kernel missed       */
+  double mov_normals_ms;    /* last sicp_register / sicp_register_batch with mov_neighbors > 0:
+                               k-NN + PCA of the movable cloud(s); 0 otherwise                    */
 } sicp_timings;
 int32_t sicp_get_timings(sicp_ctx* ctx, sicp_timings* t /*[h]*/);
 

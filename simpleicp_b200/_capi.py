@@ -17,7 +17,7 @@ LIB_PATH = PKG / "libsicp_b200.so"
 
 SICP_OK, SICP_ERR_BAD_ARG, SICP_ERR_NO_OVERLAP, SICP_ERR_TOO_FEW_CORR = 0, 1, 2, 3
 SICP_ERR_CUDA, SICP_ERR_SINGULAR, SICP_ERR_STATE = 4, 5, 6
-ABI_VERSION = 3  # include/sicp_b200.h: SICP_ABI_VERSION
+ABI_VERSION = 4  # include/sicp_b200.h: SICP_ABI_VERSION
 NN_AUTO, NN_GRID, NN_BRUTE = 0, 1, 2
 SIGN_DGEEV, SIGN_CANONICAL = 0, 1
 
@@ -59,8 +59,8 @@ class RunParams(C.Structure):
 
 
 class RegisterParams(C.Structure):
-    _fields_ = [("correspondences", C.c_int64), ("neighbors", C.c_int32), ("reserved", C.c_int32),
-                ("max_overlap_distance", C.c_double), ("run", RunParams)]
+    _fields_ = [("correspondences", C.c_int64), ("neighbors", C.c_int32), ("mov_neighbors", C.c_int32),
+                ("max_overlap_distance", C.c_double), ("run", RunParams), ("max_angle_rad", C.c_double)]
 
 
 class IterRecord(C.Structure):
@@ -81,7 +81,8 @@ class Timings(C.Structure):
                                           "normals_ms", "match_ms", "reject_solve_ms",
                                           "transform_ms")] + [("kernel_launches", C.c_int64),
                                                             ("fused_iterations", C.c_int64),
-                                                            ("rerun_iterations", C.c_int64)]
+                                                            ("rerun_iterations", C.c_int64),
+                                                            ("mov_normals_ms", C.c_double)]
 
 
 class PairResult(C.Structure):
@@ -454,9 +455,13 @@ class Engine:
         return idx
 
     def register_fused(self, X_fix, X_mov, correspondences, neighbors, max_overlap_distance,
-                       params: RunParams, transform_out=None):
+                       params: RunParams, transform_out=None, mov_neighbors: int = 0,
+                       max_angle_rad: float = -1.0):
         """SimpleICP.run as one library call (sicp_register): uploads, selection, normals, the
-        loop and the final transform, with the movable upload overlapped with the fixed-side work."""
+        loop and the final transform, with the movable upload overlapped with the fixed-side work.
+        ``mov_neighbors`` = k > 0 estimates the movable cloud's normals from k neighbours on the
+        device first (pc_mov.estimate_normals(k)); ``max_angle_rad`` (negative: off) then rejects
+        by the angle between the normals."""
         Xf, Xm = _as_f64_xyz(X_fix), _as_f64_xyz(X_mov)
         self.n_fix, self.n_mov = int(Xf.shape[0]), int(Xm.shape[0])
         rp = RegisterParams()
@@ -464,6 +469,8 @@ class Engine:
         rp.neighbors = int(neighbors)
         rp.max_overlap_distance = float(max_overlap_distance)
         rp.run = params
+        rp.mov_neighbors = int(mov_neighbors)
+        rp.max_angle_rad = float(max_angle_rad)
         out = RunResult()
         log = (IterRecord * int(params.max_iterations))()
         if transform_out is None:
@@ -478,14 +485,16 @@ class Engine:
         return out, [log[i] for i in range(out.iterations)], res, transform_out
 
     def register_batch(self, pairs, correspondences, neighbors, params: RunParams,
-                       max_overlap_distance: float = -1.0, observed=None):
+                       max_overlap_distance: float = -1.0, observed=None, mov_neighbors: int = 0,
+                       max_angle_rad: float = -1.0):
         """sicp_register_batch: SimpleICP.run for every (X_fix, X_mov) of `pairs` with one set of
         kernel launches per stage for the whole batch.  Clouds are NumPy arrays (pinned ones
         upload at link speed) or CUDA tensors; nothing is copied on the host.
 
         `max_overlap_distance` finite and > 0 runs the overlap filter per pair; `observed`, an
         (n_pairs, 6) array in radians, gives each pair its own x0 = observed values (None: those
-        of `params`).  Returns the ctypes array of PairResult (status per pair); its attribute
+        of `params`).  `mov_neighbors` / `max_angle_rad` as in register_fused, for every pair's
+        movable cloud.  Returns the ctypes array of PairResult (status per pair); its attribute
         `n_selected` holds the selected fixed points of each pair (int64)."""
         n = len(pairs)
         keep = [(_as_f64_xyz(a), _as_f64_xyz(b)) for a, b in pairs]  # keeps converted copies alive
@@ -502,6 +511,8 @@ class Engine:
         rp.neighbors = int(neighbors)
         rp.max_overlap_distance = float(max_overlap_distance)
         rp.run = params
+        rp.mov_neighbors = int(mov_neighbors)
+        rp.max_angle_rad = float(max_angle_rad)
         out = (PairResult * n)()
         n_selected = np.zeros(n, dtype=np.int64)
         self._check(self._lib.sicp_register_batch(self._h, n, fp, nf, mp, nm, C.byref(rp),

@@ -134,6 +134,11 @@ def simpleicp_batch(
     each pair starts from its own row, which is also the transform its overlap filter runs under.
     Every row is checked before any registration starts.
 
+    `mov_neighbors=k` estimates every movable cloud's normals from k neighbours (as
+    `pc_mov.estimate_normals(k)` would) and rejects correspondences by the movable planarity too;
+    `max_angle_between_normals` (degrees, needs `mov_neighbors`) also by the angle between the
+    normals.  Both are checked before any registration starts and are served by the batched engine.
+
     A pair that cannot be registered (no overlap, fewer than 6 correspondences: ordinary
     data-dependent outcomes) gets a NaN record whose `iterations` field is minus the library's
     status code; every rank still takes part in the collective.  Afterwards `on_error="raise"`
@@ -146,6 +151,7 @@ def simpleicp_batch(
     mine = shard_pairs(n_pairs, world_size, rank)
     local = np.zeros((len(mine), RECORD_LEN))
     rows = _per_pair_observed(run_kwargs, n_pairs)
+    _check_mov_kwargs(run_kwargs)
 
     def kw_of(i):
         return run_kwargs if rows is None else {**run_kwargs, "rbp_observed_values": rows[i]}
@@ -222,7 +228,7 @@ def simpleicp_batch(
 
 _BATCH_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations",
                "distance_weights", "rbp_observed_values", "rbp_observation_weights", "max_overlap_distance",
-               "want_normals"}
+               "want_normals", "mov_neighbors", "max_angle_between_normals"}
 
 
 def _batchable(kw) -> bool:
@@ -231,6 +237,14 @@ def _batchable(kw) -> bool:
     if set(kw) - _BATCH_KEYS:
         return False
     return int(kw.get("correspondences", 1000)) <= 4096 and not kw.get("want_normals", False)
+
+
+def _check_mov_kwargs(kw) -> None:
+    """mov_neighbors / max_angle_between_normals checked as register() checks them (the movable
+    point counts are checked per pair where the clouds are)."""
+    from .simpleicp import _check_mov_arguments
+
+    _check_mov_arguments(kw.get("mov_neighbors"), kw.get("max_angle_between_normals"), kw.get("mov_normals"))
 
 
 def _per_pair_observed(kw, n_pairs: int):
@@ -274,6 +288,8 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
     else:
         obs = np.zeros(6)  # every pair's x0 and observed values come from its row
     mod = float(kw.get("max_overlap_distance", np.inf))
+    k_mov = kw.get("mov_neighbors")
+    ang = kw.get("max_angle_between_normals")
     with torch.cuda.device(device):
         eng = _BATCH_ENGINES.get(int(device))
         if eng is None or not eng.alive:
@@ -286,7 +302,9 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
             pairs = [get(mine[j]) for j in ids]
             observed = None if rows is None else np.array([_observed_in_radians(rows[mine[j]]) for j in ids])
             res = eng.register_batch(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params,
-                                     mod if np.isfinite(mod) else -1.0, observed)
+                                     mod if np.isfinite(mod) else -1.0, observed,
+                                     0 if k_mov is None else int(k_mov),
+                                     -1.0 if ang is None else float(np.deg2rad(ang)))
             for j, r in zip(ids, res):
                 if r.status == 0:
                     local[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)

@@ -14,6 +14,8 @@
 //                 per batch; this needs the movable grids, so the fixed-side work below follows it
 //   select+gather rint(linspace) picks and their coordinates, all pairs in one launch
 //   normals       k-NN + PCA, blockIdx.y = pair
+//   mov normals   (mov_neighbors only) k-NN + PCA of every movable point in its pair's movable
+//                 grid, in chunks of queries; the match folds them into an effective planarity
 //   loop          per iteration ONE match launch over (pair, query) and ONE reject/solve launch
 //                 with a block per pair (the barrier-free kernel with G = 1: predictor histogram
 //                 select, or the in-block radix select when there is no usable prediction), every
@@ -89,15 +91,19 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
                  "the linearised variants have no observed or fixed parameters");
   }
   SICP_REQUIRE(any_finite, SICP_ERR_BAD_ARG, "At least one element in rbp_observation_weights must be finite.");
+  check_mov_neighbors(c, *rp);
   if (!c.batch) c.batch = new Batch();
   Batch& b = *c.batch;
   b.n_pairs = n_pairs;
   std::vector<long long> fo((size_t)n_pairs + 1, 0), mo((size_t)n_pairs + 1, 0);
-  long long Kmax = 0, max_n_fix = 0;
+  long long Kmax = 0, max_n_fix = 0, max_n_mov = 0;
   for (int i = 0; i < n_pairs; ++i) {
     SICP_REQUIRE(fix_xyz[i] && mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
     SICP_REQUIRE(n_fix[i] >= rp->neighbors && n_mov[i] >= 1, SICP_ERR_BAD_ARG,
                  "every fixed cloud needs at least `neighbors` points, every movable cloud one");
+    SICP_REQUIRE(n_mov[i] >= rp->mov_neighbors, SICP_ERR_BAD_ARG,
+                 "mov_neighbors exceeds the number of points in the movable cloud of pair " + std::to_string(i));
+    max_n_mov = std::max<long long>(max_n_mov, n_mov[i]);
     fo[(size_t)i + 1] = fo[(size_t)i] + n_fix[i];
     mo[(size_t)i + 1] = mo[(size_t)i] + n_mov[i];
     Kmax = std::max<long long>(Kmax, std::min<long long>(rp->correspondences, n_fix[i]));
@@ -256,6 +262,16 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   }
   SICP_CUDA(cudaMemcpyAsync(b.pairs.p, pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
   if (overlap) select_and_normals();
+  // pc_mov.estimate_normals(mov_neighbors) of every pair, in its own movable grid
+  b.mov_attr = rp->mov_neighbors > 0;
+  b.mov_cos_max = b.mov_attr ? mov_cos_max_of(rp->max_angle_rad) : -1.0;
+  c.tm.mov_normals_ms = 0;
+  if (b.mov_attr) {
+    b.q_nrm_eff.reserve(nq);
+    StageTimer t(c, &c.tm.mov_normals_ms);
+    batch_mov_normals_launch(c, b, rp->mov_neighbors, max_n_mov);
+    t.stop();
+  }
 
   // ---- the loop: two launches per iteration for the whole batch
   cudaEvent_t e0, e1;

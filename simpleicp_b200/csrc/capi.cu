@@ -24,6 +24,18 @@ bool is_device_ptr(const void* p) {
   return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
 }
 
+// mov_neighbors / max_angle_rad of sicp_register and sicp_register_batch (range checks that need
+// no cloud; mov_neighbors <= n_mov is checked per cloud by the callers)
+void check_mov_neighbors(const Ctx& c, const sicp_register_params& rp) {
+  if (rp.mov_neighbors == 0) return;
+  SICP_REQUIRE(rp.mov_neighbors >= 2 && rp.mov_neighbors <= 64, SICP_ERR_BAD_ARG,
+               "mov_neighbors must be 0 or between 2 and 64 (got " + std::to_string(rp.mov_neighbors) + ")");
+  SICP_REQUIRE(c.variant == SICP_VARIANT_PYTHON, SICP_ERR_BAD_ARG,
+               "the linearised variants have no movable-side attributes (mov_neighbors must be 0)");
+  SICP_REQUIRE(!(rp.max_angle_rad > 1.5707963267948966), SICP_ERR_BAD_ARG,
+               "max_angle_rad must be <= pi/2 (normals are axes), or negative for no angle test");
+}
+
 namespace {
 
 constexpr int kMaxRecords = 4096;
@@ -325,6 +337,7 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.pdl = d.pdl;
     c.keep_knn = d.keep_knn;
     c.knn_coop = d.knn_coop;
+    c.normals_scratch_mb = d.normals_scratch_mb;
   } else if (k == "nn_engine") {
     SICP_REQUIRE(value == 0 || value == 1 || value == 2, SICP_ERR_BAD_ARG, "nn_engine must be 0, 1 or 2");
     c.nn_engine = (int)value;
@@ -367,6 +380,9 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     SICP_REQUIRE(value >= 0 && value <= PageableUploader::kMaxThreads, SICP_ERR_BAD_ARG,
                  "upload_threads must be within [0, 8]");
     c.upload_threads = (int)value;
+  } else if (k == "normals_scratch_mb") {
+    SICP_REQUIRE(value >= 1 && value <= 4096, SICP_ERR_BAD_ARG, "normals_scratch_mb must be within [1, 4096]");
+    c.normals_scratch_mb = (int)value;
   } else if (k == "upload_chunk_kb") {
     SICP_REQUIRE(value >= 64 && value <= 4096, SICP_ERR_BAD_ARG, "upload_chunk_kb must be within [64, 4096]");
     c.up.chunk = (size_t)value << 10;
@@ -481,7 +497,8 @@ int32_t sicp_estimate_normals(sicp_ctx* ctx, int32_t neighbors, float* nx, float
     t.stop();
   }
   StageTimer t(c, &c.tm.normals_ms);
-  estimate_normals_launch(c, neighbors);
+  c.q_nrm.reserve(std::max<long long>(c.K, 1));
+  estimate_normals_launch(c, c.gfix, c.q_xyz.p, c.K, neighbors, c.q_nrm.p, c.keep_knn != 0, false);
   c.have_normals = true;
   if (nx || ny || nz || planarity) {
     c.stage.reserve(sizeof(float) * 4 * c.K);
@@ -537,7 +554,7 @@ int32_t sicp_set_mov_normals(sicp_ctx* ctx, const float* nx, const float* ny, co
   k_join_f4<<<(unsigned)((c.n_mov + 255) / 256), 256, 0, c.stream>>>(s, c.n_mov, c.mov_nrm.p);
   SICP_CUDA(cudaGetLastError());
   c.mov_attr = true;
-  c.mov_cos_max = (max_angle_rad >= 0.0) ? (max_angle_rad >= 1.5707963267948966 ? 0.0 : cos(max_angle_rad)) : -1.0;
+  c.mov_cos_max = mov_cos_max_of(max_angle_rad);
   c.matched = c.rejected = c.solved = false;
   sync(c);
   API_END
@@ -895,6 +912,9 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
   SICP_REQUIRE(n_fix < (1ll << 31) && n_mov < (1ll << 31), SICP_ERR_BAD_ARG,
                "clouds are limited to 2^31 - 1 points");
   SICP_REQUIRE(rp->correspondences >= 1, SICP_ERR_BAD_ARG, "correspondences must be >= 1");
+  check_mov_neighbors(c, *rp);
+  SICP_REQUIRE(rp->mov_neighbors <= n_mov, SICP_ERR_BAD_ARG,
+               "mov_neighbors exceeds the number of points in the movable cloud");
   const bool overlap = rp->max_overlap_distance > 0 && std::isfinite(rp->max_overlap_distance);
   static const bool trace = std::getenv("SICP_TRACE_RUN") != nullptr;
   const auto tr0 = std::chrono::steady_clock::now();
@@ -943,11 +963,25 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
     grid_build(c, c.gfix, c.fix_xyz.p, n_fix);
     t.stop();
   };
+  // pc_mov.estimate_normals(mov_neighbors) on the movable grid just built: the attributes
+  // sicp_set_mov_normals would install, without a host round trip (a device->host read issued
+  // while the other cloud is uploading would wait for that copy, see above)
+  c.tm.mov_normals_ms = 0;
+  auto mov_normals = [&]() {
+    if (rp->mov_neighbors <= 0) return;
+    StageTimer t(c, &c.tm.mov_normals_ms);
+    c.mov_nrm.reserve(n_mov);
+    estimate_normals_launch(c, c.gmov, c.mov_xyz.p, n_mov, rp->mov_neighbors, c.mov_nrm.p, false, true);
+    c.mov_attr = true;
+    c.mov_cos_max = mov_cos_max_of(rp->max_angle_rad);
+    t.stop();
+  };
   c.sel_idx.reserve(n_fix);
   c.tm.overlap_ms = 0;
   if (overlap) {
     build_mov();
     queue_second_copy();
+    mov_normals();  // while the fixed cloud crosses PCIe
     wait_background_upload(c);
     // PointCloud.select_in_range on all fixed points (simpleicp.py:160-170), compacted on the host
     k_iota<<<(unsigned)((n_fix + 255) / 256), 256, 0, c.stream>>>(c.sel_idx.p, n_fix);
@@ -998,7 +1032,8 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
   gather_queries_launch(c);
   {
     StageTimer t(c, &c.tm.normals_ms);
-    estimate_normals_launch(c, rp->neighbors);
+    c.q_nrm.reserve(std::max<long long>(c.K, 1));
+    estimate_normals_launch(c, c.gfix, c.q_xyz.p, c.K, rp->neighbors, c.q_nrm.p, c.keep_knn != 0, false);
     c.have_normals = true;
     t.stop();
   }
@@ -1006,6 +1041,7 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
   if (!overlap) {
     wait_background_upload(c);
     build_mov();
+    mov_normals();
   }
   tr("mov grid");
   if (n_selected) *n_selected = c.K;

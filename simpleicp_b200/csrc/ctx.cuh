@@ -93,6 +93,7 @@ struct Ctx {
   DevBuf<uint32_t> knn_pos;  // K x k record positions (cooperative k-NN kernel -> PCA kernel)
   int keep_knn = 0;          // option "keep_knn": store neighbour indices / distances for sicp_get_knn
   int knn_coop = -1;         // option "knn_coop": 1 cooperative lanes (k <= 16), 0 one thread per query, -1 by K
+  int normals_scratch_mb = 64;  // option "normals_scratch_mb": bound of the movable-normals estimate's neighbour scratch
 
   // per-iteration arrays
   DevBuf<long long> nn_idx;
@@ -210,7 +211,12 @@ struct Batch {
   DevBuf<long long> sel_idx, nn_idx;
   DevBuf<double> q_xyz, dist, m_xyz;
   DevBuf<float4> q_nrm;
-  DevBuf<uint32_t> knn_pos;        // n_pairs x Kmax x k
+  // movable-side attributes (mov_neighbors > 0): per movable point of the batch (total_mov), in its
+  // own frame, and the fixed normal + effective planarity of each match (n_pairs x Kmax)
+  DevBuf<float4> mov_nrm, q_nrm_eff;
+  bool mov_attr = false;
+  double mov_cos_max = -1.0;
+  DevBuf<uint32_t> knn_pos;        // n_pairs x Kmax x k (the movable-normals estimate reuses it)
   DevBuf<unsigned long long> binstore;  // n_pairs x LH_BINS x bin_cap
   int bin_cap = 0;
   DevBuf<uint32_t> nn_pos;
@@ -276,7 +282,14 @@ inline void launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_
   SICP_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...));
 }
 void set_state_transform(Ctx& c, const double x[6], const Rigid* T_or_null, bool reset_loop);
-void estimate_normals_launch(Ctx& c, int k);
+// k-NN (self included) + PCA of n_q queries in grid g; out[i] = (nx, ny, nz, planarity) float32.
+// The fixed side: (c.gfix, c.q_xyz, c.K, c.q_nrm) with keep_lists = option "keep_knn"; the
+// movable side: (c.gmov, c.mov_xyz, c.n_mov, c.mov_nrm), chunked: as many queries per launch as
+// option "normals_scratch_mb" holds at k x 4 bytes of neighbour positions each.
+void estimate_normals_launch(Ctx& c, const Grid& g, const double* q_xyz, long long n_q, int k, float4* out,
+                             bool keep_lists, bool chunked);
+// cos of the angle limit as sicp_set_mov_normals stores it (< 0: no angle test)
+double mov_cos_max_of(double max_angle_rad);
 void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve, bool arm_stop,
                          int rec_slot);
 void compact_residuals_launch(Ctx& c);
@@ -296,6 +309,8 @@ void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHo
 // with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud
 void batch_select_gather_launch(Ctx& c, Batch& b, bool with_list, int round_away);
 void batch_normals_launch(Ctx& c, Batch& b, int k);
+// k-NN + PCA of every movable point of every pair in its own movable grid -> Batch::mov_nrm
+void batch_mov_normals_launch(Ctx& c, Batch& b, int k, long long max_n_mov);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
 // PointCloud.select_in_range of every fixed point of the batch under its pair's DevState
 // transform: Batch::ovl_flag[i] = (squared distance to the nearest movable point < r2)
@@ -307,6 +322,11 @@ int bin_cap_for(long long K);
 
 // helpers in capi.cu
 bool is_device_ptr(const void* p);
+// queries per launch of a chunked k-NN + PCA: c.normals_scratch_mb MiB of k record positions each
+inline long long normals_chunk_queries(const Ctx& c, int k) {
+  return std::max<long long>(1024, ((long long)c.normals_scratch_mb << 20) / (4ll * k));
+}
+void check_mov_neighbors(const Ctx& c, const sicp_register_params& rp);
 
 struct StageTimer {
   Ctx& c;

@@ -581,16 +581,35 @@ struct BatchMatchArgs {
   int sphere;
 };
 template <int MG>
-__global__ void __launch_bounds__(128) k_match_batch(BatchMatchArgs a) {
+__device__ __forceinline__ void match_batch_body(const BatchMatchArgs& a, const float4* mov_nrm, float4* q_eff,
+                                                 double cos_max) {
   const PairDev pd = a.pairs[blockIdx.y];
   const long long gt = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (gt / MG >= pd.K) return;
   const long long q = pd.q_off;
   const CorrOut co{a.binstore + (size_t)blockIdx.y * LH_BINS * a.bin_cap, a.bin_cap, a.m_xyz + 3 * q, a.nn_pos + q, a.warm, a.sphere,
-                   nullptr, nullptr, -1.0};
+                   mov_nrm ? mov_nrm + pd.mov_off : nullptr, mov_nrm ? q_eff + q : nullptr, cos_max};
   match_coop_body<MG>(pd.gmov, a.state + blockIdx.y, a.q_xyz + 3 * q, a.q_nrm + q, nullptr, pd.K, 1 << 30, 1,
                       a.nn_idx + q, a.dist + q, nullptr, a.lin_hist + (size_t)blockIdx.y * (LH_BINS + 2), -1.0,
                       co, gt);
+}
+template <int MG>
+__global__ void __launch_bounds__(128) k_match_batch(BatchMatchArgs a) {
+  match_batch_body<MG>(a, nullptr, nullptr, -1.0);
+}
+// The form with movable-side attributes (mov_neighbors > 0), its own kernel so that the default
+// batch keeps its code: mov_nrm = Batch::mov_nrm (total_mov), q_eff = Batch::q_nrm_eff.  Launched
+// with 128 threads; 128 registers (instead of launch bounds) keep it free of spills (at 96 the
+// 4-lane form spills).  Only the movable-attribute batches run it.
+struct BatchMatchAttrArgs {
+  BatchMatchArgs a;
+  const float4* mov_nrm;
+  float4* q_eff;
+  double cos_max;
+};
+template <int MG>
+__global__ void __maxnreg__(128) k_match_batch_attr(BatchMatchAttrArgs m) {
+  match_batch_body<MG>(m.a, m.mov_nrm, m.q_eff, m.cos_max);
 }
 
 // Overlap filter of a batch (PointCloud.select_in_range, simpleicp.py:158-170): blockIdx.y is the
@@ -1001,7 +1020,15 @@ void batch_match_launch(Ctx& c, Batch& b, bool warm) {
   // programmatically dependent on the previous iteration's k_rs_batch (both kernels wait before
   // they touch anything the other writes; the pair descriptors are static)
   const bool pdl = c.pdl != 0;
-  if (mg == 2) launch_kernel(k_match_batch<2>, grid, dim3(128), 0, c.stream, pdl, a);
+  if (b.mov_attr) {
+    // no 2-lane form (it would spill, like the overlap kernel's): 4 lanes serve it, the result
+    // does not depend on the lanes
+    const BatchMatchAttrArgs m{a, b.mov_nrm.p, b.q_nrm_eff.p, b.mov_cos_max};
+    const dim3 grid_a((unsigned)((b.Kmax * std::max(mg, 4) + 127) / 128), b.n_pairs);
+    if (mg <= 4) launch_kernel(k_match_batch_attr<4>, grid_a, dim3(128), 0, c.stream, pdl, m);
+    else if (mg == 8) launch_kernel(k_match_batch_attr<8>, grid_a, dim3(128), 0, c.stream, pdl, m);
+    else launch_kernel(k_match_batch_attr<16>, grid_a, dim3(128), 0, c.stream, pdl, m);
+  } else if (mg == 2) launch_kernel(k_match_batch<2>, grid, dim3(128), 0, c.stream, pdl, a);
   else if (mg == 4) launch_kernel(k_match_batch<4>, grid, dim3(128), 0, c.stream, pdl, a);
   else if (mg == 8) launch_kernel(k_match_batch<8>, grid, dim3(128), 0, c.stream, pdl, a);
   else launch_kernel(k_match_batch<16>, grid, dim3(128), 0, c.stream, pdl, a);

@@ -475,55 +475,122 @@ __global__ void __launch_bounds__(128)
                     q_nrm + pd.q_off, nullptr, nullptr, blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
 
+// Movable side of a batch, one chunk of queries: blockIdx.y = pair, its movable points
+// [q0, q0 + cq) in its own movable grid; scratch pos is n_pairs x cq x k.  The grid is read
+// through a reference into the pair descriptor (a register copy of it made the cooperative
+// 12-slot form spill), and the one-thread forms are allowed 128 registers (they spilled at the
+// 64 the compiler picks by itself); all forms compile without spills.  128-thread launches.
+struct MovBatchChunk {
+  const PairDev* pairs;
+  const double* mov_xyz;  // concatenated movable clouds
+  long long q0, cq;
+  int k;
+  uint32_t* pos;
+  float4* out;            // total_mov entries
+  __device__ __forceinline__ const GridView& get(const double*& q, long long& n, uint32_t*& p,
+                                      float4*& o) const {
+    const PairDev& pd = pairs[blockIdx.y];
+    n = max(0ll, min(cq, pd.n_mov - q0));
+    q = mov_xyz + 3 * (pd.mov_off + q0);
+    p = pos + (size_t)blockIdx.y * cq * k;
+    o = out + pd.mov_off + q0;
+    return pd.gmov;
+  }
+};
+template <int MG, int KC>
+__global__ void __launch_bounds__(128) k_knn_coop_movb(MovBatchChunk a) {
+  const double* q; long long n; uint32_t* p; float4* o;
+  const GridView& g = a.get(q, n, p, o);
+  knn_coop_body<MG, KC>(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
+}
+template <int KC>
+__global__ void __launch_bounds__(128) k_knn_reg_movb(MovBatchChunk a) {
+  const double* q; long long n; uint32_t* p; float4* o;
+  const GridView& g = a.get(q, n, p, o);
+  knn_reg_body<KC>(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
+}
+__global__ void __maxnreg__(128) k_knn_single_movb(MovBatchChunk a) {
+  const double* q; long long n; uint32_t* p; float4* o;
+  const GridView& g = a.get(q, n, p, o);
+  knn_single_body(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
+}
+__global__ void __maxnreg__(128) k_pca_movb(MovBatchChunk a, int sign_mode) {
+  const double* q; long long n; uint32_t* p; float4* o;
+  const GridView& g = a.get(q, n, p, o);
+  pca_from_knn_body(g, q, n, a.k, sign_mode, p, o, nullptr, nullptr,
+                    blockIdx.x * (long long)blockDim.x + threadIdx.x);
+}
+
+// Which k-NN kernel serves n_q queries (knn_coop: 1 = cooperative lanes (k <= 16), 0 = one thread
+// per query with the list in local memory, 2 = one thread per query with the list in registers
+// (k <= 16), -1 (default) = cooperative while the search is latency-bound (few queries), one
+// thread per query with the local-memory list once the queries fill the machine (K = 100 000,
+// k = 10: faster than a register list or cooperative lanes -- the fixed-length insertion network
+// costs more than the early-exit loop saves in memory traffic).
+enum class KnnKind { Coop, Reg, Single };
+KnnKind knn_kind(const Ctx& c, int k, long long n_q) {
+  if ((k <= 16) && (c.knn_coop == 1 || (c.knn_coop < 0 && n_q <= 16384))) return KnnKind::Coop;
+  if ((k <= 16) && c.knn_coop == 2) return KnnKind::Reg;
+  return KnnKind::Single;
+}
+
 }  // namespace
 
-void estimate_normals_launch(Ctx& c, int k) {
+double mov_cos_max_of(double max_angle_rad) {
+  return (max_angle_rad >= 0.0) ? (max_angle_rad >= 1.5707963267948966 ? 0.0 : cos(max_angle_rad)) : -1.0;
+}
+
+void estimate_normals_launch(Ctx& c, const Grid& grid, const double* q_xyz, long long n_q, int k, float4* out,
+                             bool keep_lists, bool chunked) {
   SICP_REQUIRE(k >= 2 && k <= kMaxK, SICP_ERR_BAD_ARG,
                "neighbors must be between 2 and 64 (got " + std::to_string(k) + ")");
-  SICP_REQUIRE((long long)k <= c.n_fix, SICP_ERR_BAD_ARG,
-               "neighbors exceeds the number of points in the fixed cloud");
-  c.q_nrm.reserve(std::max<long long>(c.K, 1));
+  SICP_REQUIRE((long long)k <= grid.n, SICP_ERR_BAD_ARG,
+               &grid == &c.gmov ? "mov_neighbors exceeds the number of points in the movable cloud"
+                                            : "neighbors exceeds the number of points in the fixed cloud");
   // the neighbour lists leave the SM only when somebody wants to look at them (option "keep_knn")
   long long* kidx = nullptr;
   double* kd2 = nullptr;
-  if (c.keep_knn) {
-    c.knn_idx.reserve((size_t)c.K * k);
-    c.knn_d2.reserve((size_t)c.K * k);
+  if (keep_lists) {
+    c.knn_idx.reserve((size_t)n_q * k);
+    c.knn_d2.reserve((size_t)n_q * k);
     kidx = c.knn_idx.p;
     kd2 = c.knn_d2.p;
   }
-  c.knn_k = c.keep_knn ? k : 0;
-  // All k-NN kernels hand record positions to k_pca_from_knn.  knn_coop: 1 = cooperative lanes
-  // (k <= 16), 0 = one thread per query with the list in local memory, 2 = one thread per query
-  // with the list in registers (k <= 16), -1 (default) = cooperative while the search is
-  // latency-bound (few queries), one thread per query with the local-memory list once the queries
-  // fill the machine (K = 100 000, k = 10: faster than a register list or cooperative lanes — the
-  // fixed-length insertion network costs more than the early-exit loop saves in memory traffic).
-  const bool coop = (k <= 16) && (c.knn_coop == 1 || (c.knn_coop < 0 && c.K <= 16384));
-  const bool reg = (k <= 16) && c.knn_coop == 2;
-  c.knn_pos.reserve((size_t)c.K * k);
-  const GridView g = c.gfix.view();
-  if (coop) {
-    const int mg = (c.K <= 32768) ? 8 : 4;
-    const unsigned blocks = (unsigned)((c.K * mg + 127) / 128);
-    if (mg == 8) {
-      if (k <= 12) k_knn_coop<8, 12><<<blocks, 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
-      else k_knn_coop<8, 16><<<blocks, 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
+  if (keep_lists || !chunked) c.knn_k = keep_lists ? k : 0;
+  // All k-NN kernels hand record positions to k_pca_from_knn (the choice: knn_kind).  The kernel
+  // is chosen by the whole query count, so a chunked estimate runs the kernels an unchunked one
+  // would; a chunk only bounds the scratch of the positions.
+  const KnnKind kind = knn_kind(c, k, n_q);
+  const long long chunk = chunked ? std::min<long long>(n_q, normals_chunk_queries(c, k)) : n_q;
+  c.knn_pos.reserve((size_t)std::max<long long>(chunk, 1) * k);
+  const GridView g = grid.view();
+  uint32_t* pos = c.knn_pos.p;
+  for (long long q0 = 0; q0 < n_q; q0 += chunk) {
+    const long long n = std::min(chunk, n_q - q0);
+    const double* q = q_xyz + 3 * q0;
+    const unsigned blocks1 = (unsigned)((n + 127) / 128);
+    if (kind == KnnKind::Coop) {
+      const int mg = (n_q <= 32768) ? 8 : 4;
+      const unsigned blocks = (unsigned)((n * mg + 127) / 128);
+      if (mg == 8) {
+        if (k <= 12) k_knn_coop<8, 12><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
+        else k_knn_coop<8, 16><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
+      } else {
+        if (k <= 12) k_knn_coop<4, 12><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
+        else k_knn_coop<4, 16><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
+      }
+    } else if (kind == KnnKind::Reg && k <= 12) {
+      k_knn_reg<12><<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
+    } else if (kind == KnnKind::Reg) {
+      k_knn_reg<16><<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
     } else {
-      if (k <= 12) k_knn_coop<4, 12><<<blocks, 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
-      else k_knn_coop<4, 16><<<blocks, 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
+      k_knn_single<<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
     }
-  } else if (reg && k <= 12) {
-    k_knn_reg<12><<<(unsigned)((c.K + 127) / 128), 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
-  } else if (reg) {
-    k_knn_reg<16><<<(unsigned)((c.K + 127) / 128), 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
-  } else {
-    k_knn_single<<<(unsigned)((c.K + 127) / 128), 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.knn_pos.p);
+    k_pca_from_knn<<<blocks1, 128, 0, c.stream>>>(g, q, n, k, c.sign_mode, pos, out + q0,
+                                                  kidx ? kidx + q0 * k : nullptr, kd2 ? kd2 + q0 * k : nullptr);
+    SICP_CUDA(cudaGetLastError());
+    c.tm.kernel_launches += 2;
   }
-  k_pca_from_knn<<<(unsigned)((c.K + 127) / 128), 128, 0, c.stream>>>(g, c.q_xyz.p, c.K, k, c.sign_mode,
-                                                                      c.knn_pos.p, c.q_nrm.p, kidx, kd2);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 2;
 }
 
 void batch_normals_launch(Ctx& c, Batch& b, int k) {
@@ -551,6 +618,35 @@ void batch_normals_launch(Ctx& c, Batch& b, int k) {
       b.pairs.p, b.q_xyz.p, k, b.Kmax, c.sign_mode, b.knn_pos.p, b.q_nrm.p);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 2;
+}
+
+void batch_mov_normals_launch(Ctx& c, Batch& b, int k, long long max_n_mov) {
+  SICP_REQUIRE(k >= 2 && k <= kMaxK, SICP_ERR_BAD_ARG,
+               "mov_neighbors must be between 2 and 64 (got " + std::to_string(k) + ")");
+  // every pair's chunk of queries in one launch; the neighbour positions of a launch
+  // (n_pairs x cq x k x 4 bytes) stay within option "normals_scratch_mb"
+  const long long cq = std::min<long long>(max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / b.n_pairs));
+  const KnnKind kind = knn_kind(c, k, b.total_mov);
+  b.knn_pos.reserve((size_t)b.n_pairs * cq * k);
+  b.mov_nrm.reserve(std::max<long long>(b.total_mov, 1));
+  for (long long q0 = 0; q0 < max_n_mov; q0 += cq) {
+    const MovBatchChunk a{b.pairs.p, b.mov_xyz.p, q0, cq, k, b.knn_pos.p, b.mov_nrm.p};
+    const dim3 grid1((unsigned)((cq + 127) / 128), b.n_pairs);
+    if (kind == KnnKind::Coop) {
+      const dim3 grid((unsigned)((cq * 8 + 127) / 128), b.n_pairs);
+      if (k <= 12) k_knn_coop_movb<8, 12><<<grid, 128, 0, c.stream>>>(a);
+      else k_knn_coop_movb<8, 16><<<grid, 128, 0, c.stream>>>(a);
+    } else if (kind == KnnKind::Reg && k <= 12) {
+      k_knn_reg_movb<12><<<grid1, 128, 0, c.stream>>>(a);
+    } else if (kind == KnnKind::Reg) {
+      k_knn_reg_movb<16><<<grid1, 128, 0, c.stream>>>(a);
+    } else {
+      k_knn_single_movb<<<grid1, 128, 0, c.stream>>>(a);
+    }
+    k_pca_movb<<<grid1, 128, 0, c.stream>>>(a, c.sign_mode);
+    SICP_CUDA(cudaGetLastError());
+    c.tm.kernel_launches += 2;
+  }
 }
 
 }  // namespace sicp

@@ -2557,8 +2557,8 @@ void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool wa
   RSArgs& a = ba.proto;
   a = RSArgs{};
   a.dist = b.dist.p;
-  a.q_nrm = b.q_nrm.p;
-  a.pl_signed = 0;
+  a.q_nrm = b.mov_attr ? b.q_nrm_eff.p : b.q_nrm.p;  // k_finish_batch keeps the fixed normals
+  a.pl_signed = b.mov_attr ? 1 : 0;
   a.q_xyz = b.q_xyz.p;
   a.keep = b.keep.p;
   a.binstore = b.binstore.p;

@@ -129,11 +129,7 @@ class PointCloud(pd.DataFrame):
     def estimate_normals(self, neighbors: int) -> None:
         """Normals and planarity of the selected points from their k nearest neighbours."""
         idx = self.idx_selected
-        with _capi.Engine() as eng:
-            eng.set_clouds(self.X, self.X[:1])
-            eng.set_selected(idx)
-            nx, ny, nz, pl = eng.estimate_normals(neighbors)
-        self.set_normals(idx, nx, ny, nz, pl)
+        self.set_normals(idx, *estimate_normals_of(self.X, idx, neighbors))
 
     def set_normals(self, idx, nx, ny, nz, planarity) -> None:
         """Store float32 attribute columns (NaN where not estimated), as the reference does
@@ -165,6 +161,15 @@ class PointCloud(pd.DataFrame):
     def write_xyz(self, file: Path):
         """CloudCompare-style xyz text file (reference: pointcloud.py:219-226)."""
         self[_XYZ].to_csv(file, sep=" ", header=["//X", "Y", "Z"], index=False, float_format="%.3f")
+
+
+def estimate_normals_of(X, idx, neighbors: int):
+    """(nx, ny, nz, planarity) float32 of the points X[idx] (idx None: all of them) from their k
+    nearest neighbours in X, itself included: what PointCloud.estimate_normals stores."""
+    with _capi.Engine() as eng:
+        eng.set_clouds(X, X[:1])
+        eng.set_selected(idx)
+        return eng.estimate_normals(neighbors)
 
 
 def _sparse_f32_column(n: int, idx: np.ndarray, vals: np.ndarray):

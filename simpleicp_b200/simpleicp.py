@@ -56,6 +56,27 @@ def _check_arguments(distance_weights, rbp_observed_values, rbp_observation_weig
         raise SimpleICPException("At least one element in rbp_observation_weights must be finite.")
 
 
+def _check_mov_arguments(mov_neighbors, max_angle_between_normals, mov_normals=None, n_mov=None) -> None:
+    """The movable-side keywords: ``mov_neighbors`` (k of pc_mov.estimate_normals(k)) in [2, 64] and
+    at most the movable point count, not together with ``mov_normals``; ``max_angle_between_normals``
+    within [0, 90] degrees and only with movable normals."""
+    if mov_neighbors is not None:
+        if mov_normals is not None:
+            raise SimpleICPException("Give either mov_normals or mov_neighbors, not both.")
+        if isinstance(mov_neighbors, bool) or int(mov_neighbors) != mov_neighbors or not 2 <= int(mov_neighbors) <= 64:
+            raise SimpleICPException("mov_neighbors must be an integer within [2, 64].")
+        if n_mov is not None and int(mov_neighbors) > n_mov:
+            raise SimpleICPException("mov_neighbors exceeds the number of points in the movable point cloud.")
+    if max_angle_between_normals is not None:
+        if mov_normals is None and mov_neighbors is None:
+            raise SimpleICPException(
+                "max_angle_between_normals needs the normals of the movable point cloud "
+                "(mov_neighbors=k, PointCloud.estimate_normals on pc_mov, or mov_normals=...)."
+            )
+        if not 0.0 <= float(max_angle_between_normals) <= 90.0:
+            raise SimpleICPException("max_angle_between_normals must be within [0, 90] degrees.")
+
+
 def _observed_in_radians(rbp_observed_values) -> np.ndarray:
     # The reference converts in place inside np.array(rbp_observed_values) (simpleicp.py:146-148),
     # i.e. an all-integer tuple stays an integer array; kept for drop-in behaviour.
@@ -163,6 +184,7 @@ def register(
     want_normals: bool = True,
     mov_normals: Optional[Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]] = None,
     max_angle_between_normals: Optional[float] = None,
+    mov_neighbors: Optional[int] = None,
 ) -> _Result:
     """Core of both front ends: one registration on one GPU.
 
@@ -177,16 +199,13 @@ def register(
     ``mov_normals``) additionally drops correspondences whose normals differ by more than that
     angle after the distance rejection: the reference declares this step
     (``reject_wrt_to_angle_between_normals``, simpleicp.py:207) but leaves it unimplemented.
+
+    ``mov_neighbors=k`` has the effect of ``pc_mov.estimate_normals(k)`` before the run: the
+    movable attributes are estimated from k neighbours (inside the one library call when the
+    registration is fused, through ``PointCloud.estimate_normals``'s code otherwise).
     """
     _check_arguments(distance_weights, rbp_observed_values, rbp_observation_weights)
-    if max_angle_between_normals is not None:
-        if mov_normals is None:
-            raise SimpleICPException(
-                "max_angle_between_normals needs the normals of the movable point cloud "
-                "(PointCloud.estimate_normals on pc_mov, or mov_normals=...)."
-            )
-        if not 0.0 <= float(max_angle_between_normals) <= 90.0:
-            raise SimpleICPException("max_angle_between_normals must be within [0, 90] degrees.")
+    _check_mov_arguments(mov_neighbors, max_angle_between_normals, mov_normals, int(np.shape(X_mov)[0]))
     if debug_dirpath:
         _log.info(f'Write debug files to directory "{debug_dirpath}"')
         Path(debug_dirpath).mkdir(parents=True, exist_ok=True)
@@ -205,7 +224,10 @@ def register(
             # nothing but the results comes back (simpleicp_b200/_capi.py::register_fused)
             return _register_fused(eng, X_fix, X_mov, correspondences, neighbors, min_planarity,
                                    max_overlap_distance, min_change, max_iterations, distance_weights,
-                                   obs, w_obs, rbp_observation_weights, transform_out)
+                                   obs, w_obs, rbp_observation_weights, transform_out, mov_neighbors,
+                                   max_angle_between_normals)
+        if mov_neighbors is not None:
+            mov_normals = pointcloud.estimate_normals_of(X_mov, None, int(mov_neighbors))
         eng.set_clouds(X_fix, X_mov)
         n_fix = eng.n_fix
         if mov_normals is not None:
@@ -307,7 +329,7 @@ def _make_rbp(obs, rbp_observation_weights, records, iterations, x, sigma):
 
 def _register_fused(eng, X_fix, X_mov, correspondences, neighbors, min_planarity, max_overlap_distance,
                     min_change, max_iterations, distance_weights, obs, w_obs, rbp_observation_weights,
-                    transform_out) -> _Result:
+                    transform_out, mov_neighbors=None, max_angle_between_normals=None) -> _Result:
     for msg in ("Consider partial overlap of point clouds ..." if np.isfinite(max_overlap_distance) else None,
                 "Select points for correspondences in fixed point cloud ...",
                 "Estimate normals of selected points ...", "Start iterations ..."):
@@ -318,7 +340,9 @@ def _register_fused(eng, X_fix, X_mov, correspondences, neighbors, min_planarity
     try:
         out, log, residuals, X_t = eng.register_fused(
             X_fix, X_mov, correspondences, neighbors,
-            max_overlap_distance if np.isfinite(max_overlap_distance) else -1.0, params, transform_out)
+            max_overlap_distance if np.isfinite(max_overlap_distance) else -1.0, params, transform_out,
+            0 if mov_neighbors is None else int(mov_neighbors),
+            -1.0 if max_angle_between_normals is None else float(np.deg2rad(max_angle_between_normals)))
     except _capi.SicpError as e:
         raise _wrap_error(e, max_overlap_distance) from None
     records, iterations = _records(log), int(out.iterations)
