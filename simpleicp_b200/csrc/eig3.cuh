@@ -4,13 +4,17 @@
 // calls LAPACK dgeev, whose eigenvector SIGN is an artefact of its algorithm (no geometric
 // meaning) but decides the sign of every point-to-plane distance downstream (median / MAD,
 // corrpts.py:184-187).  `eig3_dgeev` therefore follows dgeev's published algorithm for a 3 x 3
-// input step by step — dgebal (a no-op for symmetric input), dgehd2 (one Householder reflector),
-// dorghr, dlahqr (double-shift QR with the Ahues-Tisseur deflation test, dlanv2 for the final
-// 2 x 2 block), dtrevc back-substitution and back-transformation, max-norm then 2-norm scaling —
-// so that eigenvalue slots and eigenvector signs come out as NumPy's do.  Measured agreement with
-// np.linalg.eig on 12 000 neighbourhood covariances of the reference's data sets: 99.8 %; the
-// rest are inputs whose deflation test sits within rounding of its threshold (one QR sweep more
-// or fewer flips two columns).  `eig3_jacobi` (cyclic Jacobi, canonical sign) is the other mode.
+// input step by step — dgebal('B') (its scaling is a no-op for symmetric input, its permutation
+// is not: a row whose off-diagonal entries are exactly zero, as on an axis-aligned wall, is
+// isolated and moved to the end), dgehd2 (one Householder reflector) and dorghr on the remaining
+// block, dlahqr (double-shift QR with the Ahues-Tisseur deflation test, dlanv2 for the final
+// 2 x 2 block), dtrevc back-substitution and back-transformation, max-norm scaling, dgebak's row
+// swap, 2-norm scaling — so that eigenvalue slots and eigenvector signs come out as NumPy's do.
+// Measured agreement with np.linalg.eig on 12 000 neighbourhood covariances of the reference's
+// data sets: 99.8 %; the rest are inputs whose deflation test sits within rounding of its
+// threshold (one QR sweep more or fewer flips two columns).  On designed covariances (exact zero
+// off-diagonals, rank 0 and 1, repeated eigenvalues) the float32 normals are bit-identical
+// (tests/test_eig3_host.py).  `eig3_jacobi` (cyclic Jacobi, canonical sign) is the other mode.
 //
 // Header-only and compilable by a host C++ compiler (tests build it with g++ and compare with
 // NumPy on the CPU).
@@ -76,6 +80,12 @@ constexpr double kEps = 2.220446049250313e-16;      // dlamch('P')
 constexpr double kSafmin = 2.2250738585072014e-308;  // dlamch('S')
 
 __host__ __device__ inline double sgn(double a, double b) { return (b >= 0.0) ? fabs(a) : -fabs(a); }
+
+__host__ __device__ inline void swap2(double& a, double& b) {
+  const double t = a;
+  a = b;
+  b = t;
+}
 
 __host__ __device__ inline double lapy2(double x, double y) {
   const double w = fmax(fabs(x), fabs(y)), z = fmin(fabs(x), fabs(y));
@@ -172,16 +182,20 @@ __host__ __device__ inline void lanv2(double& a, double& b, double& c, double& d
 
 }  // namespace dgeev3
 
-// dgeev on a symmetric 3 x 3 matrix: wr = eigenvalues in LAPACK's slot order, vr = unit
-// eigenvectors as columns with LAPACK's signs.  Returns false if the QR iteration fails.
-__host__ __device__ inline bool eig3_dgeev(const double A[3][3], double wr[3], double vr[3][3]) {
-  using namespace dgeev3;
-  double h[3][3], z[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) h[i][j] = A[i][j];
-  // dgehd2: one reflector acting on rows/columns 1..2
-  double v1[2];
-  {
+namespace dgeev3 {
+
+// dgeev after dgebal's permutation: h = P A P^T, QR on rows/columns 0..IHI (a template
+// parameter, so that the full 3 x 3 path carries no block bounds in registers); dgebak swaps the
+// eigenvector rows piv <-> 2 back.
+template <int IHI>
+__host__ __device__ inline bool dgeev_core(double h[3][3], int piv, double wr[3], double vr[3][3]) {
+  double z[3][3];
+  // dgehd2 on ilo..ihi: one reflector acting on rows/columns 1..2 (the identity unless IHI = 2)
+  z[0][0] = 1.0; z[0][1] = 0.0; z[0][2] = 0.0;
+  z[1][0] = 0.0; z[1][1] = 1.0; z[1][2] = 0.0;
+  z[2][0] = 0.0; z[2][1] = 0.0; z[2][2] = 1.0;
+  if (IHI == 2) {
+    double v1[2];
     double alpha = h[1][0];
     double x[1] = {h[2][0]};
     const double tau = larfg(2, alpha, x);
@@ -200,13 +214,15 @@ __host__ __device__ inline bool eig3_dgeev(const double A[3][3], double wr[3], d
       h[2][j] -= tau * s * v1[1];
     }
     // dorghr
-    z[0][0] = 1.0; z[0][1] = 0.0; z[0][2] = 0.0;
-    z[1][0] = 0.0; z[1][1] = 1.0 - tau * v1[0] * v1[0]; z[1][2] = -tau * v1[0] * v1[1];
-    z[2][0] = 0.0; z[2][1] = -tau * v1[1] * v1[0]; z[2][2] = 1.0 - tau * v1[1] * v1[1];
+    z[1][1] = 1.0 - tau * v1[0] * v1[0]; z[1][2] = -tau * v1[0] * v1[1];
+    z[2][1] = -tau * v1[1] * v1[0]; z[2][2] = 1.0 - tau * v1[1] * v1[1];
   }
-  // dlahqr (ilo = 0, ihi = 2, wantt, wantz)
-  const int ilo = 0, ihi = 2, i1 = 0, i2 = 2;
-  const double ulp = kEps, smlnum = kSafmin * (3.0 / kEps);
+  // dhseqr: the eigenvalues dgebal isolated
+  if (IHI < 2) wr[2] = h[2][2];
+  if (IHI < 1) wr[1] = h[1][1];
+  // dlahqr (ilo = 0, ihi = IHI, wantt, wantz with iloz = ilo, ihiz = ihi)
+  const int ilo = 0, ihi = IHI, i1 = 0, i2 = 2;
+  const double ulp = kEps, smlnum = kSafmin * ((double)(ihi - ilo + 1) / kEps);
   const int itmax = 300;
   int kdefl = 0;
   int i = ihi;
@@ -344,7 +360,7 @@ __host__ __device__ inline bool eig3_dgeev(const double A[3][3], double wr[3], d
         h[j][i] = cs * h[j][i] - sn * h[j][i - 1];
         h[j][i - 1] = t;
       }
-      for (int j = 0; j < 3; ++j) {
+      for (int j = ilo; j <= ihi; ++j) {
         const double t = cs * z[j][i - 1] + sn * z[j][i];
         z[j][i] = cs * z[j][i] - sn * z[j][i - 1];
         z[j][i - 1] = t;
@@ -374,10 +390,56 @@ __host__ __device__ inline bool eig3_dgeev(const double A[3][3], double wr[3], d
     }
     const double emax = fmax(fabs(col[0]), fmax(fabs(col[1]), fabs(col[2])));
     for (int r = 0; r < 3; ++r) col[r] /= emax;
+    // dgebak: undo dgebal's row swap before dgeev's 2-norm scaling
+    if (IHI < 2 && piv == 0) swap2(col[0], col[2]);
+    if (IHI < 2 && piv == 1) swap2(col[1], col[2]);
     const double nrm = sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
     for (int r = 0; r < 3; ++r) vr[r][ki] = col[r] / nrm;
   }
   return true;
+}
+
+// The rare blocks after an isolation, out of line: the common full-block path keeps its registers.
+#ifdef __CUDACC__
+__noinline__
+#endif
+static __host__ __device__ bool dgeev_isolated(double h[3][3], int ihi, int piv, double wr[3], double vr[3][3]) {
+  return (ihi == 1) ? dgeev_core<1>(h, piv, wr, vr) : dgeev_core<0>(h, piv, wr, vr);
+}
+
+}  // namespace dgeev3
+
+// dgeev on a symmetric 3 x 3 matrix: wr = eigenvalues in LAPACK's slot order, vr = unit
+// eigenvectors as columns with LAPACK's signs.  Returns false if the QR iteration fails.
+__host__ __device__ inline bool eig3_dgeev(const double A[3][3], double wr[3], double vr[3][3]) {
+  using namespace dgeev3;
+  double h[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) h[i][j] = A[i][j];
+  // dgebal('B'), permutation phase.  The row search (from the last row up, pushing a row whose
+  // off-diagonal entries within the active block are all exactly zero to the block's end) on a
+  // symmetric 3 x 3 input: row 2 isolated stays (and with c01 = 0 too, rows 1 and 0 follow in place:
+  // ilo = ihi = 0); else row 1 or row 0 isolated is swapped with row 2.  The column search then
+  // finds nothing: a column isolated in a symmetric block is an isolated row the search would
+  // have taken.  The scaling phase is a no-op (row and column norms are equal).  So P A P^T swaps
+  // `piv` with 2 (or nothing), QR runs on 0..ihi, and dgebak swaps the eigenvector rows back.
+  int ihi = 2, piv = 2;
+  if (h[2][0] == 0.0 && h[2][1] == 0.0) {
+    ihi = (h[1][0] == 0.0) ? 0 : 1;
+  } else if ((h[1][0] == 0.0 && h[1][2] == 0.0) || (h[0][1] == 0.0 && h[0][2] == 0.0)) {
+    piv = (h[1][0] == 0.0 && h[1][2] == 0.0) ? 1 : 0;
+    ihi = 1;
+    // columns piv <-> 2, then rows piv <-> 2, written out (constant indices keep h in registers)
+    if (piv == 0) {
+      swap2(h[0][0], h[2][2]); swap2(h[0][1], h[2][1]); swap2(h[0][2], h[2][0]); swap2(h[1][0], h[1][2]);
+    } else {
+      swap2(h[1][1], h[2][2]); swap2(h[0][1], h[0][2]); swap2(h[1][0], h[2][0]); swap2(h[1][2], h[2][1]);
+    }
+  }
+  switch (ihi) {
+    case 2: return dgeev_core<2>(h, piv, wr, vr);
+    default: return dgeev3::dgeev_isolated(h, ihi, piv, wr, vr);
+  }
 }
 
 // Eigenvalues sorted descending in w; n = unit eigenvector of the smallest eigenvalue.
@@ -399,11 +461,14 @@ __host__ __device__ inline void eig3_smallest(double c00, double c01, double c02
     const double A[3][3] = {{c00, c01, c02}, {c01, c11, c12}, {c02, c12, c22}};
     double wr[3], vr[3][3];
     if (eig3_dgeev(A, wr, vr)) {
-      // reference: idx = eig_vals.argsort()[::-1] (pointcloud.py:192) -> descending order
+      // reference: idx = eig_vals.argsort()[::-1] (pointcloud.py:192).  NumPy's argsort keeps
+      // equal values in slot order at n = 3, so after the reversal the order is descending in
+      // (value, slot): among equal eigenvalues the LOWEST slot comes last and is the normal.
       int i0 = 0, i1 = 1, i2 = 2;
-      if (wr[i0] < wr[i1]) { const int t = i0; i0 = i1; i1 = t; }
-      if (wr[i1] < wr[i2]) { const int t = i1; i1 = i2; i2 = t; }
-      if (wr[i0] < wr[i1]) { const int t = i0; i0 = i1; i1 = t; }
+      auto after = [&](int a, int b) { return wr[a] < wr[b] || (wr[a] == wr[b] && a < b); };
+      if (after(i0, i1)) { const int t = i0; i0 = i1; i1 = t; }
+      if (after(i1, i2)) { const int t = i1; i1 = i2; i2 = t; }
+      if (after(i0, i1)) { const int t = i0; i0 = i1; i1 = t; }
       w[0] = wr[i0];
       w[1] = wr[i1];
       w[2] = wr[i2];
