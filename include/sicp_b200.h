@@ -91,11 +91,8 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value);
  *        (points per occupied cell, default 3), "grid_max_rings" (ring limit before the
  *        brute-force pass takes over, default 8), "grid_sort_cells" (0/1), "host_sync_every"
  *        (iterations queued between host reads in sicp_run, default 4), "match_group" (lanes per
- *        query in the grid search: 0 = by K, 1, 4, 8, 16), "rs_blocks" (blocks of the cooperative
- *        reject/solve kernel, 0 = one per SM), "fused" (1: iterations after the first run their
- *        reject + solve in the barrier-free kernel, 0: always the cooperative kernel),
- *        "split_solve" (1: the serial part of the barrier-free kernel runs in a one-block kernel
- *        launched behind it, 0: in the kernel's last block; the results are the same bit for bit),
+ *        query in the grid search: 0 = by K, 1, 4, 8, 16), "fused" (1: iterations after the first
+ *        run their reject + solve in the barrier-free kernel, 0: always the cooperative kernel),
  *        "warm_start" (1: the grid search of an iteration starts from the previous iteration's
  *        neighbour as upper bound), "keep_knn" (see sicp_get_knn), "knn_coop" (k-NN search: 1 cooperative
  *        lanes per query (k <= 16), 0 one thread per query, -1 (default) by the number of queries),
@@ -334,15 +331,14 @@ int32_t sicp_time_stages(sicp_ctx* ctx, const sicp_run_params* p, int32_t reps, 
  * [10..12] / [14..16] radix levels done / gather barrier / sort done for the median / MAD;
  * [24],[25] radix levels used, [26],[27] candidates sorted (raw counts, not times; 0 when a
  * predictor select failed and no radix select followed); [28] path:
- * 0 radix select, 1 predictor histogram (cooperative kernel), 2 barrier-free kernel (there
- * [2] = select done, [3] = accumulation done in block 0, [4] = last block starts, [17] partials
- * reduced, [18] M assembled, [19] solve done, [9] exit).
+ * 0 cooperative kernel (radix select), 2 barrier-free kernel (there [2] = select done, [3] =
+ * accumulation done in block 0, [4] = serial tail starts, [17] partials reduced, [18] M
+ * assembled, [19] solve done, [9] exit).
  * Selection diagnostics (codes, not times; csrc/reject_solve.cuh: SelectPath, SelectOutcome):
- * [29] the selection that produced the last record's median and MAD: 0 radix, 1 predictor gather
- * of the cooperative kernel, 2 per-bin key store of the barrier-free kernel (not written by a
- * barrier-free launch that missed its prediction: the general kernel repeats that iteration);
- * [30] outcome of the predictor select of the last barrier-free launch, [31] of the last
- * cooperative-kernel launch: 0 used, > 0 the first check that failed.                          */
+ * [29] the selection that produced the last record's median and MAD: 0 radix, 2 per-bin key
+ * store of the barrier-free kernel (not written by a barrier-free launch that missed its
+ * prediction: the general kernel repeats that iteration); [30] outcome of the predictor select
+ * of the last barrier-free launch: 0 used, > 0 the first check that failed.                     */
 int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32] /*[h]*/);
 
 /* Test-only: overwrite the order-statistic predictor (median, MAD and the planarity bound of

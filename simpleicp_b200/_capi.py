@@ -22,14 +22,13 @@ NN_AUTO, NN_GRID, NN_BRUTE = 0, 1, 2
 SIGN_DGEEV, SIGN_CANONICAL = 0, 1
 
 # selection diagnostics of Engine.phase_times() (csrc/reject_solve.cuh: SelectPath, SelectOutcome)
-SLOT_SEL_PATH, SLOT_SEL_FUSED, SLOT_SEL_COOP = 29, 30, 31
-SEL_PATH_RADIX, SEL_PATH_PREDICT, SEL_PATH_BINSTORE = 0, 1, 2
-SEL_OK, SEL_NO_PREDICTION, SEL_NOT_ATTEMPTED, SEL_MEDIAN_OUTSIDE, SEL_MEDIAN_NO_BIN = 0, 1, 2, 3, 4
+SLOT_SEL_PATH, SLOT_SEL_FUSED = 29, 30
+SEL_PATH_RADIX, SEL_PATH_BINSTORE = 0, 2
+SEL_OK, SEL_NO_PREDICTION, SEL_MEDIAN_OUTSIDE = 0, 1, 3
 SEL_MEDIAN_GAP, SEL_MEDIAN_CANDIDATES, SEL_MAD_BRACKET, SEL_MAD_WINDOW = 5, 6, 7, 8
 SEL_MAD_CANDIDATES, SEL_BIN_CAP = 9, 10
 SEL_OUTCOMES = {
-    "SEL_OK": SEL_OK, "SEL_NO_PREDICTION": SEL_NO_PREDICTION, "SEL_NOT_ATTEMPTED": SEL_NOT_ATTEMPTED,
-    "SEL_MEDIAN_OUTSIDE": SEL_MEDIAN_OUTSIDE, "SEL_MEDIAN_NO_BIN": SEL_MEDIAN_NO_BIN,
+    "SEL_OK": SEL_OK, "SEL_NO_PREDICTION": SEL_NO_PREDICTION, "SEL_MEDIAN_OUTSIDE": SEL_MEDIAN_OUTSIDE,
     "SEL_MEDIAN_GAP": SEL_MEDIAN_GAP, "SEL_MEDIAN_CANDIDATES": SEL_MEDIAN_CANDIDATES,
     "SEL_MAD_BRACKET": SEL_MAD_BRACKET, "SEL_MAD_WINDOW": SEL_MAD_WINDOW,
     "SEL_MAD_CANDIDATES": SEL_MAD_CANDIDATES, "SEL_BIN_CAP": SEL_BIN_CAP,
@@ -556,12 +555,12 @@ class Engine:
         return list(us)
 
     def selection(self) -> dict:
-        """Selection diagnostics of the last reject/solve launches (phase_times slots 29..31):
-        which path produced the last record's median/MAD, and the outcome codes of the last
-        predictor attempt of the barrier-free and of the cooperative kernel."""
+        """Selection diagnostics of the last reject/solve launches (phase_times slots 29 and 30):
+        which path produced the last record's median/MAD, and the outcome code of the last
+        predictor attempt of the barrier-free kernel."""
         us = self.phase_times()
         return {"path": int(us[SLOT_SEL_PATH]), "fused": int(us[SLOT_SEL_FUSED]),
-                "coop": int(us[SLOT_SEL_COOP]), "cnt_med": int(us[26]), "cnt_edge": int(us[27])}
+                "cnt_med": int(us[26]), "cnt_edge": int(us[27])}
 
     def seed_predictor(self, med: float, mad: float, min_planarity: float):
         """Test-only (sicp_debug_seed_predictor): the predictor the next match bins with."""

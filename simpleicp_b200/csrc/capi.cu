@@ -325,13 +325,11 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.grid_target_occ = d.grid_target_occ;
     c.grid_max_rings = d.grid_max_rings;
     c.grid_sort_cells = d.grid_sort_cells;
-    c.rs_blocks = d.rs_blocks;
     c.match_group = d.match_group;
     c.host_sync_every = d.host_sync_every;
     c.upload_threads = d.upload_threads;
     c.up.chunk = d.up.chunk;
     c.fused = d.fused;
-    c.split_solve = d.split_solve;
     c.warm_start = d.warm_start;
     c.sphere_scan = d.sphere_scan;
     c.pdl = d.pdl;
@@ -367,11 +365,6 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.warm_start = (value != 0) ? 1 : 0;
   } else if (k == "fused") {
     c.fused = (value != 0) ? 1 : 0;
-  } else if (k == "split_solve") {
-    c.split_solve = (value != 0) ? 1 : 0;
-  } else if (k == "rs_blocks") {
-    SICP_REQUIRE(value >= 0 && value <= 256, SICP_ERR_BAD_ARG, "rs_blocks out of range");
-    c.rs_blocks = (int)value;
   } else if (k == "match_group") {
     SICP_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4 || value == 8 || value == 16, SICP_ERR_BAD_ARG,
                  "match_group must be 0 (auto), 1, 2, 4, 8 or 16");

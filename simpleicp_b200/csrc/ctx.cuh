@@ -64,7 +64,6 @@ struct Ctx {
   int grid_max_rings = 8;
   int host_sync_every = 4;
   int grid_sort_cells = 0;  // 1: sort the records inside each cell by index (layout only)
-  int rs_blocks = 0;     // blocks of the cooperative reject/solve kernel (0 = one per SM)
   int match_group = 0;   // lanes cooperating on one grid query: 0 = by K, else 1, 4, 8 or 16
 
   // clouds
@@ -138,8 +137,6 @@ struct Ctx {
   bool lin_hist_init = false;
   bool rsb_attr_set = false;
   bool rsf_attr_set = false;              // k_rs_fused's dynamic shared memory limit raised on this device
-  DevBuf<unsigned int> rsf_ticket;        // blocks-finished counter of the barrier-free reject/solve kernel
-  int split_solve = 1;                    // option "split_solve": 1 = its serial tail in k_rs_solve, 0 = in its last block
   DevBuf<RsSelect> rs_sel;                // k_rs_fused -> k_rs_solve
   DevBuf<RsScratch> rs_scratch;           // stores of k_rs_solve's rehearsal
   int n_fused_last = 0, n_rerun_last = 0; // last run: iterations through k_rs_fused / repeated after a missed prediction

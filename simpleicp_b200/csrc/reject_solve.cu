@@ -13,13 +13,16 @@
 //      remain.  NumPy semantics: mean of the two middle elements for even n.
 //   B  MAD = median(|d - median|) the same way (raw MAD, no 1.4826: corrpts.py:186).
 //   C  keep = |d - median| <= 3 MAD; accumulate, over the kept correspondences, the 13 x 13
-//      moment matrix M = sum phi phi^T of phi = [n (x) (p', 1), -n.q'] (73 distinct sums).  The
+//      moment matrix M = sum phi phi^T of phi = [n (x) (u, 1), d] (u = matched movable point
+//      minus the movable centre, d = the distance the match evaluated; see lm_eval).  The
 //      residual of EVERY rigid transform is phi . theta(x), so one pass over the data suffices
 //      and the non-linear least squares runs on M alone.
 //   D  block 0 / warp 0: Levenberg-Marquardt on the exact Euler model to convergence, with the
 //      reference's fixed (weight inf) / observed (0 < weight < inf) / free parameter handling.
 //   E  residuals at the solution (direct float64 evaluation, reference operation order), their
 //      mean / population std, parameter sigmas, stop rule, per-iteration record.
+// k_rs_fused / k_rs_solve below do the same without grid barriers when the previous iteration
+// left a predictor; both kernels share the solve steps (the helpers after uncertainties()).
 #include <cooperative_groups.h>
 
 #include <algorithm>
@@ -40,13 +43,18 @@ constexpr int RS_LEVELS = 6;
 constexpr int RS_CAP = 2048;       // candidate buffer (last two slots carry the selected keys)
 constexpr int RS_NACC = 26;           // accumulators per role
 constexpr int RS_NPART = 3 * RS_NACC; // partial sums per block in phase C
+constexpr int RSF_NACC = 30;             // k_rs_fused: accumulators per role (RS_NACC + the 4 of sum phi)
+constexpr int RSF_NPART = 3 * RSF_NACC;  // partial sums per block
+// Grid cap of both multi-block kernels (H100: 132 SMs; k_rs_fused also leaves one SM to
+// k_rs_solve).  The partial reduction keeps 32 x NB loads in flight per value, NB =
+// RSF_MAX_BLOCKS / 32 doubles per lane and value.
+constexpr int RSF_MAX_BLOCKS = 160;
 
 __device__ __constant__ int kShift[RS_LEVELS] = {53, 42, 31, 20, 9, 0};
 __device__ __constant__ int kWidth[RS_LEVELS] = {11, 11, 11, 11, 11, 9};
 
 struct Shared {
   unsigned int hist[LH_BINS];  // radix histogram (first RS_BINS) or prefix sums of the predictor histogram
-  int lh_i[8];
   unsigned long long sortbuf[RS_CAP];
   double red[RS_WARPS][RS_NACC];
   unsigned int scan_tmp[RS_WARPS];
@@ -864,153 +872,239 @@ __device__ void uncertainties(Shared& s, const RSArgs& a, const double* An, doub
   __syncwarp();
 }
 
-// Median and MAD from the predictor histogram the match kernel filled (reject_solve.cuh:
-// lh_bin): LH_BINS linear bins centred on the previous median, +-4 previous MADs wide.
-//   * the bins holding the two middle ranks give the median candidates;
-//   * with med somewhere in those bins, an element delta bins away has |d - med| inside
-//     ((delta-1) w, (delta+g+1) w), so cumulative symmetric counts N_in(t) bracket the MAD ranks:
-//     everything closer than t_lo - g bins is certainly below the MAD (counted, not gathered),
-//     everything farther than t_hi + g + 1 bins certainly above; the bins in between are the
-//     MAD candidates.
-// One gather pass + one grid barrier then yields both order statistics exactly (same values as
-// the radix path).  Returns SEL_OK, or — before touching global state — the SelectOutcome of the
-// first check that failed when the prediction does not bracket the ranks (first iteration, large
-// change, too many candidates): the caller falls back.
-template <bool MULTI>
-__device__ int predicted_median_mad(Shared& s, const RSArgs& a, RSWork wk, const DevState* st,
-                                    unsigned int& n1_out, double& median, double& mad) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const double pm = st->pred_med, pd = st->pred_mad;
-  constexpr int PER = (LH_BINS + RS_THREADS - 1) / RS_THREADS;
-  const int b0 = tid * PER;
-  unsigned int v[PER], sum = 0;
-#pragma unroll
-  for (int j = 0; j < PER; ++j) {
-    const int b = b0 + j;
-    v[j] = (b < LH_BINS) ? wk.lin_hist[b] : 0u;
-    sum += v[j];
-  }
-  unsigned int incl = sum;
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned int t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) s.scan_tmp[warp] = incl;
-  __syncthreads();
-  unsigned int woff = 0, total_in = 0;
-  for (int i = 0; i < RS_WARPS; ++i) {
-    if (i < warp) woff += s.scan_tmp[i];
-    total_in += s.scan_tmp[i];
-  }
-  {
-    unsigned int run = woff + incl - sum;
-#pragma unroll
-    for (int j = 0; j < PER; ++j) {
-      run += v[j];
-      if (b0 + j < LH_BINS) s.hist[b0 + j] = run;  // inclusive prefix sums
-    }
-  }
-  if (tid == 0) {
-    s.lh_i[0] = -1;
-    s.lh_i[1] = -1;
-    s.lh_i[2] = LH_BINS + 1;  // t_hi (min over t)
-    s.lh_i[3] = -1;           // t_lo (max over t)
-  }
-  __syncthreads();
-  const unsigned int* P = s.hist;
-  const unsigned int under = wk.lin_hist[LH_BINS], over = wk.lin_hist[LH_BINS + 1];
-  const unsigned int n1 = under + total_in + over;
-  n1_out = n1;
-  if (n1 == 0) return SEL_OK;
-  const unsigned int k = (n1 - 1) >> 1;
-  const bool even = ((n1 & 1u) == 0u);
-  const unsigned int k2 = k + (even ? 1u : 0u);
-  if (k < under || k2 >= under + total_in) return SEL_MEDIAN_OUTSIDE;
-  const unsigned int r = k - under, r2 = k2 - under;
-  // bins of the two middle ranks: first b with P[b] > r
-#pragma unroll
-  for (int j = 0; j < PER; ++j) {
-    const int b = b0 + j;
-    if (b < LH_BINS) {
-      const unsigned int pb = P[b], pa = (b > 0) ? P[b - 1] : 0u;
-      if (pa <= r && r < pb) s.lh_i[0] = b;
-      if (pa <= r2 && r2 < pb) s.lh_i[1] = b;
-    }
-  }
-  __syncthreads();
-  const int bm = s.lh_i[0], bm2 = s.lh_i[1];
-  if (bm < 0 || bm2 < bm) return SEL_MEDIAN_NO_BIN;
-  const int g = bm2 - bm;
-  if (g > 4) return SEL_MEDIAN_GAP;
-  const unsigned int below_m = (bm > 0) ? P[bm - 1] : 0u;
-  const unsigned int cnt_med = P[bm2] - below_m;
-  if (cnt_med > (unsigned int)(RS_CAP - 2)) return SEL_MEDIAN_CANDIDATES;
-  const unsigned int kA = r - below_m;
-  auto Nin = [&](int t) -> unsigned int {
-    const int hi = min(bm2 + t, LH_BINS - 1), lo = bm - t - 1;
-    return P[hi] - ((lo >= 0) ? P[lo] : 0u);
-  };
-  int tmin = LH_BINS + 1, tmax = -1;
-  for (int t = tid; t <= LH_BINS; t += RS_THREADS) {
-    const unsigned int nin = Nin(t);
-    if (nin >= k2 + 1u) tmin = min(tmin, t);
-    if (nin <= k) tmax = max(tmax, t);
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    tmin = min(tmin, __shfl_xor_sync(0xffffffffu, tmin, o));
-    tmax = max(tmax, __shfl_xor_sync(0xffffffffu, tmax, o));
-  }
-  if (lane == 0) {
-    atomicMin(&s.lh_i[2], tmin);
-    atomicMax(&s.lh_i[3], tmax);
-  }
-  __syncthreads();
-  const int t_hi = s.lh_i[2], t_lo = s.lh_i[3];
-  if (t_hi > LH_BINS) return SEL_MAD_BRACKET;
-  const int e_lo = max(t_lo - g, 0), e_hi = t_hi + g + 1;
-  if (bm - e_hi < 0 || bm2 + e_hi > LH_BINS - 1) return SEL_MAD_WINDOW;  // candidates must be regular bins
-  const unsigned int n_inner = (t_lo - g - 1 >= 0) ? Nin(t_lo - g - 1) : 0u;
-  const unsigned int cnt_edge = Nin(e_hi) - n_inner;
-  if (cnt_edge > (unsigned int)(RS_CAP - 2) || k < n_inner || k2 - n_inner >= cnt_edge) return SEL_MAD_CANDIDATES;
-  const unsigned int kM = k - n_inner;
-  __syncthreads();
+// ---- Solve steps shared by k_reject_solve (phases C-E) and k_rs_fused / k_rs_solve ------------
 
-  // ---- the one gather pass
-  unsigned long long* cand_med = wk.cand;
-  unsigned long long* cand_edge = wk.cand + RS_CAP;
-  for (long long i = blockIdx.x * (long long)RS_THREADS + tid; i < a.K; i += (long long)gridDim.x * RS_THREADS) {
-    if (pl_stat(a.q_nrm[i].w, a.pl_signed) >= a.stat_minpl) {
-      const double d = a.dist[i];
-      const int b = lh_bin(d, pm, pd);
-      if (b < LH_BINS) {
-        const int delta = (b < bm) ? (bm - b) : ((b > bm2) ? (b - bm2) : 0);
-        if (delta == 0) cand_med[atomicAdd(&wk.counters[0], 1u)] = f64_to_key(d);
-        if (delta >= e_lo && delta <= e_hi)
-          cand_edge[atomicAdd(&wk.counters[1], 1u)] = (unsigned long long)__double_as_longlong(d);
-      }
+// Moment update of one kept correspondence (normal nr, distance d, matched movable point p) by one
+// of the three accumulation roles of 128 threads.  Role r sums, for its two products of normal
+// components (na, nb), na (u, 1) (x) (u, 1) and nb (u, 1) (x) (u, 1) (acc[0..19]), d n_r (u, 1)
+// (acc[20..23]) and its share of the scalars: role 0 sum d^2 and the count, role 1 sum d and
+// sum d^2.  SUMPHI (k_rs_fused, 30 accumulators): also sum phi = n_r (u, 1) (acc[26..29], for
+// the mean of the residuals) and role 2's sum d.
+template <bool SUMPHI, int N>
+__device__ __forceinline__ void accumulate_moments(double (&acc)[N], const int role, const float4 nr, const double d,
+                                                   const double p0, const double p1, const double p2,
+                                                   const double* cm) {
+  const double u0 = p0 - cm[0], u1 = p1 - cm[1], u2 = p2 - cm[2];
+  const double n0 = (double)nr.x, n1d = (double)nr.y, n2 = (double)nr.z;
+  const double sc = d;  // re-centred model: the scalar entry of phi is the distance itself
+  double na, nb, nv;
+  if (role == 0) {
+    na = n0 * n0; nb = n0 * n1d; nv = n0;
+  } else if (role == 1) {
+    na = n0 * n2; nb = n1d * n1d; nv = n1d;
+  } else {
+    na = n1d * n2; nb = n2 * n2; nv = n2;
+  }
+  const double U[10] = {u0 * u0, u0 * u1, u0 * u2, u0, u1 * u1, u1 * u2, u1, u2 * u2, u2, 1.0};
+#pragma unroll
+  for (int t = 0; t < 10; ++t) {
+    acc[t] = fma(na, U[t], acc[t]);
+    acc[10 + t] = fma(nb, U[t], acc[10 + t]);
+  }
+  const double sn = sc * nv;
+  acc[20] = fma(sn, u0, acc[20]);
+  acc[21] = fma(sn, u1, acc[21]);
+  acc[22] = fma(sn, u2, acc[22]);
+  acc[23] += sn;
+  if constexpr (SUMPHI) {
+    acc[26] = fma(nv, u0, acc[26]);
+    acc[27] = fma(nv, u1, acc[27]);
+    acc[28] = fma(nv, u2, acc[28]);
+    acc[29] += nv;
+  }
+  if (role == 0) {
+    acc[24] = fma(sc, sc, acc[24]);
+    acc[25] += 1.0;
+  } else if (role == 1) {
+    acc[24] += d;
+    acc[25] = fma(d, d, acc[25]);
+  } else if constexpr (SUMPHI) {
+    acc[24] += sc;
+  }
+}
+
+// The block's partial sums: every accumulator summed over its warp, then over the four warps of
+// its role in warp order.  Thread t < 3 NACC returns value t (role t / NACC, accumulator t % NACC).
+template <int NACC>
+__device__ __forceinline__ double block_partial(const double (&acc)[NACC], double (&red)[RS_WARPS][NACC]) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int j = 0; j < NACC; ++j) {
+    const double v = warp_sum(acc[j]);
+    if (lane == 0) red[warp][j] = v;
+  }
+  __syncthreads();
+  double v = 0.0;
+  if (tid < 3 * NACC) {
+    const int r = tid / NACC, j = tid % NACC;
+    for (int ww = r; ww < RS_WARPS; ww += 3) v += red[ww][j];
+  }
+  return v;
+}
+
+// Fixed-order sum of the per-block partials, stored value-major ([value][block], G <=
+// RSF_MAX_BLOCKS): each warp owns a few values, issues the loads of all their block entries before
+// the first use (one L2 round trip, not one per value) and finishes with a shuffle tree.
+// Deterministic: the order depends on G only.
+template <int NPART>
+__device__ __forceinline__ void reduce_partials(const double* partials, const int G, double* tot) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int NO = (NPART + RS_WARPS - 1) / RS_WARPS;  // values per warp
+  constexpr int NB = RSF_MAX_BLOCKS / 32;
+  double r[NO][NB];
+#pragma unroll
+  for (int q = 0; q < NO; ++q) {
+    const int o = warp + q * RS_WARPS;
+#pragma unroll
+    for (int u = 0; u < NB; ++u) {
+      const int b = lane + 32 * u;
+      r[q][u] = (o < NPART && b < G) ? __ldcg(&partials[(size_t)o * G + b]) : 0.0;
     }
   }
-  gsync<MULTI>(wk.barrier);
-  if (blockIdx.x == 0 && tid == 0) {
-    wk.phase_t[10] = global_timer_ns();
-    wk.phase_t[24] = 0;
-    wk.phase_t[25] = 0;
-    wk.phase_t[26] = cnt_med;
-    wk.phase_t[27] = cnt_edge;
+#pragma unroll
+  for (int q = 0; q < NO; ++q) {
+    const int o = warp + q * RS_WARPS;
+    double v = 0.0;
+#pragma unroll
+    for (int u = 0; u < NB; ++u) v += r[q][u];
+    v = warp_sum(v);
+    if (lane == 0 && o < NPART) tot[o] = v;
   }
-  unsigned long long klo, khi;
-  for (int t = tid; t < (int)cnt_med; t += RS_THREADS) s.sortbuf[t] = cand_med[t];
-  __syncthreads();
-  block_select(s, s.sortbuf, (int)cnt_med, kA, 64, ~0ull, klo, khi);
-  median = even ? (a.variant ? key_to_f64(khi) : 0.5 * (key_to_f64(klo) + key_to_f64(khi))) : key_to_f64(klo);
-  __syncthreads();
-  for (int t = tid; t < (int)cnt_edge; t += RS_THREADS)
-    s.sortbuf[t] = f64_to_key(fabs(__longlong_as_double((long long)cand_edge[t]) - median));
-  __syncthreads();
-  block_select(s, s.sortbuf, (int)cnt_edge, kM, 64, ~0ull, klo, khi);
-  mad = even ? (a.variant ? key_to_f64(khi) : 0.5 * (key_to_f64(klo) + key_to_f64(khi))) : key_to_f64(klo);
-  __syncthreads();
-  return SEL_OK;
+}
+
+// Entry (r, c) of M from the reduced sums: the 6 x 10 normal-product sums, the 3 x 4 d n (x) (u, 1)
+// and sum d^2 (accumulate_moments).
+template <int NACC>
+__device__ __forceinline__ double moment_entry(const double* tot, const int r, const int c) {
+  if (r == 12 && c == 12) return tot[0 * NACC + 24];
+  if (r == 12 || c == 12) {
+    const int o = (r == 12) ? c : r;
+    return tot[(o / 4) * NACC + 20 + (o % 4)];
+  }
+  int aa = r / 4, bb = r % 4, cc = c / 4, dd = c % 4;
+  if (aa > cc) { int t = aa; aa = cc; cc = t; }
+  if (bb > dd) { int t = bb; bb = dd; dd = t; }
+  const int i6 = (aa == 0) ? cc : (aa == 1 ? 2 + cc : 5);          // (0,0)0 (0,1)1 (0,2)2 (1,1)3 (1,2)4 (2,2)5
+  const int i10 = (bb == 0) ? dd : (bb == 1 ? 3 + dd : (bb == 2 ? 5 + dd : 9));  // (1,1)4 (1,2)5 (1,3)6 (2,2)7 (2,3)8 (3,3)9
+  return tot[(i6 / 2) * NACC + (i6 % 2) * 10 + i10];
+}
+
+// Statistics of the kept distances and the distance weight of this iteration.
+struct DistStats {
+  long long n_kept;
+  double mean_d, var_d, var_d1;  // mean, population and sample variance
+  double w;
+  int skip;  // fewer than 6 correspondences or solve not requested
+};
+template <int NACC>
+__device__ __forceinline__ DistStats dist_stats(const double* tot, const RSArgs& a, const double w_state) {
+  DistStats ds;
+  ds.n_kept = (long long)(tot[0 * NACC + 25] + 0.5);
+  const long long n_kept = ds.n_kept;
+  const double sum_d = tot[1 * NACC + 24], sum_d2 = tot[1 * NACC + 25];
+  const double mean_d = (n_kept > 0) ? sum_d / (double)n_kept : nan("");
+  ds.mean_d = mean_d;
+  ds.var_d = (n_kept > 0) ? fmax(sum_d2 / (double)n_kept - mean_d * mean_d, 0.0) : nan("");
+  // the C++ driver prints the SAMPLE std of the kept distances as its "orig:0" row (simpleicp.cpp:95-100)
+  ds.var_d1 = (n_kept > 1) ? fmax(sum_d2 - (double)n_kept * mean_d * mean_d, 0.0) / (double)(n_kept - 1) : nan("");
+  double w = w_state;
+  if (a.variant) {
+    w = 1.0;
+  } else if (a.it == 0 || !(w > 0.0)) {
+    w = a.w_param;
+    if (!(w > 0.0)) w = 1.0 / ds.var_d;  // distance_weights=None: 1/std(d)^2 (simpleicp.py:233-234)
+  }
+  ds.w = w;
+  ds.skip = (n_kept < 6) || !a.do_solve;
+  return ds;
+}
+
+// The solve (warp 0): one linear solve in the linearised variants, else Levenberg-Marquardt from
+// the current parameters.
+__device__ __forceinline__ LmOut solve_iteration(Shared& s, const RSArgs& a, const DistStats& ds,
+                                                 const DevState* st, const double* cm, const double* cf,
+                                                 const int lane) {
+  LmOut lo;
+  lo.iters = 0;
+  lo.ok = 1;
+  if (!ds.skip && a.variant) {
+    lin_solve(s, st->T, cf, lane);
+    lo.iters = 1;
+    lo.ok = s.spd;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) lo.x[j] = s.delta[j];
+  } else if (!ds.skip) {
+    lm_solve(s, a, ds.w, st->x, cm, cf, lo, lane);
+  }
+  return lo;
+}
+
+// Record and loop state of the reject step (one thread); n_bf = queries the brute-force pass served.
+__device__ __forceinline__ void store_reject(const RSArgs& a, DevState* sto, sicp_iter_record* rec,
+                                             const DistStats& ds, const double median, const double mad,
+                                             const int lm_iterations, const int n_bf) {
+  rec->n_kept = ds.n_kept;
+  rec->median = median;
+  rec->mad = mad;
+  sto->pred_med = median;
+  sto->pred_mad = mad;
+  sto->pred_minpl = a.stat_minpl;
+  sto->pred_valid = (mad > 0.0 && isfinite(mad) && isfinite(median)) ? 1 : 0;
+  rec->mean_dist = ds.mean_d;
+  rec->std_dist = sqrt(a.variant ? ds.var_d1 : ds.var_d);
+  rec->distance_weight = ds.w;
+  rec->lm_iterations = lm_iterations;
+  rec->n_bruteforce = n_bf;
+  sto->n_kept = ds.n_kept;
+  sto->skip = ds.skip;
+  sto->w = ds.w;
+  if (ds.n_kept < 6 && a.do_solve && a.arm_stop) sto->stop = 2;  // too few correspondences
+}
+
+// Linearised variants: the map whose point-to-plane residuals are the reference's "A x - l",
+// (I + [alpha]x) T_in + t (c++/src/corrpts.cpp:155).
+__device__ __forceinline__ Rigid linearised_map(const double* x, const Rigid& Tin) {
+  Rigid L;
+  L.r[0] = 1.0; L.r[1] = -x[2]; L.r[2] = x[1];
+  L.r[3] = x[2]; L.r[4] = 1.0; L.r[5] = -x[0];
+  L.r[6] = -x[1]; L.r[7] = x[0]; L.r[8] = 1.0;
+  L.t[0] = x[3]; L.t[1] = x[4]; L.t[2] = x[5];
+  return rigid_compose(L, Tin);
+}
+
+// Stop rule (simpleicp.py:355-379): relative change in percent of the mean and std of the
+// residuals against the previous iteration's.
+__device__ __forceinline__ int stop_rule(const RSArgs& a, const double mean, const double sd, const double m0,
+                                         const double s0) {
+  int stop = 0;
+  if (a.it > 0) {
+    const double cmn = (m0 == 0.0) ? ((mean == 0.0) ? 0.0 : kInf) : fabs((mean - m0) / m0 * 100.0);
+    const double csd = (s0 == 0.0) ? ((sd == 0.0) ? 0.0 : kInf) : fabs((sd - s0) / s0 * 100.0);
+    stop = (cmn < a.min_change && csd < a.min_change) ? 1 : 0;
+  }
+  return stop;
+}
+
+// Residual statistics of the record, the predictor of the next iteration and the stop-rule state
+// (one thread).
+__device__ __forceinline__ void store_iteration_end(const RSArgs& a, DevState* sto, sicp_iter_record* rec,
+                                                    const double mean, const double sd, const int stop) {
+  rec->mean_res = mean;
+  rec->std_res = sd;
+  // Predictor of the NEXT iteration's order statistics: the residuals at the new transform, not
+  // the distances this iteration started from — the first solves of a registration shrink the
+  // distribution several-fold, and the next match finds (mostly) these very correspondences.
+  // median ~ mean, MAD ~ 0.8 std of the kept residuals (truncated at 3 MAD ~ 2 sigma).
+  if (sd > 0.0 && isfinite(sd) && isfinite(mean)) {
+    sto->pred_med = mean;
+    sto->pred_mad = 0.8 * sd;
+    sto->pred_valid = 1;
+  }
+  sto->prev_mean = mean;
+  sto->prev_std = sd;
+  sto->iterations_done = a.it + 1;
+  if (stop && a.arm_stop) sto->stop = 1;
+  sto->converged = stop;
 }
 
 template <bool MULTI>
@@ -1037,31 +1131,23 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
   }
 #define RS_STAMP(i) do { if (blockIdx.x == 0 && tid == 0) wk.phase_t[i] = global_timer_ns(); } while (0)
   RS_STAMP(0);
+  if (blockIdx.x == 0 && tid == 0) {
+    wk.phase_t[28] = 0;
+    wk.phase_t[29] = SEL_PATH_RADIX;
+  }
 
   // ---- A + B: median and MAD of the planarity survivors
   unsigned int n1 = 0;
   double median = 0.0, mad = 0.0;
-  int sel = SEL_NOT_ATTEMPTED;
-  if (a.hist_expected && st->pred_valid && st->pred_minpl == a.stat_minpl && st->pred_mad > 0.0)
-    sel = predicted_median_mad<MULTI>(s, a, wk, st, n1, median, mad);
-  const bool fast = sel == SEL_OK;
-  if (blockIdx.x == 0 && tid == 0) {
-    wk.phase_t[29] = fast ? SEL_PATH_PREDICT : SEL_PATH_RADIX;
-    wk.phase_t[31] = sel;
-    if (!fast) wk.phase_t[26] = wk.phase_t[27] = 0;  // the radix select writes its own counts
-  }
   sicp_iter_record* rec = a.rec;
-  if (!fast) {
+  radix_median<MULTI, 0>(s, a, wk, 0.0, n1);
+  if (n1 != 0) {
+    median = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
     __syncthreads();
-    radix_median<MULTI, 0>(s, a, wk, 0.0, n1);
-    if (n1 != 0) {
-      median = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
-      __syncthreads();
-      RS_STAMP(1);
-      unsigned int n1b = 0;
-      radix_median<MULTI, 1>(s, a, wk, median, n1b);
-      mad = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
-    }
+    RS_STAMP(1);
+    unsigned int n1b = 0;
+    radix_median<MULTI, 1>(s, a, wk, median, n1b);
+    mad = a.variant ? s.bc[1] : 0.5 * (s.bc[0] + s.bc[1]);
   }
   if (n1 == 0) {
     for (int i = blockIdx.x * RS_THREADS + tid; i < LH_BINS + 2; i += G * RS_THREADS) wk.lin_hist[i] = 0;
@@ -1075,10 +1161,8 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
   // python: |d - med| <= 3 mad (corrpts.py:176-188); linearised: not > 3 (1.4826 mad) (corrpts.cpp:61-66)
   const double lim = a.variant ? 3.0 * (1.4826 * mad) : 3.0 * mad;
   __syncthreads();
-  if (fast) RS_STAMP(1);
   RS_STAMP(2);
-  if (blockIdx.x == 0 && tid == 0) wk.phase_t[28] = fast ? 1 : 0;
-  // the predictor histogram has been consumed (or was not usable): leave it zeroed for the next match
+  // the next match fills the predictor histogram afresh: leave it zeroed
   for (int i = blockIdx.x * RS_THREADS + tid; i < LH_BINS + 2; i += G * RS_THREADS) wk.lin_hist[i] = 0;
 
   // ---- C: keep flags + moment accumulation
@@ -1094,76 +1178,28 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
     const long long i0 = blockIdx.x * chunk, i1 = min(i0 + chunk, K);
     const float4* __restrict__ qn = a.q_nrm;
     const double* __restrict__ dd = a.dist;
-    const long long* __restrict__ nn = a.nn_idx;
-    const double* __restrict__ mv = a.mov_xyz;
-    const double* __restrict__ qx = a.q_xyz;
-    auto accumulate = [&](const float4 nr, const double d, const double p0, const double p1,
-                          const double p2, const double f0, const double f1, const double f2) {
-      const double u0 = p0 - cm[0], u1 = p1 - cm[1], u2 = p2 - cm[2];
-      (void)f0;
-      (void)f1;
-      (void)f2;
-      const double n0 = (double)nr.x, n1d = (double)nr.y, n2 = (double)nr.z;
-      const double sc = d;  // re-centred model: the scalar entry of phi is the distance itself
-      double na, nb, nv;
-      if (role == 0) {
-        na = n0 * n0; nb = n0 * n1d; nv = n0;
-      } else if (role == 1) {
-        na = n0 * n2; nb = n1d * n1d; nv = n1d;
-      } else {
-        na = n1d * n2; nb = n2 * n2; nv = n2;
-      }
-      const double U[10] = {u0 * u0, u0 * u1, u0 * u2, u0, u1 * u1, u1 * u2, u1, u2 * u2, u2, 1.0};
-#pragma unroll
-      for (int t = 0; t < 10; ++t) {
-        acc[t] = fma(na, U[t], acc[t]);
-        acc[10 + t] = fma(nb, U[t], acc[10 + t]);
-      }
-      const double sn = sc * nv;
-      acc[20] = fma(sn, u0, acc[20]);
-      acc[21] = fma(sn, u1, acc[21]);
-      acc[22] = fma(sn, u2, acc[22]);
-      acc[23] += sn;
-      if (role == 0) {
-        acc[24] = fma(sc, sc, acc[24]);
-        acc[25] += 1.0;
-      } else if (role == 1) {
-        acc[24] += d;
-        acc[25] = fma(d, d, acc[25]);
-      }
-    };
-    // two elements per trip so that both dependent gather chains (nn_idx -> mov_xyz) overlap
+    const double* __restrict__ mx = a.m_xyz;
+    // two elements per trip, i and i + 128 (the order of a stride-128 loop), all loads in flight together
     for (long long i = i0 + sub; i < i1; i += 256) {
       const long long ib = i + 128;
       const bool hb = ib < i1;
+      const long long jb = hb ? ib : i;
       const float4 nrA = qn[i];
       const float4 nrB = hb ? qn[ib] : make_float4(0.f, 0.f, 0.f, -1.f);
       const double dA = dd[i], dB = hb ? dd[ib] : 0.0;
+      const double pA0 = mx[3 * i + 0], pA1 = mx[3 * i + 1], pA2 = mx[3 * i + 2];
+      const double pB0 = mx[3 * jb + 0], pB1 = mx[3 * jb + 1], pB2 = mx[3 * jb + 2];
       const bool kA = pl_keep(nrA.w, a.min_planarity, a.pl_signed) && (fabs(dA - median) <= lim);
       const bool kB = hb && pl_keep(nrB.w, a.min_planarity, a.pl_signed) && (fabs(dB - median) <= lim);
-      const long long jA = kA ? nn[i] : 0, jB = kB ? nn[ib] : 0;
-      const long long ia = kA ? i : i0, ibb = kB ? ib : i0;
-      const double pA0 = mv[3 * jA + 0], pA1 = mv[3 * jA + 1], pA2 = mv[3 * jA + 2];
-      const double pB0 = mv[3 * jB + 0], pB1 = mv[3 * jB + 1], pB2 = mv[3 * jB + 2];
-      const double fA0 = qx[3 * ia + 0], fA1 = qx[3 * ia + 1], fA2 = qx[3 * ia + 2];
-      const double fB0 = qx[3 * ibb + 0], fB1 = qx[3 * ibb + 1], fB2 = qx[3 * ibb + 2];
-      if (kA) accumulate(nrA, dA, pA0, pA1, pA2, fA0, fA1, fA2);
-      if (kB) accumulate(nrB, dB, pB0, pB1, pB2, fB0, fB1, fB2);
+      if (kA) accumulate_moments<false>(acc, role, nrA, dA, pA0, pA1, pA2, cm);
+      if (kB) accumulate_moments<false>(acc, role, nrB, dB, pB0, pB1, pB2, cm);
       if (role == 0) {
         a.keep[i] = kA ? 1 : 0;
         if (hb) a.keep[ib] = kB ? 1 : 0;
       }
     }
-#pragma unroll
-    for (int j = 0; j < RS_NACC; ++j) {
-      const double v = warp_sum(acc[j]);
-      if (lane == 0) s.red[warp][j] = v;
-    }
-    __syncthreads();
+    const double v = block_partial(acc, s.red);
     if (tid < RS_NPART) {
-      const int r = tid / RS_NACC, j = tid % RS_NACC;
-      double v = 0.0;
-      for (int ww = r; ww < RS_WARPS; ww += 3) v += s.red[ww][j];
       if (MULTI)
         wk.partials[(size_t)tid * G + blockIdx.x] = v;
       else
@@ -1176,121 +1212,33 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 
   // ---- D: block 0 reduces the partials and solves
   if (blockIdx.x == 0) {
-    if (MULTI) {
-      // fixed-order sum of the per-block partials, stored value-major ([value][block]): each warp
-      // owns a few values, reads their G block entries with coalesced, fully overlapped loads and
-      // finishes with a shuffle tree (deterministic: the order depends on G only)
-      // (all loads of a warp are issued before the first use: one L2 round trip, not 35)
-      constexpr int NO = (RS_NPART + RS_WARPS - 1) / RS_WARPS;  // values per warp
-      constexpr int NB = 8;                                      // 32 * 8 = 256 blocks max
-      double r[NO][NB];
-#pragma unroll
-      for (int q = 0; q < NO; ++q) {
-        const int o = warp + q * RS_WARPS;
-#pragma unroll
-        for (int u = 0; u < NB; ++u) {
-          const int b = lane + 32 * u;
-          r[q][u] = (o < RS_NPART && b < G) ? wk.partials[(size_t)o * G + b] : 0.0;
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < NO; ++q) {
-        const int o = warp + q * RS_WARPS;
-        double v = 0.0;
-#pragma unroll
-        for (int u = 0; u < NB; ++u) v += r[q][u];
-        v = warp_sum(v);
-        if (lane == 0 && o < RS_NPART) s.tot[o] = v;
-        if (q == 0) RS_STAMP(20);
-      }
-    }
+    if (MULTI) reduce_partials<RS_NPART>(wk.partials, G, s.tot);
     __syncthreads();
     RS_STAMP(17);
-    // assemble M (13 x 13) from T (6 x 10), V (3 x 4), S
-    for (int e = tid; e < 169; e += RS_THREADS) {
-      const int r = e / 13, c = e % 13;
-      double v;
-      if (r == 12 && c == 12) {
-        v = s.tot[0 * RS_NACC + 24];
-      } else if (r == 12 || c == 12) {
-        const int o = (r == 12) ? c : r;
-        v = s.tot[(o / 4) * RS_NACC + 20 + (o % 4)];
-      } else {
-        int aa = r / 4, bb = r % 4, cc = c / 4, dd = c % 4;
-        if (aa > cc) { int t = aa; aa = cc; cc = t; }
-        if (bb > dd) { int t = bb; bb = dd; dd = t; }
-        const int i6 = (aa == 0) ? cc : (aa == 1 ? 2 + cc : 5);          // (0,0)0 (0,1)1 (0,2)2 (1,1)3 (1,2)4 (2,2)5
-        const int i10 = (bb == 0) ? dd : (bb == 1 ? 3 + dd : (bb == 2 ? 5 + dd : 9));  // (1,1)4 (1,2)5 (1,3)6 (2,2)7 (2,3)8 (3,3)9
-        v = s.tot[(i6 / 2) * RS_NACC + (i6 % 2) * 10 + i10];
-      }
-      s.M[r][c] = v;
-    }
+    for (int e = tid; e < 169; e += RS_THREADS) s.M[e / 13][e % 13] = moment_entry<RS_NACC>(s.tot, e / 13, e % 13);
     if (tid < 13) s.th_in[tid] = (tid == 12) ? 0.0 : theta_entry(Tin, cm, cf, tid);
     __syncthreads();
     RS_STAMP(18);
     if (warp == 0) {
-      const long long n_kept = (long long)(s.tot[0 * RS_NACC + 25] + 0.5);
-      const double sum_d = s.tot[1 * RS_NACC + 24], sum_d2 = s.tot[1 * RS_NACC + 25];
-      const double mean_d = (n_kept > 0) ? sum_d / (double)n_kept : nan("");
-      const double var_d = (n_kept > 0) ? fmax(sum_d2 / (double)n_kept - mean_d * mean_d, 0.0) : nan("");
-      // the C++ driver prints the SAMPLE std of the kept distances as its "orig:0" row (simpleicp.cpp:95-100)
-      const double var_d1 = (n_kept > 1) ? fmax(sum_d2 - (double)n_kept * mean_d * mean_d, 0.0) / (double)(n_kept - 1) : nan("");
-      double w = st->w;
-      if (a.variant) {
-        w = 1.0;
-      } else if (a.it == 0 || !(w > 0.0)) {
-        w = a.w_param;
-        if (!(w > 0.0)) w = 1.0 / var_d;  // distance_weights=None: 1/std(d)^2 (simpleicp.py:233-234)
-      }
-      int skip = (n_kept < 6) || !a.do_solve;
-      LmOut lo;
-      lo.iters = 0;
-      lo.ok = 1;
-      if (!skip && a.variant) {
-        lin_solve(s, st->T, cf, lane);
-        lo.iters = 1;
-        lo.ok = s.spd;
-#pragma unroll
-        for (int j = 0; j < 6; ++j) lo.x[j] = s.delta[j];
-      } else if (!skip) {
-        lm_solve(s, a, w, st->x, cm, cf, lo, lane);
-        if (lane == 0) {
+      const DistStats ds = dist_stats<RS_NACC>(s.tot, a, st->w);
+      const LmOut lo = solve_iteration(s, a, ds, st, cm, cf, lane);
+      if (lane == 0) {
+        if (!ds.skip && !a.variant) {
           wk.phase_t[19] = global_timer_ns();
           wk.phase_t[21] = s.stamp[0];
           wk.phase_t[22] = s.stamp[1];
         }
-      }
-      if (lane == 0) {
-        rec->n_kept = n_kept;
-        rec->median = median;
-        rec->mad = mad;
-        st->pred_med = median;
-        st->pred_mad = mad;
-        st->pred_minpl = a.stat_minpl;
-        st->pred_valid = (mad > 0.0 && isfinite(mad) && isfinite(median)) ? 1 : 0;
-        rec->mean_dist = mean_d;
-        rec->std_dist = sqrt(a.variant ? var_d1 : var_d);
-        rec->distance_weight = w;
-        rec->lm_iterations = lo.iters;
-        rec->n_bruteforce = a.unresolved ? (int)a.unresolved[K] : 0;
+        const int n_bf = a.unresolved ? (int)a.unresolved[K] : 0;
         if (a.unresolved) a.unresolved[K] = 0u;  // the next match starts from a clean counter
-        st->n_kept = n_kept;
-        st->skip = skip;
-        st->w = w;
-        if (n_kept < 6 && a.do_solve && a.arm_stop) st->stop = 2;  // too few correspondences
-        if (!skip) {
+        store_reject(a, st, rec, ds, median, mad, lo.iters, n_bf);
+        if (!ds.skip) {
           for (int j = 0; j < 6; ++j) st->x_new[j] = lo.x[j];
           for (int e = 0; e < 36; ++e) st->An[e] = s.Ak[e];
           if (a.variant) {
             // cloud <- dH cloud (pointcloud.cpp:149-152), residuals of the linear model
             const Rigid dH = rigid_from_x(lo.x);
             st->T_new = rigid_compose(dH, Tin);
-            Rigid L;  // I + [alpha]x, t
-            L.r[0] = 1.0; L.r[1] = -lo.x[2]; L.r[2] = lo.x[1];
-            L.r[3] = lo.x[2]; L.r[4] = 1.0; L.r[5] = -lo.x[0];
-            L.r[6] = -lo.x[1]; L.r[7] = lo.x[0]; L.r[8] = 1.0;
-            L.t[0] = lo.x[3]; L.t[1] = lo.x[4]; L.t[2] = lo.x[5];
-            st->T_res = rigid_compose(L, Tin);
+            st->T_res = linearised_map(lo.x, Tin);
             const Rigid Hr = st->H_rep;
             st->H_rep = (a.variant == SICP_VARIANT_LINEARIZED_CPP) ? rigid_compose(Hr, dH) : rigid_compose(dH, Hr);
           } else {
@@ -1310,12 +1258,12 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
   // ---- E: residuals at the solution, in the reference's operation order
   {
     const Rigid Tn = st->T_res;
+    const double* __restrict__ mx = a.m_xyz;
     double sr = 0.0, sr2 = 0.0;
     for (long long i = blockIdx.x * (long long)RS_THREADS + tid; i < K; i += (long long)G * RS_THREADS) {
       if (!a.keep[i]) continue;
-      const long long j = a.nn_idx[i];
       double tx, ty, tz;
-      rigid_apply(Tn, a.mov_xyz[3 * j + 0], a.mov_xyz[3 * j + 1], a.mov_xyz[3 * j + 2], tx, ty, tz);
+      rigid_apply(Tn, mx[3 * i + 0], mx[3 * i + 1], mx[3 * i + 2], tx, ty, tz);
       const float4 nr = a.q_nrm[i];
       const double dx = tx - a.q_xyz[3 * i + 0], dy = ty - a.q_xyz[3 * i + 1], dz = tz - a.q_xyz[3 * i + 2];
       const double r = __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)),
@@ -1389,33 +1337,10 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
       }
     }
     if (lane == 0) {
-      rec->mean_res = mean;
-      rec->std_res = sd;
-      // Predictor of the NEXT iteration's order statistics: the residuals at the new transform, not
-      // the distances this iteration started from — the first solves of a registration shrink the
-      // distribution several-fold, and the next match finds (mostly) these very correspondences.
-      // median ~ mean, MAD ~ 0.8 std of the kept residuals (truncated at 3 MAD ~ 2 sigma).
-      if (sd > 0.0 && isfinite(sd) && isfinite(mean)) {
-        st->pred_med = mean;
-        st->pred_mad = 0.8 * sd;
-        st->pred_valid = 1;
-      }
       st->T = st->T_new;
       st->Tinv = rigid_inverse(st->T_new);
       if (!a.variant) st->H_rep = st->T_new;
-      // stop rule (simpleicp.py:355-379): relative change in percent of mean and population std
-      int stop = 0;
-      if (a.it > 0) {
-        const double m0 = st->prev_mean, s0 = st->prev_std;
-        const double cmn = (m0 == 0.0) ? ((mean == 0.0) ? 0.0 : kInf) : fabs((mean - m0) / m0 * 100.0);
-        const double csd = (s0 == 0.0) ? ((sd == 0.0) ? 0.0 : kInf) : fabs((sd - s0) / s0 * 100.0);
-        stop = (cmn < a.min_change && csd < a.min_change) ? 1 : 0;
-      }
-      st->prev_mean = mean;
-      st->prev_std = sd;
-      st->iterations_done = a.it + 1;
-      if (stop && a.arm_stop) st->stop = 1;
-      st->converged = stop;
+      store_iteration_end(a, st, rec, mean, sd, stop_rule(a, mean, sd, st->prev_mean, st->prev_std));
       wk.phase_t[9] = global_timer_ns();
     }
   }
@@ -1433,14 +1358,11 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 //              statistics are read directly — redundant, identical work on every SM, no exchange,
 //              no pass over the K correspondences.  (A first version scanned a 2-byte bin code per
 //              correspondence in every block: 38 us of 2 M thread-instructions per SM.)  Same exact
-//              order statistics as predicted_median_mad().
-//   accumulate each block streams its share of (normal, distance, matched point, fixed point) —
-//              the match kernel stored the matched point, so there is no index chase — and
-//              writes keep flags and per-block partial sums.
+//              order statistics as radix_median().
+//   accumulate each block streams its share of (normal, distance, matched point) and writes keep
+//              flags and per-block partial sums.
 //   solve      rs_tail reduces the partials in a fixed order and runs the Gauss-Newton loop: for
-//              more than one block in k_rs_solve, a one-block kernel launched behind this one
-//              (option split_solve 0: in the block that takes the LAST ticket; everybody else
-//              has already left the SM).
+//              more than one block in k_rs_solve, a one-block kernel launched behind this one.
 //   statistics mean and standard deviation of the residuals at the solution come from the moment
 //              sums themselves (sum r = theta . sum phi, sum r^2 = theta^T M theta): no residual pass
 //              and no barrier in the loop.  The residual VECTOR of the final iteration is evaluated
@@ -1450,20 +1372,13 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 // kernel changes nothing, raises state->stop = 3 and the host re-runs that iteration with the
 // general kernel (capi.cu: run_loop).
 // =============================================================================================
-constexpr int RSF_NACC = 30;             // accumulators per role
-constexpr int RSF_NPART = 3 * RSF_NACC;  // partial sums per block
-
 constexpr int RSF_TILE = 768;  // correspondences per TMA-staged tile of the moment pass
-// Grid cap of the fused kernel (H100: 132 SMs; the launch also leaves one SM to k_rs_solve).  The
-// serial tail keeps 32 x NB partial loads in flight per value, NB = RSF_MAX_BLOCKS / 32 doubles per
-// lane and value.
-constexpr int RSF_MAX_BLOCKS = 160;
 constexpr size_t RSF_PARTIALS = (size_t)RSF_NPART * RSF_MAX_BLOCKS;  // one half of ws.partials
 
 // k_rs_fused variants.  SINGLE: one block owns the whole problem (K <= 4096, and k_rs_batch) and
-// runs the serial tail itself.  TICKET: many blocks, the last one to finish runs the tail (option
-// split_solve = 0).  SPLIT: many blocks that only select and accumulate; k_rs_solve runs the tail.
-enum FusedMode : int { RSF_SINGLE = 0, RSF_TICKET = 1, RSF_SPLIT = 2 };
+// runs the serial tail itself.  SPLIT: many blocks that only select and accumulate; k_rs_solve
+// runs the tail.
+enum FusedMode : int { RSF_SINGLE = 0, RSF_SPLIT = 1 };
 
 // what the serial tail uses of the shared memory
 struct SharedTail {
@@ -1482,7 +1397,6 @@ struct SharedF : SharedTail {
   unsigned long long edgebuf[RS_CAP];  // MAD candidates (the median candidates go to s.sortbuf)
   alignas(8) uint64_t t_bar;
   double redf[RS_WARPS][RSF_NACC];
-  int is_last;
 };
 
 // k-th smallest (0-based) and its successor among n <= RS_THREADS keys in shared memory by direct
@@ -1747,48 +1661,6 @@ __device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, co
     double acc[RSF_NACC];
 #pragma unroll
     for (int j = 0; j < RSF_NACC; ++j) acc[j] = 0.0;
-    auto accumulate = [&](const float4 nr, const double d, const double p0, const double p1,
-                          const double p2, const double f0, const double f1, const double f2) {
-      const double u0 = p0 - cm[0], u1 = p1 - cm[1], u2 = p2 - cm[2];
-      (void)f0;
-      (void)f1;
-      (void)f2;
-      const double n0 = (double)nr.x, n1d = (double)nr.y, n2 = (double)nr.z;
-      const double sc = d;  // re-centred model: the scalar entry of phi is the distance itself
-      double na, nb, nv;
-      if (role == 0) {
-        na = n0 * n0; nb = n0 * n1d; nv = n0;
-      } else if (role == 1) {
-        na = n0 * n2; nb = n1d * n1d; nv = n1d;
-      } else {
-        na = n1d * n2; nb = n2 * n2; nv = n2;
-      }
-      const double U[10] = {u0 * u0, u0 * u1, u0 * u2, u0, u1 * u1, u1 * u2, u1, u2 * u2, u2, 1.0};
-#pragma unroll
-      for (int t = 0; t < 10; ++t) {
-        acc[t] = fma(na, U[t], acc[t]);
-        acc[10 + t] = fma(nb, U[t], acc[10 + t]);
-      }
-      const double sn = sc * nv;
-      acc[20] = fma(sn, u0, acc[20]);
-      acc[21] = fma(sn, u1, acc[21]);
-      acc[22] = fma(sn, u2, acc[22]);
-      acc[23] += sn;
-      // sum phi (for the mean of the residuals): n_role (x) (u, 1)
-      acc[26] = fma(nv, u0, acc[26]);
-      acc[27] = fma(nv, u1, acc[27]);
-      acc[28] = fma(nv, u2, acc[28]);
-      acc[29] += nv;
-      if (role == 0) {
-        acc[24] = fma(sc, sc, acc[24]);
-        acc[25] += 1.0;
-      } else if (role == 1) {
-        acc[24] += d;
-        acc[25] = fma(d, d, acc[25]);
-      } else {
-        acc[24] += sc;
-      }
-    };
     // tiles of RSF_TILE correspondences from shared memory (the first one has been in flight since
     // kernel entry; K <= 113 000 has a single tile per block)
     for (long long t0 = i0; t0 < i1; t0 += RSF_TILE) {
@@ -1799,7 +1671,7 @@ __device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, co
         const float4 nr = sf.t_nrm[e];
         const double d = sf.t_dist[e];
         const bool kp = pl_keep(nr.w, a.min_planarity, a.pl_signed) && (fabs(d - median) <= lim);
-        if (kp) accumulate(nr, d, sf.t_xyz[3 * e + 0], sf.t_xyz[3 * e + 1], sf.t_xyz[3 * e + 2], 0.0, 0.0, 0.0);
+        if (kp) accumulate_moments<true>(acc, role, nr, d, sf.t_xyz[3 * e + 0], sf.t_xyz[3 * e + 1], sf.t_xyz[3 * e + 2], cm);
         if (role == 0) a.keep[t0 + e] = kp ? 1 : 0;
       }
       if (t0 + RSF_TILE < i1) {
@@ -1807,18 +1679,8 @@ __device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, co
         if (tid == 0) issue_tile(t0 + RSF_TILE);
       }
     }
-#pragma unroll
-    for (int j = 0; j < RSF_NACC; ++j) {
-      const double vv = warp_sum(acc[j]);
-      if (lane == 0) sf.redf[warp][j] = vv;
-    }
-    __syncthreads();
-    if (tid < RSF_NPART) {
-      const int r = tid / RSF_NACC, j = tid % RSF_NACC;
-      double vv = 0.0;
-      for (int ww = r; ww < RS_WARPS; ww += 3) vv += sf.redf[ww][j];
-      wk.partials[(size_t)tid * G + bid] = vv;
-    }
+    const double vv = block_partial(acc, sf.redf);
+    if (tid < RSF_NPART) wk.partials[(size_t)tid * G + bid] = vv;
   } else if (have_tile) {
     mbar_wait(&sf.t_bar, tile_phase);  // never leave with a bulk copy into this block's shared memory in flight
   }
@@ -1829,30 +1691,10 @@ __device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, co
     if (bid == 0 && tid == 0) *wk.sel = RsSelect{median, mad, n1, ok ? 1 : 0};
     return;
   }
+  // one block (K <= 4096, k_rs_batch): inlined, the arguments stay where the kernel has them
   __threadfence();
   __syncthreads();
-  if constexpr (MODE == RSF_TICKET) {
-    // ---- ticket: the last block to arrive owns the serial part
-    if (tid == 0) {
-      const unsigned int t = atomicAdd(wk.ticket, 1u);
-      sf.is_last = (t == (unsigned int)G - 1u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (!sf.is_last) return;
-    __threadfence();
-    if (tid == 0) *wk.ticket = 0u;
-#ifdef SICP_RS_REHEARSE_PROBE
-    // diagnostics build (tools/build_variants.py): the last block runs the tail twice, first as
-    // the rehearsal (stamps 1 and 5), to time a warm pass (stamps 4 to 9) against a cold one
-    if (tid == 0) wk.phase_t[1] = global_timer_ns();
-    rs_tail(sf, a, wk, wk.partials, G, ok, n1, median, mad, false);
-    __syncthreads();
-    if (tid == 0) wk.phase_t[5] = global_timer_ns();
-#endif
-  }
-  // one block (K <= 4096, k_rs_batch): inlined, the arguments stay where the kernel has them
-  if constexpr (MODE == RSF_SINGLE) rs_tail_body(sf, a, wk, wk.partials, G, ok, n1, median, mad, true);
-  else rs_tail(sf, a, wk, wk.partials, G, ok, n1, median, mad, true);
+  rs_tail_body(sf, a, wk, wk.partials, G, ok, n1, median, mad, true);
 }
 
 // Not inlined, so that k_rs_solve's rehearsal and its real pass run the same code.
@@ -1906,30 +1748,7 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
     }
     return;
   }
-  {
-    // fixed-order sum of the per-block partials ([value][block] layout, all loads in flight)
-    constexpr int NO = (RSF_NPART + RS_WARPS - 1) / RS_WARPS;
-    constexpr int NB = RSF_MAX_BLOCKS / 32;
-    double r[NO][NB];
-#pragma unroll
-    for (int q = 0; q < NO; ++q) {
-      const int o = warp + q * RS_WARPS;
-#pragma unroll
-      for (int u = 0; u < NB; ++u) {
-        const int b = lane + 32 * u;
-        r[q][u] = (o < RSF_NPART && b < G) ? __ldcg(&partials[(size_t)o * G + b]) : 0.0;
-      }
-    }
-#pragma unroll
-    for (int q = 0; q < NO; ++q) {
-      const int o = warp + q * RS_WARPS;
-      double vv = 0.0;
-#pragma unroll
-      for (int u = 0; u < NB; ++u) vv += r[q][u];
-      vv = warp_sum(vv);
-      if (lane == 0 && o < RSF_NPART) sf.totf[o] = vv;
-    }
-  }
+  reduce_partials<RSF_NPART>(partials, G, sf.totf);
   __syncthreads();
   if (tid == 0) pt[17] = global_timer_ns();
   for (int e = tid; e < 169 + 13; e += RS_THREADS) {
@@ -1938,22 +1757,7 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
       sf.m1[o] = (o == 12) ? sf.totf[2 * RSF_NACC + 24] : sf.totf[(o / 4) * RSF_NACC + 26 + (o % 4)];
       continue;
     }
-    const int r = e / 13, c = e % 13;
-    double vv;
-    if (r == 12 && c == 12) {
-      vv = sf.totf[0 * RSF_NACC + 24];
-    } else if (r == 12 || c == 12) {
-      const int o = (r == 12) ? c : r;
-      vv = sf.totf[(o / 4) * RSF_NACC + 20 + (o % 4)];
-    } else {
-      int aa = r / 4, bb = r % 4, cc = c / 4, dd2 = c % 4;
-      if (aa > cc) { int t = aa; aa = cc; cc = t; }
-      if (bb > dd2) { int t = bb; bb = dd2; dd2 = t; }
-      const int i6 = (aa == 0) ? cc : (aa == 1 ? 2 + cc : 5);
-      const int i10 = (bb == 0) ? dd2 : (bb == 1 ? 3 + dd2 : (bb == 2 ? 5 + dd2 : 9));
-      vv = sf.totf[(i6 / 2) * RSF_NACC + (i6 % 2) * 10 + i10];
-    }
-    s.M[r][c] = vv;
+    s.M[e / 13][e % 13] = moment_entry<RSF_NACC>(sf.totf, e / 13, e % 13);
   }
   __syncthreads();
   if (tid == 0) pt[18] = global_timer_ns();
@@ -1961,64 +1765,21 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
   if (lane < 13) s.th_in[lane] = (lane == 12) ? 0.0 : theta_entry(Tin, cm, cf, lane);
   __syncwarp();
 
-  const long long n_kept = (long long)(sf.totf[0 * RSF_NACC + 25] + 0.5);
-  const double sum_d = sf.totf[1 * RSF_NACC + 24], sum_d2 = sf.totf[1 * RSF_NACC + 25];
-  const double mean_d = (n_kept > 0) ? sum_d / (double)n_kept : nan("");
-  const double var_d = (n_kept > 0) ? fmax(sum_d2 / (double)n_kept - mean_d * mean_d, 0.0) : nan("");
-  const double var_d1 = (n_kept > 1) ? fmax(sum_d2 - (double)n_kept * mean_d * mean_d, 0.0) / (double)(n_kept - 1) : nan("");
-  double w = w_state;
-  if (a.variant) {
-    w = 1.0;
-  } else if (a.it == 0 || !(w > 0.0)) {
-    w = a.w_param;
-    if (!(w > 0.0)) w = 1.0 / var_d;
-  }
-  const int skip = (n_kept < 6) || !a.do_solve;
-  LmOut lo;
-  lo.iters = 0;
-  lo.ok = 1;
-  if (!skip && a.variant) {
-    lin_solve(s, st->T, cf, lane);
-    lo.iters = 1;
-    lo.ok = s.spd;
-#pragma unroll
-    for (int j = 0; j < 6; ++j) lo.x[j] = s.delta[j];
-  } else if (!skip) {
-    lm_solve(s, a, w, st->x, cm, cf, lo, lane);
-  }
+  const DistStats ds = dist_stats<RSF_NACC>(sf.totf, a, w_state);
+  const LmOut lo = solve_iteration(s, a, ds, st, cm, cf, lane);
   if (lane == 0) {
     pt[19] = global_timer_ns();
     pt[21] = s.stamp[0];
     pt[22] = s.stamp[1];
-    rec->n_kept = n_kept;
-    rec->median = median;
-    rec->mad = mad;
-    sto->pred_med = median;
-    sto->pred_mad = mad;
-    sto->pred_minpl = a.stat_minpl;
-    sto->pred_valid = (mad > 0.0 && isfinite(mad) && isfinite(median)) ? 1 : 0;
-    rec->mean_dist = mean_d;
-    rec->std_dist = sqrt(a.variant ? var_d1 : var_d);
-    rec->distance_weight = w;
-    rec->lm_iterations = lo.iters;
-    rec->n_bruteforce = (int)n_bf;
-    sto->n_kept = n_kept;
-    sto->skip = skip;
-    sto->w = w;
-    if (n_kept < 6 && a.do_solve && a.arm_stop) sto->stop = 2;
+    store_reject(a, sto, rec, ds, median, mad, lo.iters, (int)n_bf);
   }
-  if (skip) return;
+  if (ds.skip) return;
   // new transform(s)
   Rigid T_new, T_res;
   const Rigid dH = rigid_from_x_warp(lo.x, lane);  // default variant: x is the transform itself
   if (a.variant) {
     T_new = rigid_compose(dH, Tin);
-    Rigid L;
-    L.r[0] = 1.0; L.r[1] = -lo.x[2]; L.r[2] = lo.x[1];
-    L.r[3] = lo.x[2]; L.r[4] = 1.0; L.r[5] = -lo.x[0];
-    L.r[6] = -lo.x[1]; L.r[7] = lo.x[0]; L.r[8] = 1.0;
-    L.t[0] = lo.x[3]; L.t[1] = lo.x[4]; L.t[2] = lo.x[5];
-    T_res = rigid_compose(L, Tin);
+    T_res = linearised_map(lo.x, Tin);
   } else {
     T_new = dH;
     T_res = T_new;
@@ -2034,17 +1795,11 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
   }
   const double sum_r2 = fmax(warp_sum(rowdot), 0.0);
   const double sum_r = warp_sum(s1);
-  const double n = (double)n_kept;
+  const double n = (double)ds.n_kept;
   const double mean = sum_r / n;
   const double sd = a.variant ? sqrt(fmax(sum_r2 - n * mean * mean, 0.0) / (n - 1.0))
                               : sqrt(fmax(sum_r2 / n - mean * mean, 0.0));
-  int stop = 0;
-  if (a.it > 0) {
-    const double m0 = prev_mean, s0 = prev_std;
-    const double cmn = (m0 == 0.0) ? ((mean == 0.0) ? 0.0 : kInf) : fabs((mean - m0) / m0 * 100.0);
-    const double csd = (s0 == 0.0) ? ((sd == 0.0) ? 0.0 : kInf) : fabs((sd - s0) / s0 * 100.0);
-    stop = (cmn < a.min_change && csd < a.min_change) ? 1 : 0;
-  }
+  const int stop = stop_rule(a, mean, sd, prev_mean, prev_std);
   if (a.variant) {
     if (lane < 6) {
       sto->sigma[lane] = nan("");
@@ -2055,7 +1810,7 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
       if (lane < 36) sto->An[lane] = s.Ak[lane];
       if (lane + 32 < 36) sto->An[lane + 32] = s.Ak[lane + 32];
       __syncwarp();
-      uncertainties(s, a, s.Ak, w, lo.x, sum_r2, n_kept, lane, sto->sigma);
+      uncertainties(s, a, s.Ak, ds.w, lo.x, sum_r2, ds.n_kept, lane, sto->sigma);
     }
     if (lane < 6) {
       const double xl = pick(lo.x, lane);
@@ -2077,19 +1832,7 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
     sto->T_res = T_res;
     sto->T = T_new;
     sto->Tinv = rigid_inverse(T_new);
-    rec->mean_res = mean;
-    rec->std_res = sd;
-    // predictor of the next iteration from the residuals at the new transform (see k_reject_solve)
-    if (sd > 0.0 && isfinite(sd) && isfinite(mean)) {
-      sto->pred_med = mean;
-      sto->pred_mad = 0.8 * sd;
-      sto->pred_valid = 1;
-    }
-    sto->prev_mean = mean;
-    sto->prev_std = sd;
-    sto->iterations_done = a.it + 1;
-    if (stop && a.arm_stop) sto->stop = 1;
-    sto->converged = stop;
+    store_iteration_end(a, sto, rec, mean, sd, stop);
     pt[9] = global_timer_ns();
   }
 }
@@ -2367,11 +2110,9 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
                          int rec_slot) {
   const long long K = c.K;
   const bool multi = K > 4096;
-  int G = 1;
-  if (multi) {
-    const int cap = (c.rs_blocks > 0) ? std::min(c.rs_blocks, c.num_sms) : std::min(c.num_sms, 256);
-    G = (int)std::min<long long>(cap, (K + RS_THREADS - 1) / RS_THREADS);
-  }
+  // one block per SM at most (every block must be resident for the grid barrier)
+  const int G = multi ? (int)std::min<long long>(std::min(c.num_sms, RSF_MAX_BLOCKS), (K + RS_THREADS - 1) / RS_THREADS)
+                      : 1;
   // workspace: two parities
   const size_t hist_n = 2ull * RS_LEVELS * RS_BINS;
   if (c.ws.hist.cap < 2 * hist_n) {
@@ -2396,8 +2137,7 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
   a.q_nrm = c.mov_attr ? c.q_nrm_eff.p : c.q_nrm.p;
   a.pl_signed = c.mov_attr ? 1 : 0;
   a.q_xyz = c.q_xyz.p;
-  a.nn_idx = c.nn_idx.p;
-  a.mov_xyz = c.mov_xyz.p;
+  a.m_xyz = c.m_xyz.p;
   a.keep = c.keep.p;
   a.resid = c.resid.p;
   a.unresolved = (c.nn_engine == SICP_NN_AUTO) ? c.unresolved.p : nullptr;
@@ -2421,7 +2161,6 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
     SICP_CUDA(cudaMemsetAsync(c.lin_hist.p, 0, (LH_BINS + 2) * sizeof(unsigned int), c.stream));
     c.lin_hist_init = true;
   }
-  a.hist_expected = c.lin_hist_pending ? 1 : 0;
   c.lin_hist_pending = false;  // the kernel leaves the histogram zeroed
 
   RSWork wk;
@@ -2459,15 +2198,12 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   const long long K = c.K;
   // K <= 4096: a single block (it never needs the host's re-run protocol, see rs_fused_body).
   // Otherwise at most one block per SM but one: k_rs_solve's block takes the SM left free while
-  // the select blocks run (both forms use the same grid, so their sums are the same bit for bit).
+  // the select blocks run.
   const int G = (K <= 4096) ? 1
                             : (int)std::min<long long>(std::min(c.num_sms - 1, RSF_MAX_BLOCKS),
                                                        std::max<long long>(1, (K + 767) / 768));
-  const bool split = G > 1 && c.split_solve;
   if (!c.rsf_attr_set) {
     SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)sizeof(SharedF)));
-    SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_TICKET>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)sizeof(SharedF)));
     SICP_CUDA(cudaFuncSetAttribute(k_rs_fused<RSF_SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)sizeof(SharedF)));
@@ -2484,10 +2220,6 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   c.keep.reserve(K);
   c.resid.reserve(K);
   c.phase_t.reserve(32);
-  if (c.rsf_ticket.p == nullptr) {
-    c.rsf_ticket.reserve(4);
-    SICP_CUDA(cudaMemsetAsync(c.rsf_ticket.p, 0, 4 * sizeof(unsigned int), c.stream));
-  }
   c.rs_sel.reserve(1);
   c.rs_scratch.reserve(1);
   RSArgs a;
@@ -2496,8 +2228,6 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   a.q_nrm = c.mov_attr ? c.q_nrm_eff.p : c.q_nrm.p;
   a.pl_signed = c.mov_attr ? 1 : 0;
   a.q_xyz = c.q_xyz.p;
-  a.nn_idx = c.nn_idx.p;
-  a.mov_xyz = c.mov_xyz.p;
   a.keep = c.keep.p;
   a.resid = c.resid.p;
   a.unresolved = (c.nn_engine == SICP_NN_AUTO) ? c.unresolved.p : nullptr;
@@ -2527,14 +2257,11 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   wk.partials_prev = c.ws.partials.p + (size_t)((it & 1) ^ 1) * RSF_PARTIALS;
   wk.phase_t = c.phase_t.p;
   wk.lin_hist = c.lin_hist.p;
-  wk.ticket = c.rsf_ticket.p;
   wk.sel = c.rs_sel.p;
   wk.scratch = c.rs_scratch.p;
   const bool pdl = c.pdl != 0;
   if (G == 1) {
     launch_kernel(k_rs_fused<RSF_SINGLE>, dim3(1), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
-  } else if (!split) {
-    launch_kernel(k_rs_fused<RSF_TICKET>, dim3(G), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
   } else {
     launch_kernel(k_rs_fused<RSF_SPLIT>, dim3(G), dim3(RS_THREADS), sizeof(SharedF), c.stream, pdl, a, wk);
     SICP_CUDA(cudaGetLastError());

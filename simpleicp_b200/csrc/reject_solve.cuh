@@ -30,7 +30,6 @@ struct DevState {
   // previous median, +-4 previous MADs wide (see lh_bin below).
   double pred_med, pred_mad, pred_minpl;
   int pred_valid;   // pred_* describe a finished reject phase of this run
-  int hist_filled;  // the last match filled the linear histogram with the current pred_*
   // Linearised variant (SICP_VARIANT_LINEARIZED*): T_res is the affine map (I + [alpha]x) T + t
   // whose point-to-plane residuals are the reference's "A x - l" (c++/src/corrpts.cpp:155);
   // H_rep is the matrix the reference driver reports (dH * H, or H * dH for the C++ driver).
@@ -57,18 +56,14 @@ __host__ __device__ inline int lh_bin(double d, double med, double mad) {
 // Slot 29: which selection produced the record's median and MAD.
 enum SelectPath : int {
   SEL_PATH_RADIX = 0,    // radix_median: iteration 0, the stage API, every fallback
-  SEL_PATH_PREDICT = 1,  // predicted_median_mad: gather pass of the cooperative kernel
   SEL_PATH_BINSTORE = 2, // fused_select: per-bin key store of k_rs_fused / k_rs_batch
 };
-// Slot 30 (last k_rs_fused / k_rs_batch launch) and slot 31 (last k_reject_solve launch): outcome
-// of the attempt to select from the predictor histogram.  0 = used, else the first check that
-// failed.  _capi.py mirrors these values.
+// Slot 30 (last k_rs_fused / k_rs_batch launch): outcome of the attempt to select from the
+// predictor histogram.  0 = used, else the first check that failed.  _capi.py mirrors these values.
 enum SelectOutcome : int {
   SEL_OK = 0,
-  SEL_NO_PREDICTION = 1,      // k_rs_fused: no histogram, no valid predictor, or one for another planarity bound
-  SEL_NOT_ATTEMPTED = 2,      // k_reject_solve: the same conditions; the radix select ran directly
+  SEL_NO_PREDICTION = 1,      // no histogram, no valid predictor, or one for another planarity bound
   SEL_MEDIAN_OUTSIDE = 3,     // a middle rank lies in the under- or overflow counter
-  SEL_MEDIAN_NO_BIN = 4,      // predicted_median_mad: no bin holds a middle rank (guard; the prefix sums rule it out)
   SEL_MEDIAN_GAP = 5,         // the bins of the two middle ranks are more than 4 bins apart
   SEL_MEDIAN_CANDIDATES = 6,  // the median bins hold more than RS_CAP - 2 members
   SEL_MAD_BRACKET = 7,        // the regular bins hold fewer than k2 + 1 members: no MAD bracket
@@ -82,8 +77,7 @@ struct RSArgs {
   const double* dist;
   const float4* q_nrm;
   const double* q_xyz;
-  const long long* nn_idx;
-  const double* mov_xyz;
+  const double* m_xyz;  // matched movable point (caller coordinates), K x 3
   uint8_t* keep;
   double* resid;
   unsigned int* unresolved;  // [K] = queries the grid left to the brute-force pass; reset by the kernel after reading
@@ -98,13 +92,12 @@ struct RSArgs {
   int it;
   int do_solve;
   int arm_stop;
-  int hist_expected;  // the preceding match launch fed lin_hist (if the predictor was valid)
+  int hist_expected;  // the preceding match launch fed lin_hist (if the predictor was valid; fused kernel)
   int variant;        // sicp_variant
   double stat_minpl;  // planarity bound of the set the median/MAD are taken over (-inf: everybody)
   // fused kernel only (k_rs_fused): what the match kernels left per correspondence
   const unsigned long long* binstore;  // LH_BINS x bin_cap: f64_to_key(distance) of the members of each predictor-histogram bin
   int bin_cap;
-  const double* m_xyz;         // matched movable point (caller coordinates), K x 3
   int want_sigma;              // evaluate the parameter sigmas even if the stop rule does not fire
   // q_nrm is the match kernel's per-iteration copy whose .w is the signed effective planarity
   // (nn.cu: effective_planarity): |w| enters both planarity tests, a set sign bit = rejected by
@@ -145,7 +138,6 @@ struct RSWork {
   unsigned long long* phase_t;  // 32 x %globaltimer stamps of block 0 (diagnostics)
   unsigned int* barrier;        // {arrival count, generation} of the grid barrier
   unsigned int* lin_hist;       // LH_BINS + 2 counters filled by the match kernels
-  unsigned int* ticket;         // fused kernel (split_solve 0): blocks finished so far (the last one solves)
   // fused kernel, split form: the other half of the double-buffered partials (the previous
   // iteration's), the select outcome and the rehearsal's store target
   const double* partials_prev;

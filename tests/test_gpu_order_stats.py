@@ -1,18 +1,16 @@
 """Exact median / MAD of every device selection path on adversarial distance distributions.
 
 Each iteration keeps the correspondences with |d - median| <= 3 MAD, where median and MAD are
-taken over the planarity survivors.  Four device implementations compute these two order
+taken over the planarity survivors.  Three device implementations compute these two order
 statistics, and which one runs depends on K, the iteration, the option "fused" and how good
 the predictor was (reject_solve.cu):
 
-  radix select                  radix_median: iteration 0, the stage API, every fallback
-  cooperative predictor gather  predicted_median_mad (k_reject_solve, iterations >= 1)
+  radix select                  radix_median (k_reject_solve): iteration 0, the stage API, every fallback
   per-bin key store             fused_select (k_rs_fused, k_rs_batch)
   in-kernel radix fallback      rs_fused_body, G == 1 (K <= 4096 or a batched pair)
 
-Slot 29 of Engine.phase_times() names the path that produced the last record; slots 30 and 31
-hold the outcome of the last predictor attempt of the barrier-free and of the cooperative
-kernel.  Engine.seed_predictor sets the predictor directly, so that any distance distribution
+Slot 29 of Engine.phase_times() names the path that produced the last record; slot 30 holds
+the outcome of the last predictor attempt of the barrier-free kernel.  Engine.seed_predictor sets the predictor directly, so that any distance distribution
 can be paired with any prediction.
 
 The harness makes every device distance reproducible on the host bit for bit: a fixed lattice
@@ -273,24 +271,16 @@ def test_radix_lockstep_stage_api(gpu, name, K):
 U_GRID = (-6.0, -3.0, -0.5, 0.0, 0.5, 3.0, 6.0)
 V_GRID = (-9, -6, -3, 0, 2, 4, 6)
 SWEEP_K = (1000, 20000, 120000)
-# codes each predictor implementation can return (reject_solve.cuh: SelectOutcome)
+# codes the predictor select can return (reject_solve.cuh: SelectOutcome)
 FUSED_CODES = {"SEL_OK", "SEL_NO_PREDICTION", "SEL_MEDIAN_OUTSIDE", "SEL_MEDIAN_GAP", "SEL_MEDIAN_CANDIDATES",
                "SEL_MAD_BRACKET", "SEL_MAD_WINDOW", "SEL_MAD_CANDIDATES", "SEL_BIN_CAP"}
-COOP_CODES = {"SEL_OK", "SEL_NOT_ATTEMPTED", "SEL_MEDIAN_OUTSIDE", "SEL_MEDIAN_GAP", "SEL_MEDIAN_CANDIDATES",
-              "SEL_MAD_BRACKET", "SEL_MAD_WINDOW", "SEL_MAD_CANDIDATES"}
-# SEL_MEDIAN_NO_BIN (predicted_median_mad only) cannot be returned: its check runs only after
-# SEL_MEDIAN_OUTSIDE's has passed, i.e. with r <= r2 < total_in = P[LH_BINS - 1].  The inclusive
-# prefix sums P rise from P[-1] = 0 <= r to P[LH_BINS - 1] > r2, so exactly one bin b has
-# P[b - 1] <= r < P[b] (and one for r2, with bm2 >= bm): the guard is defensive only.
-COOP_EXCLUDED = {"SEL_MEDIAN_NO_BIN": "the prefix sums always hold both middle ranks once they are inside "
-                                      "the regular bins (see the argument above)"}
 
 
 @functools.lru_cache(maxsize=None)
 def seeded_sweep(name, K, z0):
     """Run the whole seeded grid for one case; return what was observed."""
     case = cached_case(name, K, z0)
-    obs = {"fused": set(), "coop": set(), "paths": set(), "cnt_med_store": [], "cells": 0}
+    obs = {"fused": set(), "paths": set(), "cnt_med_store": [], "cells": 0}
     x0 = np.zeros(6)
     with new_engine(case) as e:
         assert_match_reproduced(e, case, 1.5e-3)
@@ -301,14 +291,14 @@ def seeded_sweep(name, K, z0):
             for u in U_GRID:
                 for v in V_GRID:
                     r0 = e.iterate(p, x_in=x0, want_record=True)
-                    note(obs, e.selection(), fused and K <= 4096, K)
+                    note(obs, e.selection(), fused and K <= 4096)
                     tz1 = r0.x[5]
                     d1, keep1, m, s = reference(case, tz1)
                     scale = s if s > 0 else A * 2.0 ** -10  # MAD = 0: seeds of a positive width
                     e.seed_predictor(m + u * scale, scale * 2.0 ** v, MIN_PL)
                     r1 = e.iterate(p, want_record=True)
                     sel = e.selection()
-                    note(obs, sel, fused, K)
+                    note(obs, sel, fused)
                     what = f"{name} K={K} z0={z0} fused={fused} u={u} v={v} sel={sel}"
                     assert_record(r1, case, tz1, what)
                     if fused and sel["path"] == _capi.SEL_PATH_BINSTORE:
@@ -323,15 +313,12 @@ def seeded_sweep(name, K, z0):
     return obs
 
 
-def note(obs, sel, fused, K):
-    """Record the fresh diagnostics of the last iterate(): slot 30 after a barrier-free launch,
-    slot 31 after a cooperative one (fused=0, or the host's re-run of a missed prediction).
-    fused: the iteration ran in the barrier-free kernel."""
+def note(obs, sel, fused):
+    """Record the fresh diagnostics of the last iterate(): the path, and slot 30 after a
+    barrier-free launch.  fused: the iteration ran in the barrier-free kernel."""
     obs["paths"].add(sel["path"])
     if fused:
         obs["fused"].add(sel["fused"])
-    if not fused or (K > 4096 and sel["path"] != _capi.SEL_PATH_BINSTORE):
-        obs["coop"].add(sel["coop"])
 
 
 @pytest.mark.gpu
@@ -347,26 +334,24 @@ def test_seeded_predictor_sweep(gpu, name, K):
 
 @pytest.mark.gpu
 def test_seeded_sweep_reaches_every_outcome(gpu):
-    """The sweep reaches every reason code and the success of both predictor implementations,
-    every selection path, and both selections inside fused_select (rank_select for <= 384
-    median candidates, block_select above)."""
-    fused, coop, paths, cnt = set(), set(), set(), []
+    """The sweep reaches every reason code and the success of the predictor select, every
+    selection path, and both selections inside fused_select (rank_select for <= 384 median
+    candidates, block_select above)."""
+    fused, paths, cnt = set(), set(), []
     for name in SHAPES:
         for K in SWEEP_K:
             for z0 in Z0:
                 obs = seeded_sweep(name, K, z0)
                 fused |= obs["fused"]
-                coop |= obs["coop"]
                 paths |= obs["paths"]
                 cnt += obs["cnt_med_store"]
     inv = {v: k for k, v in _capi.SEL_OUTCOMES.items()}
-    seen_f, seen_c = {inv[c] for c in fused}, {inv[c] for c in coop}
-    print(f"barrier-free outcomes {sorted(seen_f)}\ncooperative outcomes {sorted(seen_c)}\n"
+    seen_f = {inv[c] for c in fused}
+    print(f"barrier-free outcomes {sorted(seen_f)}\n"
           f"paths {sorted(paths)}, key-store cnt_med range {min(cnt)}..{max(cnt)}")
     assert seen_f == FUSED_CODES
-    assert seen_c == COOP_CODES
-    assert set(_capi.SEL_OUTCOMES) == FUSED_CODES | COOP_CODES | set(COOP_EXCLUDED)
-    assert paths == {_capi.SEL_PATH_RADIX, _capi.SEL_PATH_PREDICT, _capi.SEL_PATH_BINSTORE}
+    assert set(_capi.SEL_OUTCOMES) == FUSED_CODES
+    assert paths == {_capi.SEL_PATH_RADIX, _capi.SEL_PATH_BINSTORE}
     assert min(cnt) <= 384 < max(cnt)
 
 
@@ -389,8 +374,6 @@ def test_seeded_minpl_mismatch_falls_back(gpu, K):
             assert sel["path"] == _capi.SEL_PATH_RADIX
             if fused:
                 assert sel["fused"] == _capi.SEL_NO_PREDICTION
-            if not fused or K > 4096:
-                assert sel["coop"] == _capi.SEL_NOT_ATTEMPTED
             # the same seed with the right bound passes the guard (whether the plan then brackets
             # the ranks depends on the sample: at K = 1000 the two middle elements of an even n1
             # are often more than 4 bins of MAD / 512 apart)
@@ -401,8 +384,6 @@ def test_seeded_minpl_mismatch_falls_back(gpu, K):
             assert_record(r1, case, r0.x[5], f"K={K} fused={fused} matching bound")
             if fused:
                 assert sel["fused"] != _capi.SEL_NO_PREDICTION
-            if not fused or (K > 4096 and sel["path"] != _capi.SEL_PATH_BINSTORE):
-                assert sel["coop"] != _capi.SEL_NOT_ATTEMPTED
 
 
 # --------------------------------------------------------------------------- d. whole runs

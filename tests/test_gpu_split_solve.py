@@ -1,9 +1,9 @@
 """The serial tail of the barrier-free reject/solve kernel (reduction of the per-block partials, the
-Gauss-Newton solve, statistics, state and record stores) runs either in the kernel's last block
-(option split_solve 0) or in the one-block kernel k_rs_solve launched behind it (split_solve 1, the
-default), which first rehearses the tail on the previous iteration's partials.  Both reduce the
-same partials in the same order, so whole registrations must agree bit for bit, and nothing the
-rehearsal does may show in a result."""
+Gauss-Newton solve, statistics, state and record stores) runs in the one-block kernel k_rs_solve
+launched behind the select/accumulate grid.  With programmatic dependent launch (option pdl 1, the
+default) k_rs_solve first rehearses the tail on the previous iteration's partials while the grid
+runs; without it (pdl 0) it runs the tail once.  Nothing the rehearsal does may show in a result:
+whole registrations must agree bit for bit."""
 import numpy as np
 import pytest
 
@@ -29,8 +29,7 @@ def assert_same(a, b, what):
         assert x.shape == y.shape and np.array_equal(x, y), f"{what}: output {i} differs"
 
 
-def run(e, X_fix, X_mov, K, split, pdl=1):
-    e.set_option("split_solve", split)
+def run(e, X_fix, X_mov, K, pdl):
     e.set_option("pdl", pdl)
     n0 = e.timings()["kernel_launches"]
     res = sb.register(X_fix, X_mov, correspondences=K, engine=e, want_normals=False)
@@ -48,21 +47,40 @@ def pairs():
     return {"c3": (X_fix, X_mov, 100_000), "airborne": (A_fix, A_mov, 200_000)}
 
 
+def launches_per_iteration(e, p, fused):
+    """Kernel launches of one steady-state iterate() call, and the selection path it took."""
+    e.set_option("fused", fused)
+    for _ in range(3):
+        n0 = e.timings()["kernel_launches"]
+        rec = e.iterate(p, want_record=True)
+        n = e.timings()["kernel_launches"] - n0
+    assert rec.n_bruteforce == 0
+    return n, e.selection()["path"]
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["c3", "airborne"])
-def test_split_solve_matches_last_block_tail(gpu, pairs, name):
+def test_rehearsal_matches_plain_tail(gpu, pairs, name):
     X_fix, X_mov, K = pairs[name]
     with _capi.Engine() as e:
-        ref, launches_ticket, fused_ticket = run(e, X_fix, X_mov, K, split=0)
-    with _capi.Engine() as e:
-        new, launches_split, fused_split = run(e, X_fix, X_mov, K, split=1)
         # without PDL the solve kernel skips its rehearsal
-        nopdl, _, _ = run(e, X_fix, X_mov, K, split=1, pdl=0)
-    assert_same(ref, new, f"{name} split_solve 0 vs 1")
-    assert_same(ref, nopdl, f"{name} split_solve 1 without PDL")
-    # k_rs_solve ran: one more launch behind every launch of the select kernel
-    assert fused_split == fused_ticket
-    assert launches_split > launches_ticket
+        ref, launches_ref, fused_ref = run(e, X_fix, X_mov, K, pdl=0)
+    with _capi.Engine() as e:
+        new, launches_new, fused_new = run(e, X_fix, X_mov, K, pdl=1)
+    assert_same(ref, new, f"{name} pdl 0 vs 1")
+    assert (launches_new, fused_new) == (launches_ref, fused_ref)
+    # k_rs_solve ran: a barrier-free iteration launches one kernel more than a cooperative one
+    with _capi.Engine() as e:
+        e.set_clouds(X_fix, X_mov)
+        e.set_selected(sb.pointcloud.subsample_indices(X_fix.shape[0], K).astype(np.int64))
+        e.estimate_normals(10)
+        lsq = e.lsq_params(np.zeros(6), np.zeros(6), np.zeros(6), 1.0)
+        p = e.run_params(0.3, 1.0, 100, lsq)
+        e.iterate(p, x_in=np.zeros(6), want_record=True)
+        n_fused, path_fused = launches_per_iteration(e, p, 1)
+        n_coop, path_coop = launches_per_iteration(e, p, 0)
+    assert (path_fused, path_coop) == (_capi.SEL_PATH_BINSTORE, _capi.SEL_PATH_RADIX)
+    assert n_fused == n_coop + 1
 
 
 @pytest.mark.gpu
@@ -72,10 +90,10 @@ def test_rehearsal_leaves_no_trace(gpu, pairs):
     X_fix, X_mov, K = pairs["c3"]
     A_fix, A_mov, KA = pairs["airborne"]
     with _capi.Engine() as e:
-        ref, _, _ = run(e, X_fix, X_mov, K, split=0)
+        ref, _, _ = run(e, X_fix, X_mov, K, pdl=0)
     with _capi.Engine() as e:
-        run(e, A_fix, A_mov, KA, split=1)
-        again, _, _ = run(e, X_fix, X_mov, K, split=1)
-        twice, _, _ = run(e, X_fix, X_mov, K, split=1)
+        run(e, A_fix, A_mov, KA, pdl=1)
+        again, _, _ = run(e, X_fix, X_mov, K, pdl=1)
+        twice, _, _ = run(e, X_fix, X_mov, K, pdl=1)
     assert_same(ref, again, "c3 after airborne")
     assert_same(ref, twice, "c3 repeated")

@@ -43,14 +43,8 @@ def probe(n, K, rings=(4, 8, 12, 16)):
             seq = " ".join(f"{LABELS[i]}={t[i]:.1f}" for i in range(1, 10))
             sel = (f"med[lv={t[24]:.0f} cand={t[26]:.0f}: levels={t[10]:.1f} gather={t[11]:.1f} sort={t[12]:.1f}] "
                    f"mad[lv={t[25]:.0f} cand={t[27]:.0f}: levels={t[14]:.1f} gather={t[15]:.1f} sort={t[16]:.1f}]")
-            print("  phases(us): " + seq + f" | D: red1={t[20]:.1f} reduce={t[17]:.1f} assemble={t[18]:.1f} eval0={t[21]:.1f} chol0={t[22]:.1f} lm={t[19]:.1f} lm_it={rec_lm} fastsel={t[28]:.0f} cand={t[26]:.0f}/{t[27]:.0f}")
+            print("  phases(us): " + seq + f" | D: reduce={t[17]:.1f} assemble={t[18]:.1f} eval0={t[21]:.1f} chol0={t[22]:.1f} lm={t[19]:.1f} lm_it={rec_lm} fastsel={t[28]:.0f} cand={t[26]:.0f}/{t[27]:.0f}")
             print("  " + sel)
-        for gb in (132, 66, 33, 16):
-            e.set_option("rs_blocks", gb)
-            sw = e.time_stages(p, 20, False)
-            t = e.phase_times()
-            print(f"  rs_blocks={gb:3d}: reject_solve warm {sw['reject_solve']*1e3:6.1f} us | med {t[1]:.1f} mad {t[2]:.1f} accum {t[3]:.1f} solve {t[5]:.1f} exit {t[9]:.1f}")
-        e.set_option("rs_blocks", 0)
         for mg in (1, 4, 8, 16):
             e.set_option("match_group", mg)
             sw = e.time_stages(p, 10, False)

@@ -16,8 +16,7 @@ from bench import make_pair
 
 def stages(e, p, reps=20):
     out = {}
-    for fused, warm, split in ((0, 0, 1), (1, 1, 0), (1, 2, 0), (1, 2, 1)):
-        e.set_option("split_solve", split)
+    for fused, warm in ((0, 0), (1, 1), (1, 2)):
         e.set_option("fused", fused)
         e.set_option("warm_start", 1 if warm else 0)
         e.set_option("sphere_scan", 1 if warm == 2 else 0)
@@ -26,19 +25,18 @@ def stages(e, p, reps=20):
             e.iterate(p, want_record=True)
         sc = e.time_stages(p, reps, True)
         sw = e.time_stages(p, reps, False)
-        out[(fused, warm, split)] = (sc, sw, e.phase_times())
+        out[(fused, warm)] = (sc, sw, e.phase_times())
     return out
 
 
 def show(tag, res):
     for fused, (sc, sw, t) in res.items():
-        print(f"{tag} fused/warm/split={fused}: cold match {sc['match_grid']*1e3:6.1f} rs {sc['reject_solve']*1e3:6.1f} it {sc['iteration']*1e3:6.1f} us | "
+        print(f"{tag} fused/warm={fused}: cold match {sc['match_grid']*1e3:6.1f} rs {sc['reject_solve']*1e3:6.1f} it {sc['iteration']*1e3:6.1f} us | "
               f"warm match {sw['match_grid']*1e3:6.1f} rs {sw['reject_solve']*1e3:6.1f} it {sw['iteration']*1e3:6.1f} us | path {t[28]:.0f}")
         if t[28] == 2:
-            print(f"    fused phases (us since stamp 0): kernel entry {t[23]:.1f} plan {t[10]:.1f} scan {t[11]:.1f} median {t[12]:.1f} select {t[2]:.1f} accumulate {t[3]:.1f} last-block start {t[4]:.1f} "
+            print(f"    fused phases (us since stamp 0): kernel entry {t[23]:.1f} plan {t[10]:.1f} scan {t[11]:.1f} median {t[12]:.1f} select {t[2]:.1f} accumulate {t[3]:.1f} tail start {t[4]:.1f} "
                   f"partials {t[17]:.1f} assemble {t[18]:.1f} eval0 {t[21]:.1f} chol0 {t[22]:.1f} solve {t[19]:.1f} exit {t[9]:.1f} cand {t[26]:.0f}/{t[27]:.0f}")
-            # k_rs_solve (split_solve 1): entry, end of the rehearsal, wait released; a probe build
-            # (-DSICP_RS_REHEARSE_PROBE) stamps its rehearsal in the last block into slots 1 and 5
+            # k_rs_solve: entry, end of the rehearsal, wait released
             print(f"    solve kernel (us since stamp 0): entry {t[1]:.1f} rehearsal end {t[5]:.1f} wait released {t[6]:.1f} "
                   f"| rehearsal {t[5]-t[1]:.1f} us, real tail {t[9]-t[4]:.1f} us")
 
