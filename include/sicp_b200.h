@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SICP_ABI_VERSION 4
+#define SICP_ABI_VERSION 5
 
 typedef enum {
   SICP_OK = 0,
@@ -299,6 +299,28 @@ int32_t sicp_register_batch(sicp_ctx* ctx, int32_t n_pairs, const double* const*
                             sicp_pair_result* out /*[h] n_pairs*/,
                             int64_t* n_selected /*[h] n_pairs or NULL*/);
 
+/* ---- many scans against ONE resident fixed cloud (a map) ----------------------------------------
+ * sicp_set_map uploads a fixed cloud and builds its grid once (the cell plan sicp_register_batch
+ * would make for it).  It stays on the context until it is replaced, released (map_xyz NULL or
+ * n_map 0) or the context is destroyed; no other call (sicp_set_clouds, sicp_register,
+ * sicp_register_batch) touches it.  n_map must be below 2^32.
+ * sicp_register_to_map is SimpleICP.run (simpleicp.py:75-324) for n_scans (map, scan i) pairs,
+ * with the parameters, limits, `observed` rows, per-scan status and n_selected of
+ * sicp_register_batch: the result of scan i equals that of sicp_register_batch with the map as
+ * the fixed cloud of every pair, bit for bit.  The map is neither uploaded nor gridded again.
+ * With max_overlap_distance the overlap filter only searches the map points inside the box of
+ * each scan's movable grid mapped by its prior and grown by max_overlap_distance (plus a rounding
+ * margin): the filter's work grows with the scans' footprints, not with the map.  Survivor
+ * offsets are 32-bit: n_scans x n_map must be below 2^32 (SICP_ERR_BAD_ARG otherwise), and the
+ * filter keeps an n_scans x n_map bit mask on the device.  n_map >= neighbors is required.
+ * SICP_ERR_STATE when no map is set.                                                            */
+int32_t sicp_set_map(sicp_ctx* ctx, const double* map_xyz /*[h|d] n_map x 3*/, int64_t n_map);
+int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const* mov_xyz /*[h|d]*/,
+                             const int64_t* n_mov, const sicp_register_params* p,
+                             const double* observed /*[h] n_scans x 6, radians, or NULL*/,
+                             sicp_pair_result* out /*[h] n_scans*/,
+                             int64_t* n_selected /*[h] n_scans or NULL*/);
+
 /* ---- PointCloud.transform_by_H (pointcloud.py:205-217), final application simpleicp.py:316 -- */
 int32_t sicp_transform(sicp_ctx* ctx, const double H[16], double* mov_xyz_out /*[h|d] n_mov x 3*/);
 
@@ -313,6 +335,9 @@ typedef struct {
                                order-statistic prediction of the barrier-free kernel missed       */
   double mov_normals_ms;    /* last sicp_register / sicp_register_batch with mov_neighbors > 0:
                                k-NN + PCA of the movable cloud(s); 0 otherwise                    */
+  int64_t overlap_candidates; /* last sicp_register_to_map: bounded searches its culled overlap
+                               filter ran (map points inside the scans' grown boxes); 0 without
+                               max_overlap_distance                                               */
 } sicp_timings;
 int32_t sicp_get_timings(sicp_ctx* ctx, sicp_timings* t /*[h]*/);
 

@@ -17,7 +17,7 @@ LIB_PATH = PKG / "libsicp_b200.so"
 
 SICP_OK, SICP_ERR_BAD_ARG, SICP_ERR_NO_OVERLAP, SICP_ERR_TOO_FEW_CORR = 0, 1, 2, 3
 SICP_ERR_CUDA, SICP_ERR_SINGULAR, SICP_ERR_STATE = 4, 5, 6
-ABI_VERSION = 4  # include/sicp_b200.h: SICP_ABI_VERSION
+ABI_VERSION = 5  # include/sicp_b200.h: SICP_ABI_VERSION
 NN_AUTO, NN_GRID, NN_BRUTE = 0, 1, 2
 SIGN_DGEEV, SIGN_CANONICAL = 0, 1
 
@@ -41,7 +41,7 @@ SYMBOLS = (
     "sicp_set_normals", "sicp_set_mov_normals", "sicp_get_knn", "sicp_match", "sicp_reject", "sicp_solve",
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
-    "sicp_register_batch", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -81,7 +81,8 @@ class Timings(C.Structure):
                                           "transform_ms")] + [("kernel_launches", C.c_int64),
                                                             ("fused_iterations", C.c_int64),
                                                             ("rerun_iterations", C.c_int64),
-                                                            ("mov_normals_ms", C.c_double)]
+                                                            ("mov_normals_ms", C.c_double),
+                                                            ("overlap_candidates", C.c_int64)]
 
 
 class PairResult(C.Structure):
@@ -162,6 +163,9 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
                           C.POINTER(IterRecord), vp, C.POINTER(i64)],
         "sicp_register_batch": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(vp), C.POINTER(i64),
                                 C.POINTER(RegisterParams), vp, C.POINTER(PairResult), vp],
+        "sicp_set_map": [vp, vp, i64],
+        "sicp_register_to_map": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(RegisterParams), vp,
+                                 C.POINTER(PairResult), vp],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -294,7 +298,7 @@ class Engine:
             msg = self._lib.sicp_last_error(None).decode()
             self._h = C.c_void_p()
             raise SicpError(rc, msg)
-        self.n_fix = self.n_mov = self.K = 0
+        self.n_fix = self.n_mov = self.K = self.n_map = 0
 
     # -- plumbing
     def _check(self, rc: int):
@@ -501,17 +505,9 @@ class Engine:
         mp = (C.c_void_p * n)(*[_ptr(b) for _, b in keep])
         nf = (C.c_int64 * n)(*[int(a.shape[0]) for a, _ in keep])
         nm = (C.c_int64 * n)(*[int(b.shape[0]) for _, b in keep])
-        if observed is not None:
-            observed = np.ascontiguousarray(observed, dtype=np.float64)
-            if observed.shape != (n, 6):
-                raise ValueError(f"observed must have shape ({n}, 6), got {observed.shape}")
-        rp = RegisterParams()
-        rp.correspondences = int(correspondences)
-        rp.neighbors = int(neighbors)
-        rp.max_overlap_distance = float(max_overlap_distance)
-        rp.run = params
-        rp.mov_neighbors = int(mov_neighbors)
-        rp.max_angle_rad = float(max_angle_rad)
+        observed = self._observed_rows(observed, n)
+        rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
+                                   max_angle_rad)
         out = (PairResult * n)()
         n_selected = np.zeros(n, dtype=np.int64)
         self._check(self._lib.sicp_register_batch(self._h, n, fp, nf, mp, nm, C.byref(rp),
@@ -519,6 +515,60 @@ class Engine:
                                                   _ptr(n_selected)))
         out.n_selected = n_selected
         return out
+
+    def set_map(self, X_map):
+        """sicp_set_map: upload a fixed cloud and build its grid once; it stays on this engine
+        (``None`` releases it) and is the fixed cloud of every register_to_map call."""
+        if X_map is None:
+            self._check(self._lib.sicp_set_map(self._h, None, 0))
+            self.n_map = 0
+            return
+        X = _as_f64_xyz(X_map)
+        self._check(self._lib.sicp_set_map(self._h, _ptr(X), int(X.shape[0])))
+        self.n_map = int(X.shape[0])
+
+    def register_to_map(self, scans, correspondences, neighbors, params: RunParams,
+                        max_overlap_distance: float = -1.0, observed=None, mov_neighbors: int = 0,
+                        max_angle_rad: float = -1.0):
+        """sicp_register_to_map: register_batch with the resident map (set_map) as the fixed cloud
+        of every scan, which is neither uploaded nor gridded again, and with an overlap filter
+        that only searches the map points near each scan.  Same arguments and result as
+        register_batch, with the movable clouds `scans` in place of the pairs."""
+        n = len(scans)
+        keep = [_as_f64_xyz(X) for X in scans]  # keeps converted copies alive
+        mp = (C.c_void_p * n)(*[_ptr(X) for X in keep])
+        nm = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
+        observed = self._observed_rows(observed, n)
+        rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
+                                   max_angle_rad)
+        out = (PairResult * n)()
+        n_selected = np.zeros(n, dtype=np.int64)
+        self._check(self._lib.sicp_register_to_map(self._h, n, mp, nm, C.byref(rp),
+                                                   None if observed is None else _ptr(observed), out,
+                                                   _ptr(n_selected)))
+        out.n_selected = n_selected
+        return out
+
+    @staticmethod
+    def _observed_rows(observed, n: int):
+        if observed is None:
+            return None
+        observed = np.ascontiguousarray(observed, dtype=np.float64)
+        if observed.shape != (n, 6):
+            raise ValueError(f"observed must have shape ({n}, 6), got {observed.shape}")
+        return observed
+
+    @staticmethod
+    def _register_params(correspondences, neighbors, params: RunParams, max_overlap_distance, mov_neighbors,
+                         max_angle_rad) -> RegisterParams:
+        rp = RegisterParams()
+        rp.correspondences = int(correspondences)
+        rp.neighbors = int(neighbors)
+        rp.max_overlap_distance = float(max_overlap_distance)
+        rp.run = params
+        rp.mov_neighbors = int(mov_neighbors)
+        rp.max_angle_rad = float(max_angle_rad)
+        return rp
 
     def get_transform(self) -> np.ndarray:
         """The 4 x 4 transform the last run/solve applied to the movable cloud."""

@@ -273,7 +273,10 @@ def _per_pair_observed(kw, n_pairs: int):
 _BATCH_ENGINES: dict = {}
 
 
-def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
+def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None):
+    """The rank's share `mine` through the batched engine, `batch_size` pairs per call, records into
+    `local`.  With `map_engine` (an engine holding a map, sicp_set_map) get(i) is scan i alone and
+    every chunk is registered against that map (sicp_register_to_map)."""
     import torch
 
     from . import _capi
@@ -291,9 +294,10 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
     k_mov = kw.get("mov_neighbors")
     ang = kw.get("max_angle_between_normals")
     with torch.cuda.device(device):
-        eng = _BATCH_ENGINES.get(int(device))
+        eng = map_engine if map_engine is not None else _BATCH_ENGINES.get(int(device))
         if eng is None or not eng.alive:
             eng = _BATCH_ENGINES[int(device)] = _capi.Engine(int(device))
+        register = eng.register_to_map if map_engine is not None else eng.register_batch
         lsq = eng.lsq_params(obs, obs, [float(w) for w in obs_w], dw)
         params = eng.run_params(kw.get("min_planarity", 0.3), kw.get("min_change", 1.0),
                                 kw.get("max_iterations", 100), lsq)
@@ -301,16 +305,82 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None):
             ids = range(lo, min(lo + max(1, int(batch_size)), len(mine)))
             pairs = [get(mine[j]) for j in ids]
             observed = None if rows is None else np.array([_observed_in_radians(rows[mine[j]]) for j in ids])
-            res = eng.register_batch(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params,
-                                     mod if np.isfinite(mod) else -1.0, observed,
-                                     0 if k_mov is None else int(k_mov),
-                                     -1.0 if ang is None else float(np.deg2rad(ang)))
+            res = register(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params,
+                           mod if np.isfinite(mod) else -1.0, observed,
+                           0 if k_mov is None else int(k_mov),
+                           -1.0 if ang is None else float(np.deg2rad(ang)))
             for j, r in zip(ids, res):
                 if r.status == 0:
                     local[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)
                 else:
                     messages.append(f"pair {mine[j]}: library status {r.status}")
                     local[j] = pack_record(np.full((4, 4), np.nan), -int(r.status), 0, np.nan, np.nan)
+
+
+# run() arguments Map.register serves: those of the batched engine, without the debug output
+_MAP_KEYS = _BATCH_KEYS - {"want_normals"}
+
+
+class Map:
+    """A fixed cloud (a map) held on one GPU, against which many scans are registered.
+
+    ``Map(X_map, device=0)`` uploads the map and builds its search grid once.  Each call of
+    ``register(scans, ...)`` then registers every scan against it with the batched engine
+    (sicp_register_to_map), ``batch_size`` scans per library call: the map is neither uploaded
+    nor gridded again, and with ``max_overlap_distance`` the overlap filter only searches the map
+    points near each scan (under its prior), so the work per scan grows with its footprint, not
+    with the map.  Scan i's result is that of
+    ``register(X_map, scans[i], rbp_observed_values=row_i, max_overlap_distance=d, ...)``.
+    """
+
+    def __init__(self, X_map, device: int = 0):
+        import torch
+
+        from . import _capi
+
+        self.device = int(device)
+        with torch.cuda.device(self.device):
+            self._engine = _capi.Engine(self.device)
+            self._engine.set_map(X_map)
+        self.n_points = self._engine.n_map
+
+    def register(self, scans: Sequence[np.ndarray], *, batch_size: int = 64, on_error: str = "raise",
+                 **run_kwargs) -> np.ndarray:
+        """Register every scan against the map; returns the (n_scans, 20) record table of
+        simpleicp_batch.  ``run_kwargs`` are SimpleICP.run's arguments the batched engine serves
+        (at most 4096 correspondences); ``rbp_observed_values`` is the common 6-tuple or one row
+        per scan (degrees), each scan's prior.  A scan that cannot be registered (no overlap with
+        the map, too few correspondences) gets a NaN record whose ``iterations`` field is minus
+        the library's status code; ``on_error="raise"`` then raises BatchError with the full
+        table, ``on_error="nan"`` returns it."""
+        unknown = set(run_kwargs) - _MAP_KEYS
+        if unknown:
+            raise TypeError(f"Map.register() got unsupported arguments {sorted(unknown)}")
+        if int(run_kwargs.get("correspondences", 1000)) > 4096:
+            raise ValueError("Map.register runs one block per scan: correspondences must be <= 4096")
+        n = len(scans)
+        rows = _per_pair_observed(run_kwargs, n)
+        _check_mov_kwargs(run_kwargs)
+        local = np.zeros((n, RECORD_LEN))
+        messages: List[str] = []
+        # the survivor offsets of one call are 32-bit: scans per call x map points < 2^32
+        per_call = max(1, min(int(batch_size), ((1 << 32) - 1) // max(self.n_points, 1)))
+        _run_batched(lambda i: scans[i], list(range(n)), local, self.device, per_call, run_kwargs, messages, rows,
+                     map_engine=self._engine)
+        failed = np.flatnonzero(local[:, 16] < 0)
+        if failed.size and on_error == "raise":
+            raise BatchError(local, failed, messages)
+        return local
+
+    def close(self) -> None:
+        """Release the map and its engine."""
+        self._engine.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class BatchError(RuntimeError):

@@ -22,7 +22,12 @@
 //                 pair with its own device-resident state and stop flag
 //   finish        exact residual statistics + result record per pair, one small download
 // No host work per pair except the two copies.
+//
+// sicp_register_to_map runs the same stages (run_pairs) for scans against a map held on the
+// context (sicp_set_map, MapStore): the fixed side is the map's grid, and the overlap filter only
+// searches the map points inside each scan's box mapped by its prior (map_cull_box, map_filter).
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -68,17 +73,26 @@ void pinned_reserve(T*& p, size_t& cap, size_t n) {
   cap = n;
 }
 
-}  // namespace
+// What the stages shared by sicp_register_batch and sicp_register_to_map know about one call.
+struct PairsRun {
+  int n_pairs = 0;
+  const sicp_register_params* rp = nullptr;
+  const double* observed = nullptr;
+  bool overlap = false;
+  long long Kmax = 0, max_n_mov = 0;
+  std::vector<long long> mo;    // movable point offsets, n_pairs + 1
+  std::vector<DevState> hs;     // per-pair start state (the prior)
+  std::vector<PairDev> pd;      // descriptors; the caller fills gfix, n_fix and fix_off
+  std::vector<char> no_overlap;
+};
 
-static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, const int64_t* n_fix,
-                           const double* const* mov_xyz, const int64_t* n_mov,
-                           const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
-                           int64_t* n_selected) {
+// Argument checks of both entry points that need no cloud (the clouds are checked per pair by
+// the callers, before any device work).
+void check_pairs_params(const Ctx& c, int n_pairs, bool pointers_given, const sicp_register_params* rp) {
   SICP_REQUIRE(n_pairs >= 1 && n_pairs <= 65535, SICP_ERR_BAD_ARG, "n_pairs must be in [1, 65535]");
-  SICP_REQUIRE(fix_xyz && n_fix && mov_xyz && n_mov && rp && out, SICP_ERR_BAD_ARG, "NULL argument");
+  SICP_REQUIRE(pointers_given && rp, SICP_ERR_BAD_ARG, "NULL argument");
   SICP_REQUIRE(rp->correspondences >= 1 && rp->correspondences <= 4096, SICP_ERR_BAD_ARG,
                "the batched engine runs one block per pair: correspondences must be in [1, 4096]");
-  const bool overlap = rp->max_overlap_distance > 0 && std::isfinite(rp->max_overlap_distance);
   const sicp_run_params& p = rp->run;
   SICP_REQUIRE(p.max_iterations >= 1 && p.max_iterations <= 4096, SICP_ERR_BAD_ARG,
                "max_iterations must be in [1, 4096]");
@@ -92,44 +106,45 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   }
   SICP_REQUIRE(any_finite, SICP_ERR_BAD_ARG, "At least one element in rbp_observation_weights must be finite.");
   check_mov_neighbors(c, *rp);
-  if (!c.batch) c.batch = new Batch();
-  Batch& b = *c.batch;
-  b.n_pairs = n_pairs;
-  std::vector<long long> fo((size_t)n_pairs + 1, 0), mo((size_t)n_pairs + 1, 0);
-  long long Kmax = 0, max_n_fix = 0, max_n_mov = 0;
-  for (int i = 0; i < n_pairs; ++i) {
-    SICP_REQUIRE(fix_xyz[i] && mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
-    SICP_REQUIRE(n_fix[i] >= rp->neighbors && n_mov[i] >= 1, SICP_ERR_BAD_ARG,
-                 "every fixed cloud needs at least `neighbors` points, every movable cloud one");
-    SICP_REQUIRE(n_mov[i] >= rp->mov_neighbors, SICP_ERR_BAD_ARG,
-                 "mov_neighbors exceeds the number of points in the movable cloud of pair " + std::to_string(i));
-    max_n_mov = std::max<long long>(max_n_mov, n_mov[i]);
-    fo[(size_t)i + 1] = fo[(size_t)i] + n_fix[i];
-    mo[(size_t)i + 1] = mo[(size_t)i] + n_mov[i];
-    Kmax = std::max<long long>(Kmax, std::min<long long>(rp->correspondences, n_fix[i]));
-    max_n_fix = std::max<long long>(max_n_fix, n_fix[i]);
-  }
-  Kmax = (Kmax + 1) & ~1ll;  // even: every pair's slice of the per-query arrays starts 16-byte aligned
-  b.total_fix = fo[(size_t)n_pairs];
-  b.total_mov = mo[(size_t)n_pairs];
-  b.Kmax = Kmax;
-  cudaStream_t st = c.stream;
+}
 
-  // ---- uploads: fixed clouds on the context's stream, movable ones behind them on the copy stream
-  b.fix_xyz.reserve(3 * (size_t)b.total_fix);
+void begin_pairs(PairsRun& r, int n_pairs, const sicp_register_params* rp, const double* observed) {
+  r.n_pairs = n_pairs;
+  r.rp = rp;
+  r.observed = observed;
+  r.overlap = rp->max_overlap_distance > 0 && std::isfinite(rp->max_overlap_distance);
+  r.mo.assign((size_t)n_pairs + 1, 0);
+}
+
+// pair i's movable cloud (checked and counted) and its share of the per-query arrays
+void add_movable(PairsRun& r, int i, int64_t n_mov) {
+  SICP_REQUIRE(n_mov >= r.rp->mov_neighbors, SICP_ERR_BAD_ARG,
+               "mov_neighbors exceeds the number of points in the movable cloud of pair " + std::to_string(i));
+  r.max_n_mov = std::max<long long>(r.max_n_mov, n_mov);
+  r.mo[(size_t)i + 1] = r.mo[(size_t)i] + n_mov;
+}
+
+// The movable clouds cross PCIe on the copy stream (behind the event the caller recorded on the
+// context's stream after the last use of the buffers); ev_copy marks their arrival.
+void upload_movable(Ctx& c, Batch& b, const PairsRun& r, const double* const* mov_xyz, const int64_t* n_mov) {
   b.mov_xyz.reserve(3 * (size_t)b.total_mov);
-  SICP_CUDA(cudaEventRecord(c.ev_user, st));
-  SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
-  for (int i = 0; i < n_pairs; ++i)
-    SICP_CUDA(cudaMemcpyAsync(b.fix_xyz.p + 3 * fo[(size_t)i], fix_xyz[i], sizeof(double) * 3 * (size_t)n_fix[i],
-                              cudaMemcpyDefault, st));
-  for (int i = 0; i < n_pairs; ++i)
-    SICP_CUDA(cudaMemcpyAsync(b.mov_xyz.p + 3 * mo[(size_t)i], mov_xyz[i], sizeof(double) * 3 * (size_t)n_mov[i],
+  for (int i = 0; i < r.n_pairs; ++i)
+    SICP_CUDA(cudaMemcpyAsync(b.mov_xyz.p + 3 * r.mo[(size_t)i], mov_xyz[i], sizeof(double) * 3 * (size_t)n_mov[i],
                               cudaMemcpyDefault, c.copy_stream));
   SICP_CUDA(cudaEventRecord(c.ev_copy, c.copy_stream));
+}
 
-  // ---- per-pair buffers
+// Per-pair buffers and start states: every pair starts from its prior, observed row i (x0 =
+// observed, as SimpleICP.run does) or the common x0; the overlap filter runs under that transform
+// (H0, simpleicp.py:158-170).
+void alloc_pair_buffers(Ctx& c, Batch& b, PairsRun& r) {
+  cudaStream_t st = c.stream;
+  const int n_pairs = r.n_pairs;
+  const sicp_run_params& p = r.rp->run;
+  const long long Kmax = r.Kmax;
   const size_t nq = (size_t)n_pairs * (size_t)Kmax;
+  b.n_pairs = n_pairs;
+  b.Kmax = Kmax;
   b.pairs.reserve(n_pairs);
   b.sel_idx.reserve(nq);
   b.nn_idx.reserve(nq);
@@ -154,122 +169,230 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   SICP_CUDA(cudaMemsetAsync(b.rec.p, 0, sizeof(sicp_iter_record) * (size_t)n_pairs * (size_t)p.max_iterations, st));
   SICP_CUDA(cudaMemsetAsync(b.nn_pos.p, 0xff, sizeof(uint32_t) * nq, st));
   SICP_CUDA(cudaMemsetAsync(b.keep.p, 0, nq, st));
-  // every pair starts from its prior: observed row i (x0 = observed, as SimpleICP.run does) or the
-  // common x0; the overlap filter runs under that transform (H0, simpleicp.py:158-170)
-  std::vector<DevState> hs((size_t)n_pairs);
+  r.hs.assign((size_t)n_pairs, DevState{});
   for (int i = 0; i < n_pairs; ++i) {
-    DevState& h = hs[(size_t)i];
+    DevState& h = r.hs[(size_t)i];
     std::memset(&h, 0, sizeof(h));
-    for (int j = 0; j < 6; ++j) h.x[j] = observed ? observed[6 * i + j] : p.lsq.x0[j];
+    for (int j = 0; j < 6; ++j) h.x[j] = r.observed ? r.observed[6 * i + j] : p.lsq.x0[j];
     h.T = rigid_from_x(h.x);
     h.Tinv = rigid_inverse(h.T);
     h.T_res = h.T;
     h.H_rep = h.T;
   }
-  SICP_CUDA(cudaMemcpyAsync(b.state.p, hs.data(), sizeof(DevState) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
-  SICP_CUDA(cudaStreamSynchronize(st));  // the fixed clouds have arrived
+  SICP_CUDA(cudaMemcpyAsync(b.state.p, r.hs.data(), sizeof(DevState) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+  r.pd.assign((size_t)n_pairs, PairDev{});
+  for (auto& d : r.pd) std::memset(&d, 0, sizeof(d));
+}
 
-  // ---- fixed side: grids, subsample + gather, normals (the movable clouds are still in flight).
-  // With the overlap filter the selection needs the movable grids: only the fixed grids are
-  // built here, the rest follows the filter.
-  std::vector<PairDev> pd((size_t)n_pairs);
-  std::vector<BatchHostCloud> clouds((size_t)n_pairs);
-  std::vector<GridView> views;
-  std::vector<double> centres;
-  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = BatchHostCloud{b.fix_xyz.p + 3 * fo[(size_t)i], n_fix[i], fo[(size_t)i]};
-  {
-    StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build_batch(c, b, b.gfix, clouds, views, centres);
-    t.stop();
+// Survivor lists of the overlap filter: bounds[i] .. bounds[i + 1] is pair i's slice.  A pair
+// without a survivor is parked like a pair without enough correspondences (every later kernel
+// returns at once) and reported as SICP_ERR_NO_OVERLAP.
+void take_survivors(Ctx& c, Batch& b, PairsRun& r, const uint32_t* bounds) {
+  bool parked = false;
+  for (int i = 0; i < r.n_pairs; ++i) {
+    PairDev& d = r.pd[(size_t)i];
+    d.list_off = bounds[i];
+    d.list_len = (long long)bounds[i + 1] - (long long)bounds[i];
+    d.K = std::min<long long>(r.rp->correspondences, d.list_len);
+    if (d.list_len == 0) {
+      r.no_overlap[(size_t)i] = 1;
+      r.hs[(size_t)i].stop = 2;
+      parked = true;
+    }
   }
+  if (parked)
+    SICP_CUDA(cudaMemcpyAsync(b.state.p, r.hs.data(), sizeof(DevState) * (size_t)r.n_pairs, cudaMemcpyHostToDevice,
+                              c.stream));
+}
+
+// Overlap filter of sicp_register_batch: bounded search of every fixed point, one exclusive scan
+// over the keep flags of the whole batch, ordered scatter, and ONE read-back of the pair boundaries.
+void batch_filter(Ctx& c, Batch& b, PairsRun& r, long long max_n_fix) {
+  cudaStream_t st = c.stream;
+  const int n_pairs = r.n_pairs;
+  const long long nf = b.total_fix;
+  b.ovl_flag.reserve(nf);
+  b.ovl_scan.reserve(nf + 1);
+  b.ovl_list.reserve(std::max<long long>(nf, 1));
+  b.ovl_bounds.reserve((size_t)n_pairs + 1);
+  // r2 as sicp_register computes it
+  batch_overlap_launch(c, b, max_n_fix, r.rp->max_overlap_distance * r.rp->max_overlap_distance);
+  c.misc_counters.reserve(64);
+  scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums, c.misc_counters.p + 16);  // (its count is not used)
+  k_overlap_scatter<<<dim3((unsigned)((max_n_fix + 255) / 256), n_pairs), 256, 0, st>>>(b.pairs.p, b.ovl_flag.p,
+                                                                                     b.ovl_scan.p, b.ovl_list.p);
+  k_overlap_bounds<<<(n_pairs + 256) / 256, 256, 0, st>>>(b.pairs.p, n_pairs, b.ovl_scan.p, nf, b.ovl_bounds.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 2;
+  // keys_host (pinned, 8 n_pairs words since the grid builds) is free again
+  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.keys_host);
+  SICP_CUDA(cudaMemcpyAsync(bounds, b.ovl_bounds.p, sizeof(uint32_t) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  take_survivors(c, b, r, bounds);
+}
+
+}  // namespace
+
+// The box that holds every map point able to pass scan i's overlap filter.  A map point p passes
+// when the squared distance from q = Tinv p (rounded) to some movable point m of the scan, rounded,
+// is below r2 = r * r (rounded).  Every movable point lies in the box B of the scan's movable grid,
+// [o, o + dims h].  In exact arithmetic, |T^-1 p - m| < r gives |p - T m| < r, and T m lies in the
+// convex hull of the eight mapped corners of B, hence in their axis-aligned box grown by r.  What
+// rounding adds is bounded by a few ulps of the largest magnitude M involved (map and scan
+// coordinates, the translation): q and the mapped corners each carry a few ulps of M, Tinv is the
+// inverse of T up to a few ulps (R^T is exact, R is orthogonal to ~1e-15), and the rounded d^2 and
+// r2 move the radius by a few relative ulps.  Together that is below 1e-13 (M + r); the box is
+// grown by r + 1e-12 (M + r), ten times more (5e-6 m at UTM coordinates).  The cells are the map
+// grid's own cell_coord of the box faces: floor((v - o) / h) is monotone in v, so every point in the
+// box lies in a cell between those of its faces, and the kernel tests each candidate against the
+// box itself.
+static MapCull map_cull_box(const GridView& map, const GridView& g, const Rigid& T, double r) {
+  MapCull cu;
+  std::memset(&cu, 0, sizeof(cu));
+  const double lo_s[3] = {g.ox, g.oy, g.oz}, hi_s[3] = {g.ox + g.nx * g.h, g.oy + g.ny * g.h, g.oz + g.nz * g.h};
+  const double o[3] = {map.ox, map.oy, map.oz};
+  const int dims[3] = {map.nx, map.ny, map.nz};
+  double mag = std::max(std::fabs(T.t[0]), std::max(std::fabs(T.t[1]), std::fabs(T.t[2])));
+  for (int a = 0; a < 3; ++a) {
+    cu.lo[a] = kInf;
+    cu.hi[a] = -kInf;
+    mag = std::max(mag, std::max(std::fabs(o[a]), std::fabs(o[a] + dims[a] * map.h)));
+    mag = std::max(mag, std::max(std::fabs(lo_s[a]), std::fabs(hi_s[a])));
+  }
+  for (int k = 0; k < 8; ++k) {
+    double v[3];
+    rigid_apply(T, (k & 1) ? hi_s[0] : lo_s[0], (k & 2) ? hi_s[1] : lo_s[1], (k & 4) ? hi_s[2] : lo_s[2], v[0], v[1], v[2]);
+    for (int a = 0; a < 3; ++a) {
+      cu.lo[a] = std::min(cu.lo[a], v[a]);
+      cu.hi[a] = std::max(cu.hi[a], v[a]);
+      mag = std::max(mag, std::fabs(v[a]));
+    }
+  }
+  const double grow = r + 1e-12 * (mag + r);
+  for (int a = 0; a < 3; ++a) {
+    cu.lo[a] -= grow;
+    cu.hi[a] += grow;
+    // no map point lies below the map's box minimum o or beyond o + dims h
+    if (!(cu.hi[a] >= o[a]) || !(cu.lo[a] <= o[a] + (dims[a] + 1) * map.h)) return cu;  // rows = 0
+    auto cell = [&](double v) {
+      const double f = std::floor((v - o[a]) * map.inv_h);  // cell_coord's arithmetic, then its clamp
+      return f < 0.0 ? 0 : (f > dims[a] - 1 ? dims[a] - 1 : (int)f);
+    };
+    cu.c0[a] = cell(cu.lo[a]);
+    cu.c1[a] = cell(cu.hi[a]);
+  }
+  cu.rows = (long long)(cu.c1[1] - cu.c0[1] + 1) * (cu.c1[2] - cu.c0[2] + 1);
+  return cu;
+}
+
+// Culled overlap filter of sicp_register_to_map: a bit per (scan, map point) set by the searches
+// of the candidates in each scan's box, popcounts of the mask words, one exclusive scan over them,
+// ONE read-back of the scans' boundaries (and the search count), then the ordered compaction into
+// the survivor lists: ascending map indices per scan, as select_n_points needs them.
+static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
+  cudaStream_t st = c.stream;
+  const int n = r.n_pairs;
+  const double rr = r.rp->max_overlap_distance;
+  std::vector<MapCull> cu((size_t)n);
+  long long max_rows = 0, hint = 0;
+  for (int i = 0; i < n; ++i) {
+    cu[(size_t)i] = map_cull_box(m.view, r.pd[(size_t)i].gmov, r.hs[(size_t)i].T, rr);
+    max_rows = std::max(max_rows, cu[(size_t)i].rows);
+    hint += (long long)(cu[(size_t)i].rows * (cu[(size_t)i].c1[0] - cu[(size_t)i].c0[0] + 1) * c.grid_target_occ);
+  }
+  const long long words = (m.n + 31) / 32, nw = words * n;
+  m.culls.reserve(n);
+  m.bits.reserve(nw);
+  m.popc.reserve(nw);
+  m.popc_scan.reserve(nw + 1);
+  m.n_searched.reserve(1);
+  SICP_CUDA(cudaMemcpyAsync(m.culls.p, cu.data(), sizeof(MapCull) * (size_t)n, cudaMemcpyHostToDevice, st));
+  SICP_CUDA(cudaMemsetAsync(m.bits.p, 0, sizeof(uint32_t) * (size_t)nw, st));
+  SICP_CUDA(cudaMemsetAsync(m.n_searched.p, 0, sizeof(unsigned long long), st));
+  if (max_rows > 0) map_overlap_launch(c, b, m, m.culls.p, max_rows, rr * rr, hint);  // r2 as sicp_register computes it
+  map_bits_popc_launch(c, m.bits.p, nw, m.popc.p);
+  c.misc_counters.reserve(64);
+  scan_u32(c, m.popc.p, nw, m.popc_scan.p, m.sums, c.misc_counters.p + 16);  // (its count is not used)
+  // keys_host (pinned, 8 n_pairs words since the grid builds): n + 1 boundaries, then the count
+  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.keys_host);
+  unsigned long long* searched = b.keys_host + n + 1;
+  SICP_CUDA(cudaMemcpy2DAsync(bounds, sizeof(uint32_t), m.popc_scan.p, sizeof(uint32_t) * (size_t)words,
+                              sizeof(uint32_t), (size_t)n + 1, cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaMemcpyAsync(searched, m.n_searched.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  c.tm.overlap_candidates = (int64_t)*searched;
+  b.ovl_list.reserve(std::max<long long>(bounds[n], 1));
+  map_bits_scatter_launch(c, m.bits.p, nw, words, m.popc_scan.p, b.ovl_list.p);
+  take_survivors(c, b, r, bounds);
+}
+
+// Everything after the fixed side: descriptors, [select + normals], movable grids, [overlap filter,
+// select + normals], movable normals, the loop and the results.  fix_xyz holds the fixed
+// coordinates the descriptors' fix_off index; map (or null) is the resident map of
+// sicp_register_to_map, whose filter is the culled one.
+static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapStore* map, long long max_n_fix,
+                      sicp_pair_result* out, int64_t* n_selected) {
+  cudaStream_t st = c.stream;
+  const int n_pairs = r.n_pairs;
+  const sicp_register_params* rp = r.rp;
+  const sicp_run_params& p = rp->run;
   for (int i = 0; i < n_pairs; ++i) {
-    PairDev& d = pd[(size_t)i];
-    std::memset(&d, 0, sizeof(d));
-    d.gfix = views[(size_t)i];
-    d.n_fix = n_fix[i];
-    d.n_mov = n_mov[i];
-    d.fix_off = fo[(size_t)i];
-    d.mov_off = mo[(size_t)i];
-    d.K = std::min<long long>(rp->correspondences, n_fix[i]);
-    d.q_off = (long long)i * Kmax;
-    for (int j = 0; j < 6; ++j) d.obs[j] = observed ? observed[6 * i + j] : p.lsq.observed[j];
+    PairDev& d = r.pd[(size_t)i];
+    d.n_mov = r.mo[(size_t)i + 1] - r.mo[(size_t)i];
+    d.mov_off = r.mo[(size_t)i];
+    d.K = std::min<long long>(rp->correspondences, d.n_fix);
+    d.q_off = (long long)i * r.Kmax;
+    for (int j = 0; j < 6; ++j) d.obs[j] = r.observed ? r.observed[6 * i + j] : p.lsq.observed[j];
   }
   const int round_away = c.variant != SICP_VARIANT_PYTHON;
   auto select_and_normals = [&]() {
-    batch_select_gather_launch(c, b, overlap, round_away);
+    batch_select_gather_launch(c, b, fix_xyz, r.overlap, round_away);
     StageTimer t(c, &c.tm.normals_ms);
     batch_normals_launch(c, b, rp->neighbors);
     t.stop();
   };
-  if (!overlap) {
-    SICP_CUDA(cudaMemcpyAsync(b.pairs.p, pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+  // without the filter the selection needs only the fixed side: it runs while the movable clouds
+  // are still in flight; with it, the selection follows the filter, which needs the movable grids
+  if (!r.overlap) {
+    SICP_CUDA(cudaMemcpyAsync(b.pairs.p, r.pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
     select_and_normals();
   }
 
   // ---- movable side
   SICP_CUDA(cudaStreamWaitEvent(st, c.ev_copy, 0));
-  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = BatchHostCloud{b.mov_xyz.p + 3 * mo[(size_t)i], n_mov[i], mo[(size_t)i]};
+  std::vector<BatchHostCloud> clouds((size_t)n_pairs);
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  for (int i = 0; i < n_pairs; ++i)
+    clouds[(size_t)i] = BatchHostCloud{b.mov_xyz.p + 3 * r.mo[(size_t)i], r.pd[(size_t)i].n_mov, r.mo[(size_t)i]};
   {
     StageTimer t(c, &c.tm.grid_mov_ms);
     grid_build_batch(c, b, b.gmov, clouds, views, centres);
     t.stop();
   }
   for (int i = 0; i < n_pairs; ++i) {
-    pd[(size_t)i].gmov = views[(size_t)i];
-    for (int a = 0; a < 3; ++a) pd[(size_t)i].cm[a] = centres[(size_t)i * 3 + a];
+    r.pd[(size_t)i].gmov = views[(size_t)i];
+    for (int a = 0; a < 3; ++a) r.pd[(size_t)i].cm[a] = centres[(size_t)i * 3 + a];
   }
-  std::vector<char> no_overlap((size_t)n_pairs, 0);
+  r.no_overlap.assign((size_t)n_pairs, 0);
   c.tm.overlap_ms = 0;
-  if (overlap) {
-    // ---- overlap filter: bounded search of every fixed point, one exclusive scan over the keep
-    // flags of the whole batch, ordered scatter, and ONE read-back of the pair boundaries
-    SICP_CUDA(cudaMemcpyAsync(b.pairs.p, pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+  if (r.overlap) {
+    SICP_CUDA(cudaMemcpyAsync(b.pairs.p, r.pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
     StageTimer t(c, &c.tm.overlap_ms);
-    const long long nf = b.total_fix;
-    b.ovl_flag.reserve(nf);
-    b.ovl_scan.reserve(nf + 1);
-    b.ovl_list.reserve(std::max<long long>(nf, 1));
-    b.ovl_bounds.reserve((size_t)n_pairs + 1);
-    // r2 as sicp_register computes it
-    batch_overlap_launch(c, b, max_n_fix, rp->max_overlap_distance * rp->max_overlap_distance);
-    c.misc_counters.reserve(64);
-    scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums, c.misc_counters.p + 16);  // (its count is not used)
-    k_overlap_scatter<<<dim3((unsigned)((max_n_fix + 255) / 256), n_pairs), 256, 0, st>>>(b.pairs.p, b.ovl_flag.p,
-                                                                                       b.ovl_scan.p, b.ovl_list.p);
-    k_overlap_bounds<<<(n_pairs + 256) / 256, 256, 0, st>>>(b.pairs.p, n_pairs, b.ovl_scan.p, nf, b.ovl_bounds.p);
-    SICP_CUDA(cudaGetLastError());
-    c.tm.kernel_launches += 2;
-    // keys_host (pinned, 8 n_pairs words since the grid builds) is free again
-    uint32_t* bounds = reinterpret_cast<uint32_t*>(b.keys_host);
-    SICP_CUDA(cudaMemcpyAsync(bounds, b.ovl_bounds.p, sizeof(uint32_t) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
-    t.stop();  // synchronises the stream
-    bool parked = false;
-    for (int i = 0; i < n_pairs; ++i) {
-      PairDev& d = pd[(size_t)i];
-      d.list_off = bounds[i];
-      d.list_len = (long long)bounds[i + 1] - (long long)bounds[i];
-      d.K = std::min<long long>(rp->correspondences, d.list_len);
-      if (d.list_len == 0) {
-        // no survivor: parked like a pair without enough correspondences (every later kernel
-        // returns at once), reported as SICP_ERR_NO_OVERLAP
-        no_overlap[(size_t)i] = 1;
-        hs[(size_t)i].stop = 2;
-        parked = true;
-      }
-    }
-    if (parked)
-      SICP_CUDA(cudaMemcpyAsync(b.state.p, hs.data(), sizeof(DevState) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+    if (map) map_filter(c, b, *map, r);
+    else batch_filter(c, b, r, max_n_fix);
+    t.stop();
   }
-  SICP_CUDA(cudaMemcpyAsync(b.pairs.p, pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
-  if (overlap) select_and_normals();
+  SICP_CUDA(cudaMemcpyAsync(b.pairs.p, r.pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
+  if (r.overlap) select_and_normals();
   // pc_mov.estimate_normals(mov_neighbors) of every pair, in its own movable grid
   b.mov_attr = rp->mov_neighbors > 0;
   b.mov_cos_max = b.mov_attr ? mov_cos_max_of(rp->max_angle_rad) : -1.0;
   c.tm.mov_normals_ms = 0;
   if (b.mov_attr) {
-    b.q_nrm_eff.reserve(nq);
+    b.q_nrm_eff.reserve((size_t)n_pairs * (size_t)r.Kmax);
     StageTimer t(c, &c.tm.mov_normals_ms);
-    batch_mov_normals_launch(c, b, rp->mov_neighbors, max_n_mov);
+    batch_mov_normals_launch(c, b, rp->mov_neighbors, r.max_n_mov);
     t.stop();
   }
 
@@ -310,36 +433,166 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   c.tm.reject_solve_ms = ms;
   std::memcpy(out, b.results_host, sizeof(sicp_pair_result) * (size_t)n_pairs);
   for (int i = 0; i < n_pairs; ++i) {
-    if (no_overlap[(size_t)i]) out[i].status = SICP_ERR_NO_OVERLAP;
-    if (n_selected) n_selected[i] = pd[(size_t)i].K;
+    if (r.no_overlap[(size_t)i]) out[i].status = SICP_ERR_NO_OVERLAP;
+    if (n_selected) n_selected[i] = r.pd[(size_t)i].K;
   }
+}
+
+static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, const int64_t* n_fix,
+                           const double* const* mov_xyz, const int64_t* n_mov,
+                           const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
+                           int64_t* n_selected) {
+  check_pairs_params(c, n_pairs, fix_xyz && n_fix && mov_xyz && n_mov && out, rp);
+  PairsRun r;
+  begin_pairs(r, n_pairs, rp, observed);
+  std::vector<long long> fo((size_t)n_pairs + 1, 0);
+  long long Kmax = 0, max_n_fix = 0;
+  for (int i = 0; i < n_pairs; ++i) {
+    SICP_REQUIRE(fix_xyz[i] && mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
+    SICP_REQUIRE(n_fix[i] >= rp->neighbors && n_mov[i] >= 1, SICP_ERR_BAD_ARG,
+                 "every fixed cloud needs at least `neighbors` points, every movable cloud one");
+    add_movable(r, i, n_mov[i]);
+    fo[(size_t)i + 1] = fo[(size_t)i] + n_fix[i];
+    Kmax = std::max<long long>(Kmax, std::min<long long>(rp->correspondences, n_fix[i]));
+    max_n_fix = std::max<long long>(max_n_fix, n_fix[i]);
+  }
+  if (!c.batch) c.batch = new Batch();
+  Batch& b = *c.batch;
+  r.Kmax = (Kmax + 1) & ~1ll;  // even: every pair's slice of the per-query arrays starts 16-byte aligned
+  b.total_fix = fo[(size_t)n_pairs];
+  b.total_mov = r.mo[(size_t)n_pairs];
+  cudaStream_t st = c.stream;
+
+  // ---- uploads: fixed clouds on the context's stream, movable ones behind them on the copy stream
+  b.fix_xyz.reserve(3 * (size_t)b.total_fix);
+  SICP_CUDA(cudaEventRecord(c.ev_user, st));
+  SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
+  for (int i = 0; i < n_pairs; ++i)
+    SICP_CUDA(cudaMemcpyAsync(b.fix_xyz.p + 3 * fo[(size_t)i], fix_xyz[i], sizeof(double) * 3 * (size_t)n_fix[i],
+                              cudaMemcpyDefault, st));
+  upload_movable(c, b, r, mov_xyz, n_mov);
+  alloc_pair_buffers(c, b, r);
+  SICP_CUDA(cudaStreamSynchronize(st));  // the fixed clouds have arrived
+
+  // ---- fixed side: grids (the movable clouds are still in flight)
+  std::vector<BatchHostCloud> clouds((size_t)n_pairs);
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = BatchHostCloud{b.fix_xyz.p + 3 * fo[(size_t)i], n_fix[i], fo[(size_t)i]};
+  {
+    StageTimer t(c, &c.tm.grid_fix_ms);
+    grid_build_batch(c, b, b.gfix, clouds, views, centres);
+    t.stop();
+  }
+  for (int i = 0; i < n_pairs; ++i) {
+    r.pd[(size_t)i].gfix = views[(size_t)i];
+    r.pd[(size_t)i].n_fix = n_fix[i];
+    r.pd[(size_t)i].fix_off = fo[(size_t)i];
+  }
+  run_pairs(c, b, r, b.fix_xyz.p, nullptr, max_n_fix, out, n_selected);
+}
+
+static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
+  if (map_xyz == nullptr || n_map == 0) {
+    delete c.map;
+    c.map = nullptr;
+    return;
+  }
+  SICP_REQUIRE(n_map > 0 && n_map < (1ll << 32), SICP_ERR_BAD_ARG, "n_map must be in [1, 2^32 - 1]");
+  if (!c.batch) c.batch = new Batch();
+  if (!c.map) c.map = new MapStore();
+  MapStore& m = *c.map;
+  m.n = 0;  // no map until the new one is complete
+  m.xyz.reserve(3 * (size_t)n_map);
+  {
+    StageTimer t(c, &c.tm.upload_ms);
+    upload_to_device(c, m.xyz.p, map_xyz, sizeof(double) * 3 * (size_t)n_map);
+    t.stop();
+  }
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  {
+    StageTimer t(c, &c.tm.grid_fix_ms);
+    grid_build_batch(c, *c.batch, m.grid, {BatchHostCloud{m.xyz.p, n_map, 0}}, views, centres);
+    t.stop();
+  }
+  m.view = views[0];
+  m.n = n_map;
+}
+
+static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, const int64_t* n_mov,
+                            const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
+                            int64_t* n_selected) {
+  check_pairs_params(c, n_scans, mov_xyz && n_mov && out, rp);
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  SICP_REQUIRE(m.n >= rp->neighbors, SICP_ERR_BAD_ARG, "the map needs at least `neighbors` points");
+  SICP_REQUIRE((long long)n_scans * m.n < (1ll << 32), SICP_ERR_BAD_ARG,
+               "n_scans x n_map must be below 2^32 (32-bit survivor offsets): use fewer scans per call");
+  PairsRun r;
+  begin_pairs(r, n_scans, rp, observed);
+  for (int i = 0; i < n_scans; ++i) {
+    SICP_REQUIRE(mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
+    SICP_REQUIRE(n_mov[i] >= 1, SICP_ERR_BAD_ARG, "every movable cloud needs at least one point");
+    add_movable(r, i, n_mov[i]);
+  }
+  if (!c.batch) c.batch = new Batch();
+  Batch& b = *c.batch;
+  r.Kmax = (std::min<long long>(rp->correspondences, m.n) + 1) & ~1ll;
+  b.total_mov = r.mo[(size_t)n_scans];
+  c.tm.overlap_candidates = 0;
+  SICP_CUDA(cudaEventRecord(c.ev_user, c.stream));
+  SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
+  upload_movable(c, b, r, mov_xyz, n_mov);
+  alloc_pair_buffers(c, b, r);
+  for (int i = 0; i < n_scans; ++i) {
+    r.pd[(size_t)i].gfix = m.view;
+    r.pd[(size_t)i].n_fix = m.n;
+    r.pd[(size_t)i].fix_off = 0;
+  }
+  run_pairs(c, b, r, m.xyz.p, &m, m.n, out, n_selected);
 }
 
 }  // namespace sicp
 
 using namespace sicp;
 
+#define SICP_BATCH_API(body)                 \
+  if (!ctx) {                                \
+    sicp::set_thread_error("sicp_ctx is NULL"); \
+    return SICP_ERR_BAD_ARG;                 \
+  }                                          \
+  Ctx& c = ctx->c;                           \
+  try {                                      \
+    SICP_CUDA(cudaSetDevice(c.device));      \
+    body;                                    \
+  } catch (const sicp::Error& e) {           \
+    c.up.abandon();                          \
+    c.err = e.msg;                           \
+    sicp::set_thread_error(e.msg);           \
+    if (e.code == SICP_ERR_CUDA) cudaGetLastError(); \
+    return e.code;                           \
+  } catch (const std::exception& e) {        \
+    c.up.abandon();                          \
+    c.err = e.what();                        \
+    sicp::set_thread_error(c.err);           \
+    return SICP_ERR_CUDA;                    \
+  }                                          \
+  return SICP_OK;
+
 extern "C" int32_t sicp_register_batch(sicp_ctx* ctx, int32_t n_pairs, const double* const* fix_xyz,
                                        const int64_t* n_fix, const double* const* mov_xyz,
                                        const int64_t* n_mov, const sicp_register_params* p,
                                        const double* observed, sicp_pair_result* out, int64_t* n_selected) {
-  if (!ctx) {
-    sicp::set_thread_error("sicp_ctx is NULL");
-    return SICP_ERR_BAD_ARG;
-  }
-  Ctx& c = ctx->c;
-  try {
-    SICP_CUDA(cudaSetDevice(c.device));
-    register_batch(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected);
-  } catch (const sicp::Error& e) {
-    c.err = e.msg;
-    sicp::set_thread_error(e.msg);
-    if (e.code == SICP_ERR_CUDA) cudaGetLastError();
-    return e.code;
-  } catch (const std::exception& e) {
-    c.err = e.what();
-    sicp::set_thread_error(c.err);
-    return SICP_ERR_CUDA;
-  }
-  return SICP_OK;
+  SICP_BATCH_API(register_batch(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected))
+}
+
+extern "C" int32_t sicp_set_map(sicp_ctx* ctx, const double* map_xyz, int64_t n_map) {
+  SICP_BATCH_API(set_map(c, map_xyz, n_map))
+}
+
+extern "C" int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const* mov_xyz,
+                                        const int64_t* n_mov, const sicp_register_params* p,
+                                        const double* observed, sicp_pair_result* out, int64_t* n_selected) {
+  SICP_BATCH_API(register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected))
 }

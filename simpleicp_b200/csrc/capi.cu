@@ -203,6 +203,8 @@ void set_state_transform(Ctx& c, const double x[6], const Rigid* T_or_null, bool
   init_state(c, x, T_or_null, reset_loop);
 }
 
+void upload_to_device(Ctx& c, void* dst, const void* src, size_t bytes) { upload_cloud(c, dst, src, bytes); }
+
 }  // namespace sicp
 
 using namespace sicp;
@@ -307,6 +309,8 @@ int32_t sicp_destroy(sicp_ctx* ctx) {
   if (c.copy_stream) cudaStreamDestroy(c.copy_stream);
   delete c.batch;
   c.batch = nullptr;
+  delete c.map;
+  c.map = nullptr;
   if (c.rec_host) cudaFreeHost(c.rec_host);
   if (c.scal_host) cudaFreeHost(c.scal_host);
   delete ctx;

@@ -49,6 +49,7 @@ struct SolveWs {
 };
 
 struct Batch;
+struct MapStore;
 
 struct Ctx {
   int device = 0;
@@ -155,6 +156,7 @@ struct Ctx {
   DevBuf<unsigned char> stage;
 
   Batch* batch = nullptr;  // created by the first sicp_register_batch
+  MapStore* map = nullptr; // sicp_set_map: the resident fixed cloud of sicp_register_to_map
 };
 // what the match kernels / reject kernels see of the movable-side attributes
 inline const float4* mov_attr_nrm(Ctx& c) { return c.mov_attr ? c.mov_nrm.p : nullptr; }
@@ -242,6 +244,29 @@ struct Batch {
   }
 };
 
+// Box of one scan's overlap cull in the map frame (host-computed, batch.cu: map_cull_box): the
+// map-grid cells [c0, c1] per axis and the coordinate box [lo, hi] the candidates must lie in.
+struct MapCull {
+  double lo[3], hi[3];
+  int c0[3], c1[3];
+  long long rows;  // (c1[1] - c0[1] + 1) (c1[2] - c0[2] + 1), 0 = no candidate
+};
+
+// The resident fixed cloud of sicp_register_to_map (sicp_set_map): its coordinates and ONE grid,
+// built by grid_build_batch with the map as its only cloud, so that its cell plan is the one a
+// batch would make for it.  Every pair of a sicp_register_to_map call takes `view` as its fixed
+// grid, with fix_off = 0.
+struct MapStore {
+  DevBuf<double> xyz;
+  BatchGrid grid;
+  GridView view{};
+  long long n = 0;
+  // overlap filter: one bit per (scan, map point), its per-word popcounts and their prefix sum
+  DevBuf<uint32_t> bits, popc, popc_scan, sums;
+  DevBuf<unsigned long long> n_searched;  // bounded searches of the last filter
+  DevBuf<MapCull> culls;                  // one per scan
+};
+
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
 void grid_build(Ctx& c, Grid& g, const double* xyz_dev, long long n);
 void make_float4_copy(Ctx& c);
@@ -303,8 +328,9 @@ struct BatchHostCloud {
 };
 void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHostCloud>& clouds,
                       std::vector<GridView>& views, std::vector<double>& centres /* 3 per cloud */);
-// with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud
-void batch_select_gather_launch(Ctx& c, Batch& b, bool with_list, int round_away);
+// with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud;
+// fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::fix_xyz or MapStore::xyz)
+void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);
 void batch_normals_launch(Ctx& c, Batch& b, int k);
 // k-NN + PCA of every movable point of every pair in its own movable grid -> Batch::mov_nrm
 void batch_mov_normals_launch(Ctx& c, Batch& b, int k, long long max_n_mov);
@@ -312,6 +338,16 @@ void batch_match_launch(Ctx& c, Batch& b, bool warm);
 // PointCloud.select_in_range of every fixed point of the batch under its pair's DevState
 // transform: Batch::ovl_flag[i] = (squared distance to the nearest movable point < r2)
 void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2);
+// Culled overlap filter of sicp_register_to_map: for every scan, the map points inside its
+// MapCull box get the bounded search of batch_overlap_launch (same device code, same flag);
+// survivors set bit i of the scan's row of MapStore::bits (cleared by the caller).
+void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev, long long max_rows, double r2,
+                        long long n_candidates_hint);
+// popcounts of MapStore::bits words (n_words of them) -> popc, and the ordered compaction of the
+// set bits into list (scan[w] = exclusive prefix sum of the popcounts): ascending map indices
+void map_bits_popc_launch(Ctx& c, const uint32_t* bits, long long n_words, uint32_t* popc);
+void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, long long words_per_scan,
+                             const uint32_t* scan, uint32_t* list);
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 
@@ -324,6 +360,9 @@ inline long long normals_chunk_queries(const Ctx& c, int k) {
   return std::max<long long>(1024, ((long long)c.normals_scratch_mb << 20) / (4ll * k));
 }
 void check_mov_neighbors(const Ctx& c, const sicp_register_params& rp);
+// a whole cloud host -> device on the context's stream (pageable sources through upload.cuh's
+// staging threads), stream-ordered when it returns
+void upload_to_device(Ctx& c, void* dst, const void* src, size_t bytes);
 
 struct StageTimer {
   Ctx& c;

@@ -630,6 +630,76 @@ __global__ void __launch_bounds__(128)
                             nullptr, nullptr, nullptr, nullptr, r2, co, gt, keep + f);
 }
 
+// Culled overlap filter of sicp_register_to_map: blockIdx.y is the scan, blockIdx.x one x-row of
+// the map grid inside the scan's MapCull cells, i.e. one contiguous range of cell-sorted map
+// records.  The groups of MG lanes walk the row's records; a record inside the scan's box gets
+// k_overlap_batch's bounded search (match_coop_body<MG, true> on the same coordinates, movable
+// grid, prior and bound, so the flag is that of the batch filter bit for bit), and a survivor
+// sets the bit of its map index in the scan's row of the mask (`words` words per scan).  Points
+// outside the box cannot pass (batch.cu: map_cull_box), so they are skipped unsearched.
+template <int MG>
+__global__ void __launch_bounds__(128)
+    k_map_overlap(const PairDev* __restrict__ pairs, const DevState* __restrict__ state,
+                  const MapCull* __restrict__ culls, GridView map, double r2, long long words,
+                  uint32_t* __restrict__ bits, unsigned long long* __restrict__ n_searched) {
+  const MapCull& cu = culls[blockIdx.y];
+  if ((long long)blockIdx.x >= cu.rows) return;
+  const int ny = cu.c1[1] - cu.c0[1] + 1;
+  const int y = cu.c0[1] + (int)(blockIdx.x % (unsigned)ny), z = cu.c0[2] + (int)(blockIdx.x / (unsigned)ny);
+  const long long row = ((long long)z * map.ny + y) * map.nx;
+  // the row's end is read from shared memory in every round: held in a register across the
+  // inlined search it was spilled
+  __shared__ uint32_t row_end;
+  const uint32_t s = map.cell_start[row + cu.c0[0]];
+  if (threadIdx.x == 0) row_end = map.cell_start[row + cu.c1[0] + 1];
+  __syncthreads();
+  const PairDev& pd = pairs[blockIdx.y];
+  const CorrOut co{nullptr, 0, nullptr, nullptr, 0, 0, nullptr, nullptr, -1.0};
+  const int sub = threadIdx.x & (MG - 1);
+  uint32_t* __restrict__ mask = bits + (size_t)blockIdx.y * words;
+  // the search's flag goes to a shared slot of the group (a local variable would live in memory)
+  __shared__ uint32_t flags[128 / MG];
+  uint32_t* flag = flags + threadIdx.x / MG;
+  unsigned int searched = 0;
+  for (uint32_t p = s + threadIdx.x / MG; p < *(volatile uint32_t*)&row_end; p += 128 / MG) {
+    const Rec r = map.recs[p];  // the whole group reads the same record and takes the same branch
+    if (r.x < cu.lo[0] || r.x > cu.hi[0] || r.y < cu.lo[1] || r.y > cu.hi[1] || r.z < cu.lo[2] || r.z > cu.hi[2])
+      continue;
+    const double q[3] = {r.x, r.y, r.z};
+    match_coop_body<MG, true>(pd.gmov, state + blockIdx.y, q, nullptr, nullptr, 1, 1 << 30, 0, nullptr, nullptr,
+                              nullptr, nullptr, r2, co, sub, flag);
+    if (sub == 0) {  // the lane that wrote the flag
+      ++searched;
+      if (*flag) atomicOr(&mask[r.idx >> 5], 1u << (r.idx & 31));
+    }
+  }
+  searched = __reduce_add_sync(0xffffffffu, searched);
+  if ((threadIdx.x & 31) == 0 && searched) atomicAdd(n_searched, (unsigned long long)searched);
+}
+
+__global__ void __launch_bounds__(256) k_map_popc(const uint32_t* __restrict__ bits, long long n, uint32_t* __restrict__ popc) {
+  const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (w < n) popc[w] = (uint32_t)__popc(bits[w]);
+}
+
+// word w of scan w / per_scan holds map points 32 (w % per_scan) + b: its set bits go, in
+// ascending order, to list[scan[w] ...]
+__global__ void __launch_bounds__(256)
+    k_map_scatter(const uint32_t* __restrict__ bits, long long n, long long per_scan,
+                  const uint32_t* __restrict__ scan, uint32_t* __restrict__ list) {
+  const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (w >= n) return;
+  uint32_t v = bits[w];
+  if (!v) return;
+  uint32_t o = scan[w];
+  const uint32_t base = (uint32_t)(w % per_scan) << 5;
+  while (v) {
+    const int b = __ffs(v) - 1;
+    list[o++] = base + (uint32_t)b;
+    v &= v - 1;
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // brute-force engine (TMA staged)
 // ------------------------------------------------------------------------------------------
@@ -975,9 +1045,9 @@ __global__ void __launch_bounds__(256)
 }
 }  // namespace
 
-void batch_select_gather_launch(Ctx& c, Batch& b, bool with_list, int round_away) {
+void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away) {
   k_select_gather_batch<<<dim3((unsigned)((b.Kmax + 255) / 256), b.n_pairs), 256, 0, c.stream>>>(
-      b.pairs.p, b.fix_xyz.p, with_list ? b.ovl_list.p : nullptr, round_away, b.sel_idx.p, b.q_xyz.p);
+      b.pairs.p, fix_xyz, with_list ? b.ovl_list.p : nullptr, round_away, b.sel_idx.p, b.q_xyz.p);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
@@ -993,6 +1063,37 @@ void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2) {
   if (mg <= 4) k_overlap_batch<4><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
   else if (mg == 8) k_overlap_batch<8><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
   else k_overlap_batch<16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev, long long max_rows, double r2,
+                        long long n_candidates_hint) {
+  // lanes per search by the number of searches in flight, as batch_overlap_launch chooses them
+  // (the flags do not depend on it)
+  int mg = c.match_group;
+  if (mg == 0 || mg == 1) mg = (n_candidates_hint <= 16384) ? 16 : ((n_candidates_hint <= 65536) ? 8 : 4);
+  const dim3 grid((unsigned)max_rows, b.n_pairs);
+  const long long words = (m.n + 31) / 32;
+  if (mg <= 4)
+    k_map_overlap<4><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  else if (mg == 8)
+    k_map_overlap<8><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  else
+    k_map_overlap<16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_bits_popc_launch(Ctx& c, const uint32_t* bits, long long n_words, uint32_t* popc) {
+  k_map_popc<<<(unsigned)((n_words + 255) / 256), 256, 0, c.stream>>>(bits, n_words, popc);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, long long words_per_scan,
+                             const uint32_t* scan, uint32_t* list) {
+  k_map_scatter<<<(unsigned)((n_words + 255) / 256), 256, 0, c.stream>>>(bits, n_words, words_per_scan, scan, list);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
