@@ -12,7 +12,9 @@
  *  - Every function returns a sicp_status; sicp_last_error(ctx) gives the message.
  *  - Pointers marked [h|d] may be host or device memory (detected with
  *    cudaPointerGetAttributes); [h] must be host memory.  The caller owns every buffer it passes
- *    and allocates every output; the library never frees or keeps caller memory.
+ *    and allocates every output; the library never frees or keeps caller memory.  Any alignment
+ *    of the element type is accepted; outputs that are misaligned or on another device than the
+ *    context's are written through the library's own device buffer.
  *  - All point arrays are row-major n x 3 float64 (NumPy's layout for PointCloud.X,
  *    python/simpleicp/pointcloud.py:81-84).  Indices are int64 like NumPy's.
  *  - A context is bound to one device and one CUDA stream (e.g. torch's current stream); calls

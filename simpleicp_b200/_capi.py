@@ -224,6 +224,24 @@ def _ptr(a) -> Optional[int]:
     raise TypeError(f"unsupported buffer type {type(a)}")
 
 
+def _xyz_out_ptr(out, n: int) -> int:
+    """Address of a caller's output for n transformed points: a NumPy array or a torch tensor
+    (host, or CUDA on any device) of shape (n, 3), float64 and C-contiguous, into which the
+    library writes 24 n bytes.  Anything else raises ValueError before the library is called."""
+    if isinstance(out, np.ndarray):
+        f64, contiguous, addr = out.dtype == np.float64, out.flags.c_contiguous, out.ctypes.data
+    elif hasattr(out, "data_ptr") and hasattr(out, "is_contiguous"):
+        import torch
+
+        f64, contiguous, addr = out.dtype == torch.float64, out.is_contiguous(), out.data_ptr()
+    else:
+        raise ValueError(f"the output must be a NumPy array or a torch tensor, not {type(out).__name__}")
+    if not (f64 and contiguous and tuple(out.shape) == (n, 3)):
+        raise ValueError(f"the output must be a C-contiguous float64 array of shape ({n}, 3); got "
+                         f"{out.dtype} of shape {tuple(out.shape)}{'' if contiguous else ', not contiguous'}")
+    return addr
+
+
 def _as_f64_xyz(X):
     """(n,3) float64 C-contiguous view/copy of a NumPy array or torch tensor."""
     if isinstance(X, np.ndarray) or not hasattr(X, "data_ptr"):
@@ -480,7 +498,8 @@ class Engine:
             transform_out = pinned_empty((self.n_mov, 3), np.float64)
         nsel = C.c_int64(0)
         self._check(self._lib.sicp_register(self._h, _ptr(Xf), self.n_fix, _ptr(Xm), self.n_mov, C.byref(rp),
-                                            C.byref(out), log, _ptr(transform_out), C.byref(nsel)))
+                                            C.byref(out), log, _xyz_out_ptr(transform_out, self.n_mov),
+                                            C.byref(nsel)))
         self.K = int(nsel.value)
         n = C.c_int64(0)
         res = np.empty(int(out.n_residuals), dtype=np.float64)
@@ -584,10 +603,11 @@ class Engine:
         return rec
 
     def transform(self, H, out=None):
-        """X_mov transformed by H.  `out` may be a CUDA torch tensor (n_mov, 3) float64."""
+        """X_mov transformed by H.  `out` (None: a new pinned array) is an (n_mov, 3) float64
+        C-contiguous NumPy array or torch tensor, host or CUDA on any device."""
         if out is None:
             out = pinned_empty((self.n_mov, 3), np.float64)
-        self._check(self._lib.sicp_transform(self._h, _d16(H), _ptr(out)))
+        self._check(self._lib.sicp_transform(self._h, _d16(H), _xyz_out_ptr(out, self.n_mov)))
         return out
 
     def time_stages(self, params: RunParams, reps: int, flush_l2: bool, outer_only: bool = False) -> dict:

@@ -567,13 +567,13 @@ using namespace sicp;
     SICP_CUDA(cudaSetDevice(c.device));      \
     body;                                    \
   } catch (const sicp::Error& e) {           \
-    c.up.abandon();                          \
+    c.up.cancel();                           \
     c.err = e.msg;                           \
     sicp::set_thread_error(e.msg);           \
     if (e.code == SICP_ERR_CUDA) cudaGetLastError(); \
     return e.code;                           \
   } catch (const std::exception& e) {        \
-    c.up.abandon();                          \
+    c.up.cancel();                           \
     c.err = e.what();                        \
     sicp::set_thread_error(c.err);           \
     return SICP_ERR_CUDA;                    \

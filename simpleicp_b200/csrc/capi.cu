@@ -13,15 +13,15 @@ namespace sicp {
 static thread_local std::string g_thread_error;
 void set_thread_error(const std::string& m) { g_thread_error = m; }
 
-bool is_device_ptr(const void* p) {
-  if (!p) return false;
+int device_of_ptr(const void* p) {
+  if (!p) return -1;
   cudaPointerAttributes at;
   cudaError_t e = cudaPointerGetAttributes(&at, p);
   if (e != cudaSuccess) {
     cudaGetLastError();
-    return false;
+    return -1;
   }
-  return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+  return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) ? at.device : -1;
 }
 
 // mov_neighbors / max_angle_rad of sicp_register and sicp_register_batch (range checks that need
@@ -221,14 +221,14 @@ using namespace sicp;
 #define API_END                                              \
   }                                                          \
   catch (const sicp::Error& e) {                             \
-    c.up.abandon();                                          \
+    c.up.cancel();                                           \
     c.err = e.msg;                                           \
     sicp::set_thread_error(e.msg);                           \
     if (e.code == SICP_ERR_CUDA) cudaGetLastError();         \
     return e.code;                                           \
   }                                                          \
   catch (const std::exception& e) {                          \
-    c.up.abandon();                                          \
+    c.up.cancel();                                           \
     c.err = e.what();                                        \
     sicp::set_thread_error(c.err);                           \
     return SICP_ERR_CUDA;                                    \
@@ -857,9 +857,12 @@ int32_t sicp_get_residuals(sicp_ctx* ctx, double* residuals, int64_t cap, int64_
   API_END
 }
 
+// k_transform stores 16-byte vectors at out + 48 i: only an aligned output on the context's own
+// device takes them directly; host outputs, misaligned ones and those on another device are
+// written through the staging buffer
 static void transform_to(Ctx& c, const Rigid& T, double* mov_xyz_out) {
   StageTimer t(c, &c.tm.transform_ms);
-  if (is_device_ptr(mov_xyz_out)) {
+  if (device_of_ptr(mov_xyz_out) == c.device && reinterpret_cast<uintptr_t>(mov_xyz_out) % 16 == 0) {
     transform_launch(c, T, c.mov_xyz.p, mov_xyz_out, c.n_mov);
   } else {
     c.stage.reserve(sizeof(double) * 3 * c.n_mov);

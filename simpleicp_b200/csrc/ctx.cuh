@@ -354,7 +354,8 @@ void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 int bin_cap_for(long long K);
 
 // helpers in capi.cu
-bool is_device_ptr(const void* p);
+// device ordinal of device (or managed) memory, -1 for host memory
+int device_of_ptr(const void* p);
 // queries per launch of a chunked k-NN + PCA: c.normals_scratch_mb MiB of k record positions each
 inline long long normals_chunk_queries(const Ctx& c, int k) {
   return std::max<long long>(1024, ((long long)c.normals_scratch_mb << 20) / (4ll * k));

@@ -31,7 +31,7 @@ __global__ void __launch_bounds__(256) k_bbox(const double* __restrict__ xyz, lo
     for (int a = 0; a < 3; ++a) {
       double v = xyz[3 * i + a];
       mn[a] = fmin(mn[a], v);
-      mx[a] = fmax(mx[a], v);
+      mx[a] = fmax(mx[a], v != v ? kInf : v);  // fmax drops NaN: count it as +inf, which the host refuses
     }
   }
   __shared__ double smn[8][3], smx[8][3];
@@ -396,7 +396,7 @@ __global__ void __launch_bounds__(256) k_bbox_batch(const CloudPlan* __restrict_
     for (int a = 0; a < 3; ++a) {
       const double v = xyz[3 * i + a];
       mn[a] = fmin(mn[a], v);
-      mx[a] = fmax(mx[a], v);
+      mx[a] = fmax(mx[a], v != v ? kInf : v);  // fmax drops NaN: count it as +inf, which the host refuses
     }
   }
   __shared__ double smn[8][3], smx[8][3];

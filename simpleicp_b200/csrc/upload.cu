@@ -118,6 +118,11 @@ void PageableUploader::abandon() noexcept {
   in_flight_ = false;
 }
 
+void PageableUploader::cancel() noexcept {
+  abandon();
+  for (int t = 0; t < n_used_; ++t) cudaStreamSynchronize(ws_[t]);
+}
+
 void PageableUploader::finish(cudaStream_t target) {
   if (!in_flight_) return;
   abandon();

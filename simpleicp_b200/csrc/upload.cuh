@@ -41,8 +41,12 @@ struct PageableUploader {
   // Wait for the workers (host side: src has been read completely) and make `target` wait for
   // their transfers (device side).  Throws sicp::Error if a worker failed.  No-op when idle.
   void finish(cudaStream_t target);
-  // Host-side wait only (error paths): never throws.
+  // Host-side wait only: never throws.
   void abandon() noexcept;
+  // Error paths: abandon(), then wait until the DMA the workers queued has landed.  The failing
+  // call may not have made any stream wait for it, and the next call may copy into the same
+  // device buffer from another stream.  Never throws.
+  void cancel() noexcept;
   bool active() const { return in_flight_; }
 
  private:
