@@ -31,6 +31,9 @@
 extern "C" {
 #endif
 
+/* The version changes when a struct layout or an existing entry point's meaning changes.  Added
+ * entry points leave it as it is (sicp_get_batch_outputs came in at version 5): bindings look
+ * them up by name. */
 #define SICP_ABI_VERSION 5
 
 typedef enum {
@@ -322,6 +325,35 @@ int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const
                              const double* observed /*[h] n_scans x 6, radians, or NULL*/,
                              sicp_pair_result* out /*[h] n_scans*/,
                              int64_t* n_selected /*[h] n_scans or NULL*/);
+
+/* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
+ * sicp_register_batch and sicp_register_to_map report per pair only the record above.  This call
+ * returns what else sicp_register returns, for every pair of the LAST successful call of either
+ * on this context: X_mov_transformed (transform_by_H, pointcloud.py:205-217, as at
+ * simpleicp.py:316), the final distance residuals (simpleicp.py:324, 4th return value), the
+ * per-iteration records and the applied transform.  Those two calls only leave these on the
+ * device; all the work happens here, and they stay readable (any number of times, same bits)
+ * until the next sicp_register_batch, sicp_register_to_map or sicp_set_map on the context.
+ *  - SICP_ERR_STATE: before any such call, after sicp_set_map, or after a batch / map call that
+ *    returned an error (each of the three clears the outputs on entry; only a successful return
+ *    of the first two makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
+ *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose
+ *    status was not SICP_OK (SICP_ERR_NO_OVERLAP included) is ever written.
+ *  - mov_xyz_out[i]: pair i's movable cloud (n_mov[i] x 3) moved by the transform the run applied,
+ *    bit for bit what sicp_transform gives for that cloud with T[i].
+ *  - residuals[i]: the final residuals in kept order (the order of selection), out[i].n_kept
+ *    values: those whose two-pass mean / std are out[i].mean_res / std_res.
+ *  - log: entry i * max_iterations + j is pair i's record of iteration j for j < out[i].iterations,
+ *    zero beyond; max_iterations is that call's run.max_iterations.  As in sicp_register's log,
+ *    the last row's mean_res / std_res are the exact two-pass values (out[i]'s).
+ *  - T: row-major 4 x 4 transform applied to pair i's cloud (what sicp_get_transform reports after
+ *    sicp_register): out[i].H, except under SICP_VARIANT_LINEARIZED_CPP, where H = H * dH is a
+ *    different product of the same increments.                                                   */
+int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
+                               double* const* mov_xyz_out /*[h|d] per pair n_mov[i] x 3, or NULL*/,
+                               double* const* residuals   /*[h|d] per pair out[i].n_kept, or NULL*/,
+                               sicp_iter_record* log      /*[h] n_pairs x max_iterations, or NULL*/,
+                               double* T                  /*[h] n_pairs x 16, or NULL*/);
 
 /* ---- PointCloud.transform_by_H (pointcloud.py:205-217), final application simpleicp.py:316 -- */
 int32_t sicp_transform(sicp_ctx* ctx, const double H[16], double* mov_xyz_out /*[h|d] n_mov x 3*/);

@@ -41,7 +41,7 @@ SYMBOLS = (
     "sicp_set_normals", "sicp_set_mov_normals", "sicp_get_knn", "sicp_match", "sicp_reject", "sicp_solve",
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
-    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -166,6 +166,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_set_map": [vp, vp, i64],
         "sicp_register_to_map": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(RegisterParams), vp,
                                  C.POINTER(PairResult), vp],
+        "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -173,7 +174,12 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_debug_grid_params": [vp, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(i32)],
     }
     for name, args in sigs.items():
-        fn = getattr(lib, name)
+        # entry points added without a layout change keep the version: a library that predates
+        # one of them is refused by name
+        fn = getattr(lib, name, None)
+        if fn is None:
+            raise ImportError(f"{lib_path} does not export {name}: rebuild with "
+                              f"`python -m simpleicp_b200._build --force`")
         fn.argtypes = args
         fn.restype = i32
     lib.sicp_xyz_load.argtypes = [C.c_char_p, C.POINTER(C.POINTER(dbl)), C.POINTER(i64)]
@@ -533,6 +539,7 @@ class Engine:
                                                   None if observed is None else _ptr(observed), out,
                                                   _ptr(n_selected)))
         out.n_selected = n_selected
+        out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
         return out
 
     def set_map(self, X_map):
@@ -566,7 +573,26 @@ class Engine:
                                                    None if observed is None else _ptr(observed), out,
                                                    _ptr(n_selected)))
         out.n_selected = n_selected
+        out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
         return out
+
+    def batch_outputs(self, result):
+        """sicp_get_batch_outputs for `result`, the PairResult array the last register_batch /
+        register_to_map on this engine returned: per pair (X_mov_transformed, residuals, log, T)
+        -- the transformed movable cloud (pinned NumPy), the final residuals in kept order, the
+        IterRecord of every iteration run and the applied 4 x 4 transform -- or None for a pair
+        whose status is not SICP_OK."""
+        n, it = len(result), int(result.max_iterations)
+        ok = [result[i].status == SICP_OK for i in range(n)]
+        X = [pinned_empty((int(result.n_mov[i]), 3), np.float64) if ok[i] else None for i in range(n)]
+        R = [np.empty(int(result[i].n_kept), dtype=np.float64) if ok[i] else None for i in range(n)]
+        log = (IterRecord * (n * it))()
+        T = np.zeros((n, 16))
+        self._check(self._lib.sicp_get_batch_outputs(
+            self._h, n, (C.c_void_p * n)(*[_ptr(x) for x in X]), (C.c_void_p * n)(*[_ptr(r) for r in R]), log,
+            T.ctypes.data_as(C.POINTER(C.c_double))))
+        return [(X[i], R[i], [log[i * it + j] for j in range(result[i].iterations)], T[i].reshape(4, 4))
+                if ok[i] else None for i in range(n)]
 
     @staticmethod
     def _observed_rows(observed, n: int):

@@ -112,8 +112,9 @@ def simpleicp_batch(
     on_error: str = "raise",
     batch_size: int = 64,
     engine: str = "batched",
+    full_output: bool = False,
     **run_kwargs,
-) -> np.ndarray:
+):
     """Register every pair; returns the (n_pairs, 20) record table on every rank.
 
     `pairs` is a sequence or a generator function i -> (X_fix, X_mov) (so that ranks only
@@ -144,12 +145,21 @@ def simpleicp_batch(
     status code; every rank still takes part in the collective.  Afterwards `on_error="raise"`
     raises BatchError (same on every rank, `.table` holds the full table, `.failed` the pair
     numbers), `on_error="nan"` just returns the table.
+
+    `full_output=True` returns `(table, results)` instead, with the same table.  `results[i]` is
+    what `register` returns for pair i -- `H`, `X_mov_transformed`, `rbp` with the estimated
+    uncertainties, `residuals`, `records`, `iterations`, `converged`; fields the batched engine
+    has no equivalent for are None -- and None for a pair that failed or belongs to another rank
+    (only the table is exchanged between ranks).  Pairs served per pair (`engine="pool"`, more
+    than 4096 correspondences, `register_fn`) give the objects `register` / `register_fn`
+    returned.  BatchError then carries `.results` too.
     """
     if n_pairs is None:
         n_pairs = len(pairs)  # type: ignore[arg-type]
     get = pairs if callable(pairs) else (lambda i: pairs[i])  # type: ignore[index]
     mine = shard_pairs(n_pairs, world_size, rank)
     local = np.zeros((len(mine), RECORD_LEN))
+    found: List = [None] * len(mine)  # full_output: the result object of each pair of the share
     rows = _per_pair_observed(run_kwargs, n_pairs)
     _check_mov_kwargs(run_kwargs)
 
@@ -160,9 +170,12 @@ def simpleicp_batch(
         last = res.records[res.iterations - 1]
         return pack_record(res.H, res.iterations, last["n_kept"], last["mean_res"], last["std_res"])
 
-    def guarded(fn, Xf, Xm, **kw):
+    def guarded(fn, j, Xf, Xm, **kw):
         try:
-            return record(fn(Xf, Xm, **kw))
+            res = fn(Xf, Xm, **kw)
+            if full_output:
+                found[j] = res
+            return record(res)
         except Exception as e:  # noqa: BLE001 — recorded per pair, reported after the gather
             code = getattr(getattr(e, "__cause__", None) or e, "code", None)
             msg = str(e)
@@ -175,9 +188,11 @@ def simpleicp_batch(
     if register_fn is not None:
         for j, i in enumerate(mine):
             Xf, Xm = get(i)
-            local[j] = guarded(register_fn, Xf, Xm, **kw_of(i))
+            local[j] = guarded(register_fn, j, Xf, Xm, **kw_of(i))
     elif engine == "batched" and _batchable(run_kwargs):
-        _run_batched(get, mine, local, device, batch_size, run_kwargs, messages, rows)
+        # results= only when asked for: the default call is unchanged
+        _run_batched(get, mine, local, device, batch_size, run_kwargs, messages, rows,
+                     **({"results": found} if full_output else {}))
     else:
         import threading
 
@@ -201,7 +216,7 @@ def simpleicp_batch(
                         if j is None:
                             break
                         Xf, Xm = get(mine[j])
-                        local[j] = guarded(register, Xf, Xm, engine=eng, **kw_of(mine[j]))
+                        local[j] = guarded(register, j, Xf, Xm, engine=eng, **kw_of(mine[j]))
             except Exception as e:  # surfaced after the join
                 errors.append(e)
 
@@ -220,10 +235,15 @@ def simpleicp_batch(
 
         dev = torch.device("cuda", device) if dist.get_backend() == "nccl" else torch.device("cpu")
     table = gather_records(local, n_pairs, world_size, rank, dist, dev)
+    results = None
+    if full_output:
+        results = [None] * n_pairs
+        for j, i in enumerate(mine):
+            results[i] = found[j]
     failed = np.flatnonzero(table[:, 16] < 0)
     if failed.size and on_error == "raise":
-        raise BatchError(table, failed, messages)
-    return table
+        raise BatchError(table, failed, messages, results)
+    return (table, results) if full_output else table
 
 
 _BATCH_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations",
@@ -273,10 +293,12 @@ def _per_pair_observed(kw, n_pairs: int):
 _BATCH_ENGINES: dict = {}
 
 
-def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None):
+def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None, results=None):
     """The rank's share `mine` through the batched engine, `batch_size` pairs per call, records into
     `local`.  With `map_engine` (an engine holding a map, sicp_set_map) get(i) is scan i alone and
-    every chunk is registered against that map (sicp_register_to_map)."""
+    every chunk is registered against that map (sicp_register_to_map).  With `results` (a list of
+    len(mine)) the full output of every pair that succeeded goes there too, fetched after each call
+    (sicp_get_batch_outputs) because the next one reuses the library's buffers."""
     import torch
 
     from . import _capi
@@ -315,6 +337,26 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, 
                 else:
                     messages.append(f"pair {mine[j]}: library status {r.status}")
                     local[j] = pack_record(np.full((4, 4), np.nan), -int(r.status), 0, np.nan, np.nan)
+            if results is not None:
+                for k, (j, r, o) in enumerate(zip(ids, res, eng.batch_outputs(res))):
+                    if o is not None:
+                        results[j] = _batch_result(r, o, obs if observed is None else observed[k], obs_w)
+
+
+def _batch_result(r, outputs, obs, rbp_observation_weights):
+    """register()'s result object for one pair of a batched call: its PairResult `r` and its
+    sicp_get_batch_outputs part `outputs`; `obs` is the pair's prior in radians."""
+    from .simpleicp import _make_rbp, _records, _Result
+
+    X_t, residuals, log, _ = outputs
+    records, iterations = _records(log), int(r.iterations)
+    res = _Result()
+    res.H = np.array(r.H).reshape(4, 4)
+    res.X_mov_transformed, res.residuals, res.records = X_t, residuals, records
+    res.rbp = _make_rbp(obs, rbp_observation_weights, records, iterations, np.array(r.x), np.array(r.sigma))
+    res.iterations, res.converged = iterations, bool(r.converged)
+    res.idx_selected = res.normals = res.timings = res.loop_ms = res.initial_stats = None
+    return res
 
 
 # run() arguments Map.register serves: those of the batched engine, without the debug output
@@ -345,14 +387,17 @@ class Map:
         self.n_points = self._engine.n_map
 
     def register(self, scans: Sequence[np.ndarray], *, batch_size: int = 64, on_error: str = "raise",
-                 **run_kwargs) -> np.ndarray:
+                 full_output: bool = False, **run_kwargs):
         """Register every scan against the map; returns the (n_scans, 20) record table of
         simpleicp_batch.  ``run_kwargs`` are SimpleICP.run's arguments the batched engine serves
         (at most 4096 correspondences); ``rbp_observed_values`` is the common 6-tuple or one row
         per scan (degrees), each scan's prior.  A scan that cannot be registered (no overlap with
         the map, too few correspondences) gets a NaN record whose ``iterations`` field is minus
         the library's status code; ``on_error="raise"`` then raises BatchError with the full
-        table, ``on_error="nan"`` returns it."""
+        table, ``on_error="nan"`` returns it.  ``full_output=True`` returns ``(table, results)``
+        as simpleicp_batch does: ``results[i]`` is register()'s result object for scan i
+        (``X_mov_transformed`` in the map's frame, residuals, records, uncertainties), None for
+        a scan that failed."""
         unknown = set(run_kwargs) - _MAP_KEYS
         if unknown:
             raise TypeError(f"Map.register() got unsupported arguments {sorted(unknown)}")
@@ -362,15 +407,16 @@ class Map:
         rows = _per_pair_observed(run_kwargs, n)
         _check_mov_kwargs(run_kwargs)
         local = np.zeros((n, RECORD_LEN))
+        results = [None] * n if full_output else None
         messages: List[str] = []
         # the survivor offsets of one call are 32-bit: scans per call x map points < 2^32
         per_call = max(1, min(int(batch_size), ((1 << 32) - 1) // max(self.n_points, 1)))
         _run_batched(lambda i: scans[i], list(range(n)), local, self.device, per_call, run_kwargs, messages, rows,
-                     map_engine=self._engine)
+                     map_engine=self._engine, **({"results": results} if full_output else {}))
         failed = np.flatnonzero(local[:, 16] < 0)
         if failed.size and on_error == "raise":
-            raise BatchError(local, failed, messages)
-        return local
+            raise BatchError(local, failed, messages, results)
+        return (local, results) if full_output else local
 
     def close(self) -> None:
         """Release the map and its engine."""
@@ -384,11 +430,12 @@ class Map:
 
 
 class BatchError(RuntimeError):
-    """Some pairs of a batch could not be registered; `.table` is the complete record table."""
+    """Some pairs of a batch could not be registered; `.table` is the complete record table,
+    `.results` the per-pair results of a `full_output=True` call (None otherwise)."""
 
-    def __init__(self, table, failed, messages):
+    def __init__(self, table, failed, messages, results=None):
         codes = sorted({int(-table[i, 16]) for i in failed})
         super().__init__(f"{len(failed)} of {len(table)} pairs failed (pairs {failed[:8].tolist()}"
                          f"{' ...' if len(failed) > 8 else ''}, status codes {codes})"
                          + (f"; first local message: {messages[0]}" if messages else ""))
-        self.table, self.failed, self.messages = table, failed, messages
+        self.table, self.failed, self.messages, self.results = table, failed, messages, results

@@ -26,7 +26,11 @@
 // sicp_register_to_map runs the same stages (run_pairs) for scans against a map held on the
 // context (sicp_set_map, MapStore): the fixed side is the map's grid, and the overlap filter only
 // searches the map points inside each scan's box mapped by its prior (map_cull_box, map_filter).
+//
+// sicp_get_batch_outputs returns what either call left on the device and did not download:
+// transformed clouds, residual vectors, the per-iteration log and the applied transforms.
 #include <algorithm>
+#include <cstddef>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -436,12 +440,115 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
     if (r.no_overlap[(size_t)i]) out[i].status = SICP_ERR_NO_OVERLAP;
     if (n_selected) n_selected[i] = r.pd[(size_t)i].K;
   }
+  // what sicp_get_batch_outputs needs of this call (host bookkeeping only)
+  b.out_n_pairs = n_pairs;
+  b.out_max_iterations = p.max_iterations;
+  b.out_mo = r.mo;
+  b.out_n_kept.resize((size_t)n_pairs);
+  b.out_status.resize((size_t)n_pairs);
+  b.out_iterations.resize((size_t)n_pairs);
+  b.out_mean_std.resize(2 * (size_t)n_pairs);
+  for (int i = 0; i < n_pairs; ++i) {
+    b.out_n_kept[(size_t)i] = out[i].n_kept;
+    b.out_status[(size_t)i] = out[i].status;
+    b.out_iterations[(size_t)i] = out[i].iterations;
+    b.out_mean_std[2 * (size_t)i] = out[i].mean_res;
+    b.out_mean_std[2 * (size_t)i + 1] = out[i].std_res;
+  }
+  b.out_valid = true;
+}
+
+// sicp_get_batch_outputs: everything is read from the buffers the last run_pairs left behind.
+// One launch transforms the requested clouds, one compacts the requested residual vectors, one
+// copy brings the log and one the transforms; each requested pair's slice then goes to the
+// caller's memory with its own copy (any memory kind, any alignment).
+static void get_batch_outputs(Ctx& c, int n_pairs, double* const* mov_xyz_out, double* const* residuals,
+                              sicp_iter_record* log, double* T) {
+  SICP_REQUIRE(c.batch && c.batch->out_valid, SICP_ERR_STATE,
+               "no batch outputs: no sicp_register_batch / sicp_register_to_map has succeeded since the last "
+               "sicp_set_map");
+  Batch& b = *c.batch;
+  SICP_REQUIRE(n_pairs == b.out_n_pairs, SICP_ERR_BAD_ARG,
+               "n_pairs must equal the last batched call's (" + std::to_string(b.out_n_pairs) + ")");
+  cudaStream_t st = c.stream;
+  const int n = n_pairs;
+  const auto ok = [&](int i) { return b.out_status[(size_t)i] == SICP_OK; };
+  const auto n_mov = [&](int i) { return b.out_mo[(size_t)i + 1] - b.out_mo[(size_t)i]; };
+  // requested pairs: transforms first, then residual vectors (with their output offsets)
+  std::vector<int> ids;
+  std::vector<long long> off;
+  long long max_n_mov = 0, n_res = 0;
+  if (mov_xyz_out)
+    for (int i = 0; i < n; ++i)
+      if (ok(i) && mov_xyz_out[i]) {
+        ids.push_back(i);
+        max_n_mov = std::max(max_n_mov, n_mov(i));
+      }
+  const int n_xyz = (int)ids.size();
+  if (residuals)
+    for (int i = 0; i < n; ++i)
+      if (ok(i) && residuals[i] && b.out_n_kept[(size_t)i] > 0) {
+        ids.push_back(i);
+        off.push_back(n_res);
+        n_res += b.out_n_kept[(size_t)i];
+      }
+  const int n_rv = (int)ids.size() - n_xyz;
+  if (!ids.empty()) {
+    b.out_ids.reserve(ids.size());
+    SICP_CUDA(cudaMemcpyAsync(b.out_ids.p, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, st));
+  }
+  if (n_xyz > 0) {
+    b.xyz_out.reserve(3 * (size_t)b.out_mo[(size_t)n]);
+    batch_transform_launch(c, b, b.out_ids.p, n_xyz, max_n_mov, b.xyz_out.p);
+    for (int j = 0; j < n_xyz; ++j) {
+      const int i = ids[(size_t)j];
+      copy_any(c, mov_xyz_out[i], b.xyz_out.p + 3 * b.out_mo[(size_t)i], sizeof(double) * 3 * (size_t)n_mov(i));
+    }
+  }
+  if (n_rv > 0) {
+    b.out_off.reserve(off.size());
+    b.resid_out.reserve((size_t)n_res);
+    SICP_CUDA(cudaMemcpyAsync(b.out_off.p, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice, st));
+    batch_residuals_launch(c, b, b.out_ids.p + n_xyz, n_rv, b.out_off.p, b.resid_out.p);
+    for (int j = 0; j < n_rv; ++j) {
+      const int i = ids[(size_t)(n_xyz + j)];
+      copy_any(c, residuals[i], b.resid_out.p + off[(size_t)j], sizeof(double) * (size_t)b.out_n_kept[(size_t)i]);
+    }
+  }
+  const size_t it_max = (size_t)b.out_max_iterations;
+  if (log) {
+    pinned_reserve(b.rec_host, b.rec_cap, (size_t)n * it_max);
+    SICP_CUDA(cudaMemcpyAsync(b.rec_host, b.rec.p, sizeof(sicp_iter_record) * (size_t)n * it_max,
+                              cudaMemcpyDeviceToHost, st));
+  }
+  if (T) {
+    pinned_reserve(b.T_host, b.T_cap, (size_t)n);
+    SICP_CUDA(cudaMemcpy2DAsync(b.T_host, sizeof(Rigid), reinterpret_cast<const char*>(b.state.p) + offsetof(DevState, T),
+                                sizeof(DevState), sizeof(Rigid), (size_t)n, cudaMemcpyDeviceToHost, st));
+  }
+  SICP_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) {
+    if (!ok(i)) continue;
+    if (log) {
+      const size_t done = std::min<size_t>((size_t)b.out_iterations[(size_t)i], it_max);
+      sicp_iter_record* dst = log + (size_t)i * it_max;
+      std::memcpy(dst, b.rec_host + (size_t)i * it_max, sizeof(sicp_iter_record) * done);
+      std::memset(dst + done, 0, sizeof(sicp_iter_record) * (it_max - done));
+      // the last row carries the exact two-pass statistics, as sicp_register's log does
+      if (done > 0) {
+        dst[done - 1].mean_res = b.out_mean_std[2 * (size_t)i];
+        dst[done - 1].std_res = b.out_mean_std[2 * (size_t)i + 1];
+      }
+    }
+    if (T) H_from_rigid(b.T_host[i], T + 16 * (size_t)i);
+  }
 }
 
 static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, const int64_t* n_fix,
                            const double* const* mov_xyz, const int64_t* n_mov,
                            const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
                            int64_t* n_selected) {
+  if (c.batch) c.batch->out_valid = false;
   check_pairs_params(c, n_pairs, fix_xyz && n_fix && mov_xyz && n_mov && out, rp);
   PairsRun r;
   begin_pairs(r, n_pairs, rp, observed);
@@ -493,6 +600,7 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
 }
 
 static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
+  if (c.batch) c.batch->out_valid = false;
   if (map_xyz == nullptr || n_map == 0) {
     delete c.map;
     c.map = nullptr;
@@ -523,6 +631,7 @@ static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
 static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, const int64_t* n_mov,
                             const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
                             int64_t* n_selected) {
+  if (c.batch) c.batch->out_valid = false;
   check_pairs_params(c, n_scans, mov_xyz && n_mov && out, rp);
   SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
   MapStore& m = *c.map;
@@ -595,4 +704,9 @@ extern "C" int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const do
                                         const int64_t* n_mov, const sicp_register_params* p,
                                         const double* observed, sicp_pair_result* out, int64_t* n_selected) {
   SICP_BATCH_API(register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected))
+}
+
+extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double* const* mov_xyz_out,
+                                          double* const* residuals, sicp_iter_record* log, double* T) {
+  SICP_BATCH_API(get_batch_outputs(c, n_pairs, mov_xyz_out, residuals, log, T))
 }

@@ -36,6 +36,11 @@ void check_mov_neighbors(const Ctx& c, const sicp_register_params& rp) {
                "max_angle_rad must be <= pi/2 (normals are axes), or negative for no angle test");
 }
 
+void copy_any(Ctx& c, void* dst, const void* src, size_t bytes) {
+  if (bytes == 0) return;
+  SICP_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, c.stream));
+}
+
 namespace {
 
 constexpr int kMaxRecords = 4096;
@@ -92,11 +97,6 @@ __global__ void k_join_f4(const float* __restrict__ in, long long K, float4* __r
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= K) return;
   out[i] = make_float4(in[i], in[K + i], in[2 * K + i], in[3 * K + i]);
-}
-
-void copy_any(Ctx& c, void* dst, const void* src, size_t bytes) {
-  if (bytes == 0) return;
-  SICP_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, c.stream));
 }
 
 void sync(Ctx& c) { SICP_CUDA(cudaStreamSynchronize(c.stream)); }

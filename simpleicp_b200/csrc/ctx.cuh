@@ -237,10 +237,29 @@ struct Batch {
   size_t flags_cap = 0, results_cap = 0;
   unsigned long long* keys_host = nullptr;   // pinned: bounding boxes / occupancies
   size_t keys_cap = 0;
+  // What sicp_get_batch_outputs reads of the last sicp_register_batch / sicp_register_to_map.
+  // out_valid is cleared on entry of those two calls and of sicp_set_map, and set only when one of
+  // the two returns successfully; the vectors are per pair of that call.
+  bool out_valid = false;
+  int out_n_pairs = 0, out_max_iterations = 0;
+  std::vector<long long> out_mo, out_n_kept;  // movable point offsets (n_pairs + 1), kept residuals
+  std::vector<int> out_status, out_iterations; // sicp_status (SICP_ERR_NO_OVERLAP included), iterations run
+  std::vector<double> out_mean_std;            // exact mean / std of the final residuals, 2 per pair
+  // buffers of sicp_get_batch_outputs: transformed clouds (total_mov points, the offsets of
+  // mov_xyz), compacted residuals, the ids and residual offsets of the requested pairs
+  DevBuf<double> xyz_out, resid_out;
+  DevBuf<int> out_ids;
+  DevBuf<long long> out_off;
+  sicp_iter_record* rec_host = nullptr;      // pinned: the downloaded log
+  size_t rec_cap = 0;
+  Rigid* T_host = nullptr;                   // pinned: DevState::T of every pair
+  size_t T_cap = 0;
   ~Batch() {
     if (flags_host) cudaFreeHost(flags_host);
     if (results_host) cudaFreeHost(results_host);
     if (keys_host) cudaFreeHost(keys_host);
+    if (rec_host) cudaFreeHost(rec_host);
+    if (T_host) cudaFreeHost(T_host);
   }
 };
 
@@ -350,12 +369,19 @@ void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, lo
                              const uint32_t* scan, uint32_t* list);
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
+// sicp_get_batch_outputs, for the n_ids pairs ids (device) of the last batched run: the movable
+// clouds moved by DevState::T into out at their Batch::mov_xyz offsets, and the final residuals
+// in kept order into out + off[j] (device)
+void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, long long max_n_mov, double* out);
+void batch_residuals_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const long long* off, double* out);
 
 int bin_cap_for(long long K);
 
 // helpers in capi.cu
 // device ordinal of device (or managed) memory, -1 for host memory
 int device_of_ptr(const void* p);
+// bytes between any two of host, device and other-device memory, on the context's stream
+void copy_any(Ctx& c, void* dst, const void* src, size_t bytes);
 // queries per launch of a chunked k-NN + PCA: c.normals_scratch_mb MiB of k record positions each
 inline long long normals_chunk_queries(const Ctx& c, int k) {
   return std::max<long long>(1024, ((long long)c.normals_scratch_mb << 20) / (4ll * k));

@@ -1906,6 +1906,19 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_rs_batch(BatchRsArgs b) {
   rs_fused_body<RSF_SINGLE>(a, wk, 1, 0, *reinterpret_cast<SharedF*>(rsf_smem));
 }
 
+// Residual of query i at the final transform Tn, in the reference's operation order
+// (optimization.py:117-124): the matched movable point moved by Tn, minus the fixed point, dotted
+// with the fixed normal.  The only definition: k_finish_batch takes its statistics from it,
+// k_final_residuals and k_batch_residuals return it.
+__device__ __forceinline__ double final_residual(const Rigid& Tn, const double* m_xyz, const double* q_xyz,
+                                                 const float4* q_nrm, long long i) {
+  double tx, ty, tz;
+  rigid_apply(Tn, m_xyz[3 * i + 0], m_xyz[3 * i + 1], m_xyz[3 * i + 2], tx, ty, tz);
+  const float4 nr = q_nrm[i];
+  const double dx = tx - q_xyz[3 * i + 0], dy = ty - q_xyz[3 * i + 1], dz = tz - q_xyz[3 * i + 2];
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)), __dmul_rn(dz, (double)nr.z));
+}
+
 // End of a batched run, one block per pair: residuals of the kept correspondences at the final
 // transform (reference operation order), their exact two-pass mean / std, and the result record.
 __global__ void __launch_bounds__(256)
@@ -1922,13 +1935,7 @@ __global__ void __launch_bounds__(256)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const Rigid Tn = st.T_res;
   const bool have = st.iterations_done > 0;
-  auto resid_of = [&](long long i) {
-    double tx, ty, tz;
-    rigid_apply(Tn, m_xyz[3 * (q + i) + 0], m_xyz[3 * (q + i) + 1], m_xyz[3 * (q + i) + 2], tx, ty, tz);
-    const float4 nr = q_nrm[q + i];
-    const double dx = tx - q_xyz[3 * (q + i) + 0], dy = ty - q_xyz[3 * (q + i) + 1], dz = tz - q_xyz[3 * (q + i) + 2];
-    return __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)), __dmul_rn(dz, (double)nr.z));
-  };
+  auto resid_of = [&](long long i) { return final_residual(Tn, m_xyz, q_xyz, q_nrm, q + i); };
   double acc = 0.0, cnt = 0.0;
   if (have)
     for (long long i = threadIdx.x; i < K; i += 256)
@@ -2001,12 +2008,43 @@ __global__ void __launch_bounds__(256)
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= K || !keep[i]) return;
   const Rigid Tn = st->T_res;
-  double tx, ty, tz;
-  rigid_apply(Tn, m_xyz[3 * i + 0], m_xyz[3 * i + 1], m_xyz[3 * i + 2], tx, ty, tz);
-  const float4 nr = q_nrm[i];
-  const double dx = tx - q_xyz[3 * i + 0], dy = ty - q_xyz[3 * i + 1], dz = tz - q_xyz[3 * i + 2];
-  resid[i] = __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)),
-                       __dmul_rn(dz, (double)nr.z));
+  resid[i] = final_residual(Tn, m_xyz, q_xyz, q_nrm, i);
+}
+
+// sicp_get_batch_outputs: the final residual vector of every listed pair in kept order, one block
+// per pair.  K <= 4096, so the block walks the keep flags in slices of 256 and scans each one
+// (ballot within a warp, warp totals through shared memory): an ordered compaction.  Pair ids[j]
+// writes out[off[j] ..], at most its n_kept values.
+__global__ void __launch_bounds__(256)
+    k_batch_residuals(const PairDev* __restrict__ pairs, const DevState* __restrict__ state,
+                      const uint8_t* __restrict__ keep, const double* __restrict__ m_xyz,
+                      const double* __restrict__ q_xyz, const float4* __restrict__ q_nrm,
+                      const int* __restrict__ ids, const long long* __restrict__ off, double* __restrict__ out) {
+  const int pair = ids[blockIdx.x];
+  const PairDev& pd = pairs[pair];
+  const DevState& st = state[pair];
+  const long long q = pd.q_off, K = pd.K, cap = st.n_kept;
+  double* dst = out + off[blockIdx.x];
+  __shared__ int warp_n[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const Rigid Tn = st.T_res;
+  long long base = 0;  // kept entries before this slice
+  for (long long s = 0; s < K; s += 256) {
+    const long long i = s + threadIdx.x;
+    const bool k = i < K && keep[q + i];
+    const unsigned int m = __ballot_sync(0xffffffffu, k);
+    if (lane == 0) warp_n[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < 8; ++w) {
+      before += (w < warp) ? warp_n[w] : 0;
+      total += warp_n[w];
+    }
+    const long long pos = base + before + __popc(m & ((1u << lane) - 1u));
+    if (k && pos < cap) dst[pos] = final_residual(Tn, m_xyz, q_xyz, q_nrm, q + i);
+    base += total;
+    __syncthreads();
+  }
 }
 
 // Exact statistics of the compacted residuals: mean first, then the squared deviations from it
@@ -2317,6 +2355,14 @@ void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool wa
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations) {
   k_finish_batch<<<b.n_pairs, 256, 0, c.stream>>>(b.pairs.p, b.state.p, b.keep.p, b.m_xyz.p, b.q_xyz.p, b.q_nrm.p,
                                                   c.variant, max_iterations, b.results.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void batch_residuals_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const long long* off, double* out) {
+  // the fixed normals, as k_finish_batch
+  k_batch_residuals<<<n_ids, 256, 0, c.stream>>>(b.pairs.p, b.state.p, b.keep.p, b.m_xyz.p, b.q_xyz.p, b.q_nrm.p,
+                                                 ids, off, out);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
