@@ -326,6 +326,38 @@ int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const
                              sicp_pair_result* out /*[h] n_scans*/,
                              int64_t* n_selected /*[h] n_scans or NULL*/);
 
+/* ---- growing the map and reading it back -------------------------------------------------------
+ * sicp_map_insert appends to the map, for every voxel of size voxel_size it does not occupy, the
+ * first new point that falls into it.  C is the concatenation of the n_clouds clouds in call
+ * order, cloud i moved by H[16 i .. 16 i + 15] (row-major 4 x 4, bit for bit what sicp_transform
+ * gives for that cloud and H) or, with H NULL, taken as it is.  key(p) = (floor(p.x / v),
+ * floor(p.y / v), floor(p.z / v)) in IEEE double with a real division, compared as doubles.
+ * Point C[j] is added iff its three coordinates are finite (NaN / inf points are skipped), no map
+ * point has its key and no finite C[j'] with j' < j has its key.  The new map is the old one, in
+ * its order, followed by the added points in ascending j; nothing is removed or moved.  The map's
+ * grid is rebuilt by sicp_set_map's builder, so the grown map registers exactly as a fresh
+ * sicp_set_map of the same points.  n_added[i] (if not NULL) = the points cloud i added.
+ *  - SICP_ERR_STATE: no map.  SICP_ERR_BAD_ARG, before any device work: n_clouds < 1, a negative
+ *    n[i], a NULL xyz[i] with n[i] > 0 (empty clouds add nothing), a non-finite H entry, a
+ *    voxel_size that is not finite and > 0, or n_map + sum n[i] >= 2^32.
+ *  - The map is replaced only when the new one is complete: after an error it is unchanged.
+ *    Device memory peaks at about two maps plus the staged clouds; the staging buffers (about
+ *    100 bytes per point of the largest insert) stay on the context for the next insert.
+ *  - The grid builder of sicp_set_map needs finite bounding-box extents, of the finite new points
+ *    and of the grown map: points whose coordinates on one axis are more than DBL_MAX apart
+ *    (e.g. near +1e308 and -1e308) are refused with SICP_ERR_BAD_ARG ("point cloud contains
+ *    non-finite coordinates") after the upload, and the map is unchanged.
+ *  - Clears the batch outputs, as sicp_set_map does.
+ *  - Each new point walks the map-grid cells its voxel covers: about (v / h + 2)^3 of them for a
+ *    map cell size h, so a voxel far larger than the map's cells costs accordingly.
+ * sicp_get_map sets *n to the map's size and copies min(*n, cap) points, in map order, into xyz
+ * (none when xyz is NULL).  SICP_ERR_STATE: no map.                                              */
+int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                        const int64_t* n /*[h]*/, const double* H /*[h] n_clouds x 16, or NULL*/,
+                        double voxel_size, int64_t* n_added /*[h] n_clouds, or NULL*/);
+int32_t sicp_get_map(sicp_ctx* ctx, double* xyz /*[h|d] cap x 3, or NULL*/, int64_t cap,
+                     int64_t* n /*[h]*/);
+
 /* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
  * sicp_register_batch and sicp_register_to_map report per pair only the record above.  This call
  * returns what else sicp_register returns, for every pair of the LAST successful call of either
@@ -333,10 +365,11 @@ int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const
  * simpleicp.py:316), the final distance residuals (simpleicp.py:324, 4th return value), the
  * per-iteration records and the applied transform.  Those two calls only leave these on the
  * device; all the work happens here, and they stay readable (any number of times, same bits)
- * until the next sicp_register_batch, sicp_register_to_map or sicp_set_map on the context.
- *  - SICP_ERR_STATE: before any such call, after sicp_set_map, or after a batch / map call that
- *    returned an error (each of the three clears the outputs on entry; only a successful return
- *    of the first two makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
+ * until the next sicp_register_batch, sicp_register_to_map, sicp_set_map or sicp_map_insert on the
+ * context.
+ *  - SICP_ERR_STATE: before any such call, after sicp_set_map or sicp_map_insert, or after a
+ *    batch / map call that returned an error (each of the four clears the outputs on entry; only a
+ *    successful return of the first two makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
  *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose
  *    status was not SICP_OK (SICP_ERR_NO_OVERLAP included) is ever written.
  *  - mov_xyz_out[i]: pair i's movable cloud (n_mov[i] x 3) moved by the transform the run applied,

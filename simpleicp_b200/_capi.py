@@ -41,7 +41,8 @@ SYMBOLS = (
     "sicp_set_normals", "sicp_set_mov_normals", "sicp_get_knn", "sicp_match", "sicp_reject", "sicp_solve",
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
-    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs",
+    "sicp_map_insert", "sicp_get_map", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -167,6 +168,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_register_to_map": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(RegisterParams), vp,
                                  C.POINTER(PairResult), vp],
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
+        "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
+        "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -575,6 +578,32 @@ class Engine:
         out.n_selected = n_selected
         out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
         return out
+
+    def map_insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
+        """sicp_map_insert: append to the resident map, per voxel of `voxel_size` it does not
+        occupy, the first finite point of `clouds` (in order) falling into it, cloud i moved by
+        H[i] first when `H` (n_clouds x 4 x 4) is given.  Returns the points each cloud added
+        (int64)."""
+        n = len(clouds)
+        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
+        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
+        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
+        if H is not None:
+            H = np.ascontiguousarray(H, dtype=np.float64)
+            if H.shape != (n, 4, 4):
+                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
+        added = np.zeros(n, dtype=np.int64)
+        self._check(self._lib.sicp_map_insert(self._h, n, ptrs, counts, _ptr(H), float(voxel_size), _ptr(added)))
+        self.n_map += int(added.sum())
+        return added
+
+    def get_map(self) -> np.ndarray:
+        """sicp_get_map: the resident map, (n_map, 3) float64 in map order."""
+        n = C.c_int64(0)
+        self._check(self._lib.sicp_get_map(self._h, None, 0, C.byref(n)))
+        X = np.empty((int(n.value), 3), dtype=np.float64)
+        self._check(self._lib.sicp_get_map(self._h, _ptr(X), X.shape[0], C.byref(n)))
+        return X
 
     def batch_outputs(self, result):
         """sicp_get_batch_outputs for `result`, the PairResult array the last register_batch /

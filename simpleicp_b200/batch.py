@@ -373,6 +373,8 @@ class Map:
     points near each scan (under its prior), so the work per scan grows with its footprint, not
     with the map.  Scan i's result is that of
     ``register(X_map, scans[i], rbp_observed_values=row_i, max_overlap_distance=d, ...)``.
+    ``insert(clouds, H, voxel_size=v)`` grows the map on the device by what the scans saw (one
+    new point per voxel the map does not occupy) and ``points()`` reads it back.
     """
 
     def __init__(self, X_map, device: int = 0):
@@ -417,6 +419,47 @@ class Map:
         if failed.size and on_error == "raise":
             raise BatchError(local, failed, messages, results)
         return (local, results) if full_output else local
+
+    def insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
+        """Grow the map on the device: for every voxel of edge ``voxel_size`` the map does not
+        occupy, append the first new point that falls into it (sicp_map_insert).
+
+        ``clouds`` is a sequence of (n_i, 3) NumPy arrays or CUDA tensors, taken in order; ``H``
+        is None or an (n_clouds, 4, 4) array moving cloud i into the map's frame first, e.g.
+        ``table[:, :16].reshape(-1, 4, 4)`` of the scans ``register`` registered.  A voxel is the
+        key floor(p / voxel_size) per axis; points with a NaN or inf coordinate are skipped.  The
+        map keeps its points and order and gets the added ones at its end, and registers as
+        ``Map(points)`` of the same points would.  Returns the number of points each cloud added
+        (int64)."""
+        v = float(voxel_size)
+        if not (np.isfinite(v) and v > 0):
+            raise ValueError(f"voxel_size must be finite and > 0, got {voxel_size}")
+        clouds = list(clouds)
+        if not clouds:
+            raise ValueError("insert needs at least one cloud")
+        for i, X in enumerate(clouds):
+            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
+                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
+        if H is not None:
+            H = np.asarray(H, dtype=np.float64)
+            if H.shape != (len(clouds), 4, 4):
+                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
+            if not np.isfinite(H).all():
+                raise ValueError("H must be finite")
+        import torch
+
+        with torch.cuda.device(self.device):
+            added = self._engine.map_insert(clouds, H, voxel_size=v)
+        self.n_points = self._engine.n_map
+        return added
+
+    def points(self) -> np.ndarray:
+        """The map as it stands, (n_points, 3) float64 in map order (a copy): the points it was
+        made of followed by those ``insert`` added.  ``sb.write_xyz(path, m.points())`` saves it."""
+        import torch
+
+        with torch.cuda.device(self.device):
+            return self._engine.get_map()
 
     def close(self) -> None:
         """Release the map and its engine."""

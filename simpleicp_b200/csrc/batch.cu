@@ -68,6 +68,71 @@ __global__ void k_overlap_bounds(const PairDev* __restrict__ pairs, int n_pairs,
   if (i <= n_pairs) bounds[i] = scan[i < n_pairs ? pairs[i].fix_off : total];
 }
 
+// sicp_map_insert, one thread per point j of the concatenated clouds (cloud i owns [off[i],
+// off[i + 1])): the point moved by its cloud's transform when there are transforms (T != NULL;
+// rigid_apply as k_transform, in place, scalar accesses since clouds start at any point offset),
+// and fin[j] = all three coordinates finite.
+__global__ void __launch_bounds__(256)
+    k_insert_stage(double* __restrict__ xyz, long long n, const uint32_t* __restrict__ off, int n_clouds,
+                   const Rigid* __restrict__ T, uint32_t* __restrict__ fin) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  double x = xyz[3 * j + 0], y = xyz[3 * j + 1], z = xyz[3 * j + 2];
+  if (T) {
+    int lo = 0, hi = n_clouds;  // off[lo] <= j < off[hi]: the last cloud starting at or before j
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (off[mid] <= (unsigned long long)j) lo = mid;
+      else hi = mid;
+    }
+    double ox, oy, oz;
+    rigid_apply(T[lo], x, y, z, ox, oy, oz);
+    xyz[3 * j + 0] = x = ox;
+    xyz[3 * j + 1] = y = oy;
+    xyz[3 * j + 2] = z = oz;
+  }
+  fin[j] = (isfinite(x) && isfinite(y) && isfinite(z)) ? 1u : 0u;
+}
+
+// the finite points in ascending j (scan = exclusive prefix sum of fin) with their j
+__global__ void __launch_bounds__(256)
+    k_insert_compact(const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ fin,
+                     const uint32_t* __restrict__ scan, double* __restrict__ fin_xyz, uint32_t* __restrict__ fin_idx) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n || !fin[j]) return;
+  const long long f = scan[j];
+  fin_xyz[3 * f + 0] = xyz[3 * j + 0];
+  fin_xyz[3 * f + 1] = xyz[3 * j + 1];
+  fin_xyz[3 * f + 2] = xyz[3 * j + 2];
+  fin_idx[f] = (uint32_t)j;
+}
+
+// the added points in ascending j, written after the map's points (out = the new map + 3 n_map)
+__global__ void __launch_bounds__(256)
+    k_insert_scatter(const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ flag,
+                     const uint32_t* __restrict__ scan, double* __restrict__ out) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n || !flag[j]) return;
+  const long long o = scan[j];
+  out[3 * o + 0] = xyz[3 * j + 0];
+  out[3 * o + 1] = xyz[3 * j + 1];
+  out[3 * o + 2] = xyz[3 * j + 2];
+}
+
+// bounds[i] = S[off[i]] for i <= n_clouds (off[n_clouds] = n, S[n] = the total): cloud i added
+// bounds[i + 1] - bounds[i] points
+__global__ void k_insert_bounds(const uint32_t* __restrict__ off, int n_clouds, const uint32_t* __restrict__ scan,
+                                uint32_t* __restrict__ bounds) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i <= n_clouds) bounds[i] = scan[off[i]];
+}
+
+template <typename T>
+void swap_buf(DevBuf<T>& a, DevBuf<T>& b) {
+  std::swap(a.p, b.p);
+  std::swap(a.cap, b.cap);
+}
+
 template <typename T>
 void pinned_reserve(T*& p, size_t& cap, size_t n) {
   if (n <= cap) return;
@@ -662,6 +727,132 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
   run_pairs(c, b, r, m.xyz.p, &m, m.n, out, n_selected);
 }
 
+// sicp_map_insert.  The clouds are staged into one buffer and moved there; their finite points
+// are compacted in order and gridded as one cloud; k_map_insert_flags flags the points to add (a
+// voxel key no map point has, first of its key among the new points); one scan + an ordered
+// scatter append them after the map's points in a fresh buffer, which gets its grid from set_map's
+// grid_build_batch call.  Only then are the two swapped in, so a failure leaves the map as it was,
+// and the grown map is the one set_map would make of the same points.  Peak device memory: the
+// old and the new map (coordinates and grid) plus the staged clouds.
+static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
+                       double voxel, int64_t* n_added) {
+  if (c.batch) c.batch->out_valid = false;
+  SICP_REQUIRE(n_clouds >= 1, SICP_ERR_BAD_ARG, "n_clouds must be >= 1");
+  SICP_REQUIRE(xyz && n, SICP_ERR_BAD_ARG, "NULL argument");
+  SICP_REQUIRE(std::isfinite(voxel) && voxel > 0, SICP_ERR_BAD_ARG, "voxel_size must be finite and > 0");
+  constexpr long long kMany = 1ll << 40;  // saturation of the point count (the limit below is 2^32)
+  std::vector<long long> off((size_t)n_clouds + 1, 0);
+  for (int i = 0; i < n_clouds; ++i) {
+    SICP_REQUIRE(n[i] >= 0, SICP_ERR_BAD_ARG, "cloud " + std::to_string(i) + " has a negative point count");
+    SICP_REQUIRE(n[i] == 0 || xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
+    off[(size_t)i + 1] = std::min<long long>(off[(size_t)i] + std::min<long long>(n[i], kMany), kMany);
+  }
+  if (H)
+    for (int j = 0; j < 16 * n_clouds; ++j)
+      SICP_REQUIRE(std::isfinite(H[j]), SICP_ERR_BAD_ARG, "H has non-finite entries");
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  const long long nt = off[(size_t)n_clouds];
+  SICP_REQUIRE(m.n + nt < (1ll << 32), SICP_ERR_BAD_ARG,
+               "n_map + the points of the clouds must be below 2^32 (the limit of sicp_set_map)");
+  if (n_added) std::fill(n_added, n_added + n_clouds, 0);
+  if (nt == 0) return;
+  if (!c.batch) c.batch = new Batch();
+  Batch& b = *c.batch;
+  cudaStream_t st = c.stream;
+
+  // ---- stage and move the clouds, flag and compact their finite points
+  m.ins_xyz.reserve(3 * (size_t)nt);
+  for (int i = 0; i < n_clouds; ++i)
+    if (n[i] > 0) upload_to_device(c, m.ins_xyz.p + 3 * off[(size_t)i], xyz[i], sizeof(double) * 3 * (size_t)n[i]);
+  const std::vector<uint32_t> off32(off.begin(), off.end());
+  m.ins_off.reserve((size_t)n_clouds + 1);
+  SICP_CUDA(cudaMemcpyAsync(m.ins_off.p, off32.data(), sizeof(uint32_t) * off32.size(), cudaMemcpyHostToDevice, st));
+  const Rigid* T = nullptr;
+  if (H) {
+    std::vector<Rigid> hT((size_t)n_clouds);
+    for (int i = 0; i < n_clouds; ++i) hT[(size_t)i] = rigid_from_H(H + 16 * (size_t)i);  // as sicp_transform
+    m.ins_T.reserve((size_t)n_clouds);
+    SICP_CUDA(cudaMemcpyAsync(m.ins_T.p, hT.data(), sizeof(Rigid) * hT.size(), cudaMemcpyHostToDevice, st));
+    T = m.ins_T.p;
+  }
+  const unsigned blocks = (unsigned)((nt + 255) / 256);
+  m.fin_flag.reserve((size_t)nt);
+  m.fin_scan.reserve((size_t)nt + 1);
+  k_insert_stage<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T, m.fin_flag.p);
+  c.tm.kernel_launches += 1;
+  c.misc_counters.reserve(64);
+  scan_u32(c, m.fin_flag.p, nt, m.fin_scan.p, m.sums, c.misc_counters.p + 16);  // (its count is not used)
+  pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
+  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.fin_scan.p + nt, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  const long long n_fin = m.bounds_host[0];
+  if (n_fin == 0) return;  // nothing finite, nothing added
+  m.fin_xyz.reserve(3 * (size_t)n_fin);
+  m.fin_idx.reserve((size_t)n_fin);
+  k_insert_compact<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.fin_flag.p, m.fin_scan.p, m.fin_xyz.p, m.fin_idx.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+
+  // ---- the points to add, and how many per cloud (one read-back)
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  grid_build_batch(c, b, m.gnew, {BatchHostCloud{m.fin_xyz.p, n_fin, 0}}, views, centres);
+  m.ins_flag.reserve((size_t)nt);
+  m.ins_scan.reserve((size_t)nt + 1);
+  SICP_CUDA(cudaMemsetAsync(m.ins_flag.p, 0, sizeof(uint32_t) * (size_t)nt, st));
+  map_insert_flags_launch(c, m.view, views[0], m.fin_xyz.p, m.fin_idx.p, n_fin, voxel, m.ins_flag.p);
+  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums, c.misc_counters.p + 16);
+  m.ins_bounds.reserve((size_t)n_clouds + 1);
+  k_insert_bounds<<<(n_clouds + 256) / 256, 256, 0, st>>>(m.ins_off.p, n_clouds, m.ins_scan.p, m.ins_bounds.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_bounds.p, sizeof(uint32_t) * ((size_t)n_clouds + 1),
+                            cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  const long long added = m.bounds_host[n_clouds];
+  if (added > 0) {
+    // ---- the grown map in fresh buffers, then swapped in (DevBuf::reserve drops what it held)
+    const long long n_new = m.n + added;
+    m.xyz_next.reserve(3 * (size_t)n_new);
+    SICP_CUDA(cudaMemcpyAsync(m.xyz_next.p, m.xyz.p, sizeof(double) * 3 * (size_t)m.n, cudaMemcpyDeviceToDevice, st));
+    k_insert_scatter<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p + 3 * m.n);
+    SICP_CUDA(cudaGetLastError());
+    c.tm.kernel_launches += 1;
+    grid_build_batch(c, b, m.grid_next, {BatchHostCloud{m.xyz_next.p, n_new, 0}}, views, centres);  // as set_map
+    SICP_CUDA(cudaStreamSynchronize(st));
+    swap_buf(m.xyz, m.xyz_next);
+    swap_buf(m.grid.recs, m.grid_next.recs);
+    swap_buf(m.grid.cell_table, m.grid_next.cell_table);
+    swap_buf(m.grid.fill, m.grid_next.fill);
+    swap_buf(m.grid.cid, m.grid_next.cid);
+    swap_buf(m.grid.block_sums, m.grid_next.block_sums);
+    m.view = views[0];
+    m.n = n_new;
+    // the old map's buffers: one map stays resident between inserts
+    m.xyz_next.release();
+    m.grid_next.recs.release();
+    m.grid_next.cell_table.release();
+    m.grid_next.fill.release();
+    m.grid_next.cid.release();
+    m.grid_next.block_sums.release();
+  }
+  if (n_added)
+    for (int i = 0; i < n_clouds; ++i) n_added[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];
+}
+
+static void get_map(Ctx& c, double* xyz, int64_t cap, int64_t* n) {
+  SICP_REQUIRE(n, SICP_ERR_BAD_ARG, "n is NULL");
+  SICP_REQUIRE(cap >= 0, SICP_ERR_BAD_ARG, "cap must be >= 0");
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  const MapStore& m = *c.map;
+  *n = m.n;
+  if (xyz && cap > 0) {
+    copy_any(c, xyz, m.xyz.p, sizeof(double) * 3 * (size_t)std::min<long long>(m.n, cap));
+    SICP_CUDA(cudaStreamSynchronize(c.stream));
+  }
+}
+
 }  // namespace sicp
 
 using namespace sicp;
@@ -704,6 +895,15 @@ extern "C" int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const do
                                         const int64_t* n_mov, const sicp_register_params* p,
                                         const double* observed, sicp_pair_result* out, int64_t* n_selected) {
   SICP_BATCH_API(register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected))
+}
+
+extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                   const double* H, double voxel_size, int64_t* n_added) {
+  SICP_BATCH_API(map_insert(c, n_clouds, xyz, n, H, voxel_size, n_added))
+}
+
+extern "C" int32_t sicp_get_map(sicp_ctx* ctx, double* xyz, int64_t cap, int64_t* n) {
+  SICP_BATCH_API(get_map(c, xyz, cap, n))
 }
 
 extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double* const* mov_xyz_out,

@@ -284,6 +284,22 @@ struct MapStore {
   DevBuf<uint32_t> bits, popc, popc_scan, sums;
   DevBuf<unsigned long long> n_searched;  // bounded searches of the last filter
   DevBuf<MapCull> culls;                  // one per scan
+  // sicp_map_insert (batch.cu: map_insert): the clouds of one call, moved and concatenated
+  // (ins_xyz), their finite points compacted in order (fin_xyz, with their index in ins_xyz in
+  // fin_idx) and gridded as one cloud (gnew); a keep flag per point of ins_xyz, its prefix sum and
+  // the per-cloud boundaries of that sum.  These staging buffers grow to the largest insert (about
+  // 100 B per point) and stay allocated, also across sicp_set_map, like the batch's buffers.
+  // xyz_next / grid_next receive the grown map, which is then swapped in; they are released after
+  // the swap, so an insert's peak is about two maps and one map stays resident between inserts.
+  DevBuf<double> ins_xyz, fin_xyz, xyz_next;
+  DevBuf<uint32_t> fin_flag, fin_scan, fin_idx, ins_flag, ins_scan, ins_off, ins_bounds;
+  DevBuf<Rigid> ins_T;
+  BatchGrid gnew, grid_next;
+  uint32_t* bounds_host = nullptr;  // pinned: n_clouds + 1 boundaries
+  size_t bounds_cap = 0;
+  ~MapStore() {
+    if (bounds_host) cudaFreeHost(bounds_host);
+  }
 };
 
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
@@ -367,6 +383,11 @@ void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev,
 void map_bits_popc_launch(Ctx& c, const uint32_t* bits, long long n_words, uint32_t* popc);
 void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, long long words_per_scan,
                              const uint32_t* scan, uint32_t* list);
+// sicp_map_insert's occupancy test (nn.cu: k_map_insert_flags): for each of the n_fin points of
+// fin_xyz (gridded in fresh), flag[fin_idx[f]] = 1 when no point of the map grid and no point of
+// fresh with a smaller index has the same voxel key floor(p / voxel) (flag is zeroed by the caller)
+void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh, const double* fin_xyz,
+                             const uint32_t* fin_idx, long long n_fin, double voxel, uint32_t* flag);
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 // sicp_get_batch_outputs, for the n_ids pairs ids (device) of the last batched run: the movable

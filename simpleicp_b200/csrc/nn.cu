@@ -17,6 +17,8 @@
 //           coordinates, and the per-lane winners are combined with a warp-shuffle min-reduction.
 // Ties are broken towards the lower original index in both.
 #include <algorithm>
+#include <cfloat>
+#include <climits>
 
 #include "ctx.cuh"
 
@@ -700,6 +702,65 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// ---- sicp_map_insert: one new point per voxel the map does not occupy ----------------------
+// key(p) = (floor(p.x / v), floor(p.y / v), floor(p.z / v)) with IEEE double division, compared
+// as doubles.  Only records inside the box of p's voxel can share its key:
+//   a point q with key k on an axis has fl(q / v) in [k, k + 1) (fl(q / v) = k when |k| >= 2^53,
+//   where k + 1 rounds to k).  Division is correctly rounded, so q / v lies within u|k + 1| + u|k|
+//   + 2^-1075 of [k, k + 1] (u = 2^-53; the last term covers a quotient in the subnormal range),
+//   i.e. q lies in [k v, (k + 1) v] grown by u (|k| + |k + 1|) v + v 2^-1075.  The computed faces
+//   lo = k v and hi = (k + 1) v are each within u of their value, plus 2^-1075 below the normal
+//   range, and |lo| + |hi| >= (1 - 2u) v while both are finite.  So the box [lo, hi] grown by
+//   4u (|lo| + |hi|) + 2^-1072 holds every such q; the kernel grows it by
+//   g = 1e-12 (|lo| + |hi|) + 1e-300, over a thousand times more.  A face that overflows (or
+//   inf - inf) opens that axis to the whole line.
+// The cells are the grid's own cell_coord of the grown faces: a rounded product, a floor and a
+// clamp are each monotone, and the builder binned every record with the same cell_coord, so a
+// record inside the box lies in a cell between those of the faces (also when they clamp: a box
+// beyond the grid only walks its edge cells, whose records then fail the key test).  In a cubic
+// x-fastest grid each (y, z) row of that range is one contiguous range of records.
+__device__ __forceinline__ bool voxel_taken(const GridView& g, const double lo[3], const double hi[3], double v,
+                                            const double k[3], long long below) {
+  const int x0 = cell_coord(lo[0], g.ox, g.inv_h, g.nx), x1 = cell_coord(hi[0], g.ox, g.inv_h, g.nx);
+  const int y0 = cell_coord(lo[1], g.oy, g.inv_h, g.ny), y1 = cell_coord(hi[1], g.oy, g.inv_h, g.ny);
+  const int z0 = cell_coord(lo[2], g.oz, g.inv_h, g.nz), z1 = cell_coord(hi[2], g.oz, g.inv_h, g.nz);
+  for (int z = z0; z <= z1; ++z)
+    for (int y = y0; y <= y1; ++y) {
+      const long long row = ((long long)z * g.ny + y) * g.nx;
+      const uint32_t e = g.cell_start[row + x1 + 1];
+      for (uint32_t p = g.cell_start[row + x0]; p < e; ++p) {
+        const Rec r = g.recs[p];
+        if (r.idx >= below || r.x < lo[0] || r.x > hi[0] || r.y < lo[1] || r.y > hi[1] || r.z < lo[2] || r.z > hi[2])
+          continue;
+        if (floor(__ddiv_rn(r.x, v)) == k[0] && floor(__ddiv_rn(r.y, v)) == k[1] && floor(__ddiv_rn(r.z, v)) == k[2])
+          return true;
+      }
+    }
+  return false;
+}
+
+// One thread per finite new point f (fin_xyz, the compacted points gridded in `fresh`, Rec::idx =
+// f): it is added unless a map record has its key or a fresh record with a smaller index does.
+__global__ void __launch_bounds__(256)
+    k_map_insert_flags(GridView map, GridView fresh, const double* __restrict__ fin_xyz,
+                       const uint32_t* __restrict__ fin_idx, long long n_fin, double v, uint32_t* __restrict__ flag) {
+  const long long f = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (f >= n_fin) return;
+  double k[3], lo[3], hi[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    k[a] = floor(__ddiv_rn(fin_xyz[3 * f + a], v));
+    const double l = k[a] * v, h = (k[a] + 1.0) * v;
+    const double g = 1e-12 * (fabs(l) + fabs(h)) + 1e-300;
+    lo[a] = l - g;
+    hi[a] = h + g;
+    if (!(lo[a] >= -DBL_MAX)) lo[a] = -kInf;  // overflow or NaN
+    if (!(hi[a] <= DBL_MAX)) hi[a] = kInf;
+  }
+  if (voxel_taken(map, lo, hi, v, k, LLONG_MAX) || voxel_taken(fresh, lo, hi, v, k, f)) return;
+  flag[fin_idx[f]] = 1u;
+}
+
 // ------------------------------------------------------------------------------------------
 // brute-force engine (TMA staged)
 // ------------------------------------------------------------------------------------------
@@ -1094,6 +1155,15 @@ void map_bits_popc_launch(Ctx& c, const uint32_t* bits, long long n_words, uint3
 void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, long long words_per_scan,
                              const uint32_t* scan, uint32_t* list) {
   k_map_scatter<<<(unsigned)((n_words + 255) / 256), 256, 0, c.stream>>>(bits, n_words, words_per_scan, scan, list);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh, const double* fin_xyz,
+                             const uint32_t* fin_idx, long long n_fin, double voxel, uint32_t* flag) {
+  if (n_fin <= 0) return;
+  k_map_insert_flags<<<(unsigned)((n_fin + 255) / 256), 256, 0, c.stream>>>(map, fresh, fin_xyz, fin_idx, n_fin, voxel,
+                                                                            flag);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

@@ -54,5 +54,14 @@ ov = [(p[0][p[0][:, 0] < 20], p[1][p[1][:, 0] > 10]) for p in pairs] + [(pairs[0
 tab_o = sb.simpleicp_batch(ov, engine="batched", correspondences=500, max_overlap_distance=0.5,
                            rbp_observed_values=np.zeros((len(ov), 6)), on_error="nan")
 assert np.isfinite(tab_o[:-1]).all() and tab_o[-1, 16] == -_capi.SICP_ERR_NO_OVERLAP
+# map insert: with H (a NaN point, an empty cloud, a cloud at an odd point offset), without H, and
+# one that adds nothing
+with sb.Map(X_fix[:30_000]) as mp:
+    ins = [X_mov[:1001].copy(), np.zeros((0, 3)), X_mov[1001:3000]]
+    ins[0][5, 1] = np.nan
+    k1 = mp.insert(ins, np.stack([H_true, np.eye(4), H_true]), voxel_size=0.05)
+    k2 = mp.insert([X_mov[3000:9000] + 0.01], voxel_size=0.2)
+    k3 = mp.insert([mp.points()[:500]], voxel_size=0.05)
+    assert k1.sum() > 0 and k2.sum() > 0 and k3.sum() == 0 and mp.n_points == 30_000 + k1.sum() + k2.sum()
 print("ok", a.iterations, m.iterations, int(tab[:, 16].sum()), c.iterations, d.iterations, f.iterations, g.iterations, l.iterations,
       float(np.linalg.norm(c.H - H_true)), float(np.linalg.norm(l.T - H_true)))
