@@ -417,7 +417,7 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   auto select_and_normals = [&]() {
     batch_select_gather_launch(c, b, fix_xyz, r.overlap, round_away);
     StageTimer t(c, &c.tm.normals_ms);
-    batch_normals_launch(c, b, rp->neighbors);
+    normals_launch(c, &b, false, rp->neighbors);
     t.stop();
   };
   // without the filter the selection needs only the fixed side: it runs while the movable clouds
@@ -461,7 +461,8 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   if (b.mov_attr) {
     b.q_nrm_eff.reserve((size_t)n_pairs * (size_t)r.Kmax);
     StageTimer t(c, &c.tm.mov_normals_ms);
-    batch_mov_normals_launch(c, b, rp->mov_neighbors, r.max_n_mov);
+    b.max_n_mov = r.max_n_mov;
+    normals_launch(c, &b, true, rp->mov_neighbors);
     t.stop();
   }
 

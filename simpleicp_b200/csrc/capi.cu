@@ -495,7 +495,7 @@ int32_t sicp_estimate_normals(sicp_ctx* ctx, int32_t neighbors, float* nx, float
   }
   StageTimer t(c, &c.tm.normals_ms);
   c.q_nrm.reserve(std::max<long long>(c.K, 1));
-  estimate_normals_launch(c, c.gfix, c.q_xyz.p, c.K, neighbors, c.q_nrm.p, c.keep_knn != 0, false);
+  normals_launch(c, nullptr, false, neighbors);
   c.have_normals = true;
   if (nx || ny || nz || planarity) {
     c.stage.reserve(sizeof(float) * 4 * c.K);
@@ -971,7 +971,7 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
     if (rp->mov_neighbors <= 0) return;
     StageTimer t(c, &c.tm.mov_normals_ms);
     c.mov_nrm.reserve(n_mov);
-    estimate_normals_launch(c, c.gmov, c.mov_xyz.p, n_mov, rp->mov_neighbors, c.mov_nrm.p, false, true);
+    normals_launch(c, nullptr, true, rp->mov_neighbors);
     c.mov_attr = true;
     c.mov_cos_max = mov_cos_max_of(rp->max_angle_rad);
     t.stop();
@@ -1033,7 +1033,7 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
   {
     StageTimer t(c, &c.tm.normals_ms);
     c.q_nrm.reserve(std::max<long long>(c.K, 1));
-    estimate_normals_launch(c, c.gfix, c.q_xyz.p, c.K, rp->neighbors, c.q_nrm.p, c.keep_knn != 0, false);
+    normals_launch(c, nullptr, false, rp->neighbors);
     c.have_normals = true;
     t.stop();
   }

@@ -199,7 +199,7 @@ struct BatchGrid {
 
 struct Batch {
   int n_pairs = 0;
-  long long Kmax = 0, total_fix = 0, total_mov = 0;
+  long long Kmax = 0, total_fix = 0, total_mov = 0, max_n_mov = 0;  // max_n_mov: the largest movable cloud
   DevBuf<double> fix_xyz, mov_xyz;  // concatenated clouds
   BatchGrid gfix, gmov;
   DevBuf<unsigned int> occ;
@@ -339,12 +339,14 @@ inline void launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_
   SICP_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...));
 }
 void set_state_transform(Ctx& c, const double x[6], const Rigid* T_or_null, bool reset_loop);
-// k-NN (self included) + PCA of n_q queries in grid g; out[i] = (nx, ny, nz, planarity) float32.
-// The fixed side: (c.gfix, c.q_xyz, c.K, c.q_nrm) with keep_lists = option "keep_knn"; the
-// movable side: (c.gmov, c.mov_xyz, c.n_mov, c.mov_nrm), chunked: as many queries per launch as
-// option "normals_scratch_mb" holds at k x 4 bytes of neighbour positions each.
-void estimate_normals_launch(Ctx& c, const Grid& g, const double* q_xyz, long long n_q, int k, float4* out,
-                             bool keep_lists, bool chunked);
+// k-NN (self included) + PCA of every query of one side; out[i] = (nx, ny, nz, planarity) float32.
+// b == nullptr, the one-pair context: the fixed side (c.gfix, c.q_xyz, c.K -> c.q_nrm, the lists
+// kept under option "keep_knn") or the movable side (c.gmov, c.mov_xyz, c.n_mov -> c.mov_nrm).
+// b != nullptr, a batch: every pair's selected fixed points in its fixed grid (Batch::q_xyz ->
+// Batch::q_nrm) or its movable points in its own movable grid (Batch::mov_xyz -> Batch::mov_nrm).
+// The movable side is chunked: as many queries per launch as option "normals_scratch_mb" holds at
+// k x 4 bytes of neighbour positions each.
+void normals_launch(Ctx& c, Batch* b, bool movable, int k);
 // cos of the angle limit as sicp_set_mov_normals stores it (< 0: no angle test)
 double mov_cos_max_of(double max_angle_rad);
 void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve, bool arm_stop,
@@ -366,9 +368,6 @@ void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHo
 // with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud;
 // fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::fix_xyz or MapStore::xyz)
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);
-void batch_normals_launch(Ctx& c, Batch& b, int k);
-// k-NN + PCA of every movable point of every pair in its own movable grid -> Batch::mov_nrm
-void batch_mov_normals_launch(Ctx& c, Batch& b, int k, long long max_n_mov);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
 // PointCloud.select_in_range of every fixed point of the batch under its pair's DevState
 // transform: Batch::ovl_flag[i] = (squared distance to the nearest movable point < r2)

@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <climits>
+#include <type_traits>
 
 #include "ctx.cuh"
 
@@ -1104,6 +1105,23 @@ __global__ void __launch_bounds__(256)
   dst[1] = src[1];
   dst[2] = src[2];
 }
+
+// Lanes per query of the grid match family: option match_group when it names a lane count, else
+// by the number n_q of queries in flight -- 16 while the search is latency-bound (few queries),
+// fewer once there are enough queries to fill the machine and issue slots become the limit.  A
+// family without the forms below min_lanes (they would spill) runs min_lanes; the results do not
+// depend on the lanes.
+int match_lanes(const Ctx& c, long long n_q, int min_lanes) {
+  const int mg = (c.match_group > 1) ? c.match_group : ((n_q <= 16384) ? 16 : ((n_q <= 65536) ? 8 : 4));
+  return std::max(mg, min_lanes);
+}
+
+// launch(std::integral_constant<int, L>{}) for the form L == lanes among the forms Ls of a family
+template <int... Ls, class F>
+void with_lanes(int lanes, F&& launch) {
+  const bool found = ((lanes == Ls && (launch(std::integral_constant<int, Ls>{}), true)) || ...);
+  SICP_REQUIRE(found, SICP_ERR_BAD_ARG, "no " + std::to_string(lanes) + "-lane match kernel");
+}
 }  // namespace
 
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away) {
@@ -1114,34 +1132,24 @@ void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool wi
 }
 
 void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2) {
-  // lanes per query by the number of queries in flight, as in batch_match_launch; the result does
-  // not depend on it, and the 2-lane form (which spills) is served by 4 lanes
-  const long long total = b.total_fix;
-  int mg = c.match_group;
-  if (mg == 0 || mg == 1) mg = (total <= 16384) ? 16 : ((total <= 65536) ? 8 : 4);
-  const dim3 grid((unsigned)((max_n_fix * std::max(mg, 4) + 127) / 128), b.n_pairs);
-  uint32_t* keep = b.ovl_flag.p;
-  if (mg <= 4) k_overlap_batch<4><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
-  else if (mg == 8) k_overlap_batch<8><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
-  else k_overlap_batch<16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, keep);
+  const int mg = match_lanes(c, b.total_fix, 4);
+  const dim3 grid((unsigned)((max_n_fix * mg + 127) / 128), b.n_pairs);
+  with_lanes<4, 8, 16>(mg, [&](auto L) {
+    k_overlap_batch<decltype(L)::value>
+        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, b.ovl_flag.p);
+  });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
 
 void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev, long long max_rows, double r2,
                         long long n_candidates_hint) {
-  // lanes per search by the number of searches in flight, as batch_overlap_launch chooses them
-  // (the flags do not depend on it)
-  int mg = c.match_group;
-  if (mg == 0 || mg == 1) mg = (n_candidates_hint <= 16384) ? 16 : ((n_candidates_hint <= 65536) ? 8 : 4);
   const dim3 grid((unsigned)max_rows, b.n_pairs);
   const long long words = (m.n + 31) / 32;
-  if (mg <= 4)
-    k_map_overlap<4><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
-  else if (mg == 8)
-    k_map_overlap<8><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
-  else
-    k_map_overlap<16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  with_lanes<4, 8, 16>(match_lanes(c, n_candidates_hint, 4), [&](auto L) {
+    k_map_overlap<decltype(L)::value>
+        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
@@ -1183,26 +1191,21 @@ void batch_match_launch(Ctx& c, Batch& b, bool warm) {
   a.nn_pos = b.nn_pos.p;
   a.warm = warm ? 1 : 0;
   a.sphere = c.sphere_scan;
-  // lanes per query as in the single-pair launch, by the number of queries in flight
-  const long long total = b.Kmax * b.n_pairs;
-  int mg = c.match_group;
-  if (mg == 0 || mg == 1) mg = (total <= 16384) ? 16 : ((total <= 65536) ? 8 : 4);
+  const int mg = match_lanes(c, b.Kmax * b.n_pairs, b.mov_attr ? 4 : 2);
   const dim3 grid((unsigned)((b.Kmax * mg + 127) / 128), b.n_pairs);
   // programmatically dependent on the previous iteration's k_rs_batch (both kernels wait before
   // they touch anything the other writes; the pair descriptors are static)
   const bool pdl = c.pdl != 0;
   if (b.mov_attr) {
-    // no 2-lane form (it would spill, like the overlap kernel's): 4 lanes serve it, the result
-    // does not depend on the lanes
     const BatchMatchAttrArgs m{a, b.mov_nrm.p, b.q_nrm_eff.p, b.mov_cos_max};
-    const dim3 grid_a((unsigned)((b.Kmax * std::max(mg, 4) + 127) / 128), b.n_pairs);
-    if (mg <= 4) launch_kernel(k_match_batch_attr<4>, grid_a, dim3(128), 0, c.stream, pdl, m);
-    else if (mg == 8) launch_kernel(k_match_batch_attr<8>, grid_a, dim3(128), 0, c.stream, pdl, m);
-    else launch_kernel(k_match_batch_attr<16>, grid_a, dim3(128), 0, c.stream, pdl, m);
-  } else if (mg == 2) launch_kernel(k_match_batch<2>, grid, dim3(128), 0, c.stream, pdl, a);
-  else if (mg == 4) launch_kernel(k_match_batch<4>, grid, dim3(128), 0, c.stream, pdl, a);
-  else if (mg == 8) launch_kernel(k_match_batch<8>, grid, dim3(128), 0, c.stream, pdl, a);
-  else launch_kernel(k_match_batch<16>, grid, dim3(128), 0, c.stream, pdl, a);
+    with_lanes<4, 8, 16>(mg, [&](auto L) {
+      launch_kernel(k_match_batch_attr<decltype(L)::value>, grid, dim3(128), 0, c.stream, pdl, m);
+    });
+  } else {
+    with_lanes<2, 4, 8, 16>(mg, [&](auto L) {
+      launch_kernel(k_match_batch<decltype(L)::value>, grid, dim3(128), 0, c.stream, pdl, a);
+    });
+  }
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
@@ -1249,21 +1252,12 @@ void match_launch(Ctx& c, bool with_distance, double* out_d2, cudaEvent_t mid, b
         c.gmov.view(), c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
         with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
   } else {
-    // lanes per query: 16 while the search is latency-bound (few queries), fewer once there are
-    // enough queries to fill the machine and issue slots become the limit
-    int mg = c.match_group;
-    if (mg == 0) mg = (K <= 16384) ? 16 : ((K <= 65536) ? 8 : 4);
-    const long long threads = K * mg;
-    const unsigned blocks = (unsigned)((threads + 127) / 128);
-#define SICP_LAUNCH_COOP(N)                                                                          \
-  launch_kernel(k_match_grid_coop<N>, dim3(blocks), dim3(128), 0, c.stream, pdl, c.gmov.view(),       \
-                c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax, with_distance ? 1 : 0, \
-                c.nn_idx.p, out, c.unresolved.p, lh, cap2, co)
-    if (mg == 2) SICP_LAUNCH_COOP(2);
-    else if (mg == 4) SICP_LAUNCH_COOP(4);
-    else if (mg == 8) SICP_LAUNCH_COOP(8);
-    else SICP_LAUNCH_COOP(16);
-#undef SICP_LAUNCH_COOP
+    const int mg = match_lanes(c, K, 2);
+    with_lanes<2, 4, 8, 16>(mg, [&](auto L) {
+      launch_kernel(k_match_grid_coop<decltype(L)::value>, dim3((unsigned)((K * mg + 127) / 128)), dim3(128), 0,
+                    c.stream, pdl, c.gmov.view(), c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
+                    with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
+    });
   }
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;

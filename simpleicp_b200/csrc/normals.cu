@@ -31,7 +31,7 @@ constexpr int kMaxK = 64;
 //     used to prune rows of the next ring and for the termination proof
 //     (k-th best <= distance to every unexplored cell);
 //   * the final k rounds emit the neighbours in (distance, index) order as record positions.
-// The covariance / eigen-solve run in a second kernel, one thread per query (k_pca_from_knn): in
+// The covariance / eigen-solve run in a second kernel, one thread per query (k_pca): in
 // this one three of four lanes would idle through the ~2000-instruction dgeev walk.  It reads
 // the neighbours from the cell-sorted records the search just touched (L2-hot), not from the
 // caller-order cloud.  Ordering (distance, then original index) and the summation order of mean
@@ -200,7 +200,7 @@ __device__ __forceinline__ void knn_coop_body(const GridView& g, const double* _
 
 // One thread per query, 16 < k <= 64 (the reference's webots test uses k = 40): a sorted list of
 // record POSITIONS in a dynamically indexed (local-memory) array, ties by original index through
-// the records as everywhere, written to knn_pos for k_pca_from_knn.
+// the records as everywhere, written to knn_pos for k_pca.
 struct TopKPos {
   double d2[kMaxK];
   uint32_t pos[kMaxK];
@@ -293,24 +293,6 @@ __device__ __forceinline__ void knn_single_body(const GridView& g, const double*
   for (int j = 0; j < k; ++j) knn_pos[i * k + j] = (j < tk.n) ? tk.pos[j] : 0xffffffffu;
 }
 
-__global__ void __launch_bounds__(128)
-    k_knn_single(GridView g, const double* __restrict__ q_xyz, long long K, int k, uint32_t* __restrict__ knn_pos) {
-  knn_single_body(g, q_xyz, K, k, knn_pos, blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-__global__ void __launch_bounds__(128)
-    k_knn_single_batch(const PairDev* __restrict__ pairs, const double* __restrict__ q_xyz, int k, long long Kmax,
-                       uint32_t* __restrict__ knn_pos) {
-  const PairDev pd = pairs[blockIdx.y];
-  knn_single_body(pd.gfix, q_xyz + 3 * pd.q_off, pd.K, k, knn_pos + (size_t)blockIdx.y * Kmax * k,
-                  blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-
-template <int MG, int KC>
-__global__ void __launch_bounds__(128)
-    k_knn_coop(GridView g, const double* __restrict__ q_xyz, long long K, int k, uint32_t* __restrict__ knn_pos) {
-  knn_coop_body<MG, KC>(g, q_xyz, K, k, knn_pos, blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-
 // covariance (np.cov, ddof = 1) + eigen-solve + float32 store from the neighbour positions; the
 // arithmetic of knn_pca_body, the points taken from the cell-sorted records
 __device__ __forceinline__ void pca_from_knn_body(const GridView& g, const double* __restrict__ q_xyz, long long K,
@@ -367,14 +349,6 @@ __device__ __forceinline__ void pca_from_knn_body(const GridView& g, const doubl
   o.z = (float)nn[2];
   o.w = (float)((w[1] - w[2]) / w[0]);
   q_nrm[i] = o;
-}
-
-__global__ void __launch_bounds__(128)
-    k_pca_from_knn(GridView g, const double* __restrict__ q_xyz, long long K, int k, int sign_mode,
-                   const uint32_t* __restrict__ knn_pos, float4* __restrict__ q_nrm,
-                   long long* __restrict__ knn_idx, double* __restrict__ knn_d2) {
-  pca_from_knn_body(g, q_xyz, K, k, sign_mode, knn_pos, q_nrm, knn_idx, knn_d2,
-                    blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
 
 // One thread per query with the list in REGISTERS (k <= KC <= 16): the insertion network of the
@@ -444,94 +418,110 @@ __device__ __forceinline__ void knn_reg_body(const GridView& g, const double* __
     if (j >= KC - k) knn_pos[i * k + (j - (KC - k))] = L.p[j];
 }
 
-template <int KC>
-__global__ void __launch_bounds__(128)
-    k_knn_reg(GridView g, const double* __restrict__ q_xyz, long long K, int k, uint32_t* __restrict__ knn_pos) {
-  knn_reg_body<KC>(g, q_xyz, K, k, knn_pos, blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-template <int KC>
-__global__ void __launch_bounds__(128)
-    k_knn_reg_batch(const PairDev* __restrict__ pairs, const double* __restrict__ q_xyz, int k, long long Kmax,
-                    uint32_t* __restrict__ knn_pos) {
-  const PairDev pd = pairs[blockIdx.y];
-  knn_reg_body<KC>(pd.gfix, q_xyz + 3 * pd.q_off, pd.K, k, knn_pos + (size_t)blockIdx.y * Kmax * k,
-                   blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-
-// batched forms: blockIdx.y = pair
-template <int MG, int KC>
-__global__ void __launch_bounds__(128)
-    k_knn_coop_batch(const PairDev* __restrict__ pairs, const double* __restrict__ q_xyz, int k, long long Kmax,
-                     uint32_t* __restrict__ knn_pos) {
-  const PairDev pd = pairs[blockIdx.y];
-  knn_coop_body<MG, KC>(pd.gfix, q_xyz + 3 * pd.q_off, pd.K, k, knn_pos + (size_t)blockIdx.y * Kmax * k,
-                        blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-__global__ void __launch_bounds__(128)
-    k_pca_from_knn_batch(const PairDev* __restrict__ pairs, const double* __restrict__ q_xyz, int k, long long Kmax,
-                         int sign_mode, const uint32_t* __restrict__ knn_pos, float4* __restrict__ q_nrm) {
-  const PairDev pd = pairs[blockIdx.y];
-  pca_from_knn_body(pd.gfix, q_xyz + 3 * pd.q_off, pd.K, k, sign_mode, knn_pos + (size_t)blockIdx.y * Kmax * k,
-                    q_nrm + pd.q_off, nullptr, nullptr, blockIdx.x * (long long)blockDim.x + threadIdx.x);
-}
-
-// Movable side of a batch, one chunk of queries: blockIdx.y = pair, its movable points
-// [q0, q0 + cq) in its own movable grid; scratch pos is n_pairs x cq x k.  The grid is read
-// through a reference into the pair descriptor (a register copy of it made the cooperative
-// 12-slot form spill), and the one-thread forms are allowed 128 registers (they spilled at the
-// 64 the compiler picks by itself); all forms compile without spills.  128-thread launches.
-struct MovBatchChunk {
-  const PairDev* pairs;
-  const double* mov_xyz;  // concatenated movable clouds
-  long long q0, cq;
+// Where the queries of a k-NN + PCA launch come from.  get<S>() resolves, per block, the grid, the
+// queries, their count, the neighbour-position scratch and the output slice.  The pair descriptor
+// is read through a reference: a register copy of it made the cooperative and register-list forms
+// spill.
+enum class Src {
+  One,      // one grid g: q_xyz[n] -> out[n], pos n x k, knn_idx / knn_d2 of option "keep_knn"
+  PairFix,  // blockIdx.y = pair: its K selected fixed points at q_off, in its fixed grid
+  PairMov,  // blockIdx.y = pair: its movable points [q0, q0 + n), in its own movable grid
+};
+struct KnnQueries {
+  GridView g;            // One
+  const PairDev* pairs;  // PairFix, PairMov
+  const double* q_xyz;   // One: the queries; PairFix: Batch::q_xyz; PairMov: Batch::mov_xyz
+  float4* out;           // One: n entries; PairFix: Batch::q_nrm; PairMov: Batch::mov_nrm
+  long long n;           // One: the queries; PairFix, PairMov: pos rows per pair
+  long long q0;          // PairMov: first movable point of the chunk
   int k;
   uint32_t* pos;
-  float4* out;            // total_mov entries
-  __device__ __forceinline__ const GridView& get(const double*& q, long long& n, uint32_t*& p,
-                                      float4*& o) const {
-    const PairDev& pd = pairs[blockIdx.y];
-    n = max(0ll, min(cq, pd.n_mov - q0));
-    q = mov_xyz + 3 * (pd.mov_off + q0);
-    p = pos + (size_t)blockIdx.y * cq * k;
-    o = out + pd.mov_off + q0;
-    return pd.gmov;
+  long long* knn_idx;
+  double* knn_d2;
+  template <Src S>
+  __device__ __forceinline__ const GridView& get(const double*& q, long long& nq, uint32_t*& p, float4*& o) const {
+    if constexpr (S == Src::One) {
+      q = q_xyz;
+      nq = n;
+      p = pos;
+      o = out;
+      return g;
+    } else {
+      const PairDev& pd = pairs[blockIdx.y];
+      p = pos + (size_t)blockIdx.y * n * k;
+      if constexpr (S == Src::PairFix) {
+        q = q_xyz + 3 * pd.q_off;
+        nq = pd.K;
+        o = out + pd.q_off;
+        return pd.gfix;
+      } else {
+        q = q_xyz + 3 * (pd.mov_off + q0);
+        nq = max(0ll, min(n, pd.n_mov - q0));
+        o = out + pd.mov_off + q0;
+        return pd.gmov;
+      }
+    }
   }
 };
-template <int MG, int KC>
-__global__ void __launch_bounds__(128) k_knn_coop_movb(MovBatchChunk a) {
+
+// 128-thread blocks.  The one-thread-per-query kernels get up to 128 registers: at the 64 the
+// compiler picks by itself they spill.
+template <int MG, int KC, Src S>
+__global__ void __launch_bounds__(128) k_knn_coop(const KnnQueries a) {
   const double* q; long long n; uint32_t* p; float4* o;
-  const GridView& g = a.get(q, n, p, o);
+  const GridView& g = a.get<S>(q, n, p, o);
   knn_coop_body<MG, KC>(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
-template <int KC>
-__global__ void __launch_bounds__(128) k_knn_reg_movb(MovBatchChunk a) {
+template <int KC, Src S>
+__global__ void __launch_bounds__(128) k_knn_reg(const KnnQueries a) {
   const double* q; long long n; uint32_t* p; float4* o;
-  const GridView& g = a.get(q, n, p, o);
+  const GridView& g = a.get<S>(q, n, p, o);
   knn_reg_body<KC>(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
-__global__ void __maxnreg__(128) k_knn_single_movb(MovBatchChunk a) {
+template <Src S>
+__global__ void __launch_bounds__(128, 4) k_knn_single(const KnnQueries a) {
   const double* q; long long n; uint32_t* p; float4* o;
-  const GridView& g = a.get(q, n, p, o);
+  const GridView& g = a.get<S>(q, n, p, o);
   knn_single_body(g, q, n, a.k, p, blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
-__global__ void __maxnreg__(128) k_pca_movb(MovBatchChunk a, int sign_mode) {
+template <Src S>
+__global__ void __launch_bounds__(128, 4) k_pca(const KnnQueries a, int sign_mode) {
   const double* q; long long n; uint32_t* p; float4* o;
-  const GridView& g = a.get(q, n, p, o);
-  pca_from_knn_body(g, q, n, a.k, sign_mode, p, o, nullptr, nullptr,
+  const GridView& g = a.get<S>(q, n, p, o);
+  const bool keep = S == Src::One;
+  pca_from_knn_body(g, q, n, a.k, sign_mode, p, o, keep ? a.knn_idx : nullptr, keep ? a.knn_d2 : nullptr,
                     blockIdx.x * (long long)blockDim.x + threadIdx.x);
 }
 
-// Which k-NN kernel serves n_q queries (knn_coop: 1 = cooperative lanes (k <= 16), 0 = one thread
-// per query with the list in local memory, 2 = one thread per query with the list in registers
-// (k <= 16), -1 (default) = cooperative while the search is latency-bound (few queries), one
-// thread per query with the local-memory list once the queries fill the machine (K = 100 000,
-// k = 10: faster than a register list or cooperative lanes -- the fixed-length insertion network
-// costs more than the early-exit loop saves in memory traffic).
-enum class KnnKind { Coop, Reg, Single };
-KnnKind knn_kind(const Ctx& c, int k, long long n_q) {
-  if ((k <= 16) && (c.knn_coop == 1 || (c.knn_coop < 0 && n_q <= 16384))) return KnnKind::Coop;
-  if ((k <= 16) && c.knn_coop == 2) return KnnKind::Reg;
-  return KnnKind::Single;
+// The k-NN and the PCA of one launch: `rows` queries per pair (n_y pairs, 1 for Src::One).  The
+// k-NN kernel is chosen by the query count n_all of the whole estimate, so a chunk runs the kernels
+// an unchunked estimate would; a chunk only bounds the scratch of the positions.  Option knn_coop:
+// 1 = cooperative lanes (k <= 16), 0 = one thread per query with the list in local memory, 2 = one
+// thread per query with the list in registers (k <= 16), -1 (default) = cooperative while the
+// search is latency-bound (few queries), one thread per query with the local-memory list once the
+// queries fill the machine (K = 100 000, k = 10: faster than a register list or cooperative lanes
+// -- the fixed-length insertion network costs more than the early-exit loop saves in memory
+// traffic).  The neighbours are exact, so the choice does not change the normals.
+template <Src S>
+void knn_pca_launch(Ctx& c, const KnnQueries& a, long long rows, unsigned n_y, long long n_all) {
+  const int k = a.k;
+  const dim3 grid1((unsigned)((rows + 127) / 128), n_y);
+  if (k <= 16 && (c.knn_coop == 1 || (c.knn_coop < 0 && n_all <= 16384))) {
+    const int mg = (n_all <= 32768) ? 8 : 4;
+    const dim3 grid((unsigned)((rows * mg + 127) / 128), n_y);
+    if (mg == 8 && k <= 12) k_knn_coop<8, 12, S><<<grid, 128, 0, c.stream>>>(a);
+    else if (mg == 8) k_knn_coop<8, 16, S><<<grid, 128, 0, c.stream>>>(a);
+    else if (k <= 12) k_knn_coop<4, 12, S><<<grid, 128, 0, c.stream>>>(a);
+    else k_knn_coop<4, 16, S><<<grid, 128, 0, c.stream>>>(a);
+  } else if (k <= 16 && c.knn_coop == 2) {
+    if (k <= 12) k_knn_reg<12, S><<<grid1, 128, 0, c.stream>>>(a);
+    else k_knn_reg<16, S><<<grid1, 128, 0, c.stream>>>(a);
+  } else {
+    k_knn_single<S><<<grid1, 128, 0, c.stream>>>(a);
+  }
+  k_pca<S><<<grid1, 128, 0, c.stream>>>(a, c.sign_mode);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 2;
 }
 
 }  // namespace
@@ -540,112 +530,61 @@ double mov_cos_max_of(double max_angle_rad) {
   return (max_angle_rad >= 0.0) ? (max_angle_rad >= 1.5707963267948966 ? 0.0 : cos(max_angle_rad)) : -1.0;
 }
 
-void estimate_normals_launch(Ctx& c, const Grid& grid, const double* q_xyz, long long n_q, int k, float4* out,
-                             bool keep_lists, bool chunked) {
+void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
+  const std::string name = movable ? "mov_neighbors" : "neighbors";
   SICP_REQUIRE(k >= 2 && k <= kMaxK, SICP_ERR_BAD_ARG,
-               "neighbors must be between 2 and 64 (got " + std::to_string(k) + ")");
-  SICP_REQUIRE((long long)k <= grid.n, SICP_ERR_BAD_ARG,
-               &grid == &c.gmov ? "mov_neighbors exceeds the number of points in the movable cloud"
-                                            : "neighbors exceeds the number of points in the fixed cloud");
-  // the neighbour lists leave the SM only when somebody wants to look at them (option "keep_knn")
-  long long* kidx = nullptr;
-  double* kd2 = nullptr;
-  if (keep_lists) {
-    c.knn_idx.reserve((size_t)n_q * k);
-    c.knn_d2.reserve((size_t)n_q * k);
-    kidx = c.knn_idx.p;
-    kd2 = c.knn_d2.p;
-  }
-  if (keep_lists || !chunked) c.knn_k = keep_lists ? k : 0;
-  // All k-NN kernels hand record positions to k_pca_from_knn (the choice: knn_kind).  The kernel
-  // is chosen by the whole query count, so a chunked estimate runs the kernels an unchunked one
-  // would; a chunk only bounds the scratch of the positions.
-  const KnnKind kind = knn_kind(c, k, n_q);
-  const long long chunk = chunked ? std::min<long long>(n_q, normals_chunk_queries(c, k)) : n_q;
-  c.knn_pos.reserve((size_t)std::max<long long>(chunk, 1) * k);
-  const GridView g = grid.view();
-  uint32_t* pos = c.knn_pos.p;
-  for (long long q0 = 0; q0 < n_q; q0 += chunk) {
-    const long long n = std::min(chunk, n_q - q0);
-    const double* q = q_xyz + 3 * q0;
-    const unsigned blocks1 = (unsigned)((n + 127) / 128);
-    if (kind == KnnKind::Coop) {
-      const int mg = (n_q <= 32768) ? 8 : 4;
-      const unsigned blocks = (unsigned)((n * mg + 127) / 128);
-      if (mg == 8) {
-        if (k <= 12) k_knn_coop<8, 12><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
-        else k_knn_coop<8, 16><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
-      } else {
-        if (k <= 12) k_knn_coop<4, 12><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
-        else k_knn_coop<4, 16><<<blocks, 128, 0, c.stream>>>(g, q, n, k, pos);
-      }
-    } else if (kind == KnnKind::Reg && k <= 12) {
-      k_knn_reg<12><<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
-    } else if (kind == KnnKind::Reg) {
-      k_knn_reg<16><<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
-    } else {
-      k_knn_single<<<blocks1, 128, 0, c.stream>>>(g, q, n, k, pos);
+               name + " must be between 2 and 64 (got " + std::to_string(k) + ")");
+  KnnQueries a{};
+  a.k = k;
+  if (b == nullptr) {
+    const Grid& grid = movable ? c.gmov : c.gfix;
+    const long long n_q = movable ? c.n_mov : c.K;
+    SICP_REQUIRE((long long)k <= grid.n, SICP_ERR_BAD_ARG,
+                 name + " exceeds the number of points in the " + (movable ? "movable" : "fixed") + " cloud");
+    // the neighbour lists leave the SM only when somebody wants to look at them (option "keep_knn")
+    const bool keep = !movable && c.keep_knn != 0;
+    if (keep) {
+      c.knn_idx.reserve((size_t)n_q * k);
+      c.knn_d2.reserve((size_t)n_q * k);
     }
-    k_pca_from_knn<<<blocks1, 128, 0, c.stream>>>(g, q, n, k, c.sign_mode, pos, out + q0,
-                                                  kidx ? kidx + q0 * k : nullptr, kd2 ? kd2 + q0 * k : nullptr);
-    SICP_CUDA(cudaGetLastError());
-    c.tm.kernel_launches += 2;
+    if (!movable) c.knn_k = keep ? k : 0;
+    const long long chunk = movable ? std::min<long long>(n_q, normals_chunk_queries(c, k)) : n_q;
+    c.knn_pos.reserve((size_t)std::max<long long>(chunk, 1) * k);
+    a.g = grid.view();
+    a.pos = c.knn_pos.p;
+    for (long long q0 = 0; q0 < n_q; q0 += chunk) {
+      a.n = std::min(chunk, n_q - q0);
+      a.q_xyz = (movable ? c.mov_xyz.p : c.q_xyz.p) + 3 * q0;
+      a.out = (movable ? c.mov_nrm.p : c.q_nrm.p) + q0;
+      a.knn_idx = keep ? c.knn_idx.p + q0 * k : nullptr;
+      a.knn_d2 = keep ? c.knn_d2.p + q0 * k : nullptr;
+      knn_pca_launch<Src::One>(c, a, a.n, 1, n_q);
+    }
+    return;
   }
-}
-
-void batch_normals_launch(Ctx& c, Batch& b, int k) {
-  SICP_REQUIRE(k >= 2 && k <= kMaxK, SICP_ERR_BAD_ARG,
-               "neighbors must be between 2 and 64 (got " + std::to_string(k) + ")");
-  const long long total = b.Kmax * b.n_pairs;
-  const bool coop = (k <= 16) && (c.knn_coop == 1 || (c.knn_coop < 0 && total <= 16384));
-  const bool reg = (k <= 16) && c.knn_coop == 2;
-  b.knn_pos.reserve((size_t)b.n_pairs * b.Kmax * k);
-  if (coop) {
-    const dim3 grid((unsigned)((b.Kmax * 8 + 127) / 128), b.n_pairs);
-    if (k <= 12) k_knn_coop_batch<8, 12><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.q_xyz.p, k, b.Kmax, b.knn_pos.p);
-    else k_knn_coop_batch<8, 16><<<grid, 128, 0, c.stream>>>(b.pairs.p, b.q_xyz.p, k, b.Kmax, b.knn_pos.p);
-  } else if (reg && k <= 12) {
-    k_knn_reg_batch<12><<<dim3((unsigned)((b.Kmax + 127) / 128), b.n_pairs), 128, 0, c.stream>>>(
-        b.pairs.p, b.q_xyz.p, k, b.Kmax, b.knn_pos.p);
-  } else if (reg) {
-    k_knn_reg_batch<16><<<dim3((unsigned)((b.Kmax + 127) / 128), b.n_pairs), 128, 0, c.stream>>>(
-        b.pairs.p, b.q_xyz.p, k, b.Kmax, b.knn_pos.p);
-  } else {
-    k_knn_single_batch<<<dim3((unsigned)((b.Kmax + 127) / 128), b.n_pairs), 128, 0, c.stream>>>(
-        b.pairs.p, b.q_xyz.p, k, b.Kmax, b.knn_pos.p);
+  a.pairs = b->pairs.p;
+  if (!movable) {
+    b->knn_pos.reserve((size_t)b->n_pairs * b->Kmax * k);
+    a.q_xyz = b->q_xyz.p;
+    a.out = b->q_nrm.p;
+    a.n = b->Kmax;
+    a.pos = b->knn_pos.p;
+    knn_pca_launch<Src::PairFix>(c, a, b->Kmax, b->n_pairs, b->Kmax * b->n_pairs);
+    return;
   }
-  k_pca_from_knn_batch<<<dim3((unsigned)((b.Kmax + 127) / 128), b.n_pairs), 128, 0, c.stream>>>(
-      b.pairs.p, b.q_xyz.p, k, b.Kmax, c.sign_mode, b.knn_pos.p, b.q_nrm.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 2;
-}
-
-void batch_mov_normals_launch(Ctx& c, Batch& b, int k, long long max_n_mov) {
-  SICP_REQUIRE(k >= 2 && k <= kMaxK, SICP_ERR_BAD_ARG,
-               "mov_neighbors must be between 2 and 64 (got " + std::to_string(k) + ")");
   // every pair's chunk of queries in one launch; the neighbour positions of a launch
   // (n_pairs x cq x k x 4 bytes) stay within option "normals_scratch_mb"
-  const long long cq = std::min<long long>(max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / b.n_pairs));
-  const KnnKind kind = knn_kind(c, k, b.total_mov);
-  b.knn_pos.reserve((size_t)b.n_pairs * cq * k);
-  b.mov_nrm.reserve(std::max<long long>(b.total_mov, 1));
-  for (long long q0 = 0; q0 < max_n_mov; q0 += cq) {
-    const MovBatchChunk a{b.pairs.p, b.mov_xyz.p, q0, cq, k, b.knn_pos.p, b.mov_nrm.p};
-    const dim3 grid1((unsigned)((cq + 127) / 128), b.n_pairs);
-    if (kind == KnnKind::Coop) {
-      const dim3 grid((unsigned)((cq * 8 + 127) / 128), b.n_pairs);
-      if (k <= 12) k_knn_coop_movb<8, 12><<<grid, 128, 0, c.stream>>>(a);
-      else k_knn_coop_movb<8, 16><<<grid, 128, 0, c.stream>>>(a);
-    } else if (kind == KnnKind::Reg && k <= 12) {
-      k_knn_reg_movb<12><<<grid1, 128, 0, c.stream>>>(a);
-    } else if (kind == KnnKind::Reg) {
-      k_knn_reg_movb<16><<<grid1, 128, 0, c.stream>>>(a);
-    } else {
-      k_knn_single_movb<<<grid1, 128, 0, c.stream>>>(a);
-    }
-    k_pca_movb<<<grid1, 128, 0, c.stream>>>(a, c.sign_mode);
-    SICP_CUDA(cudaGetLastError());
-    c.tm.kernel_launches += 2;
+  const long long cq =
+      std::min<long long>(b->max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / b->n_pairs));
+  b->knn_pos.reserve((size_t)b->n_pairs * cq * k);
+  b->mov_nrm.reserve(std::max<long long>(b->total_mov, 1));
+  a.q_xyz = b->mov_xyz.p;
+  a.out = b->mov_nrm.p;
+  a.n = cq;
+  a.pos = b->knn_pos.p;
+  for (long long q0 = 0; q0 < b->max_n_mov; q0 += cq) {
+    a.q0 = q0;
+    knn_pca_launch<Src::PairMov>(c, a, cq, b->n_pairs, b->total_mov);
   }
 }
 

@@ -2142,6 +2142,29 @@ __global__ void __launch_bounds__(256)
     if (flags & (1u << j)) out[pos++] = resid[base + j];
 }
 
+// The arguments every reject/solve launch takes from the run parameters and the variant /
+// movable-attribute policy: with movable-side attributes the kernels read the match kernels'
+// copy of the normals, whose .w is the signed effective planarity; the linearised variants take
+// the median / MAD over every correspondence.  The launchers add their own pointers and flags.
+RSArgs rs_args(const Ctx& c, const sicp_run_params& p, int it, bool mov_attr, const float4* q_nrm,
+               const float4* q_nrm_eff) {
+  RSArgs a{};
+  a.q_nrm = mov_attr ? q_nrm_eff : q_nrm;
+  a.pl_signed = mov_attr ? 1 : 0;
+  a.min_planarity = p.min_planarity;
+  a.variant = c.variant;
+  a.stat_minpl = c.variant ? -kInf : p.min_planarity;
+  a.min_change = p.min_change;
+  a.w_param = p.lsq.distance_weight;
+  for (int j = 0; j < 6; ++j) {
+    a.obs[j] = p.lsq.observed[j];
+    a.wobs[j] = p.lsq.obs_weight[j];
+  }
+  a.it = it;
+  a.do_solve = 1;
+  return a;
+}
+
 }  // namespace
 
 void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve, bool arm_stop,
@@ -2169,11 +2192,9 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
   const int par = c.rs_parity;
   c.rs_parity ^= 1;
 
-  RSArgs a;
+  RSArgs a = rs_args(c, p, it, c.mov_attr, c.q_nrm.p, c.q_nrm_eff.p);
   a.K = K;
   a.dist = c.dist.p;
-  a.q_nrm = c.mov_attr ? c.q_nrm_eff.p : c.q_nrm.p;
-  a.pl_signed = c.mov_attr ? 1 : 0;
   a.q_xyz = c.q_xyz.p;
   a.m_xyz = c.m_xyz.p;
   a.keep = c.keep.p;
@@ -2181,17 +2202,7 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
   a.unresolved = (c.nn_engine == SICP_NN_AUTO) ? c.unresolved.p : nullptr;
   a.state = c.dev_state.p;
   a.rec = c.ws.rec.p + rec_slot;
-  a.min_planarity = p.min_planarity;
-  a.variant = c.variant;
-  a.stat_minpl = c.variant ? -kInf : p.min_planarity;
-  a.min_change = p.min_change;
-  a.w_param = p.lsq.distance_weight;
-  for (int j = 0; j < 6; ++j) {
-    a.obs[j] = p.lsq.observed[j];
-    a.wobs[j] = p.lsq.obs_weight[j];
-  }
   for (int j = 0; j < 3; ++j) a.cm[j] = c.mov_center[j];
-  a.it = it;
   a.do_solve = do_solve ? 1 : 0;
   a.arm_stop = arm_stop ? 1 : 0;
   c.lin_hist.reserve(LH_BINS + 2);
@@ -2260,29 +2271,16 @@ void rs_fused_launch(Ctx& c, const sicp_run_params& p, int it, bool arm_stop, in
   c.phase_t.reserve(32);
   c.rs_sel.reserve(1);
   c.rs_scratch.reserve(1);
-  RSArgs a;
+  RSArgs a = rs_args(c, p, it, c.mov_attr, c.q_nrm.p, c.q_nrm_eff.p);
   a.K = K;
   a.dist = c.dist.p;
-  a.q_nrm = c.mov_attr ? c.q_nrm_eff.p : c.q_nrm.p;
-  a.pl_signed = c.mov_attr ? 1 : 0;
   a.q_xyz = c.q_xyz.p;
   a.keep = c.keep.p;
   a.resid = c.resid.p;
   a.unresolved = (c.nn_engine == SICP_NN_AUTO) ? c.unresolved.p : nullptr;
   a.state = c.dev_state.p;
   a.rec = c.ws.rec.p + rec_slot;
-  a.min_planarity = p.min_planarity;
-  a.variant = c.variant;
-  a.stat_minpl = c.variant ? -kInf : p.min_planarity;
-  a.min_change = p.min_change;
-  a.w_param = p.lsq.distance_weight;
-  for (int j = 0; j < 6; ++j) {
-    a.obs[j] = p.lsq.observed[j];
-    a.wobs[j] = p.lsq.obs_weight[j];
-  }
   for (int j = 0; j < 3; ++j) a.cm[j] = c.mov_center[j];
-  a.it = it;
-  a.do_solve = 1;
   a.arm_stop = arm_stop ? 1 : 0;
   a.hist_expected = c.lin_hist_pending ? 1 : 0;
   c.lin_hist_pending = false;  // the kernel leaves the histogram zeroed
@@ -2319,24 +2317,15 @@ void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool wa
     c.rsb_attr_set = true;
   }
   BatchRsArgs ba;
+  // k_finish_batch keeps the fixed normals; k_rs_batch replaces a.obs by the pair's PairDev::obs
   RSArgs& a = ba.proto;
-  a = RSArgs{};
+  a = rs_args(c, p, it, b.mov_attr, b.q_nrm.p, b.q_nrm_eff.p);
   a.dist = b.dist.p;
-  a.q_nrm = b.mov_attr ? b.q_nrm_eff.p : b.q_nrm.p;  // k_finish_batch keeps the fixed normals
-  a.pl_signed = b.mov_attr ? 1 : 0;
   a.q_xyz = b.q_xyz.p;
   a.keep = b.keep.p;
   a.binstore = b.binstore.p;
   a.bin_cap = b.bin_cap;
   a.m_xyz = b.m_xyz.p;
-  a.min_planarity = p.min_planarity;
-  a.variant = c.variant;
-  a.stat_minpl = c.variant ? -kInf : p.min_planarity;
-  a.min_change = p.min_change;
-  a.w_param = p.lsq.distance_weight;
-  for (int j = 0; j < 6; ++j) a.wobs[j] = p.lsq.obs_weight[j];  // a.obs: per pair, PairDev::obs
-  a.it = it;
-  a.do_solve = 1;
   a.arm_stop = 1;
   a.hist_expected = 1;  // every batched match feeds the per-pair histogram (when its predictor is valid)
   a.want_sigma = want_sigma ? 1 : 0;

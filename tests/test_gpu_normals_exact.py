@@ -327,26 +327,29 @@ def test_room_movable_normals_one_call_equals_staged(gpu):
 
 @pytest.mark.gpu
 def test_room_batch_equals_register(gpu):
-    """The batched engine (k_pca_from_knn_batch on the fixed side, k_pca_movb on the movable side)
-    on room pairs at both origins against register pair by pair."""
+    """The batched engine (the k-NN + PCA kernels over the batch's fixed side and, with
+    mov_neighbors, its movable side) under every knn_coop choice, on room pairs at both origins,
+    against register pair by pair."""
     pairs = [room_pair(), room_pair(ORIGINS["utm"])]
     with _capi.Engine() as e:
         lsq = e.lsq_params(np.zeros(6), np.zeros(6), np.zeros(6), 1.0)
         params = e.run_params(0.3, FIXED_ITERATIONS["min_change"], FIXED_ITERATIONS["max_iterations"], lsq)
         for mov_k, angle in ((0, None), (10, 10.0)):
-            for mb in (64, 1):
-                e.reset_options()
-                e.set_option("normals_scratch_mb", mb)
-                res = e.register_batch(pairs, 1000, 10, params, mov_neighbors=mov_k,
-                                       max_angle_rad=-1.0 if angle is None else float(np.deg2rad(angle)))
-                e.reset_options()
-                for i, (Xf, Xm) in enumerate(pairs):
-                    kw = {} if mov_k == 0 else {"mov_neighbors": mov_k, "max_angle_between_normals": angle}
-                    r = sb.register(Xf, Xm, engine=e, want_normals=False, **kw, **FIXED_ITERATIONS)
-                    what = f"pair {i} mov_neighbors {mov_k} scratch {mb}"
-                    b = res[i]
-                    assert b.status == 0, what
-                    assert b.iterations == r.iterations and b.n_kept == r.records[-1]["n_kept"], what
-                    tol = np.full((4, 4), 1e-12)
-                    tol[:3, 3] *= max(1.0, np.abs(Xm).max())
-                    assert (np.abs(np.array(b.H).reshape(4, 4) - r.H) <= tol).all(), what
+            for coop in (-1, 0, 1, 2):
+                for mb in (64, 1):
+                    e.reset_options()
+                    e.set_option("knn_coop", coop)
+                    e.set_option("normals_scratch_mb", mb)
+                    res = e.register_batch(pairs, 1000, 10, params, mov_neighbors=mov_k,
+                                           max_angle_rad=-1.0 if angle is None else float(np.deg2rad(angle)))
+                    e.reset_options()
+                    for i, (Xf, Xm) in enumerate(pairs):
+                        kw = {} if mov_k == 0 else {"mov_neighbors": mov_k, "max_angle_between_normals": angle}
+                        r = sb.register(Xf, Xm, engine=e, want_normals=False, **kw, **FIXED_ITERATIONS)
+                        what = f"pair {i} mov_neighbors {mov_k} knn_coop {coop} scratch {mb}"
+                        b = res[i]
+                        assert b.status == 0, what
+                        assert b.iterations == r.iterations and b.n_kept == r.records[-1]["n_kept"], what
+                        tol = np.full((4, 4), 1e-12)
+                        tol[:3, 3] *= max(1.0, np.abs(Xm).max())
+                        assert (np.abs(np.array(b.H).reshape(4, 4) - r.H) <= tol).all(), what
