@@ -37,7 +37,7 @@ def _nvcc() -> str:
 
 def _digest() -> str:
     h = hashlib.sha256()
-    for f in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.cpp")) +
+    for f in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) + list(CSRC.glob("*.cpp")) +
                     [PKG.parent / "include" / "sicp_b200.h", CLI_SRC]):
         h.update(f.name.encode())
         h.update(f.read_bytes())

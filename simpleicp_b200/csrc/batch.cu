@@ -8,7 +8,7 @@
 // pair dimension instead:
 //   upload        one cudaMemcpyAsync per cloud straight from the caller's (pinned) arrays; the
 //                 movable clouds cross PCIe while the fixed-side work runs
-//   grids         segmented counting sort over all clouds of a side (grid.cu: grid_build_batch)
+//   grids         segmented counting sort over all clouds of a side (grid.cu: grid_build)
 //   overlap       (max_overlap_distance only) bounded search of every fixed point under its pair's
 //                 prior, one scan + ordered scatter into per-pair survivor lists, one read-back
 //                 per batch; this needs the movable grids, so the fixed-side work below follows it
@@ -127,20 +127,8 @@ __global__ void k_insert_bounds(const uint32_t* __restrict__ off, int n_clouds, 
   if (i <= n_clouds) bounds[i] = scan[off[i]];
 }
 
-template <typename T>
-void swap_buf(DevBuf<T>& a, DevBuf<T>& b) {
-  std::swap(a.p, b.p);
-  std::swap(a.cap, b.cap);
-}
-
-template <typename T>
-void pinned_reserve(T*& p, size_t& cap, size_t n) {
-  if (n <= cap) return;
-  if (p) cudaFreeHost(p);
-  p = nullptr;
-  SICP_CUDA(cudaMallocHost(&p, n * sizeof(T)));
-  cap = n;
-}
+// the cell policy of every grid of this file: both sides of a batch, the map and its inserts
+CellPolicy batch_policy(const Ctx& c) { return CellPolicy{CellPolicy::kBatch, c.grid_target_occ}; }
 
 // What the stages shared by sicp_register_batch and sicp_register_to_map know about one call.
 struct PairsRun {
@@ -286,15 +274,14 @@ void batch_filter(Ctx& c, Batch& b, PairsRun& r, long long max_n_fix) {
   b.ovl_bounds.reserve((size_t)n_pairs + 1);
   // r2 as sicp_register computes it
   batch_overlap_launch(c, b, max_n_fix, r.rp->max_overlap_distance * r.rp->max_overlap_distance);
-  c.misc_counters.reserve(64);
-  scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums, c.misc_counters.p + 16);  // (its count is not used)
+  scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums);
   k_overlap_scatter<<<dim3((unsigned)((max_n_fix + 255) / 256), n_pairs), 256, 0, st>>>(b.pairs.p, b.ovl_flag.p,
                                                                                      b.ovl_scan.p, b.ovl_list.p);
   k_overlap_bounds<<<(n_pairs + 256) / 256, 256, 0, st>>>(b.pairs.p, n_pairs, b.ovl_scan.p, nf, b.ovl_bounds.p);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 2;
-  // keys_host (pinned, 8 n_pairs words since the grid builds) is free again
-  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.keys_host);
+  pinned_reserve(b.ovl_host, b.ovl_host_cap, (size_t)n_pairs + 1);
+  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.ovl_host);
   SICP_CUDA(cudaMemcpyAsync(bounds, b.ovl_bounds.p, sizeof(uint32_t) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
   SICP_CUDA(cudaStreamSynchronize(st));
   take_survivors(c, b, r, bounds);
@@ -380,11 +367,11 @@ static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
   SICP_CUDA(cudaMemsetAsync(m.n_searched.p, 0, sizeof(unsigned long long), st));
   if (max_rows > 0) map_overlap_launch(c, b, m, m.culls.p, max_rows, rr * rr, hint);  // r2 as sicp_register computes it
   map_bits_popc_launch(c, m.bits.p, nw, m.popc.p);
-  c.misc_counters.reserve(64);
-  scan_u32(c, m.popc.p, nw, m.popc_scan.p, m.sums, c.misc_counters.p + 16);  // (its count is not used)
-  // keys_host (pinned, 8 n_pairs words since the grid builds): n + 1 boundaries, then the count
-  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.keys_host);
-  unsigned long long* searched = b.keys_host + n + 1;
+  scan_u32(c, m.popc.p, nw, m.popc_scan.p, m.sums);
+  // n + 1 boundaries, then the count
+  pinned_reserve(b.ovl_host, b.ovl_host_cap, (size_t)n + 2);
+  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.ovl_host);
+  unsigned long long* searched = b.ovl_host + n + 1;
   SICP_CUDA(cudaMemcpy2DAsync(bounds, sizeof(uint32_t), m.popc_scan.p, sizeof(uint32_t) * (size_t)words,
                               sizeof(uint32_t), (size_t)n + 1, cudaMemcpyDeviceToHost, st));
   SICP_CUDA(cudaMemcpyAsync(searched, m.n_searched.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -429,14 +416,14 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
 
   // ---- movable side
   SICP_CUDA(cudaStreamWaitEvent(st, c.ev_copy, 0));
-  std::vector<BatchHostCloud> clouds((size_t)n_pairs);
+  std::vector<HostCloud> clouds((size_t)n_pairs);
   std::vector<GridView> views;
   std::vector<double> centres;
   for (int i = 0; i < n_pairs; ++i)
-    clouds[(size_t)i] = BatchHostCloud{b.mov_xyz.p + 3 * r.mo[(size_t)i], r.pd[(size_t)i].n_mov, r.mo[(size_t)i]};
+    clouds[(size_t)i] = HostCloud{b.mov_xyz.p + 3 * r.mo[(size_t)i], r.pd[(size_t)i].n_mov, r.mo[(size_t)i]};
   {
     StageTimer t(c, &c.tm.grid_mov_ms);
-    grid_build_batch(c, b, b.gmov, clouds, views, centres);
+    grid_build(c, b.gmov, clouds, batch_policy(c), views, centres);
     t.stop();
   }
   for (int i = 0; i < n_pairs; ++i) {
@@ -648,13 +635,13 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   SICP_CUDA(cudaStreamSynchronize(st));  // the fixed clouds have arrived
 
   // ---- fixed side: grids (the movable clouds are still in flight)
-  std::vector<BatchHostCloud> clouds((size_t)n_pairs);
+  std::vector<HostCloud> clouds((size_t)n_pairs);
   std::vector<GridView> views;
   std::vector<double> centres;
-  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = BatchHostCloud{b.fix_xyz.p + 3 * fo[(size_t)i], n_fix[i], fo[(size_t)i]};
+  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = HostCloud{b.fix_xyz.p + 3 * fo[(size_t)i], n_fix[i], fo[(size_t)i]};
   {
     StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build_batch(c, b, b.gfix, clouds, views, centres);
+    grid_build(c, b.gfix, clouds, batch_policy(c), views, centres);
     t.stop();
   }
   for (int i = 0; i < n_pairs; ++i) {
@@ -673,7 +660,6 @@ static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
     return;
   }
   SICP_REQUIRE(n_map > 0 && n_map < (1ll << 32), SICP_ERR_BAD_ARG, "n_map must be in [1, 2^32 - 1]");
-  if (!c.batch) c.batch = new Batch();
   if (!c.map) c.map = new MapStore();
   MapStore& m = *c.map;
   m.n = 0;  // no map until the new one is complete
@@ -687,7 +673,7 @@ static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
   std::vector<double> centres;
   {
     StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build_batch(c, *c.batch, m.grid, {BatchHostCloud{m.xyz.p, n_map, 0}}, views, centres);
+    grid_build(c, m.grid, {HostCloud{m.xyz.p, n_map, 0}}, batch_policy(c), views, centres);
     t.stop();
   }
   m.view = views[0];
@@ -732,7 +718,7 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
 // are compacted in order and gridded as one cloud; k_map_insert_flags flags the points to add (a
 // voxel key no map point has, first of its key among the new points); one scan + an ordered
 // scatter append them after the map's points in a fresh buffer, which gets its grid from set_map's
-// grid_build_batch call.  Only then are the two swapped in, so a failure leaves the map as it was,
+// grid_build call.  Only then are the two swapped in, so a failure leaves the map as it was,
 // and the grown map is the one set_map would make of the same points.  Peak device memory: the
 // old and the new map (coordinates and grid) plus the staged clouds.
 static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
@@ -758,8 +744,6 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
                "n_map + the points of the clouds must be below 2^32 (the limit of sicp_set_map)");
   if (n_added) std::fill(n_added, n_added + n_clouds, 0);
   if (nt == 0) return;
-  if (!c.batch) c.batch = new Batch();
-  Batch& b = *c.batch;
   cudaStream_t st = c.stream;
 
   // ---- stage and move the clouds, flag and compact their finite points
@@ -782,8 +766,7 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
   m.fin_scan.reserve((size_t)nt + 1);
   k_insert_stage<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T, m.fin_flag.p);
   c.tm.kernel_launches += 1;
-  c.misc_counters.reserve(64);
-  scan_u32(c, m.fin_flag.p, nt, m.fin_scan.p, m.sums, c.misc_counters.p + 16);  // (its count is not used)
+  scan_u32(c, m.fin_flag.p, nt, m.fin_scan.p, m.sums);
   pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
   SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.fin_scan.p + nt, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   SICP_CUDA(cudaStreamSynchronize(st));
@@ -798,12 +781,12 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
   // ---- the points to add, and how many per cloud (one read-back)
   std::vector<GridView> views;
   std::vector<double> centres;
-  grid_build_batch(c, b, m.gnew, {BatchHostCloud{m.fin_xyz.p, n_fin, 0}}, views, centres);
+  grid_build(c, m.gnew, {HostCloud{m.fin_xyz.p, n_fin, 0}}, batch_policy(c), views, centres);
   m.ins_flag.reserve((size_t)nt);
   m.ins_scan.reserve((size_t)nt + 1);
   SICP_CUDA(cudaMemsetAsync(m.ins_flag.p, 0, sizeof(uint32_t) * (size_t)nt, st));
   map_insert_flags_launch(c, m.view, views[0], m.fin_xyz.p, m.fin_idx.p, n_fin, voxel, m.ins_flag.p);
-  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums, c.misc_counters.p + 16);
+  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums);
   m.ins_bounds.reserve((size_t)n_clouds + 1);
   k_insert_bounds<<<(n_clouds + 256) / 256, 256, 0, st>>>(m.ins_off.p, n_clouds, m.ins_scan.p, m.ins_bounds.p);
   SICP_CUDA(cudaGetLastError());
@@ -820,23 +803,15 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
     k_insert_scatter<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p + 3 * m.n);
     SICP_CUDA(cudaGetLastError());
     c.tm.kernel_launches += 1;
-    grid_build_batch(c, b, m.grid_next, {BatchHostCloud{m.xyz_next.p, n_new, 0}}, views, centres);  // as set_map
+    grid_build(c, m.grid_next, {HostCloud{m.xyz_next.p, n_new, 0}}, batch_policy(c), views, centres);  // as set_map
     SICP_CUDA(cudaStreamSynchronize(st));
-    swap_buf(m.xyz, m.xyz_next);
-    swap_buf(m.grid.recs, m.grid_next.recs);
-    swap_buf(m.grid.cell_table, m.grid_next.cell_table);
-    swap_buf(m.grid.fill, m.grid_next.fill);
-    swap_buf(m.grid.cid, m.grid_next.cid);
-    swap_buf(m.grid.block_sums, m.grid_next.block_sums);
+    m.xyz.swap(m.xyz_next);
+    m.grid.swap(m.grid_next);
     m.view = views[0];
     m.n = n_new;
     // the old map's buffers: one map stays resident between inserts
     m.xyz_next.release();
-    m.grid_next.recs.release();
-    m.grid_next.cell_table.release();
-    m.grid_next.fill.release();
-    m.grid_next.cid.release();
-    m.grid_next.block_sums.release();
+    m.grid_next.release();
   }
   if (n_added)
     for (int i = 0; i < n_clouds; ++i) n_added[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];

@@ -285,6 +285,7 @@ int32_t sicp_create(int32_t device, void* cuda_stream, sicp_ctx** out) {
     c.ws.scal.reserve(256);
     c.ws.counters.reserve(64);
     c.ws.minkey.reserve(16);
+    c.misc_counters.reserve(16);
     c.dev_state.reserve(1);
     SICP_CUDA(cudaMemsetAsync(c.dev_state.p, 0, sizeof(DevState), c.stream));
     SICP_CUDA(cudaStreamSynchronize(c.stream));
@@ -313,6 +314,7 @@ int32_t sicp_destroy(sicp_ctx* ctx) {
   c.map = nullptr;
   if (c.rec_host) cudaFreeHost(c.rec_host);
   if (c.scal_host) cudaFreeHost(c.scal_host);
+  if (c.grid_host) cudaFreeHost(c.grid_host);
   delete ctx;
   return SICP_OK;
 }
@@ -443,7 +445,7 @@ int32_t sicp_set_clouds(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, con
   c.gfix.built = false;
   {
     StageTimer t(c, &c.tm.grid_mov_ms);
-    grid_build(c, c.gmov, c.mov_xyz.p, n_mov);
+    grid_build_pair(c, c.gmov, c.mov_xyz.p, n_mov);
     make_float4_copy(c);
     t.stop();
   }
@@ -490,7 +492,7 @@ int32_t sicp_estimate_normals(sicp_ctx* ctx, int32_t neighbors, float* nx, float
   require_selected(c);
   if (!c.gfix.built) {
     StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build(c, c.gfix, c.fix_xyz.p, c.n_fix);
+    grid_build_pair(c, c.gfix, c.fix_xyz.p, c.n_fix);
     t.stop();
   }
   StageTimer t(c, &c.tm.normals_ms);
@@ -954,13 +956,13 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
   };
   auto build_mov = [&]() {
     StageTimer t(c, &c.tm.grid_mov_ms);
-    grid_build(c, c.gmov, c.mov_xyz.p, n_mov);
+    grid_build_pair(c, c.gmov, c.mov_xyz.p, n_mov);
     make_float4_copy(c);
     t.stop();
   };
   auto build_fix = [&]() {
     StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build(c, c.gfix, c.fix_xyz.p, n_fix);
+    grid_build_pair(c, c.gfix, c.fix_xyz.p, n_fix);
     t.stop();
   };
   // pc_mov.estimate_normals(mov_neighbors) on the movable grid just built: the attributes
@@ -1149,11 +1151,14 @@ int32_t sicp_debug_grid_params(sicp_ctx* ctx, int32_t side, double o[3], double*
   SICP_REQUIRE(o && h && dims, SICP_ERR_BAD_ARG, "NULL argument");
   const Grid& g = (side == 0) ? c.gfix : c.gmov;
   SICP_REQUIRE(g.built, SICP_ERR_STATE, "that grid has not been built");
-  for (int a = 0; a < 3; ++a) {
-    o[a] = g.o[a];
-    dims[a] = g.dims[a];
-  }
-  *h = g.h;
+  const GridView& v = g.view;
+  o[0] = v.ox;
+  o[1] = v.oy;
+  o[2] = v.oz;
+  dims[0] = v.nx;
+  dims[1] = v.ny;
+  dims[2] = v.nz;
+  *h = v.h;
   API_END
 }
 

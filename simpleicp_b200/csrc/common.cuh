@@ -6,6 +6,7 @@
 
 #include <limits>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/sicp_b200.h"
@@ -58,7 +59,21 @@ struct DevBuf {
     SICP_CUDA(cudaMalloc(&p, (n + 8) * sizeof(T)));
     cap = n;
   }
+  void swap(DevBuf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+  }
 };
+
+// pinned host buffer of at least n elements, grown on demand (contents not kept)
+template <typename T>
+void pinned_reserve(T*& p, size_t& cap, size_t n) {
+  if (n <= cap) return;
+  if (p) cudaFreeHost(p);
+  p = nullptr;
+  SICP_CUDA(cudaMallocHost(&p, n * sizeof(T)));
+  cap = n;
+}
 
 // ------------------------------------------------------------------------------------------
 // Geometry types

@@ -1,40 +1,52 @@
 // ctx.cuh — the context behind sicp_ctx and the stage entry points each .cu implements.
 #pragma once
 #include "common.cuh"
+#include "grid_plan.h"
 #include "reject_solve.cuh"
 #include "upload.cuh"
 
 namespace sicp {
 
-// Cell-sorted copy of one cloud + its uniform grid (HBM resident, L2 resident for <= ~2M points).
-struct Grid {
-  DevBuf<Rec> recs;              // n points, sorted by cell
-  DevBuf<uint32_t> cell_start;   // n_cells + 1
+// Cell-sorted records and cell table of the clouds of one grid build (grid.cu: grid_build), HBM
+// resident (L2 resident for <= ~2M points).
+struct GridBufs {
+  DevBuf<Rec> recs;              // the points of all clouds, sorted by cell within each cloud
+  DevBuf<uint32_t> cell_table;   // every cloud's cells + 1 end sentinel: global record positions
   DevBuf<uint32_t> cid;          // scratch: cell id per point
   DevBuf<uint32_t> fill;         // scratch: per-cell counter
   DevBuf<uint32_t> block_sums;   // scratch for the scan
-  double o[3] = {0, 0, 0};
-  double h = 1.0;
-  int dims[3] = {1, 1, 1};
-  long long n = 0;
-  long long n_cells = 0;
-  long long n_occupied = 0;
-  bool built = false;
-  GridView view() const {
-    GridView v;
-    v.recs = recs.p;
-    v.cell_start = cell_start.p;
-    v.ox = o[0];
-    v.oy = o[1];
-    v.oz = o[2];
-    v.h = h;
-    v.inv_h = 1.0 / h;
-    v.nx = dims[0];
-    v.ny = dims[1];
-    v.nz = dims[2];
-    v.n_points = n;
-    return v;
+  void swap(GridBufs& o) {
+    recs.swap(o.recs);
+    cell_table.swap(o.cell_table);
+    cid.swap(o.cid);
+    fill.swap(o.fill);
+    block_sums.swap(o.block_sums);
   }
+  void release() {
+    recs.release();
+    cell_table.release();
+    cid.release();
+    fill.release();
+    block_sums.release();
+  }
+};
+
+// One cloud of a grid build (filled by the host from the bounding boxes).
+struct CloudPlan {
+  const double* xyz;
+  long long n;
+  long long rec_base;   // position of its first record in the shared record array (= point offset)
+  long long cell_base;  // first entry of its cell table in the shared table
+  double ox, oy, oz, h, inv_h;
+  int nx, ny, nz, pad;
+};
+
+// A grid of the one-pair context (sicp_set_clouds, sicp_estimate_normals, sicp_register): one
+// cloud under the one-pair cell policy (grid.cu: grid_build_pair).
+struct Grid {
+  GridBufs bufs;
+  GridView view{};
+  bool built = false;
 };
 
 // Workspace of the fused reject + solve kernel (all device memory).
@@ -128,8 +140,13 @@ struct Ctx {
   DevBuf<DevState> dev_state;
   int rs_parity = 0;
   DevBuf<unsigned int> compact_sums;
-  DevBuf<unsigned long long> bbox_keys;   // grid build scratch (kept apart from the select workspace)
-  DevBuf<unsigned int> misc_counters;     // grid build / API scratch counters
+  // grid build scratch (grid.cu: grid_build), kept apart from the select workspace
+  DevBuf<unsigned long long> bbox_keys;   // 6 per cloud
+  DevBuf<unsigned int> grid_occ;          // occupied cells per cloud
+  DevBuf<CloudPlan> grid_plans;           // the plan table of a build of several clouds
+  unsigned long long* grid_host = nullptr;  // pinned: bounding-box keys, then occupancies
+  size_t grid_host_cap = 0;
+  DevBuf<unsigned int> misc_counters;     // API scratch counters
   DevBuf<unsigned char> flush_buf;        // 256 MiB scratch for cold-L2 measurements
   DevBuf<unsigned long long> phase_t;     // %globaltimer stamps of the reject/solve kernel
   DevBuf<unsigned int> grid_bar;          // grid barrier of the cooperative reject/solve kernel
@@ -181,30 +198,11 @@ struct PairDev {
   double obs[6];               // rbp_observed_values of this pair (radians)
 };
 
-// One cloud of a batched grid build (filled by the host from the bounding boxes).
-struct CloudPlan {
-  const double* xyz;
-  long long n;
-  long long rec_base;   // position of its first record in the shared record array (= point offset)
-  long long cell_base;  // first entry of its cell table in the shared table
-  double ox, oy, oz, h, inv_h;
-  int nx, ny, nz, pad;
-};
-
-// The grids of one side (all fixed or all movable clouds of a batch): one record array, one cell table.
-struct BatchGrid {
-  DevBuf<Rec> recs;
-  DevBuf<uint32_t> cell_table, fill, cid, block_sums;
-};
-
 struct Batch {
   int n_pairs = 0;
   long long Kmax = 0, total_fix = 0, total_mov = 0, max_n_mov = 0;  // max_n_mov: the largest movable cloud
   DevBuf<double> fix_xyz, mov_xyz;  // concatenated clouds
-  BatchGrid gfix, gmov;
-  DevBuf<unsigned int> occ;
-  DevBuf<unsigned long long> bbox_keys;
-  DevBuf<CloudPlan> plans;
+  GridBufs gfix, gmov;
   DevBuf<PairDev> pairs;
   // per-query arrays, n_pairs x Kmax
   DevBuf<long long> sel_idx, nn_idx;
@@ -235,8 +233,8 @@ struct Batch {
   int* flags_host = nullptr;                 // pinned
   sicp_pair_result* results_host = nullptr;  // pinned
   size_t flags_cap = 0, results_cap = 0;
-  unsigned long long* keys_host = nullptr;   // pinned: bounding boxes / occupancies
-  size_t keys_cap = 0;
+  unsigned long long* ovl_host = nullptr;    // pinned: what the overlap filters read back
+  size_t ovl_host_cap = 0;
   // What sicp_get_batch_outputs reads of the last sicp_register_batch / sicp_register_to_map.
   // out_valid is cleared on entry of those two calls and of sicp_set_map, and set only when one of
   // the two returns successfully; the vectors are per pair of that call.
@@ -257,7 +255,7 @@ struct Batch {
   ~Batch() {
     if (flags_host) cudaFreeHost(flags_host);
     if (results_host) cudaFreeHost(results_host);
-    if (keys_host) cudaFreeHost(keys_host);
+    if (ovl_host) cudaFreeHost(ovl_host);
     if (rec_host) cudaFreeHost(rec_host);
     if (T_host) cudaFreeHost(T_host);
   }
@@ -272,12 +270,12 @@ struct MapCull {
 };
 
 // The resident fixed cloud of sicp_register_to_map (sicp_set_map): its coordinates and ONE grid,
-// built by grid_build_batch with the map as its only cloud, so that its cell plan is the one a
-// batch would make for it.  Every pair of a sicp_register_to_map call takes `view` as its fixed
-// grid, with fix_off = 0.
+// built by grid_build with the map as its only cloud and the batch cell policy, so that its cell
+// plan is the one a batch would make for it.  Every pair of a sicp_register_to_map call takes
+// `view` as its fixed grid, with fix_off = 0.
 struct MapStore {
   DevBuf<double> xyz;
-  BatchGrid grid;
+  GridBufs grid;
   GridView view{};
   long long n = 0;
   // overlap filter: one bit per (scan, map point), its per-word popcounts and their prefix sum
@@ -294,7 +292,7 @@ struct MapStore {
   DevBuf<double> ins_xyz, fin_xyz, xyz_next;
   DevBuf<uint32_t> fin_flag, fin_scan, fin_idx, ins_flag, ins_scan, ins_off, ins_bounds;
   DevBuf<Rigid> ins_T;
-  BatchGrid gnew, grid_next;
+  GridBufs gnew, grid_next;
   uint32_t* bounds_host = nullptr;  // pinned: n_clouds + 1 boundaries
   size_t bounds_cap = 0;
   ~MapStore() {
@@ -303,12 +301,21 @@ struct MapStore {
 };
 
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
-void grid_build(Ctx& c, Grid& g, const double* xyz_dev, long long n);
+struct HostCloud {
+  const double* xyz_dev;
+  long long n;
+  long long point_off;  // first record of this cloud in the shared record array
+};
+// The grids of clouds in g, one segmented counting sort; views[i] is cloud i's grid, centres
+// (3 per cloud) the centre o + 0.5 dims h of its box.  Cell sizes follow the policy (grid_plan.h).
+void grid_build(Ctx& c, GridBufs& g, const std::vector<HostCloud>& clouds, const CellPolicy& policy,
+                std::vector<GridView>& views, std::vector<double>& centres);
+// one cloud under the one-pair cell policy, into a grid of the one-pair context
+void grid_build_pair(Ctx& c, Grid& g, const double* xyz_dev, long long n);
 void make_float4_copy(Ctx& c);
 // Exclusive prefix sum of n uint32 values (four launches): out[0 .. n], out[n] = the total.
-// block_sums is scratch; n_nonzero (device) is incremented by the number of non-zero inputs.
-void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums,
-              unsigned int* n_nonzero);
+// block_sums is scratch.
+void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums);
 
 // 1-NN of K transformed queries into the movable cloud; fused point-to-plane distance.
 // If out_d2 != nullptr the squared NN distance is written instead of the plane distance epilogue
@@ -358,13 +365,6 @@ void transform_launch(Ctx& c, const Rigid& T, const double* in_dev, double* out_
 void gather_queries_launch(Ctx& c);
 
 // batched launches
-struct BatchHostCloud {
-  const double* xyz_dev;
-  long long n;
-  long long point_off;  // first record of this cloud in the shared record array
-};
-void grid_build_batch(Ctx& c, Batch& b, BatchGrid& bg, const std::vector<BatchHostCloud>& clouds,
-                      std::vector<GridView>& views, std::vector<double>& centres /* 3 per cloud */);
 // with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud;
 // fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::fix_xyz or MapStore::xyz)
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);

@@ -1249,13 +1249,13 @@ void match_launch(Ctx& c, bool with_distance, double* out_d2, cudaEvent_t mid, b
   const int rmax = use_bf ? c.grid_max_rings : (1 << 30);
   if (c.match_group == 1) {
     k_match_grid<<<(unsigned)((K + 127) / 128), 128, 0, c.stream>>>(
-        c.gmov.view(), c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
+        c.gmov.view, c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
         with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
   } else {
     const int mg = match_lanes(c, K, 2);
     with_lanes<2, 4, 8, 16>(mg, [&](auto L) {
       launch_kernel(k_match_grid_coop<decltype(L)::value>, dim3((unsigned)((K * mg + 127) / 128)), dim3(128), 0,
-                    c.stream, pdl, c.gmov.view(), c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
+                    c.stream, pdl, c.gmov.view, c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
                     with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
     });
   }

@@ -539,7 +539,7 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
   if (b == nullptr) {
     const Grid& grid = movable ? c.gmov : c.gfix;
     const long long n_q = movable ? c.n_mov : c.K;
-    SICP_REQUIRE((long long)k <= grid.n, SICP_ERR_BAD_ARG,
+    SICP_REQUIRE((long long)k <= grid.view.n_points, SICP_ERR_BAD_ARG,
                  name + " exceeds the number of points in the " + (movable ? "movable" : "fixed") + " cloud");
     // the neighbour lists leave the SM only when somebody wants to look at them (option "keep_knn")
     const bool keep = !movable && c.keep_knn != 0;
@@ -550,7 +550,7 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
     if (!movable) c.knn_k = keep ? k : 0;
     const long long chunk = movable ? std::min<long long>(n_q, normals_chunk_queries(c, k)) : n_q;
     c.knn_pos.reserve((size_t)std::max<long long>(chunk, 1) * k);
-    a.g = grid.view();
+    a.g = grid.view;
     a.pos = c.knn_pos.p;
     for (long long q0 = 0; q0 < n_q; q0 += chunk) {
       a.n = std::min(chunk, n_q - q0);

@@ -36,6 +36,7 @@ from scipy.spatial import cKDTree
 from oracle import simpleicp_oracle as O
 
 from simpleicp_b200 import _capi
+from test_grid_plan import first_plan
 
 U = 2.0 ** -10                                  # lattice unit (m)
 KMAX = 2 ** 25                                  # bound on every coordinate difference, in units
@@ -560,18 +561,6 @@ def faces_rounded_away(o_a, h, lo, hi, step):
     return out
 
 
-def planned_grid(X, target=3.0):
-    """The cell size and dims grid.cu picks on its first attempt (kept when the occupancy it
-    measures is within a factor 1.6 of the target, which the sliver layout below ensures)."""
-    lo = X.min(0)
-    ext = X.max(0) - lo
-    e = np.sort(ext)
-    emax = max(e[2], 1e-12)
-    area = max(e[2] * max(e[1], 1e-3 * emax), 1e-300)
-    h = max(float(np.sqrt(target * area / len(X))), emax * 1e-6)
-    return lo, h, tuple(int(max(1, np.floor(x / h) + 1)) for x in ext)
-
-
 def sliver_cloud(n_base, with_queries):
     """A dense sheet (~3 points per 4 cm cell, 2 m x 4 m at the UTM origin) and, ten cells above
     it, 8 slivers across y faces (neighbour rows of ring 1, or the guard) and 4 across x faces
@@ -584,7 +573,7 @@ def sliver_cloud(n_base, with_queries):
     nq = 12
     n = n_base + (3 if with_queries else 2) * nq
     o = base.min(0)
-    _, h, _ = planned_grid(np.concatenate((base, np.tile(o, (n - n_base, 1)))))
+    _, h, _, _ = first_plan(np.concatenate((base, np.tile(o, (n - n_base, 1)))))
     dims = tuple(int(np.floor((base[:, a].max() - o[a]) / h) + 1) for a in range(2))
     zc = o[2] + 10.5 * h
     xmid = o[0] + (dims[0] // 2 + 0.5) * h
@@ -595,7 +584,7 @@ def sliver_cloud(n_base, with_queries):
     assert len(fy) == 8 and len(fx) == 4
     Q, P, C = np.concatenate((Qy, Qx)), np.concatenate((Py, Px)), np.concatenate((Cy, Cx))
     X = np.concatenate(((Q,) if with_queries else ()) + (P, C, base))
-    plan = planned_grid(X)
+    plan = first_plan(X)[:3]  # the first attempt's plan, kept: its occupancy is in the band
     assert plan[1] == h and np.array_equal(plan[0], o), "the slivers changed the planned grid"
     return X, Q, plan
 

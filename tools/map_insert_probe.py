@@ -40,8 +40,9 @@ def thin_on_host(M, clouds, v):
 
 
 def first_cell_plan(P, occ=3.0, cap=1 << 25):
-    """The cell size and dims grid_build_batch (grid.cu) picks for one cloud before it refines
-    from the measured occupancy, which it skips when the cell cap binds (as for these maps)."""
+    """The cell size and dims grid_build (grid.cu) picks for one cloud under the batch policy
+    (grid_plan.h: first_cell_plan) before it refines from the measured occupancy, which it skips
+    when the cell cap binds (as for these maps)."""
     ext = P.max(axis=0) - P.min(axis=0)
     e = np.sort(ext)
     emax = max(e[2], 1e-12)
