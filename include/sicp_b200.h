@@ -358,6 +358,44 @@ int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xy
 int32_t sicp_get_map(sicp_ctx* ctx, double* xyz /*[h|d] cap x 3, or NULL*/, int64_t cap,
                      int64_t* n /*[h]*/);
 
+/* ---- how well clouds fit the map: cloud-to-map distances --------------------------------------
+ * sicp_map_distances gives every point of n_clouds clouds its nearest map point within
+ * max_distance, and with neighbors = k > 0 its signed distance along that map point's normal.
+ *  - Points: cloud i moved by H[16 i .. 16 i + 15] (row-major 4 x 4), bit for bit what
+ *    sicp_transform gives for that cloud and H, or with H NULL taken as it is.
+ *  - Nearest point: for a point p with three finite coordinates (after the move), the map point
+ *    with the smallest squared distance d2 = (dx dx + dy dy) + dz dz (the search's d2 may contract
+ *    to fused multiply-adds), the lower map index among ties.  p is within iff d2 < fl(max_distance^2),
+ *    the comparison of sicp_select_in_range (cKDTree's distance_upper_bound).  Then idx = that map
+ *    index and dist2 = its d2.  A finite point with nothing within the bound gets idx -1 and
+ *    dist2 +inf; a point with a NaN or inf coordinate gets idx -1 and dist2 NaN and is not counted.
+ *  - neighbors = k > 0: the normal (nx, ny, nz) and planarity of the matched map point m are the
+ *    float32 values sicp_estimate_normals(k) gives for m with the map as the fixed cloud (m's k
+ *    nearest map points, m included, under option "sign_mode").  plane_dist = ((px - mx) nx +
+ *    (py - my) ny) + (pz - mz) nz in double, the float32 normal promoted, no fused multiply-add:
+ *    sicp_match's point-to-plane expression, moved point minus map point.  planarity = that
+ *    planarity.  Both are NaN where idx is -1.
+ *  - n_within[i]: the within points of cloud i.
+ *  - A NULL array skips that output and a NULL entry skips that cloud (any memory kind otherwise).
+ *  - SICP_ERR_STATE: no map.  SICP_ERR_BAD_ARG, before any device work: n_clouds < 1, a negative
+ *    n[i], a NULL xyz[i] with n[i] > 0 (empty clouds are fine), a non-finite H entry, a
+ *    max_distance that is not finite and > 0 (an unbounded search is not offered), k neither 0
+ *    nor in [2, 64], k above n_map, plane_dist or planarity given with k = 0, or sum n[i] >= 2^32.
+ *  - Nothing else changes: the map, the batch outputs (sicp_get_batch_outputs), the one-pair state
+ *    (sicp_get_knn, sicp_get_residuals) and sicp_timings' fields except kernel_launches.
+ *  - Cost: a bound r walks about (2 r / h + 1)^3 map cells per point, h being the map grid's cell
+ *    size; the normals add one k-NN + PCA per within point.  Device memory: the insert's staging
+ *    buffers (about 40 B per point) plus 28 B per point and 40 B per within point, and the k-NN
+ *    scratch of option "normals_scratch_mb"; they stay on the context like the insert's.        */
+int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                           const int64_t* n /*[h]*/, const double* H /*[h] n_clouds x 16, or NULL*/,
+                           double max_distance, int32_t neighbors /*0: no normals*/,
+                           int64_t* const* idx        /*[h|d] per cloud n[i], or NULL*/,
+                           double* const* dist2       /*[h|d] per cloud n[i], or NULL*/,
+                           double* const* plane_dist  /*[h|d] per cloud n[i], or NULL*/,
+                           float* const* planarity    /*[h|d] per cloud n[i], or NULL*/,
+                           int64_t* n_within          /*[h] n_clouds, or NULL*/);
+
 /* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
  * sicp_register_batch and sicp_register_to_map report per pair only the record above.  This call
  * returns what else sicp_register returns, for every pair of the LAST successful call of either

@@ -42,7 +42,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs",
-    "sicp_map_insert", "sicp_get_map", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_map_insert", "sicp_get_map", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -170,6 +170,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
+        "sicp_map_distances": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, i32, C.POINTER(vp), C.POINTER(vp),
+                               C.POINTER(vp), C.POINTER(vp), vp],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -596,6 +598,37 @@ class Engine:
         self._check(self._lib.sicp_map_insert(self._h, n, ptrs, counts, _ptr(H), float(voxel_size), _ptr(added)))
         self.n_map += int(added.sum())
         return added
+
+    def map_distances(self, clouds, H=None, *, max_distance: float, neighbors: int = 0):
+        """sicp_map_distances: the nearest map point of every point of `clouds` (cloud i moved by
+        H[i] first when `H` (n_clouds x 4 x 4) is given) whose squared distance is below
+        max_distance^2.  Returns (idx, dist2, plane_dist, planarity, n_within): per cloud the map
+        index (int64, -1 where none) and the squared distance (float64, +inf beyond the bound, NaN
+        for a non-finite point); with `neighbors` = k > 0 per cloud the signed distance along the
+        matched map point's normal (float64) and its planarity (float32), both NaN where idx is -1,
+        else None; and the within points of each cloud (int64)."""
+        n = len(clouds)
+        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
+        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
+        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
+        if H is not None:
+            H = np.ascontiguousarray(H, dtype=np.float64)
+            if H.shape != (n, 4, 4):
+                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
+        k = int(neighbors)
+        sizes = [int(c) for c in counts]
+        idx = [np.empty(m, dtype=np.int64) for m in sizes]
+        d2 = [np.empty(m, dtype=np.float64) for m in sizes]
+        pd = [np.empty(m, dtype=np.float64) for m in sizes] if k > 0 else None
+        pl = [np.empty(m, dtype=np.float32) for m in sizes] if k > 0 else None
+        n_within = np.zeros(n, dtype=np.int64)
+
+        def arr(a):
+            return None if a is None else (C.c_void_p * n)(*[_ptr(x) for x in a])
+
+        self._check(self._lib.sicp_map_distances(self._h, n, ptrs, counts, _ptr(H), float(max_distance), k, arr(idx),
+                                                 arr(d2), arr(pd), arr(pl), _ptr(n_within)))
+        return idx, d2, pd, pl, n_within
 
     def get_map(self) -> np.ndarray:
         """sicp_get_map: the resident map, (n_map, 3) float64 in map order."""

@@ -7,6 +7,7 @@ residuals — over NCCL (gloo on CPU-only hosts for the tests of the sharding lo
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -375,6 +376,8 @@ class Map:
     ``register(X_map, scans[i], rbp_observed_values=row_i, max_overlap_distance=d, ...)``.
     ``insert(clouds, H, voxel_size=v)`` grows the map on the device by what the scans saw (one
     new point per voxel the map does not occupy) and ``points()`` reads it back.
+    ``distances(clouds, H, max_distance=d)`` tells how well clouds fit the map: every point's
+    nearest map point within d, with fitness and inlier RMSE per cloud.
     """
 
     def __init__(self, X_map, device: int = 0):
@@ -453,6 +456,47 @@ class Map:
         self.n_points = self._engine.n_map
         return added
 
+    def distances(self, clouds, H=None, *, max_distance: float, neighbors: Optional[int] = None
+                  ) -> List["CloudDistances"]:
+        """How well each cloud fits the map: the nearest map point of every point within
+        ``max_distance`` (sicp_map_distances), one CloudDistances per cloud.
+
+        ``clouds`` and ``H`` are as in ``insert``.  The rows of the table ``register`` returns for
+        the scans that registered plug in: with ``ok = [i for i in range(len(scans)) if t[i, 16] > 0]``,
+        ``m.distances([scans[i] for i in ok], t[ok, :16].reshape(-1, 4, 4), max_distance=0.5)``
+        (a scan that failed has a NaN H, which is refused).  A point is within
+        when its squared distance to the nearest map point is below max_distance^2 (cKDTree's
+        ``distance_upper_bound``); ties go to the lower map index.  ``neighbors`` = k also gives
+        the signed distance along the matched map point's normal and its planarity, estimated from
+        the k nearest map points as ``estimate_normals(k)`` would with the map as the fixed cloud.
+        The search walks about (2 max_distance / h + 1)^3 map cells per point for a map cell size
+        h, so the bound is required and finite."""
+        r = float(max_distance)
+        if not (np.isfinite(r) and r > 0):
+            raise ValueError(f"max_distance must be finite and > 0, got {max_distance}")
+        k = 0 if neighbors is None else int(neighbors)
+        if neighbors is not None and not (2 <= k <= 64 and k <= self.n_points):
+            raise ValueError(f"neighbors must be between 2 and 64 and at most the map's {self.n_points} points, "
+                             f"got {neighbors}")
+        clouds = list(clouds)
+        if not clouds:
+            raise ValueError("distances needs at least one cloud")
+        for i, X in enumerate(clouds):
+            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
+                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
+        if H is not None:
+            H = np.asarray(H, dtype=np.float64)
+            if H.shape != (len(clouds), 4, 4):
+                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
+            if not np.isfinite(H).all():
+                raise ValueError("H must be finite")
+        import torch
+
+        with torch.cuda.device(self.device):
+            idx, d2, pd, pl, n_within = self._engine.map_distances(clouds, H, max_distance=r, neighbors=k)
+        return [CloudDistances.of(idx[i], d2[i], None if pd is None else pd[i], None if pl is None else pl[i],
+                                  int(n_within[i])) for i in range(len(clouds))]
+
     def points(self) -> np.ndarray:
         """The map as it stands, (n_points, 3) float64 in map order (a copy): the points it was
         made of followed by those ``insert`` added.  ``sb.write_xyz(path, m.points())`` saves it."""
@@ -470,6 +514,35 @@ class Map:
 
     def __exit__(self, *exc):
         self.close()
+
+
+@dataclass
+class CloudDistances:
+    """One cloud's fit to the map (Map.distances).  Per point: ``index`` of the nearest map point
+    within the bound (int64, -1 where there is none), its ``distance`` (sqrt of the squared
+    distance: +inf beyond the bound, NaN for a point with a NaN or inf coordinate), and with
+    ``neighbors`` the signed ``plane_distance`` along that map point's normal and its
+    ``planarity`` (NaN where index is -1; None without ``neighbors``).  Per cloud: ``n_within``,
+    ``fitness`` = n_within / n over all n points as Open3D's evaluate_registration counts it (NaN
+    for an empty cloud), and ``rmse`` = the root mean square distance of the within points (NaN
+    when there are none)."""
+
+    index: np.ndarray
+    distance: np.ndarray
+    plane_distance: Optional[np.ndarray]
+    planarity: Optional[np.ndarray]
+    n_within: int
+    fitness: float
+    rmse: float
+
+    @classmethod
+    def of(cls, index, dist2, plane_distance, planarity, n_within: int) -> "CloudDistances":
+        index, dist2 = np.asarray(index), np.asarray(dist2, dtype=np.float64)
+        n = len(index)
+        inside = dist2[index >= 0]
+        fitness = n_within / n if n else float("nan")
+        rmse = float(np.sqrt(np.mean(inside))) if inside.size else float("nan")
+        return cls(index, np.sqrt(dist2), plane_distance, planarity, int(n_within), fitness, rmse)
 
 
 class BatchError(RuntimeError):

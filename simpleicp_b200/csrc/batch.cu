@@ -127,6 +127,41 @@ __global__ void k_insert_bounds(const uint32_t* __restrict__ off, int n_clouds, 
   if (i <= n_clouds) bounds[i] = scan[off[i]];
 }
 
+// sicp_map_distances, one thread per point j: the coordinates of its matched map point, at its
+// place among the within points (scan = exclusive prefix sum of the within flags)
+__global__ void __launch_bounds__(256)
+    k_dist_gather(const double* __restrict__ map_xyz, const long long* __restrict__ idx, long long n,
+                  const uint32_t* __restrict__ within, const uint32_t* __restrict__ scan, double* __restrict__ m_xyz) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n || !within[j]) return;
+  const long long f = scan[j], m = idx[j];
+  m_xyz[3 * f + 0] = map_xyz[3 * m + 0];
+  m_xyz[3 * f + 1] = map_xyz[3 * m + 1];
+  m_xyz[3 * f + 2] = map_xyz[3 * m + 2];
+}
+
+// the signed distance of point j along its matched map point's normal, plane_distance's expression
+// (nn.cu): ((px - mx) nx + (py - my) ny) + (pz - mz) nz in double, the float32 normal promoted, no
+// fused multiply-add; and that normal's planarity.  NaN for a point without a match.
+__global__ void __launch_bounds__(256)
+    k_dist_plane(const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ within,
+                 const uint32_t* __restrict__ scan, const double* __restrict__ m_xyz, const float4* __restrict__ nrm,
+                 double* __restrict__ plane, float* __restrict__ planarity) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  if (!within[j]) {
+    plane[j] = __longlong_as_double(0x7ff8000000000000ll);
+    planarity[j] = __int_as_float(0x7fc00000);
+    return;
+  }
+  const long long f = scan[j];
+  const float4 nr = nrm[f];
+  const double dx = xyz[3 * j + 0] - m_xyz[3 * f + 0], dy = xyz[3 * j + 1] - m_xyz[3 * f + 1],
+               dz = xyz[3 * j + 2] - m_xyz[3 * f + 2];
+  plane[j] = __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)), __dmul_rn(dz, (double)nr.z));
+  planarity[j] = nr.w;
+}
+
 // the cell policy of every grid of this file: both sides of a batch, the map and its inserts
 CellPolicy batch_policy(const Ctx& c) { return CellPolicy{CellPolicy::kBatch, c.grid_target_occ}; }
 
@@ -714,20 +749,13 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
   run_pairs(c, b, r, m.xyz.p, &m, m.n, out, n_selected);
 }
 
-// sicp_map_insert.  The clouds are staged into one buffer and moved there; their finite points
-// are compacted in order and gridded as one cloud; k_map_insert_flags flags the points to add (a
-// voxel key no map point has, first of its key among the new points); one scan + an ordered
-// scatter append them after the map's points in a fresh buffer, which gets its grid from set_map's
-// grid_build call.  Only then are the two swapped in, so a failure leaves the map as it was,
-// and the grown map is the one set_map would make of the same points.  Peak device memory: the
-// old and the new map (coordinates and grid) plus the staged clouds.
-static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
-                       double voxel, int64_t* n_added) {
-  if (c.batch) c.batch->out_valid = false;
+// The clouds of sicp_map_insert and sicp_map_distances, checked before any device work: their
+// offsets in the concatenation, n_clouds + 1 of them, the count saturated at 2^40 (both callers'
+// limits are below 2^32).
+static std::vector<long long> check_clouds(int n_clouds, const double* const* xyz, const int64_t* n, const double* H) {
   SICP_REQUIRE(n_clouds >= 1, SICP_ERR_BAD_ARG, "n_clouds must be >= 1");
   SICP_REQUIRE(xyz && n, SICP_ERR_BAD_ARG, "NULL argument");
-  SICP_REQUIRE(std::isfinite(voxel) && voxel > 0, SICP_ERR_BAD_ARG, "voxel_size must be finite and > 0");
-  constexpr long long kMany = 1ll << 40;  // saturation of the point count (the limit below is 2^32)
+  constexpr long long kMany = 1ll << 40;
   std::vector<long long> off((size_t)n_clouds + 1, 0);
   for (int i = 0; i < n_clouds; ++i) {
     SICP_REQUIRE(n[i] >= 0, SICP_ERR_BAD_ARG, "cloud " + std::to_string(i) + " has a negative point count");
@@ -737,16 +765,15 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
   if (H)
     for (int j = 0; j < 16 * n_clouds; ++j)
       SICP_REQUIRE(std::isfinite(H[j]), SICP_ERR_BAD_ARG, "H has non-finite entries");
-  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
-  MapStore& m = *c.map;
-  const long long nt = off[(size_t)n_clouds];
-  SICP_REQUIRE(m.n + nt < (1ll << 32), SICP_ERR_BAD_ARG,
-               "n_map + the points of the clouds must be below 2^32 (the limit of sicp_set_map)");
-  if (n_added) std::fill(n_added, n_added + n_clouds, 0);
-  if (nt == 0) return;
-  cudaStream_t st = c.stream;
+  return off;
+}
 
-  // ---- stage and move the clouds, flag and compact their finite points
+// The clouds uploaded into MapStore::ins_xyz (off from check_clouds, nt = off[n_clouds] > 0 points)
+// and moved there by k_insert_stage, which also writes fin_flag.
+static void stage_clouds(Ctx& c, MapStore& m, int n_clouds, const double* const* xyz, const int64_t* n,
+                         const double* H, const std::vector<long long>& off) {
+  cudaStream_t st = c.stream;
+  const long long nt = off[(size_t)n_clouds];
   m.ins_xyz.reserve(3 * (size_t)nt);
   for (int i = 0; i < n_clouds; ++i)
     if (n[i] > 0) upload_to_device(c, m.ins_xyz.p + 3 * off[(size_t)i], xyz[i], sizeof(double) * 3 * (size_t)n[i]);
@@ -761,11 +788,36 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
     SICP_CUDA(cudaMemcpyAsync(m.ins_T.p, hT.data(), sizeof(Rigid) * hT.size(), cudaMemcpyHostToDevice, st));
     T = m.ins_T.p;
   }
-  const unsigned blocks = (unsigned)((nt + 255) / 256);
   m.fin_flag.reserve((size_t)nt);
-  m.fin_scan.reserve((size_t)nt + 1);
-  k_insert_stage<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T, m.fin_flag.p);
+  k_insert_stage<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T, m.fin_flag.p);
   c.tm.kernel_launches += 1;
+}
+
+// sicp_map_insert.  The clouds are staged into one buffer and moved there; their finite points
+// are compacted in order and gridded as one cloud; k_map_insert_flags flags the points to add (a
+// voxel key no map point has, first of its key among the new points); one scan + an ordered
+// scatter append them after the map's points in a fresh buffer, which gets its grid from set_map's
+// grid_build call.  Only then are the two swapped in, so a failure leaves the map as it was,
+// and the grown map is the one set_map would make of the same points.  Peak device memory: the
+// old and the new map (coordinates and grid) plus the staged clouds.
+static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
+                       double voxel, int64_t* n_added) {
+  if (c.batch) c.batch->out_valid = false;
+  SICP_REQUIRE(std::isfinite(voxel) && voxel > 0, SICP_ERR_BAD_ARG, "voxel_size must be finite and > 0");
+  const std::vector<long long> off = check_clouds(n_clouds, xyz, n, H);
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  const long long nt = off[(size_t)n_clouds];
+  SICP_REQUIRE(m.n + nt < (1ll << 32), SICP_ERR_BAD_ARG,
+               "n_map + the points of the clouds must be below 2^32 (the limit of sicp_set_map)");
+  if (n_added) std::fill(n_added, n_added + n_clouds, 0);
+  if (nt == 0) return;
+  cudaStream_t st = c.stream;
+
+  // ---- stage and move the clouds, flag and compact their finite points
+  stage_clouds(c, m, n_clouds, xyz, n, H, off);
+  const unsigned blocks = (unsigned)((nt + 255) / 256);
+  m.fin_scan.reserve((size_t)nt + 1);
   scan_u32(c, m.fin_flag.p, nt, m.fin_scan.p, m.sums);
   pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
   SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.fin_scan.p + nt, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
@@ -829,6 +881,82 @@ static void get_map(Ctx& c, double* xyz, int64_t cap, int64_t* n) {
   }
 }
 
+// sicp_map_distances.  The clouds are staged and moved as sicp_map_insert's are; k_map_nearest
+// finds each point's nearest map point within the bound (nn.cu); one scan over the within flags
+// gives the per-cloud counts (one read-back) and the places of the within points, whose matched
+// map points are gathered and get the normal estimate of sicp_estimate_normals in the map grid;
+// k_dist_plane then writes the plane distances.  Every output is written to MapStore buffers and
+// copied per cloud to the caller's arrays.  Nothing else of the context changes: the map, the
+// batch outputs and the one-pair state stay as they are.
+static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
+                          double max_distance, int k, int64_t* const* idx, double* const* dist2,
+                          double* const* plane_dist, float* const* planarity, int64_t* n_within) {
+  SICP_REQUIRE(std::isfinite(max_distance) && max_distance > 0, SICP_ERR_BAD_ARG,
+               "max_distance must be finite and > 0");
+  SICP_REQUIRE(k == 0 || (k >= 2 && k <= 64), SICP_ERR_BAD_ARG,
+               "neighbors must be 0 or between 2 and 64 (got " + std::to_string(k) + ")");
+  SICP_REQUIRE(k > 0 || (!plane_dist && !planarity), SICP_ERR_BAD_ARG,
+               "plane_dist and planarity need the map's normals: neighbors must be > 0");
+  const std::vector<long long> off = check_clouds(n_clouds, xyz, n, H);
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  SICP_REQUIRE(k <= m.n, SICP_ERR_BAD_ARG, "neighbors exceeds the number of map points");
+  const long long nt = off[(size_t)n_clouds];
+  SICP_REQUIRE(nt < (1ll << 32), SICP_ERR_BAD_ARG, "the points of the clouds must be below 2^32 (32-bit offsets)");
+  if (n_within) std::fill(n_within, n_within + n_clouds, 0);
+  if (nt == 0) return;
+  cudaStream_t st = c.stream;
+  const unsigned blocks = (unsigned)((nt + 255) / 256);
+
+  // ---- nearest map point of every staged point, within flags and their per-cloud counts
+  stage_clouds(c, m, n_clouds, xyz, n, H, off);
+  m.dst_idx.reserve((size_t)nt);
+  m.dst_d2.reserve((size_t)nt);
+  m.ins_flag.reserve((size_t)nt);
+  m.ins_scan.reserve((size_t)nt + 1);
+  map_nearest_launch(c, m.view, m.ins_xyz.p, nt, max_distance * max_distance, m.dst_idx.p, m.dst_d2.p, m.ins_flag.p);
+  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums);
+  m.ins_bounds.reserve((size_t)n_clouds + 1);
+  k_insert_bounds<<<(n_clouds + 256) / 256, 256, 0, st>>>(m.ins_off.p, n_clouds, m.ins_scan.p, m.ins_bounds.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
+  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_bounds.p, sizeof(uint32_t) * ((size_t)n_clouds + 1),
+                            cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  const long long n_in = m.bounds_host[n_clouds];
+
+  // ---- normals of the matched map points and the plane distances
+  if (k > 0) {
+    m.dst_plane.reserve((size_t)nt);
+    m.dst_pl.reserve((size_t)nt);
+    if (n_in > 0) {
+      m.dst_mxyz.reserve(3 * (size_t)n_in);
+      m.dst_nrm.reserve((size_t)n_in);
+      k_dist_gather<<<blocks, 256, 0, st>>>(m.xyz.p, m.dst_idx.p, nt, m.ins_flag.p, m.ins_scan.p, m.dst_mxyz.p);
+      SICP_CUDA(cudaGetLastError());
+      c.tm.kernel_launches += 1;
+      map_normals_launch(c, m.view, m.dst_mxyz.p, n_in, k, m.dst_nrm.p, m.dst_pos);
+    }
+    k_dist_plane<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.dst_mxyz.p, m.dst_nrm.p,
+                                         m.dst_plane.p, m.dst_pl.p);
+    SICP_CUDA(cudaGetLastError());
+    c.tm.kernel_launches += 1;
+  }
+
+  // ---- each requested cloud's slice to the caller (any memory kind)
+  for (int i = 0; i < n_clouds; ++i) {
+    const size_t s = (size_t)off[(size_t)i], cnt = (size_t)n[i];
+    if (idx && idx[i]) copy_any(c, idx[i], m.dst_idx.p + s, sizeof(long long) * cnt);
+    if (dist2 && dist2[i]) copy_any(c, dist2[i], m.dst_d2.p + s, sizeof(double) * cnt);
+    if (plane_dist && plane_dist[i]) copy_any(c, plane_dist[i], m.dst_plane.p + s, sizeof(double) * cnt);
+    if (planarity && planarity[i]) copy_any(c, planarity[i], m.dst_pl.p + s, sizeof(float) * cnt);
+  }
+  SICP_CUDA(cudaStreamSynchronize(st));
+  if (n_within)
+    for (int i = 0; i < n_clouds; ++i) n_within[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];
+}
+
 }  // namespace sicp
 
 using namespace sicp;
@@ -880,6 +1008,14 @@ extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double
 
 extern "C" int32_t sicp_get_map(sicp_ctx* ctx, double* xyz, int64_t cap, int64_t* n) {
   SICP_BATCH_API(get_map(c, xyz, cap, n))
+}
+
+extern "C" int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                      const double* H, double max_distance, int32_t neighbors, int64_t* const* idx,
+                                      double* const* dist2, double* const* plane_dist, float* const* planarity,
+                                      int64_t* n_within) {
+  SICP_BATCH_API(map_distances(c, n_clouds, xyz, n, H, max_distance, neighbors, idx, dist2, plane_dist, planarity,
+                               n_within))
 }
 
 extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double* const* mov_xyz_out,

@@ -293,6 +293,18 @@ struct MapStore {
   DevBuf<uint32_t> fin_flag, fin_scan, fin_idx, ins_flag, ins_scan, ins_off, ins_bounds;
   DevBuf<Rigid> ins_T;
   GridBufs gnew, grid_next;
+  // sicp_map_distances (batch.cu: map_distances) stages its clouds in ins_xyz (with ins_off,
+  // ins_T, fin_flag) and takes ins_flag / ins_scan / ins_bounds for its within flags, their prefix
+  // sum and the per-cloud boundaries.  Its own buffers, per staged point: the map index and d2
+  // of the nearest map point, and with normals the plane distance and planarity (28 B); per
+  // within point: the matched map point's coordinates and its (normal, planarity) (40 B); and the
+  // k-NN positions of one chunk of option "normals_scratch_mb".  They stay allocated like the
+  // insert's staging buffers.
+  DevBuf<long long> dst_idx;
+  DevBuf<double> dst_d2, dst_plane, dst_mxyz;
+  DevBuf<float> dst_pl;
+  DevBuf<float4> dst_nrm;
+  DevBuf<uint32_t> dst_pos;
   uint32_t* bounds_host = nullptr;  // pinned: n_clouds + 1 boundaries
   size_t bounds_cap = 0;
   ~MapStore() {
@@ -387,6 +399,18 @@ void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, lo
 // fresh with a smaller index has the same voxel key floor(p / voxel) (flag is zeroed by the caller)
 void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh, const double* fin_xyz,
                              const uint32_t* fin_idx, long long n_fin, double voxel, uint32_t* flag);
+// sicp_map_distances' bounded nearest search (nn.cu: k_map_nearest), one lane group per point j of
+// xyz (n points): the nearest map point (lowest index among ties) when its d2 < cap2 ->
+// idx[j], d2[j], within[j] = 1; else idx -1, within 0 and d2 +inf (finite point) or NaN (a NaN or
+// inf coordinate).
+void map_nearest_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double cap2, long long* idx,
+                        double* d2, uint32_t* within);
+// k-NN (self included) + PCA of n query points in the map grid (normals.cu: the estimate of
+// sicp_estimate_normals, chunked by option "normals_scratch_mb"): out[i] = (nx, ny, nz,
+// planarity) float32; pos is the caller's scratch, grown to one chunk.  Nothing of the one-pair
+// context is written.
+void map_normals_launch(Ctx& c, const GridView& map, const double* q_xyz, long long n, int k, float4* out,
+                        DevBuf<uint32_t>& pos);
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 // sicp_get_batch_outputs, for the n_ids pairs ids (device) of the last batched run: the movable

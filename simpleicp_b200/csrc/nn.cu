@@ -762,6 +762,95 @@ __global__ void __launch_bounds__(256)
   flag[fin_idx[f]] = 1u;
 }
 
+// ---- sicp_map_distances: the nearest map point of a point, within a bound --------------------
+// MG lanes per point run grid_nn's ring expansion with the rows of each ring dealt over the lanes
+// and reduced after the ring.  guard is the distance from the point to the nearest face behind
+// which unexplored cells remain, less 1e-9 h (cell assignment rounds at the 1e-13 level), so every
+// unexplored point lies farther than guard.  The search stops when
+//   best <= guard^2   the best point is the nearest, ties included, or
+//   guard^2 >= cap2   no unexplored point is within the bound: whether the nearest is within is
+//                     decided by best alone (best < cap2 <= guard^2 is the first case).
+// The first is grid_nn's rule; the second replaces its cap2 stop at the first point under the
+// bound, which answers only yes or no.  A row is skipped when its distance to the point, less the
+// same margin, exceeds min(best, cap2) (1e-12 relative slack): it holds nothing nearer than the
+// lane's best, which bounds the group's, and nothing within the bound.
+template <int MG>
+__global__ void __launch_bounds__(128)
+    k_map_nearest(GridView g, const double* __restrict__ xyz, long long n, double cap2, long long* __restrict__ idx,
+                  double* __restrict__ d2, uint32_t* __restrict__ within) {
+  const long long j = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / MG;
+  const int sub = threadIdx.x & (MG - 1);
+  if (j >= n) return;  // a whole group leaves together
+  const unsigned int gmask = ((1u << MG) - 1u) << ((threadIdx.x & 31) & ~(MG - 1));
+  const double qx = xyz[3 * j + 0], qy = xyz[3 * j + 1], qz = xyz[3 * j + 2];
+  if (!(isfinite(qx) && isfinite(qy) && isfinite(qz))) {
+    if (sub == 0) {
+      idx[j] = -1;
+      d2[j] = __longlong_as_double(0x7ff8000000000000ll);
+      within[j] = 0u;
+    }
+    return;
+  }
+  const int cx = cell_coord(qx, g.ox, g.inv_h, g.nx);
+  const int cy = cell_coord(qy, g.oy, g.inv_h, g.ny);
+  const int cz = cell_coord(qz, g.oz, g.inv_h, g.nz);
+  const uint32_t* __restrict__ cs = g.cell_start;
+  const double marg = 1e-9 * g.h;
+  double best = kInf;
+  long long bidx = -1;
+  uint32_t bpos = 0;
+  // r stays below the grid's largest dimension: once the ring's block covers the grid, guard is inf
+  for (int r = 1;; ++r) {
+    const int x0 = cx - r, x1 = cx + r, y0 = cy - r, y1 = cy + r, z0 = cz - r, z1 = cz + r;
+    const int xa = max(x0, 0), xb = min(x1, g.nx - 1);
+    // the ring's (y, z) rows clamped to the grid: at most ny nz < 2^25 of them
+    const int ya = max(y0, 0), yb = min(y1, g.ny - 1), za = max(z0, 0), zb = min(z1, g.nz - 1);
+    const int nyr = yb - ya + 1, items = nyr * (zb - za + 1);
+    int zr = sub / nyr, yr = sub - zr * nyr;
+    for (int t = sub; t < items; t += MG, yr += MG) {
+      while (yr >= nyr) {
+        yr -= nyr;
+        ++zr;
+      }
+      const int y = ya + yr, z = za + zr;
+      const double by = fmax(fmax((g.oy + y * g.h) - qy, qy - (g.oy + (y + 1) * g.h)) - marg, 0.0);
+      const double bz = fmax(fmax((g.oz + z * g.h) - qz, qz - (g.oz + (z + 1) * g.h)) - marg, 0.0);
+      if (by * by + bz * bz > fmin(best, cap2) * (1.0 + 1e-12)) continue;
+      const long long row = ((long long)z * g.ny + y) * g.nx;
+      if (r == 1 || y == y0 || y == y1 || z == z0 || z == z1) {
+        scan_range(g.recs, cs[row + xa], cs[row + xb + 1], qx, qy, qz, best, bidx, bpos);
+      } else {
+        if (x0 >= 0) scan_range(g.recs, cs[row + x0], cs[row + x0 + 1], qx, qy, qz, best, bidx, bpos);
+        if (x1 < g.nx) scan_range(g.recs, cs[row + x1], cs[row + x1 + 1], qx, qy, qz, best, bidx, bpos);
+      }
+    }
+#pragma unroll
+    for (int o = MG / 2; o > 0; o >>= 1) {
+      const double od = __shfl_xor_sync(gmask, best, o, MG);
+      const long long oi = __shfl_xor_sync(gmask, bidx, o, MG);
+      if (od < best || (od == best && oi >= 0 && (bidx < 0 || oi < bidx))) {
+        best = od;
+        bidx = oi;
+      }
+    }
+    double guard = kInf;
+    if (x0 > 0) guard = fmin(guard, qx - (g.ox + x0 * g.h));
+    if (x1 < g.nx - 1) guard = fmin(guard, (g.ox + (x1 + 1) * g.h) - qx);
+    if (y0 > 0) guard = fmin(guard, qy - (g.oy + y0 * g.h));
+    if (y1 < g.ny - 1) guard = fmin(guard, (g.oy + (y1 + 1) * g.h) - qy);
+    if (z0 > 0) guard = fmin(guard, qz - (g.oz + z0 * g.h));
+    if (z1 < g.nz - 1) guard = fmin(guard, (g.oz + (z1 + 1) * g.h) - qz);
+    if (guard >= kInf) break;  // the block covers the whole grid
+    guard -= marg;
+    if (guard > 0.0 && (best <= guard * guard || guard * guard >= cap2)) break;
+  }
+  if (sub != 0) return;
+  const bool in = best < cap2;  // strict: cKDTree distance_upper_bound semantics, as k_range_keep
+  idx[j] = in ? bidx : -1;
+  d2[j] = in ? best : kInf;
+  within[j] = in ? 1u : 0u;
+}
+
 // ------------------------------------------------------------------------------------------
 // brute-force engine (TMA staged)
 // ------------------------------------------------------------------------------------------
@@ -1172,6 +1261,21 @@ void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh,
   if (n_fin <= 0) return;
   k_map_insert_flags<<<(unsigned)((n_fin + 255) / 256), 256, 0, c.stream>>>(map, fresh, fin_xyz, fin_idx, n_fin, voxel,
                                                                             flag);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+// Lanes per point by the point count, the rule of match_lanes without its option: 16 while the
+// search is latency-bound (few points), fewer once the points fill the machine.  The result does
+// not depend on the lanes.
+void map_nearest_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double cap2, long long* idx,
+                        double* d2, uint32_t* within) {
+  if (n <= 0) return;
+  const int mg = (n <= 16384) ? 16 : ((n <= 65536) ? 8 : 4);
+  with_lanes<4, 8, 16>(mg, [&](auto L) {
+    constexpr int M = decltype(L)::value;
+    k_map_nearest<M><<<(unsigned)((n * M + 127) / 128), 128, 0, c.stream>>>(map, xyz, n, cap2, idx, d2, within);
+  });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

@@ -588,4 +588,22 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
   }
 }
 
+// the queries are map points, so each finds itself among its k neighbours, as the fixed points of
+// sicp_estimate_normals do; knn_idx / knn_d2 stay null, so k_pca keeps no lists
+void map_normals_launch(Ctx& c, const GridView& map, const double* q_xyz, long long n, int k, float4* out,
+                        DevBuf<uint32_t>& pos) {
+  const long long chunk = std::min<long long>(n, normals_chunk_queries(c, k));
+  pos.reserve((size_t)std::max<long long>(chunk, 1) * k);
+  KnnQueries a{};
+  a.k = k;
+  a.g = map;
+  a.pos = pos.p;
+  for (long long q0 = 0; q0 < n; q0 += chunk) {
+    a.n = std::min(chunk, n - q0);
+    a.q_xyz = q_xyz + 3 * q0;
+    a.out = out + q0;
+    knn_pca_launch<Src::One>(c, a, a.n, 1, n);
+  }
+}
+
 }  // namespace sicp

@@ -63,5 +63,11 @@ with sb.Map(X_fix[:30_000]) as mp:
     k2 = mp.insert([X_mov[3000:9000] + 0.01], voxel_size=0.2)
     k3 = mp.insert([mp.points()[:500]], voxel_size=0.05)
     assert k1.sum() > 0 and k2.sum() > 0 and k3.sum() == 0 and mp.n_points == 30_000 + k1.sum() + k2.sum()
+    # map distances: with H and normals (the same odd-offset, NaN and empty clouds), without either,
+    # and a cloud entirely beyond the bound
+    d1 = mp.distances(ins, np.stack([H_true, np.eye(4), H_true]), max_distance=0.5, neighbors=10)
+    d2 = mp.distances([X_mov[3000:9000]], max_distance=0.2)
+    d3 = mp.distances([X_mov[:100] + 1e4], max_distance=0.5, neighbors=30)
+    assert d1[0].n_within > 0 and d1[1].n_within == 0 and d2[0].n_within > 0 and d3[0].n_within == 0
 print("ok", a.iterations, m.iterations, int(tab[:, 16].sum()), c.iterations, d.iterations, f.iterations, g.iterations, l.iterations,
       float(np.linalg.norm(c.H - H_true)), float(np.linalg.norm(l.T - H_true)))
