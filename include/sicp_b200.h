@@ -358,6 +358,37 @@ int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xy
 int32_t sicp_get_map(sicp_ctx* ctx, double* xyz /*[h|d] cap x 3, or NULL*/, int64_t cap,
                      int64_t* n /*[h]*/);
 
+/* ---- shrinking the map: crop around positions, thin to one point per voxel --------------------
+ * sicp_map_crop keeps the map points near any of n_centers centres (x, y, z rows, in the map's
+ * frame): with d = p - c rounded in double per axis and d2 = (dx dx + dy dy) + dz dz in double
+ * with no fused multiply-add, map point p is kept iff d2 < fl(radius^2) for at least one centre c
+ * (the strict comparison of sicp_select_in_range and sicp_map_distances).
+ * sicp_map_thin keeps one map point per voxel: with key(p) = (floor(p.x / v), floor(p.y / v),
+ * floor(p.z / v)) as sicp_map_insert computes it, map point j is kept iff no map point j' < j has
+ * its key.  Thinning a map M thus gives the points of inserting M[1:] into a map of M[:1], and
+ * later inserts at the same v keep the map at one point per voxel.
+ * Common to both:
+ *  - The new map is the kept points in their old order; nothing is moved or reordered.
+ *    n_removed (if not NULL) = the points removed.
+ *  - When nothing is removed, the map and its grid stay as they are (no rebuild).  Otherwise the
+ *    grid is rebuilt by sicp_set_map's builder, so the shrunk map registers and gives distances
+ *    exactly as a fresh sicp_set_map of the same points.
+ *  - SICP_ERR_STATE: no map.  SICP_ERR_BAD_ARG, before any device work: n_centers < 1, centers
+ *    NULL, a non-finite centre coordinate, or a radius / voxel_size that is not finite and > 0.
+ *    SICP_ERR_NO_OVERLAP: a crop that would keep no point (a map is never empty).
+ *  - The map is replaced only when the new one is complete: after an error it is unchanged.
+ *  - Clears the batch outputs, as sicp_map_insert does.
+ *  - Device memory peaks at about two maps (the old and the new one, coordinates and grid) plus
+ *    8 bytes per map point of keep flags and their prefix sum, which stay on the context like the
+ *    insert's staging buffers.
+ *  - Cost: the crop is one pass over the map, O(n_map x n_centers) distance tests in the worst case
+ *    (a point stops at its first centre within radius), plus the rebuild.  The thin walks, per map
+ *    point, the map-grid cells its voxel covers, about (v / h + 2)^3 for a map cell size h, as an
+ *    inserted point does, plus the rebuild.                                                      */
+int32_t sicp_map_crop(sicp_ctx* ctx, int32_t n_centers, const double* centers /*[h] n_centers x 3*/,
+                      double radius, int64_t* n_removed /*[h] or NULL*/);
+int32_t sicp_map_thin(sicp_ctx* ctx, double voxel_size, int64_t* n_removed /*[h] or NULL*/);
+
 /* ---- how well clouds fit the map: cloud-to-map distances --------------------------------------
  * sicp_map_distances gives every point of n_clouds clouds its nearest map point within
  * max_distance, and with neighbors = k > 0 its signed distance along that map point's normal.
@@ -403,10 +434,11 @@ int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const*
  * simpleicp.py:316), the final distance residuals (simpleicp.py:324, 4th return value), the
  * per-iteration records and the applied transform.  Those two calls only leave these on the
  * device; all the work happens here, and they stay readable (any number of times, same bits)
- * until the next sicp_register_batch, sicp_register_to_map, sicp_set_map or sicp_map_insert on the
- * context.
- *  - SICP_ERR_STATE: before any such call, after sicp_set_map or sicp_map_insert, or after a
- *    batch / map call that returned an error (each of the four clears the outputs on entry; only a
+ * until the next sicp_register_batch, sicp_register_to_map, sicp_set_map, sicp_map_insert,
+ * sicp_map_crop or sicp_map_thin on the context.
+ *  - SICP_ERR_STATE: before any such call, after sicp_set_map, sicp_map_insert, sicp_map_crop or
+ *    sicp_map_thin, or after a
+ *    batch / map call that returned an error (each of these clears the outputs on entry; only a
  *    successful return of the first two makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
  *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose
  *    status was not SICP_OK (SICP_ERR_NO_OVERLAP included) is ever written.

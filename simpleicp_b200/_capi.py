@@ -42,7 +42,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs",
-    "sicp_map_insert", "sicp_get_map", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -170,6 +170,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
+        "sicp_map_crop": [vp, i32, vp, dbl, C.POINTER(i64)],
+        "sicp_map_thin": [vp, dbl, C.POINTER(i64)],
         "sicp_map_distances": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, i32, C.POINTER(vp), C.POINTER(vp),
                                C.POINTER(vp), C.POINTER(vp), vp],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
@@ -637,6 +639,23 @@ class Engine:
         X = np.empty((int(n.value), 3), dtype=np.float64)
         self._check(self._lib.sicp_get_map(self._h, _ptr(X), X.shape[0], C.byref(n)))
         return X
+
+    def map_crop(self, centers, radius: float) -> int:
+        """sicp_map_crop: keep the map points whose squared distance to at least one of `centers`
+        ((n, 3) float64) is below radius^2, in map order.  Returns the points removed."""
+        c = np.ascontiguousarray(np.asarray(centers, dtype=np.float64).reshape(-1, 3))
+        removed = C.c_int64(0)
+        self._check(self._lib.sicp_map_crop(self._h, c.shape[0], _ptr(c), float(radius), C.byref(removed)))
+        self.n_map -= int(removed.value)
+        return int(removed.value)
+
+    def map_thin(self, voxel_size: float) -> int:
+        """sicp_map_thin: keep the first map point of every voxel key floor(p / voxel_size), in map
+        order.  Returns the points removed."""
+        removed = C.c_int64(0)
+        self._check(self._lib.sicp_map_thin(self._h, float(voxel_size), C.byref(removed)))
+        self.n_map -= int(removed.value)
+        return int(removed.value)
 
     def batch_outputs(self, result):
         """sicp_get_batch_outputs for `result`, the PairResult array the last register_batch /

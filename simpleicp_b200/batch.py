@@ -378,6 +378,10 @@ class Map:
     new point per voxel the map does not occupy) and ``points()`` reads it back.
     ``distances(clouds, H, max_distance=d)`` tells how well clouds fit the map: every point's
     nearest map point within d, with fitness and inlier RMSE per cloud.
+    ``crop(centers, radius=R)`` shrinks the map on the device to the points within R of the given
+    positions (a local map around the sensor, so a loop that keeps inserting stays bounded), and
+    ``thin(voxel_size=v)`` to one point per voxel (a dense base map); both keep the points' order
+    and leave a map that registers as ``Map(points)`` of the same points would.
     """
 
     def __init__(self, X_map, device: int = 0):
@@ -497,9 +501,52 @@ class Map:
         return [CloudDistances.of(idx[i], d2[i], None if pd is None else pd[i], None if pl is None else pl[i],
                                   int(n_within[i])) for i in range(len(clouds))]
 
+    def crop(self, centers, *, radius: float) -> int:
+        """Shrink the map on the device to the surroundings of ``centers`` (sicp_map_crop): keep
+        the map points within ``radius`` of at least one centre, in their order, e.g.
+        ``m.crop(table[ok, :16].reshape(-1, 4, 4)[:, :3, 3], radius=100.0)`` for the positions of
+        the scans just registered.  ``centers`` is one (3,) position or an (n, 3) array in the
+        map's frame.  Point p is kept iff (dx dx + dy dy) + dz dz < radius^2 for some centre
+        (d = p - c, each operation rounded in double).  Returns the number of points removed; a
+        crop that would keep no point raises the library's SicpError (code 2,
+        SICP_ERR_NO_OVERLAP) and leaves the map as it was."""
+        c = np.asarray(centers, dtype=np.float64)
+        if c.shape == (3,):
+            c = c.reshape(1, 3)
+        if c.ndim != 2 or c.shape[1] != 3 or c.shape[0] < 1:
+            raise ValueError(f"centers must have shape (3,) or (n, 3) with n >= 1, got {c.shape}")
+        if not np.isfinite(c).all():
+            raise ValueError("centers must be finite")
+        r = float(radius)
+        if not (np.isfinite(r) and r > 0):
+            raise ValueError(f"radius must be finite and > 0, got {radius}")
+        import torch
+
+        with torch.cuda.device(self.device):
+            removed = self._engine.map_crop(c, r)
+        self.n_points = self._engine.n_map
+        return removed
+
+    def thin(self, *, voxel_size: float) -> int:
+        """Thin the map on the device to one point per voxel (sicp_map_thin): of the map points
+        that share a voxel key floor(p / voxel_size) (``insert``'s key), the first in map order is
+        kept.  The kept points keep their order, and later inserts at the same voxel size keep the
+        map at one point per voxel.  Meant for a dense base map (``Map(X_tls)``).  Returns the
+        number of points removed."""
+        v = float(voxel_size)
+        if not (np.isfinite(v) and v > 0):
+            raise ValueError(f"voxel_size must be finite and > 0, got {voxel_size}")
+        import torch
+
+        with torch.cuda.device(self.device):
+            removed = self._engine.map_thin(v)
+        self.n_points = self._engine.n_map
+        return removed
+
     def points(self) -> np.ndarray:
         """The map as it stands, (n_points, 3) float64 in map order (a copy): the points it was
-        made of followed by those ``insert`` added.  ``sb.write_xyz(path, m.points())`` saves it."""
+        made of followed by those ``insert`` added, less those ``crop`` and ``thin`` removed.
+        ``sb.write_xyz(path, m.points())`` saves it."""
         import torch
 
         with torch.cuda.device(self.device):

@@ -119,6 +119,41 @@ __global__ void __launch_bounds__(256)
   out[3 * o + 2] = xyz[3 * j + 2];
 }
 
+// sicp_map_crop, one thread per map point j: keep[j] = 1 iff d2 < r2 for at least one of the n_c
+// centres cen, where d2 = (dx dx + dy dy) + dz dz with d = p - c and every operation rounded on
+// its own (no fused multiply-add), else 0.  The block reads the centres through shared memory,
+// kCropChunk at a time, and stops at the first chunk boundary where all its points are kept.
+constexpr int kCropChunk = 256;
+__global__ void __launch_bounds__(256)
+    k_map_crop_flags(const double* __restrict__ xyz, long long n, const double* __restrict__ cen, int n_c, double r2,
+                     uint32_t* __restrict__ keep) {
+  __shared__ double s[3 * kCropChunk];
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  double x = 0.0, y = 0.0, z = 0.0;
+  if (j < n) {
+    x = xyz[3 * j + 0];
+    y = xyz[3 * j + 1];
+    z = xyz[3 * j + 2];
+  }
+  bool hit = false;
+  for (int c0 = 0; c0 < n_c; c0 += kCropChunk) {
+    // block-uniform: every thread has finished reading the previous chunk
+    if (__syncthreads_and(hit || j >= n)) break;
+    const int m = min(kCropChunk, n_c - c0);
+    for (int i = threadIdx.x; i < 3 * m; i += blockDim.x) s[i] = cen[3 * (long long)c0 + i];
+    __syncthreads();
+    if (hit || j >= n) continue;
+    for (int i = 0; i < m; ++i) {
+      const double dx = __dsub_rn(x, s[3 * i + 0]), dy = __dsub_rn(y, s[3 * i + 1]), dz = __dsub_rn(z, s[3 * i + 2]);
+      if (__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) < r2) {
+        hit = true;
+        break;
+      }
+    }
+  }
+  if (j < n) keep[j] = hit ? 1u : 0u;
+}
+
 // bounds[i] = S[off[i]] for i <= n_clouds (off[n_clouds] = n, S[n] = the total): cloud i added
 // bounds[i + 1] - bounds[i] points
 __global__ void k_insert_bounds(const uint32_t* __restrict__ off, int n_clouds, const uint32_t* __restrict__ scan,
@@ -793,6 +828,24 @@ static void stage_clouds(Ctx& c, MapStore& m, int n_clouds, const double* const*
   c.tm.kernel_launches += 1;
 }
 
+// The last step of every call that replaces the map (insert, crop, thin): the new map's n_new
+// points are in MapStore::xyz_next; they get their grid from set_map's grid_build call, and only
+// then are the two swapped in, so a failure leaves the map as it was, and the new map is the one
+// set_map would make of the same points.  The old map's buffers are released after the swap: one
+// map stays resident between calls.
+static void swap_in_next_map(Ctx& c, MapStore& m, long long n_new) {
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  grid_build(c, m.grid_next, {HostCloud{m.xyz_next.p, n_new, 0}}, batch_policy(c), views, centres);  // as set_map
+  SICP_CUDA(cudaStreamSynchronize(c.stream));
+  m.xyz.swap(m.xyz_next);
+  m.grid.swap(m.grid_next);
+  m.view = views[0];
+  m.n = n_new;
+  m.xyz_next.release();
+  m.grid_next.release();
+}
+
 // sicp_map_insert.  The clouds are staged into one buffer and moved there; their finite points
 // are compacted in order and gridded as one cloud; k_map_insert_flags flags the points to add (a
 // voxel key no map point has, first of its key among the new points); one scan + an ordered
@@ -855,15 +908,7 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
     k_insert_scatter<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p + 3 * m.n);
     SICP_CUDA(cudaGetLastError());
     c.tm.kernel_launches += 1;
-    grid_build(c, m.grid_next, {HostCloud{m.xyz_next.p, n_new, 0}}, batch_policy(c), views, centres);  // as set_map
-    SICP_CUDA(cudaStreamSynchronize(st));
-    m.xyz.swap(m.xyz_next);
-    m.grid.swap(m.grid_next);
-    m.view = views[0];
-    m.n = n_new;
-    // the old map's buffers: one map stays resident between inserts
-    m.xyz_next.release();
-    m.grid_next.release();
+    swap_in_next_map(c, m, n_new);
   }
   if (n_added)
     for (int i = 0; i < n_clouds; ++i) n_added[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];
@@ -879,6 +924,69 @@ static void get_map(Ctx& c, double* xyz, int64_t cap, int64_t* n) {
     copy_any(c, xyz, m.xyz.p, sizeof(double) * 3 * (size_t)std::min<long long>(m.n, cap));
     SICP_CUDA(cudaStreamSynchronize(c.stream));
   }
+}
+
+// The end of sicp_map_crop and sicp_map_thin: the map points whose keep flag (MapStore::ins_flag,
+// one per map point) is set become the new map, in map order.  One scan and one read-back of the
+// kept count; when every point is kept nothing else happens (the map and its grid stay as they
+// are); otherwise k_insert_scatter writes the kept points into xyz_next and swap_in_next_map makes
+// them the map.  A map is never empty: keeping no point is SICP_ERR_NO_OVERLAP with the map
+// unchanged.  Returns the points removed.
+static long long keep_flagged(Ctx& c, MapStore& m) {
+  cudaStream_t st = c.stream;
+  const long long n = m.n;
+  scan_u32(c, m.ins_flag.p, n, m.ins_scan.p, m.sums);
+  pinned_reserve(m.bounds_host, m.bounds_cap, 1);
+  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_scan.p + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  const long long kept = m.bounds_host[0];
+  SICP_REQUIRE(kept > 0, SICP_ERR_NO_OVERLAP, "no map point would be kept (a map is never empty): the map is unchanged");
+  if (kept == n) return 0;
+  m.xyz_next.reserve(3 * (size_t)kept);
+  k_insert_scatter<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(m.xyz.p, n, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  swap_in_next_map(c, m, kept);
+  return n - kept;
+}
+
+// sicp_map_crop: keep the map points within radius of at least one centre (k_map_crop_flags).
+static void map_crop(Ctx& c, int n_centers, const double* centers, double radius, int64_t* n_removed) {
+  if (c.batch) c.batch->out_valid = false;
+  SICP_REQUIRE(n_centers >= 1, SICP_ERR_BAD_ARG, "n_centers must be >= 1");
+  SICP_REQUIRE(centers, SICP_ERR_BAD_ARG, "centers is NULL");
+  for (long long i = 0; i < 3ll * n_centers; ++i)
+    SICP_REQUIRE(std::isfinite(centers[i]), SICP_ERR_BAD_ARG, "centers has non-finite coordinates");
+  SICP_REQUIRE(std::isfinite(radius) && radius > 0, SICP_ERR_BAD_ARG, "radius must be finite and > 0");
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  if (n_removed) *n_removed = 0;
+  cudaStream_t st = c.stream;
+  m.crop_c.reserve(3 * (size_t)n_centers);
+  SICP_CUDA(cudaMemcpyAsync(m.crop_c.p, centers, sizeof(double) * 3 * (size_t)n_centers, cudaMemcpyHostToDevice, st));
+  m.ins_flag.reserve((size_t)m.n);
+  m.ins_scan.reserve((size_t)m.n + 1);
+  // r2 = fl(radius^2), as sicp_select_in_range and sicp_map_distances compute it
+  k_map_crop_flags<<<(unsigned)((m.n + 255) / 256), 256, 0, st>>>(m.xyz.p, m.n, m.crop_c.p, n_centers,
+                                                                  radius * radius, m.ins_flag.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  const long long removed = keep_flagged(c, m);
+  if (n_removed) *n_removed = removed;
+}
+
+// sicp_map_thin: keep the first map point of every voxel key (k_map_thin_flags, nn.cu).
+static void map_thin(Ctx& c, double voxel, int64_t* n_removed) {
+  if (c.batch) c.batch->out_valid = false;
+  SICP_REQUIRE(std::isfinite(voxel) && voxel > 0, SICP_ERR_BAD_ARG, "voxel_size must be finite and > 0");
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  if (n_removed) *n_removed = 0;
+  m.ins_flag.reserve((size_t)m.n);
+  m.ins_scan.reserve((size_t)m.n + 1);
+  map_thin_flags_launch(c, m.view, m.xyz.p, m.n, voxel, m.ins_flag.p);
+  const long long removed = keep_flagged(c, m);
+  if (n_removed) *n_removed = removed;
 }
 
 // sicp_map_distances.  The clouds are staged and moved as sicp_map_insert's are; k_map_nearest
@@ -1008,6 +1116,15 @@ extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double
 
 extern "C" int32_t sicp_get_map(sicp_ctx* ctx, double* xyz, int64_t cap, int64_t* n) {
   SICP_BATCH_API(get_map(c, xyz, cap, n))
+}
+
+extern "C" int32_t sicp_map_crop(sicp_ctx* ctx, int32_t n_centers, const double* centers, double radius,
+                                 int64_t* n_removed) {
+  SICP_BATCH_API(map_crop(c, n_centers, centers, radius, n_removed))
+}
+
+extern "C" int32_t sicp_map_thin(sicp_ctx* ctx, double voxel_size, int64_t* n_removed) {
+  SICP_BATCH_API(map_thin(c, voxel_size, n_removed))
 }
 
 extern "C" int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

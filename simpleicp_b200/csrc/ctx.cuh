@@ -305,6 +305,10 @@ struct MapStore {
   DevBuf<float> dst_pl;
   DevBuf<float4> dst_nrm;
   DevBuf<uint32_t> dst_pos;
+  // sicp_map_crop / sicp_map_thin (batch.cu: map_crop, map_thin) take ins_flag / ins_scan for a
+  // keep flag per map point and its prefix sum (8 B per map point, kept like the staging buffers),
+  // and write the kept points into xyz_next; crop_c holds the crop's centres.
+  DevBuf<double> crop_c;
   uint32_t* bounds_host = nullptr;  // pinned: n_clouds + 1 boundaries
   size_t bounds_cap = 0;
   ~MapStore() {
@@ -399,6 +403,10 @@ void map_bits_scatter_launch(Ctx& c, const uint32_t* bits, long long n_words, lo
 // fresh with a smaller index has the same voxel key floor(p / voxel) (flag is zeroed by the caller)
 void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh, const double* fin_xyz,
                              const uint32_t* fin_idx, long long n_fin, double voxel, uint32_t* flag);
+// sicp_map_thin's keep flags (nn.cu: k_map_thin_flags): keep[j] = 1 for each of the n map points
+// xyz (gridded in map, in map order) when no map point j' < j has its voxel key floor(p / voxel),
+// else 0
+void map_thin_flags_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double voxel, uint32_t* keep);
 // sicp_map_distances' bounded nearest search (nn.cu: k_map_nearest), one lane group per point j of
 // xyz (n points): the nearest map point (lowest index among ties) when its d2 < cap2 ->
 // idx[j], d2[j], within[j] = 1; else idx -1, within 0 and d2 +inf (finite point) or NaN (a NaN or

@@ -740,6 +740,21 @@ __device__ __forceinline__ bool voxel_taken(const GridView& g, const double lo[3
   return false;
 }
 
+// The voxel key k of point p (three doubles) and the grown box [lo, hi] of its voxel, as above.
+__device__ __forceinline__ void voxel_box(const double* __restrict__ p, double v, double k[3], double lo[3],
+                                          double hi[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    k[a] = floor(__ddiv_rn(p[a], v));
+    const double l = k[a] * v, h = (k[a] + 1.0) * v;
+    const double g = 1e-12 * (fabs(l) + fabs(h)) + 1e-300;
+    lo[a] = l - g;
+    hi[a] = h + g;
+    if (!(lo[a] >= -DBL_MAX)) lo[a] = -kInf;  // overflow or NaN
+    if (!(hi[a] <= DBL_MAX)) hi[a] = kInf;
+  }
+}
+
 // One thread per finite new point f (fin_xyz, the compacted points gridded in `fresh`, Rec::idx =
 // f): it is added unless a map record has its key or a fresh record with a smaller index does.
 __global__ void __launch_bounds__(256)
@@ -748,18 +763,21 @@ __global__ void __launch_bounds__(256)
   const long long f = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (f >= n_fin) return;
   double k[3], lo[3], hi[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    k[a] = floor(__ddiv_rn(fin_xyz[3 * f + a], v));
-    const double l = k[a] * v, h = (k[a] + 1.0) * v;
-    const double g = 1e-12 * (fabs(l) + fabs(h)) + 1e-300;
-    lo[a] = l - g;
-    hi[a] = h + g;
-    if (!(lo[a] >= -DBL_MAX)) lo[a] = -kInf;  // overflow or NaN
-    if (!(hi[a] <= DBL_MAX)) hi[a] = kInf;
-  }
+  voxel_box(fin_xyz + 3 * f, v, k, lo, hi);
   if (voxel_taken(map, lo, hi, v, k, LLONG_MAX) || voxel_taken(fresh, lo, hi, v, k, f)) return;
   flag[fin_idx[f]] = 1u;
+}
+
+// ---- sicp_map_thin: one map point per voxel -------------------------------------------------
+// One thread per map point j (xyz in map order, gridded in `map`, Rec::idx = j): keep[j] = 1 iff no
+// map point with a smaller index has its key (the grid builder admits finite points only).
+__global__ void __launch_bounds__(256)
+    k_map_thin_flags(GridView map, const double* __restrict__ xyz, long long n, double v, uint32_t* __restrict__ keep) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  double k[3], lo[3], hi[3];
+  voxel_box(xyz + 3 * j, v, k, lo, hi);
+  keep[j] = voxel_taken(map, lo, hi, v, k, j) ? 0u : 1u;
 }
 
 // ---- sicp_map_distances: the nearest map point of a point, within a bound --------------------
@@ -1261,6 +1279,13 @@ void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh,
   if (n_fin <= 0) return;
   k_map_insert_flags<<<(unsigned)((n_fin + 255) / 256), 256, 0, c.stream>>>(map, fresh, fin_xyz, fin_idx, n_fin, voxel,
                                                                             flag);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_thin_flags_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double voxel, uint32_t* keep) {
+  if (n <= 0) return;
+  k_map_thin_flags<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(map, xyz, n, voxel, keep);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

@@ -69,5 +69,18 @@ with sb.Map(X_fix[:30_000]) as mp:
     d2 = mp.distances([X_mov[3000:9000]], max_distance=0.2)
     d3 = mp.distances([X_mov[:100] + 1e4], max_distance=0.5, neighbors=30)
     assert d1[0].n_within > 0 and d1[1].n_within == 0 and d2[0].n_within > 0 and d3[0].n_within == 0
+    # map crop and thin: several centres (more than one shared-memory chunk), one that removes
+    # nothing, one that would remove everything (refused, the map unchanged), and a thin
+    n0 = mp.n_points
+    cen = np.concatenate([mp.points()[::97][:300], np.full((3, 3), 1e4)])
+    c1 = mp.crop(cen, radius=0.3)
+    c2 = mp.crop(cen[:5], radius=1e4)
+    try:
+        mp.crop(np.full(3, 1e5), radius=1.0)
+        raise AssertionError("a crop that keeps nothing must be refused")
+    except _capi.SicpError as err:
+        assert err.code == _capi.SICP_ERR_NO_OVERLAP
+    t1 = mp.thin(voxel_size=0.1)
+    assert c1 > 0 and c2 == 0 and t1 > 0 and mp.n_points == n0 - c1 - t1
 print("ok", a.iterations, m.iterations, int(tab[:, 16].sum()), c.iterations, d.iterations, f.iterations, g.iterations, l.iterations,
       float(np.linalg.norm(c.H - H_true)), float(np.linalg.norm(l.T - H_true)))
