@@ -97,7 +97,10 @@ __global__ void __launch_bounds__(256) k_cell_count(const CloudPlan* __restrict_
   if (threadIdx.x == 0 && n_first) atomicAdd(&occ[blockIdx.y], (unsigned int)n_first);
 }
 
-// ---- 3-kernel exclusive scan over uint32 (n up to 2^27) ------------------------------------
+// ---- 3-kernel exclusive scan over uint32 ------------------------------------------------------
+// Any n below 2^32 whose total is below 2^32 (the outputs are uint32): k_scan_blocksums walks the
+// ceil(n / 4096) block sums 1024 at a time with a carry.  tests/test_gpu_scale.py runs it at
+// 2^27 + 4097 elements (a map crop) and at totals of about 3.9e9 (the map filter's survivors).
 __global__ void __launch_bounds__(256) k_scan_reduce(const uint32_t* __restrict__ in, long long n,
                                                      uint32_t* __restrict__ block_sums) {
   long long base = (long long)blockIdx.x * kScanItems;
