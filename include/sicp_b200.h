@@ -509,6 +509,12 @@ int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32] /*[h]*/);
  * median and MAD, which is what tests use this for.                                            */
 int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double min_planarity);
 
+/* Test-only: the number of queries the last match answered from the certificate of its warm
+ * start (the search skipped because the neighbour provably cannot have changed; DESIGN.md §3.2).
+ * 0 when the last match could not use certificates (brute-force engine, match_group 1, no
+ * distance).                                                                                    */
+int32_t sicp_debug_match_counts(sicp_ctx* ctx, int64_t* n_certified /*[h]*/);
+
 /* Test-only: the uniform grid the searches run on.  side 0 = the fixed cloud's grid (k-NN of the
  * normals; built by sicp_estimate_normals), 1 = the movable cloud's grid (correspondences; built
  * by sicp_set_clouds).  o = origin (the cloud's bounding-box minimum), h = cell size, dims = cells

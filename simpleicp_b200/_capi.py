@@ -43,7 +43,7 @@ SYMBOLS = (
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs",
     "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
-    "sicp_debug_seed_predictor", "sicp_debug_grid_params",
+    "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
 
@@ -178,6 +178,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
         "sicp_debug_seed_predictor": [vp, dbl, dbl, dbl],
+        "sicp_debug_match_counts": [vp, C.POINTER(i64)],
         "sicp_debug_grid_params": [vp, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(i32)],
     }
     for name, args in sigs.items():
@@ -742,6 +743,12 @@ class Engine:
     def seed_predictor(self, med: float, mad: float, min_planarity: float):
         """Test-only (sicp_debug_seed_predictor): the predictor the next match bins with."""
         self._check(self._lib.sicp_debug_seed_predictor(self._h, float(med), float(mad), float(min_planarity)))
+
+    def match_counts(self) -> int:
+        """Test-only (sicp_debug_match_counts): queries the last match answered from a certificate."""
+        n = C.c_int64(0)
+        self._check(self._lib.sicp_debug_match_counts(self._h, C.byref(n)))
+        return int(n.value)
 
     def grid_params(self, side: str = "mov"):
         """Test-only (sicp_debug_grid_params): (origin, cell size, dims) of the movable ("mov") or

@@ -1145,6 +1145,18 @@ int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double 
   API_END
 }
 
+int32_t sicp_debug_match_counts(sicp_ctx* ctx, int64_t* n_certified) {
+  API_BEGIN(ctx)
+  SICP_REQUIRE(n_certified != nullptr, SICP_ERR_BAD_ARG, "n_certified is NULL");
+  unsigned int n = 0;
+  if (c.cert_slot >= 0) {
+    SICP_CUDA(cudaMemcpyAsync(&n, c.cert_count.p + c.cert_slot, sizeof(n), cudaMemcpyDeviceToHost, c.stream));
+    sync(c);
+  }
+  *n_certified = (int64_t)n;
+  API_END
+}
+
 int32_t sicp_debug_grid_params(sicp_ctx* ctx, int32_t side, double o[3], double* h, int32_t dims[3]) {
   API_BEGIN(ctx)
   SICP_REQUIRE(side == 0 || side == 1, SICP_ERR_BAD_ARG, "side must be 0 (fixed) or 1 (movable)");

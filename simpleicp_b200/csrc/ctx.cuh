@@ -115,8 +115,19 @@ struct Ctx {
   int bin_cap = 0;
   DevBuf<double> m_xyz;              // K x 3: matched movable point, caller coordinates
   DevBuf<uint32_t> nn_pos;           // K: record position of the last match (warm start of the next one)
-  bool nn_pos_valid = false;         // nn_pos belongs to the current movable grid and selection
+  // nn_pos, cert_c, cert_rho, m_xyz and nn_idx were all written by the last match with distance,
+  // on the current movable grid and selection.  The certificates make this a correctness
+  // contract, not a hint: a match answered from a certificate returns m_xyz and nn_idx as they
+  // are.  Whatever rebuilds gmov, changes the selection or writes m_xyz or nn_idx outside such a
+  // match must clear the flag.
+  bool nn_pos_valid = false;
   long long nn_pos_K = 0;
+  // certificates of the one-pair grid match (nn.cu: MatchCert), 28 B per query, valid with nn_pos
+  DevBuf<double> cert_c;             // K x 3
+  DevBuf<float> cert_rho;            // K
+  DevBuf<unsigned int> cert_count;   // 2: queries answered from a certificate, by launch parity
+  int cert_next = 0;                 // counter of the next certifying launch
+  int cert_slot = -1;                // counter of the last match; -1: it could not certify
   int warm_start = 1;                // option "warm_start"
   int sphere_scan = 1;               // option "sphere_scan"
   int pdl = 1;                       // option "pdl": programmatic dependent launch between the two kernels of an iteration

@@ -64,6 +64,43 @@ __device__ __forceinline__ void scan_range(const Rec* __restrict__ recs, uint32_
   }
 }
 
+// consider() that also keeps sec, the smallest d2 among the visited records other than the
+// winner (certificate of the warm-started match, below).  A record at the winner's position is
+// not a second point: the warm-start record every lane starts from, and the last record that
+// scan_range re-reads as padding, come back with the winner's position.  A record that loses
+// (or is displaced) lost to a record earlier in the (d2, idx) order, so sec never holds the winner.
+__device__ __forceinline__ void consider_sec(const Rec& r, uint32_t pos, double qx, double qy, double qz,
+                                             double& best, long long& bidx, uint32_t& bpos, double& sec) {
+  const double dx = r.x - qx, dy = r.y - qy, dz = r.z - qz;
+  const double d2 = dx * dx + dy * dy + dz * dz;
+  if (pos == bpos) return;
+  if (d2 < best || (d2 == best && r.idx < bidx)) {
+    sec = fmin(sec, best);
+    best = d2;
+    bidx = r.idx;
+    bpos = pos;
+  } else {
+    sec = fmin(sec, d2);
+  }
+}
+
+__device__ __forceinline__ void scan_range_sec(const Rec* __restrict__ recs, uint32_t s, uint32_t e,
+                                               double qx, double qy, double qz, double& best,
+                                               long long& bidx, uint32_t& bpos, double& sec) {
+  for (uint32_t i = s; i < e; i += 4) {
+    const uint32_t last = e - 1;
+    const uint32_t i1 = min(i + 1, last), i2 = min(i + 2, last), i3 = min(i + 3, last);
+    const Rec r0 = recs[i];
+    const Rec r1 = recs[i1];
+    const Rec r2 = recs[i2];
+    const Rec r3 = recs[i3];
+    consider_sec(r0, i, qx, qy, qz, best, bidx, bpos, sec);
+    consider_sec(r1, i1, qx, qy, qz, best, bidx, bpos, sec);
+    consider_sec(r2, i2, qx, qy, qz, best, bidx, bpos, sec);
+    consider_sec(r3, i3, qx, qy, qz, best, bidx, bpos, sec);
+  }
+}
+
 // Returns true when (best, bidx) is proven to be the nearest neighbour.
 // cap2 >= 0: the caller only needs to know on which side of cap2 the squared nearest-neighbour
 // distance lies (overlap filter, PointCloud.select_in_range): the search may stop as soon as any
@@ -196,6 +233,22 @@ __device__ __forceinline__ float effective_planarity(const CorrOut& co, const Ri
   co.q_eff[qi] = make_float4(nr.x, nr.y, nr.z, w);
   return fabsf(w);
 }
+// Certificate of the one-pair warm-started match (DESIGN §3.2, "certificate"): a search that
+// finishes in the warm sphere scan proves that the record it found stays the strict nearest
+// neighbour of every query within rho of the query it searched, c.  The next match of the same
+// query skips its search while the moved query is provably inside that ball.  Part of the
+// warm-start state: valid exactly where nn_pos is.
+#ifndef SICP_CERT_SKIN
+#define SICP_CERT_SKIN 0.125f  // skin of the sphere scan that writes a certificate, in cells
+#endif
+constexpr float kCertSkin = SICP_CERT_SKIN;
+struct MatchCert {
+  double* c;              // K x 3: the moved query of the search that wrote the certificate
+  float* rho;             // K: radius of the certified ball, rounded down; <= 0: no certificate
+  unsigned int* n_cert;   // queries of this launch answered from their certificate
+  unsigned int* n_clear;  // the next launch's counter: zeroed here (ctx.cuh: cert_count)
+};
+
 __device__ __forceinline__ void store_matched(const CorrOut& co, long long qi, double x, double y, double z) {
   if (co.m_xyz) {
     co.m_xyz[3 * qi + 0] = x;
@@ -244,13 +297,16 @@ __global__ void __launch_bounds__(128)
 // those loads are in flight — with one thread per query a K = 1000 search took 27 us.
 // KEEP (overlap filter of a batch, with_distance = 0, unlimited rings): instead of nn_idx and the
 // squared distance, keep[qi] = (d2 < cap2), the comparison of k_range_keep (capi.cu).
-template <int MG, bool KEEP = false>
+// CERT (one-pair match only): read and write the certificates of `cert` (MatchCert above);
+// cert.rho is null when the launch keeps none (with_distance = 0).
+template <int MG, bool KEEP = false, bool CERT = false>
 __device__ __forceinline__ void match_coop_body(
     const GridView& g, const DevState* __restrict__ st, const double* __restrict__ q_xyz,
     const float4* __restrict__ q_nrm, const double* __restrict__ mov_xyz, long long K, int rmax,
     int with_distance, long long* __restrict__ nn_idx, double* __restrict__ out,
     unsigned int* __restrict__ unresolved, unsigned int* __restrict__ lin_hist, double cap2,
-    const CorrOut& co, const long long gt, uint32_t* __restrict__ keep = nullptr) {
+    const CorrOut& co, const long long gt, uint32_t* __restrict__ keep = nullptr,
+    const MatchCert& cert = MatchCert{}) {
   const long long qi = gt / MG;
   const int sub = threadIdx.x & (MG - 1);
   pdl_launch_dependents();
@@ -258,11 +314,36 @@ __device__ __forceinline__ void match_coop_body(
   // the query's coordinates do not depend on the previous kernel: on their way before the wait
   const double px = q_xyz[3 * qi + 0], py = q_xyz[3 * qi + 1], pz = q_xyz[3 * qi + 2];
   pdl_wait();
+  if constexpr (CERT) {
+    if (gt == 0 && cert.n_clear) *cert.n_clear = 0u;
+  }
   if (st->stop) return;
   const unsigned int gmask = (MG == 32) ? 0xffffffffu : (((1u << MG) - 1u) << ((threadIdx.x & 31) & ~(MG - 1)));
   const Rigid Tinv = st->Tinv;
   double qx, qy, qz;
   rigid_apply(Tinv, px, py, pz, qx, qy, qz);
+  if constexpr (CERT) {
+    // Fast path: |q - c| < rho (computed norm times 1 + 1e-12, an upper bound) proves that the
+    // full search would return the record at nn_pos[qi] again, as the strict winner (DESIGN §3.2).
+    // nn_idx, nn_pos, m_xyz and the certificate keep their values; only the epilogue runs.  A
+    // non-finite q fails the comparison.  The matched point is requested with the certificate.
+    if (co.warm) {
+      const double ex = qx - cert.c[3 * qi + 0], ey = qy - cert.c[3 * qi + 1], ez = qz - cert.c[3 * qi + 2];
+      const float rho = cert.rho[qi];
+      const double mx = co.m_xyz[3 * qi + 0], my = co.m_xyz[3 * qi + 1], mz = co.m_xyz[3 * qi + 2];
+      if (sqrt(ex * ex + ey * ey + ez * ez) * (1.0 + 1e-12) < (double)rho) {
+        if (sub != 0) return;
+        const unsigned int am = __activemask();
+        if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(cert.n_cert, (unsigned int)__popc(am));
+        const float4 nr = q_nrm[qi];
+        const Rec m{mx, my, mz, co.mov_nrm ? nn_idx[qi] : -1};
+        const double d = plane_distance_rec(st->T, m, px, py, pz, nr);
+        out[qi] = d;
+        lin_hist_add(st, lin_hist, effective_planarity(co, st->T, qi, m.idx, nr), d, co.binstore, co.bin_cap, qi);
+        return;
+      }
+    }
+  }
   const int cx = cell_coord(qx, g.ox, g.inv_h, g.nx);
   const int cy = cell_coord(qy, g.oy, g.inv_h, g.ny);
   const int cz = cell_coord(qz, g.oz, g.inv_h, g.nz);
@@ -298,8 +379,24 @@ __device__ __forceinline__ void match_coop_body(
   const float marg = 1e-3f + 4e-7f * fmaxf(fmaxf(fabsf(fqx), fabsf(fqy)),
                                            fmaxf(fabsf(fqz), (float)max(g.nx, max(g.ny, g.nz))));
   const double inv_h2 = g.inv_h * g.inv_h;
-  auto sphere_scan = [&](const int rs, const int max_rows) -> bool {
-    const float Rc = sqrtf(__double2float_ru(best * inv_h2)) * (1.0f + 1e-6f) + marg;  // radius in cells, rounded up
+  // With a certificate to write (S true), the scan prunes with the skin: rows and chords are
+  // bounded by (sqrt(best) + kCertSkin h)^2 instead of best, a superset of the same candidates
+  // (the result does not change), it keeps sec (consider_sec) and sets rho.
+  float rho = 0.0f;
+  auto sphere_scan = [&](auto S, const int rs, const int max_rows) -> bool {
+    constexpr bool SK = decltype(S)::value;
+    // squared pruning radius in cells, rounded up; ties are still visited (1e-12)
+    auto lim_of = [&](double b) -> float {
+      if constexpr (SK) {
+        const float r = __fadd_ru(__fsqrt_ru(__double2float_ru(b * (1.0 + 1e-12) * inv_h2)), kCertSkin);
+        return __fmul_ru(r, r);
+      } else {
+        return __double2float_ru(b * (1.0 + 1e-12) * inv_h2);
+      }
+    };
+    double sec = kInf;
+    float Rc = sqrtf(__double2float_ru(best * inv_h2)) * (1.0f + 1e-6f) + marg;  // radius in cells, rounded up
+    if constexpr (SK) Rc += kCertSkin;
     const int ya = min(max(__float2int_rd(fqy - Rc), 0), g.ny - 1), yb = min(max(__float2int_rd(fqy + Rc), 0), g.ny - 1);
     const int za = min(max(__float2int_rd(fqz - Rc), 0), g.nz - 1), zb = min(max(__float2int_rd(fqz + Rc), 0), g.nz - 1);
     const int nyb = yb - ya + 1;
@@ -307,7 +404,7 @@ __device__ __forceinline__ void match_coop_body(
     if (rows > max_rows) return false;
     // (yr, zr) walk the box with stride MG, kept incrementally (no division per row)
     int zr = sub / nyb, yr = sub - zr * nyb;
-    float limc = __double2float_ru(best * (1.0 + 1e-12) * inv_h2);  // strictly farther rows only: ties are still visited
+    float limc = lim_of(best);
     double best_seen = best;
     for (int t = sub; t < (int)rows; t += MG, yr += MG) {
       while (yr >= nyb) {
@@ -317,7 +414,7 @@ __device__ __forceinline__ void match_coop_body(
       const int yy = ya + yr, zz = za + zr;
       if (best != best_seen) {
         best_seen = best;
-        limc = __double2float_ru(best * (1.0 + 1e-12) * inv_h2);
+        limc = lim_of(best);
       }
       const float by = fmaxf(fabsf(fqy - ((float)yy + 0.5f)) - 0.5f - marg, 0.0f);
       const float bz = fmaxf(fabsf(fqz - ((float)zz + 0.5f)) - 0.5f - marg, 0.0f);
@@ -332,6 +429,8 @@ __device__ __forceinline__ void match_coop_body(
         const int le = min(xe, cx - rs - 1), rb = max(xs, cx + rs + 1);
         if (xs <= le) scan_range(g.recs, cs[row + xs], cs[row + le + 1], qx, qy, qz, best, bidx, bpos);
         if (rb <= xe) scan_range(g.recs, cs[row + rb], cs[row + xe + 1], qx, qy, qz, best, bidx, bpos);
+      } else if constexpr (SK) {  // rs = 0: the warm-start scan
+        scan_range_sec(g.recs, cs[row + xs], cs[row + xe + 1], qx, qy, qz, best, bidx, bpos, sec);
       } else {
         scan_range(g.recs, cs[row + xs], cs[row + xe + 1], qx, qy, qz, best, bidx, bpos);
       }
@@ -341,11 +440,32 @@ __device__ __forceinline__ void match_coop_body(
       const double od = __shfl_xor_sync(gmask, best, o, MG);
       const long long oi = __shfl_xor_sync(gmask, bidx, o, MG);
       const uint32_t op = __shfl_xor_sync(gmask, bpos, o, MG);
-      if (od < best || (od == best && oi >= 0 && (bidx < 0 || oi < bidx))) {
+      if constexpr (SK) {
+        // the pair's loser is a second point unless it is the winner's record (bidx >= 0 in
+        // every lane: the scan starts from the warm-start record)
+        const double osec = __shfl_xor_sync(gmask, sec, o, MG);
+        const bool take = od < best || (od == best && oi < bidx);
+        sec = fmin(sec, osec);
+        if (op != bpos) sec = fmin(sec, take ? best : od);
+        if (take) {
+          best = od;
+          bidx = oi;
+          bpos = op;
+        }
+      } else if (od < best || (od == best && oi >= 0 && (bidx < 0 || oi < bidx))) {
         best = od;
         bidx = oi;
         bpos = op;
       }
+    }
+    if constexpr (SK) {
+      // U >= |c - m| and L <= |c - j| for every other record j: sec bounds the visited ones (the
+      // computed squared distances are within a few ulps), and every record the scan skipped lies
+      // farther than sqrt(lim_of(best)) cells: each lane pruned with lim_of(its best) >=
+      // lim_of(the group's best), rounded up, with the margins of the row bounds
+      const double L = fmin(sqrt(sec) * (1.0 - 1e-14), sqrt((double)lim_of(best)) * g.h * (1.0 - 1e-6));
+      const double U = sqrt(best) * (1.0 + 1e-14);
+      rho = __double2float_rd((L - U) * 0.5 - 1e-12 * L);
     }
     return true;
   };
@@ -355,7 +475,7 @@ __device__ __forceinline__ void match_coop_body(
   // iteration of a registration) the old neighbour is a poor bound — several cells — while the
   // true one is almost surely in the query's own row: ring 1 first, it prunes with the bound it
   // has and leaves a much smaller sphere to the scan after it.
-  if (use_sphere && best < kInf && sphere_scan(0, 4 * MG)) resolved = true;
+  if (use_sphere && best < kInf && sphere_scan(std::integral_constant<bool, CERT>{}, 0, 4 * MG)) resolved = true;
   for (int r = 1; !resolved; ++r) {
     const int x0 = cx - r, x1 = cx + r;
     const int xa = max(x0, 0), xb = min(x1, g.nx - 1);
@@ -521,7 +641,7 @@ __device__ __forceinline__ void match_coop_body(
     }
     // a point is known now: finish inside its sphere instead of growing the cube ring by ring
     // (best is uniform across the group after the reduction, so the whole group takes one branch)
-    if (use_sphere && best < kInf && sphere_scan(r, 64 * MG)) {  // ~15 instructions per pruned row: cheaper than the next rings up to there
+    if (use_sphere && best < kInf && sphere_scan(std::false_type{}, r, 64 * MG)) {  // ~15 instructions per pruned row: cheaper than the next rings up to there
       resolved = true;
       break;
     }
@@ -535,6 +655,16 @@ __device__ __forceinline__ void match_coop_body(
     return;
   }
   if (co.nn_pos) co.nn_pos[qi] = resolved ? bpos : 0xffffffffu;
+  if constexpr (CERT) {
+    if (cert.rho) {
+      if (rho > 0.0f) {
+        cert.c[3 * qi + 0] = qx;
+        cert.c[3 * qi + 1] = qy;
+        cert.c[3 * qi + 2] = qz;
+      }
+      cert.rho[qi] = rho;
+    }
+  }
   if (!resolved) {
     const unsigned int slot = atomicAdd(&unresolved[K], 1u);
     unresolved[slot] = (unsigned int)qi;
@@ -561,9 +691,9 @@ __global__ void __launch_bounds__(128)
                       const float4* __restrict__ q_nrm, const double* __restrict__ mov_xyz,
                       long long K, int rmax, int with_distance, long long* __restrict__ nn_idx,
                       double* __restrict__ out, unsigned int* __restrict__ unresolved,
-                      unsigned int* __restrict__ lin_hist, double cap2, CorrOut co) {
-  match_coop_body<MG>(g, st, q_xyz, q_nrm, mov_xyz, K, rmax, with_distance, nn_idx, out, unresolved,
-                      lin_hist, cap2, co, blockIdx.x * (long long)blockDim.x + threadIdx.x);
+                      unsigned int* __restrict__ lin_hist, double cap2, CorrOut co, MatchCert cert) {
+  match_coop_body<MG, false, true>(g, st, q_xyz, q_nrm, mov_xyz, K, rmax, with_distance, nn_idx, out, unresolved,
+                                   lin_hist, cap2, co, blockIdx.x * (long long)blockDim.x + threadIdx.x, nullptr, cert);
 }
 
 // Batched form: blockIdx.y is the pair, everything else comes from its descriptor.  The ring
@@ -1355,14 +1485,21 @@ void match_launch(Ctx& c, bool with_distance, double* out_d2, cudaEvent_t mid, b
   reserve_binstore(c);
   c.m_xyz.reserve(3 * std::max<long long>(K, 1));
   c.nn_pos.reserve(std::max<long long>(K, 1));
+  c.cert_c.reserve(3 * std::max<long long>(K, 1));
+  c.cert_rho.reserve(std::max<long long>(K, 1));
+  if (c.cert_count.p == nullptr) {
+    c.cert_count.reserve(2);
+    SICP_CUDA(cudaMemsetAsync(c.cert_count.p, 0, 2 * sizeof(unsigned int), c.stream));
+  }
   const bool warm = with_distance && c.warm_start && c.nn_pos_valid && c.nn_pos_K == K;
   const CorrOut co = with_distance ? CorrOut{c.binstore.p, c.bin_cap, c.m_xyz.p, c.nn_pos.p, warm ? 1 : 0, c.sphere_scan,
                                              mov_attr_nrm(c), mov_attr_eff(c), c.mov_cos_max}
                                    : CorrOut{nullptr, 0, nullptr, nullptr, 0, 0, nullptr, nullptr, -1.0};
-  if (with_distance) {
-    c.nn_pos_valid = (c.nn_engine != SICP_NN_BRUTE) && c.match_group != 1;
-    c.nn_pos_K = K;
-  }
+  // A match without distance overwrites nn_idx, which the certificates of the next warm match
+  // keep: it ends the warm-start state like a new selection does.
+  c.nn_pos_valid = with_distance && (c.nn_engine != SICP_NN_BRUTE) && c.match_group != 1;
+  if (with_distance) c.nn_pos_K = K;
+  c.cert_slot = -1;
   double* out = with_distance ? c.dist.p : out_d2;
   if (c.nn_engine == SICP_NN_BRUTE) {
     bf_launch(c, with_distance, out, true);
@@ -1381,11 +1518,20 @@ void match_launch(Ctx& c, bool with_distance, double* out_d2, cudaEvent_t mid, b
         c.gmov.view, c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
         with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
   } else {
+    // every match with distance writes the certificate of each query it searches (none where it
+    // cannot prove one), so they are valid wherever nn_pos is; the launch counts into one of the
+    // two counters and zeroes the other for the next
+    MatchCert cert{nullptr, nullptr, nullptr, nullptr};
+    if (with_distance) {
+      c.cert_slot = c.cert_next;
+      c.cert_next ^= 1;
+      cert = MatchCert{c.cert_c.p, c.cert_rho.p, c.cert_count.p + c.cert_slot, c.cert_count.p + (c.cert_slot ^ 1)};
+    }
     const int mg = match_lanes(c, K, 2);
     with_lanes<2, 4, 8, 16>(mg, [&](auto L) {
       launch_kernel(k_match_grid_coop<decltype(L)::value>, dim3((unsigned)((K * mg + 127) / 128)), dim3(128), 0,
                     c.stream, pdl, c.gmov.view, c.dev_state.p, c.q_xyz.p, c.q_nrm.p, c.mov_xyz.p, K, rmax,
-                    with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co);
+                    with_distance ? 1 : 0, c.nn_idx.p, out, c.unresolved.p, lh, cap2, co, cert);
     });
   }
   SICP_CUDA(cudaGetLastError());
