@@ -326,6 +326,39 @@ int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const
                              sicp_pair_result* out /*[h] n_scans*/,
                              int64_t* n_selected /*[h] n_scans or NULL*/);
 
+/* ---- many pairs drawn from ONE set of clouds (scan sequences, loop closures, several priors) ----
+ * sicp_register_pairs registers n_pairs pairs whose clouds come from n_clouds clouds: pair i is
+ * (xyz[fix_id[i]], xyz[mov_id[i]]).
+ *  - Equality: out[i] and n_selected[i] equal, bit for bit, what sicp_register_batch returns for
+ *    pair i of the expanded list (fix_xyz[i] = xyz[fix_id[i]], mov_xyz[i] = xyz[mov_id[i]]) with
+ *    the same p and observed: every field, every variant, with and without max_overlap_distance
+ *    and mov_neighbors.  sicp_get_batch_outputs afterwards returns the same bits as after that
+ *    call (transformed clouds, residuals, log, T).
+ *  - Shared clouds: fix_id[i] == mov_id[i] is allowed, a cloud may be fixed in one pair and movable
+ *    in another, and a cloud no pair references is not read (its pointer may be NULL).
+ *  - Done once per cloud: each referenced cloud is uploaded once (any memory kind) and gridded once
+ *    under sicp_register_batch's cell plan; that grid is both its fixed and its movable grid.  With
+ *    mov_neighbors, each cloud that is movable in some pair gets its normals estimated once.  The
+ *    loop is per pair, as in sicp_register_batch.
+ *  - SICP_ERR_BAD_ARG, before any device work: the checks of sicp_register_batch's parameters
+ *    (n_pairs in [1, 65535], correspondences <= 4096, ...), n_clouds < 1, an id outside
+ *    [0, n_clouds), a referenced cloud with a NULL pointer or no point, a cloud that is fixed in a
+ *    pair with fewer than `neighbors` points, a cloud that is movable in a pair with fewer than
+ *    mov_neighbors points, sum n over the referenced clouds >= 2^32, or sum over pairs of
+ *    n[fix_id[i]] >= 2^32 (the overlap filter's keep flags and their prefix sum are per pair and
+ *    32-bit).
+ *  - The map (sicp_set_map) is not touched.  sicp_timings: upload_ms is the upload of the clouds,
+ *    grid_fix_ms the single grid build, grid_mov_ms 0.
+ *  - Device memory: the clouds once (24 B per point) and their one grid, plus sicp_register_batch's
+ *    per-pair buffers and 4 B of overlap flags per fixed point of each pair.                   */
+int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                            const int64_t* n /*[h] n_clouds*/, int32_t n_pairs,
+                            const int32_t* fix_id /*[h] n_pairs*/, const int32_t* mov_id /*[h] n_pairs*/,
+                            const sicp_register_params* p,
+                            const double* observed /*[h] n_pairs x 6, radians, or NULL*/,
+                            sicp_pair_result* out /*[h] n_pairs*/,
+                            int64_t* n_selected /*[h] n_pairs or NULL*/);
+
 /* ---- growing the map and reading it back -------------------------------------------------------
  * sicp_map_insert appends to the map, for every voxel of size voxel_size it does not occupy, the
  * first new point that falls into it.  C is the concatenation of the n_clouds clouds in call
@@ -428,18 +461,18 @@ int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const*
                            int64_t* n_within          /*[h] n_clouds, or NULL*/);
 
 /* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
- * sicp_register_batch and sicp_register_to_map report per pair only the record above.  This call
- * returns what else sicp_register returns, for every pair of the LAST successful call of either
- * on this context: X_mov_transformed (transform_by_H, pointcloud.py:205-217, as at
+ * sicp_register_batch, sicp_register_to_map and sicp_register_pairs report per pair only the
+ * record above.  This call returns what else sicp_register returns, for every pair of the LAST
+ * successful call of any of them on this context: X_mov_transformed (transform_by_H, pointcloud.py:205-217, as at
  * simpleicp.py:316), the final distance residuals (simpleicp.py:324, 4th return value), the
  * per-iteration records and the applied transform.  Those two calls only leave these on the
  * device; all the work happens here, and they stay readable (any number of times, same bits)
- * until the next sicp_register_batch, sicp_register_to_map, sicp_set_map, sicp_map_insert,
- * sicp_map_crop or sicp_map_thin on the context.
+ * until the next sicp_register_batch, sicp_register_to_map, sicp_register_pairs, sicp_set_map,
+ * sicp_map_insert, sicp_map_crop or sicp_map_thin on the context.
  *  - SICP_ERR_STATE: before any such call, after sicp_set_map, sicp_map_insert, sicp_map_crop or
  *    sicp_map_thin, or after a
- *    batch / map call that returned an error (each of these clears the outputs on entry; only a
- *    successful return of the first two makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
+ *    batch / map / pairs call that returned an error (each of these clears the outputs on entry;
+ *    only a successful return of the first three makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
  *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose
  *    status was not SICP_OK (SICP_ERR_NO_OVERLAP included) is ever written.
  *  - mov_xyz_out[i]: pair i's movable cloud (n_mov[i] x 3) moved by the transform the run applied,
@@ -470,7 +503,7 @@ typedef struct {
                                in the barrier-free kernel (all but the first, normally)          */
   int64_t rerun_iterations; /* ... iterations repeated through the general kernel because the
                                order-statistic prediction of the barrier-free kernel missed       */
-  double mov_normals_ms;    /* last sicp_register / sicp_register_batch with mov_neighbors > 0:
+  double mov_normals_ms;    /* last sicp_register / batched call with mov_neighbors > 0:
                                k-NN + PCA of the movable cloud(s); 0 otherwise                    */
   int64_t overlap_candidates; /* last sicp_register_to_map: bounded searches its culled overlap
                                filter ran (map points inside the scans' grown boxes); 0 without

@@ -2,7 +2,8 @@
 
 Drop-in names of the reference package (python/simpleicp/__init__.py:12-14):
 ``SimpleICP``, ``PointCloud``, ``RigidBodyParameters``; plus the functional form
-``simpleicp(X_fix, X_mov, **kwargs)`` and the batched / multi-GPU ``simpleicp_batch``.
+``simpleicp(X_fix, X_mov, **kwargs)``, the batched / multi-GPU ``simpleicp_batch`` and
+``simpleicp_edges`` (many pairs drawn from one set of clouds).
 """
 __version__ = "0.1.0"
 
@@ -13,11 +14,11 @@ _logging.getLogger(__name__).addHandler(_logging.NullHandler())
 from .simpleicp import SimpleICP, SimpleICPException, simpleicp, register  # noqa: E402
 from .pointcloud import PointCloud, PointCloudException  # noqa: E402
 from .optimization import RigidBodyParameters, Parameter  # noqa: E402
-from .batch import Map, BatchError, simpleicp_batch, shard_pairs, tile_slabs, close_engine_pool  # noqa: E402
+from .batch import Map, BatchError, simpleicp_batch, simpleicp_edges, shard_pairs, tile_slabs, close_engine_pool  # noqa: E402
 from ._capi import read_xyz, write_xyz  # noqa: E402
 from .linearized import simpleicp_linearized  # noqa: E402
 
 __all__ = [
     "SimpleICP", "SimpleICPException", "PointCloud", "PointCloudException", "RigidBodyParameters",
-    "Parameter", "simpleicp", "simpleicp_linearized", "register", "simpleicp_batch", "Map", "BatchError", "shard_pairs", "tile_slabs", "close_engine_pool", "read_xyz", "write_xyz",
+    "Parameter", "simpleicp", "simpleicp_linearized", "register", "simpleicp_batch", "simpleicp_edges", "Map", "BatchError", "shard_pairs", "tile_slabs", "close_engine_pool", "read_xyz", "write_xyz",
 ]

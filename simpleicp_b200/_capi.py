@@ -41,7 +41,7 @@ SYMBOLS = (
     "sicp_set_normals", "sicp_set_mov_normals", "sicp_get_knn", "sicp_match", "sicp_reject", "sicp_solve",
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
-    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_get_batch_outputs",
+    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_get_batch_outputs",
     "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
@@ -167,6 +167,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_set_map": [vp, vp, i64],
         "sicp_register_to_map": [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(RegisterParams), vp,
                                  C.POINTER(PairResult), vp],
+        "sicp_register_pairs": [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i32), C.POINTER(i32),
+                                C.POINTER(RegisterParams), vp, C.POINTER(PairResult), vp],
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
@@ -584,6 +586,42 @@ class Engine:
         out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
         return out
 
+    def register_pairs(self, clouds, pairs, correspondences, neighbors, params: RunParams,
+                       max_overlap_distance: float = -1.0, observed=None, mov_neighbors: int = 0,
+                       max_angle_rad: float = -1.0):
+        """sicp_register_pairs: register_batch for pairs drawn from one set of clouds.  `clouds` is a
+        sequence of (n_i, 3) NumPy arrays or CUDA tensors, None for a cloud no pair uses; `pairs`
+        is (n_pairs, 2) of (fixed, movable) indices into `clouds`.  Each referenced cloud is
+        uploaded and gridded once (and with `mov_neighbors` given its normals once), and pair i's
+        result equals, bit for bit, register_batch's for (clouds[pairs[i, 0]], clouds[pairs[i, 1]]).
+        Same other arguments and result as register_batch (`n_mov` is the size of each pair's
+        movable cloud), so batch_outputs works on it."""
+        ids = np.asarray(pairs)
+        if ids.ndim != 2 or ids.shape[1] != 2 or ids.shape[0] < 1 or not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError(f"pairs must be integers of shape (n_pairs, 2) with n_pairs >= 1, got {ids.dtype} "
+                             f"of shape {ids.shape}")
+        if ids.min() < -(1 << 31) or ids.max() >= (1 << 31):
+            raise ValueError("cloud ids must fit in int32")  # the library checks [0, n_clouds)
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        n, m = ids.shape[0], len(clouds)
+        keep = [None if X is None else _as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
+        ptrs = (C.c_void_p * m)(*[_ptr(X) for X in keep])
+        counts = (C.c_int64 * m)(*[0 if X is None else int(X.shape[0]) for X in keep])
+        fix, mov = np.ascontiguousarray(ids[:, 0]), np.ascontiguousarray(ids[:, 1])
+        observed = self._observed_rows(observed, n)
+        rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
+                                   max_angle_rad)
+        out = (PairResult * n)()
+        n_selected = np.zeros(n, dtype=np.int64)
+        self._check(self._lib.sicp_register_pairs(
+            self._h, m, ptrs, counts, n, fix.ctypes.data_as(C.POINTER(C.c_int32)),
+            mov.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(rp), None if observed is None else _ptr(observed), out,
+            _ptr(n_selected)))
+        out.n_selected = n_selected
+        # an id out of range was refused above
+        out.n_mov, out.max_iterations = np.array([counts[j] for j in mov], dtype=np.int64), int(params.max_iterations)
+        return out
+
     def map_insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
         """sicp_map_insert: append to the resident map, per voxel of `voxel_size` it does not
         occupy, the first finite point of `clouds` (in order) falling into it, cloud i moved by
@@ -660,7 +698,7 @@ class Engine:
 
     def batch_outputs(self, result):
         """sicp_get_batch_outputs for `result`, the PairResult array the last register_batch /
-        register_to_map on this engine returned: per pair (X_mov_transformed, residuals, log, T)
+        register_to_map / register_pairs on this engine returned: per pair (X_mov_transformed, residuals, log, T)
         -- the transformed movable cloud (pinned NumPy), the final residuals in kept order, the
         IterRecord of every iteration run and the applied 4 x 4 transform -- or None for a pair
         whose status is not SICP_OK."""

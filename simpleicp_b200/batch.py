@@ -230,6 +230,13 @@ def simpleicp_batch(
             messages.append(repr(errors[0]))
             done = np.isfinite(local[:, 16]) & (local[:, 16] != 0)
             local[~done] = pack_record(np.full((4, 4), np.nan), -99, 0, np.nan, np.nan)
+    return _gather_share(local, found, mine, n_pairs, rank, world_size, dist, device, on_error, full_output, messages)
+
+
+def _gather_share(local, found, mine, n_pairs, rank, world_size, dist, device, on_error, full_output, messages):
+    """The end of simpleicp_batch and simpleicp_edges: the rank's records `local` (and with
+    full_output its result objects `found`, both in the order of its share `mine`) all-gathered
+    into the table, BatchError per `on_error`, the return value."""
     dev = None
     if dist is not None and world_size > 1:
         import torch
@@ -247,9 +254,76 @@ def simpleicp_batch(
     return (table, results) if full_output else table
 
 
+def simpleicp_edges(clouds: Sequence, edges, *, rank: int = 0, world_size: int = 1, dist=None, device: int = 0,
+                    batch_size: int = 64, on_error: str = "raise", full_output: bool = False, **run_kwargs):
+    """Register many pairs drawn from one set of clouds; returns simpleicp_batch's (n_edges, 20)
+    record table on every rank.
+
+    `clouds` is a sequence of (n_i, 3) NumPy arrays or CUDA tensors; `edges` is (n_edges, 2) of
+    integer (fixed, movable) indices into it, e.g. the edges (i, i + 1) and (i, i + 2) of a scan
+    sequence, loop-closure candidates, or one pair repeated under several priors.  Edge i's row
+    equals that of ``simpleicp_batch([(clouds[a], clouds[b]) for a, b in edges], ...)`` bit for
+    bit, but every cloud a library call uses is uploaded and gridded once per call, and with
+    `mov_neighbors` given its normals once, however many edges share it (sicp_register_pairs).
+
+    Edges are taken in order, `batch_size` per library call; each call passes only the clouds its
+    edges reference (edge_chunks).  Edge i belongs to rank i % world_size, and only the table is
+    exchanged.  ``rbp_observed_values`` is the common 6-tuple or one row per edge (degrees), each
+    edge's prior.  The run() arguments served are those of the batched engine without
+    ``want_normals`` (at most 4096 correspondences); anything else is a TypeError.  `on_error`,
+    `full_output` and BatchError are as in simpleicp_batch."""
+    unknown = set(run_kwargs) - _EDGE_KEYS
+    if unknown:
+        raise TypeError(f"simpleicp_edges() got unsupported arguments {sorted(unknown)}")
+    if int(run_kwargs.get("correspondences", 1000)) > 4096:
+        raise ValueError("simpleicp_edges runs one block per edge: correspondences must be <= 4096")
+    e = _check_edges(edges, len(clouds))
+    n = e.shape[0]
+    rows = _per_pair_observed(run_kwargs, n)
+    _check_mov_kwargs(run_kwargs)
+    mine = shard_pairs(n, world_size, rank)
+    local = np.zeros((len(mine), RECORD_LEN))
+    found: List = [None] * len(mine)
+    messages: List[str] = []
+    _run_batched(lambda i: clouds[i], mine, local, device, batch_size, run_kwargs, messages, rows, edges=e,
+                 **({"results": found} if full_output else {}))
+    return _gather_share(local, found, mine, n, rank, world_size, dist, device, on_error, full_output, messages)
+
+
+def _check_edges(edges, n_clouds: int) -> np.ndarray:
+    """edges as an (n_edges, 2) int64 array of indices into n_clouds clouds, or ValueError."""
+    e = np.asarray(edges)
+    if e.ndim != 2 or e.shape[1] != 2:
+        raise ValueError(f"edges must have shape (n_edges, 2), got {e.shape}")
+    if e.size and not np.issubdtype(e.dtype, np.integer):
+        raise ValueError(f"edges must hold integer cloud indices, got {e.dtype}")
+    e = e.astype(np.int64)
+    if e.size and (e.min() < 0 or e.max() >= n_clouds):
+        raise ValueError(f"edges must index the {n_clouds} clouds: every entry in [0, {n_clouds})")
+    return e
+
+
+def edge_chunks(edges: np.ndarray, mine: Sequence[int], batch_size: int):
+    """The library calls of simpleicp_edges for a rank's share `mine` (edge numbers, in order):
+    `batch_size` edges per call, in order.  Each call is (js, cloud_ids, local_edges): the positions
+    js in `mine` of its edges, the clouds it passes (ascending indices into the caller's clouds:
+    exactly those its edges reference) and its edges remapped to positions in cloud_ids, so that
+    cloud_ids[local_edges[k]] == edges[mine[js[k]]]."""
+    bs = max(1, int(batch_size))
+    out = []
+    for lo in range(0, len(mine), bs):
+        js = np.arange(lo, min(lo + bs, len(mine)))
+        cloud_ids, inv = np.unique(edges[np.asarray(mine, dtype=np.int64)[js]], return_inverse=True)
+        out.append((js, cloud_ids, inv.reshape(-1, 2)))
+    return out
+
+
 _BATCH_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations",
                "distance_weights", "rbp_observed_values", "rbp_observation_weights", "max_overlap_distance",
                "want_normals", "mov_neighbors", "max_angle_between_normals"}
+# run() arguments simpleicp_edges serves (sicp_register_pairs): the batched engine's, without the
+# debug output
+_EDGE_KEYS = _BATCH_KEYS - {"want_normals"}
 
 
 def _batchable(kw) -> bool:
@@ -294,10 +368,13 @@ def _per_pair_observed(kw, n_pairs: int):
 _BATCH_ENGINES: dict = {}
 
 
-def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None, results=None):
+def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None, results=None,
+                 edges=None):
     """The rank's share `mine` through the batched engine, `batch_size` pairs per call, records into
     `local`.  With `map_engine` (an engine holding a map, sicp_set_map) get(i) is scan i alone and
-    every chunk is registered against that map (sicp_register_to_map).  With `results` (a list of
+    every chunk is registered against that map (sicp_register_to_map).  With `edges` (n_edges x 2
+    cloud indices) get(i) is cloud i, pair i is edge i, and every chunk passes the clouds its edges
+    reference (edge_chunks, sicp_register_pairs).  With `results` (a list of
     len(mine)) the full output of every pair that succeeded goes there too, fetched after each call
     (sicp_get_batch_outputs) because the next one reuses the library's buffers."""
     import torch
@@ -324,14 +401,17 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, 
         lsq = eng.lsq_params(obs, obs, [float(w) for w in obs_w], dw)
         params = eng.run_params(kw.get("min_planarity", 0.3), kw.get("min_change", 1.0),
                                 kw.get("max_iterations", 100), lsq)
-        for lo in range(0, len(mine), max(1, int(batch_size))):
-            ids = range(lo, min(lo + max(1, int(batch_size)), len(mine)))
-            pairs = [get(mine[j]) for j in ids]
+        bs = max(1, int(batch_size))
+        chunks = (edge_chunks(edges, mine, bs) if edges is not None else
+                  [(range(lo, min(lo + bs, len(mine))), None, None) for lo in range(0, len(mine), bs)])
+        for ids, cloud_ids, local_edges in chunks:
             observed = None if rows is None else np.array([_observed_in_radians(rows[mine[j]]) for j in ids])
-            res = register(pairs, kw.get("correspondences", 1000), kw.get("neighbors", 10), params,
-                           mod if np.isfinite(mod) else -1.0, observed,
-                           0 if k_mov is None else int(k_mov),
-                           -1.0 if ang is None else float(np.deg2rad(ang)))
+            args = (kw.get("correspondences", 1000), kw.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0,
+                    observed, 0 if k_mov is None else int(k_mov), -1.0 if ang is None else float(np.deg2rad(ang)))
+            if edges is None:
+                res = register([get(mine[j]) for j in ids], *args)
+            else:
+                res = eng.register_pairs([get(int(c)) for c in cloud_ids], local_edges, *args)
             for j, r in zip(ids, res):
                 if r.status == 0:
                     local[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)

@@ -27,7 +27,11 @@
 // context (sicp_set_map, MapStore): the fixed side is the map's grid, and the overlap filter only
 // searches the map points inside each scan's box mapped by its prior (map_cull_box, map_filter).
 //
-// sicp_get_batch_outputs returns what either call left on the device and did not download:
+// sicp_register_pairs runs them too for pairs drawn from one set of clouds: each cloud is
+// uploaded, gridded and (as a movable cloud) given its normals once, whatever number of pairs
+// uses it (register_pairs).
+//
+// sicp_get_batch_outputs returns what any of these calls left on the device and did not download:
 // transformed clouds, residual vectors, the per-iteration log and the applied transforms.
 #include <algorithm>
 #include <cstddef>
@@ -49,15 +53,16 @@ __global__ void k_gather_flags(const DevState* __restrict__ st, int n, int* __re
 }
 
 // Ordered compaction of the overlap filter: with S the exclusive prefix sum of the keep flags of
-// all fixed points of the batch, pair i's survivors are the slice [S[fo[i]], S[fo[i+1]]) of the
-// list, in ascending point order; each holds its index inside its own cloud.
+// all pairs' fixed points and fo[i] pair i's flag offset, pair i's survivors are the slice
+// [S[fo[i]], S[fo[i+1]]) of the list, in ascending point order; each holds its index inside its
+// own cloud.
 __global__ void __launch_bounds__(256)
     k_overlap_scatter(const PairDev* __restrict__ pairs, const uint32_t* __restrict__ keep,
                       const uint32_t* __restrict__ scan, uint32_t* __restrict__ list) {
   const PairDev& pd = pairs[blockIdx.y];
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= pd.n_fix) return;
-  const long long g = pd.fix_off + i;
+  const long long g = pd.flag_off + i;
   if (keep[g]) list[scan[g]] = (uint32_t)i;
 }
 
@@ -65,7 +70,7 @@ __global__ void __launch_bounds__(256)
 __global__ void k_overlap_bounds(const PairDev* __restrict__ pairs, int n_pairs, const uint32_t* __restrict__ scan,
                                  long long total, uint32_t* __restrict__ bounds) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i <= n_pairs) bounds[i] = scan[i < n_pairs ? pairs[i].fix_off : total];
+  if (i <= n_pairs) bounds[i] = scan[i < n_pairs ? pairs[i].flag_off : total];
 }
 
 // sicp_map_insert, one thread per point j of the concatenated clouds (cloud i owns [off[i],
@@ -200,16 +205,23 @@ __global__ void __launch_bounds__(256)
 // the cell policy of every grid of this file: both sides of a batch, the map and its inserts
 CellPolicy batch_policy(const Ctx& c) { return CellPolicy{CellPolicy::kBatch, c.grid_target_occ}; }
 
-// What the stages shared by sicp_register_batch and sicp_register_to_map know about one call.
+// What the stages shared by sicp_register_batch, sicp_register_to_map and sicp_register_pairs
+// know about one call.
 struct PairsRun {
   int n_pairs = 0;
   const sicp_register_params* rp = nullptr;
   const double* observed = nullptr;
   bool overlap = false;
   long long Kmax = 0, max_n_mov = 0;
-  std::vector<long long> mo;    // movable point offsets, n_pairs + 1
+  std::vector<long long> mo;    // prefix sums of the pairs' movable point counts, n_pairs + 1
   std::vector<DevState> hs;     // per-pair start state (the prior)
-  std::vector<PairDev> pd;      // descriptors; the caller fills gfix, n_fix and fix_off
+  // descriptors; the caller fills gfix, n_fix, fix_off, flag_off and mov_off, and with mov_built
+  // also gmov and cm (the movable grids exist already: run_pairs does not build them)
+  std::vector<PairDev> pd;
+  bool mov_built = false;
+  // pairs whose descriptors the movable-normals estimate runs over, one per distinct movable cloud;
+  // empty: every pair's (each owns its movable cloud)
+  std::vector<int> mov_first;
   std::vector<char> no_overlap;
 };
 
@@ -332,9 +344,10 @@ void take_survivors(Ctx& c, Batch& b, PairsRun& r, const uint32_t* bounds) {
                               c.stream));
 }
 
-// Overlap filter of sicp_register_batch: bounded search of every fixed point, one exclusive scan
-// over the keep flags of the whole batch, ordered scatter, and ONE read-back of the pair boundaries.
-void batch_filter(Ctx& c, Batch& b, PairsRun& r, long long max_n_fix) {
+// Overlap filter of sicp_register_batch and sicp_register_pairs: bounded search of every fixed
+// point of every pair (coordinates in fix_xyz), one exclusive scan over the keep flags of the whole
+// batch, ordered scatter, and ONE read-back of the pair boundaries.
+void batch_filter(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, long long max_n_fix) {
   cudaStream_t st = c.stream;
   const int n_pairs = r.n_pairs;
   const long long nf = b.total_fix;
@@ -343,7 +356,7 @@ void batch_filter(Ctx& c, Batch& b, PairsRun& r, long long max_n_fix) {
   b.ovl_list.reserve(std::max<long long>(nf, 1));
   b.ovl_bounds.reserve((size_t)n_pairs + 1);
   // r2 as sicp_register computes it
-  batch_overlap_launch(c, b, max_n_fix, r.rp->max_overlap_distance * r.rp->max_overlap_distance);
+  batch_overlap_launch(c, b, fix_xyz, max_n_fix, r.rp->max_overlap_distance * r.rp->max_overlap_distance);
   scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums);
   k_overlap_scatter<<<dim3((unsigned)((max_n_fix + 255) / 256), n_pairs), 256, 0, st>>>(b.pairs.p, b.ovl_flag.p,
                                                                                      b.ovl_scan.p, b.ovl_list.p);
@@ -452,10 +465,10 @@ static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
   take_survivors(c, b, r, bounds);
 }
 
-// Everything after the fixed side: descriptors, [select + normals], movable grids, [overlap filter,
-// select + normals], movable normals, the loop and the results.  fix_xyz holds the fixed
-// coordinates the descriptors' fix_off index; map (or null) is the resident map of
-// sicp_register_to_map, whose filter is the culled one.
+// Everything after the fixed side: descriptors, [select + normals], movable grids (unless the
+// caller built them), [overlap filter, select + normals], movable normals, the loop and the
+// results.  fix_xyz holds the fixed coordinates the descriptors' fix_off index; map (or null) is
+// the resident map of sicp_register_to_map, whose filter is the culled one.
 static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapStore* map, long long max_n_fix,
                       sicp_pair_result* out, int64_t* n_selected) {
   cudaStream_t st = c.stream;
@@ -465,7 +478,6 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   for (int i = 0; i < n_pairs; ++i) {
     PairDev& d = r.pd[(size_t)i];
     d.n_mov = r.mo[(size_t)i + 1] - r.mo[(size_t)i];
-    d.mov_off = r.mo[(size_t)i];
     d.K = std::min<long long>(rp->correspondences, d.n_fix);
     d.q_off = (long long)i * r.Kmax;
     for (int j = 0; j < 6; ++j) d.obs[j] = r.observed ? r.observed[6 * i + j] : p.lsq.observed[j];
@@ -485,20 +497,24 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   }
 
   // ---- movable side
-  SICP_CUDA(cudaStreamWaitEvent(st, c.ev_copy, 0));
-  std::vector<HostCloud> clouds((size_t)n_pairs);
-  std::vector<GridView> views;
-  std::vector<double> centres;
-  for (int i = 0; i < n_pairs; ++i)
-    clouds[(size_t)i] = HostCloud{b.mov_xyz.p + 3 * r.mo[(size_t)i], r.pd[(size_t)i].n_mov, r.mo[(size_t)i]};
-  {
-    StageTimer t(c, &c.tm.grid_mov_ms);
-    grid_build(c, b.gmov, clouds, batch_policy(c), views, centres);
-    t.stop();
-  }
-  for (int i = 0; i < n_pairs; ++i) {
-    r.pd[(size_t)i].gmov = views[(size_t)i];
-    for (int a = 0; a < 3; ++a) r.pd[(size_t)i].cm[a] = centres[(size_t)i * 3 + a];
+  if (!r.mov_built) {
+    SICP_CUDA(cudaStreamWaitEvent(st, c.ev_copy, 0));
+    std::vector<HostCloud> clouds((size_t)n_pairs);
+    std::vector<GridView> views;
+    std::vector<double> centres;
+    for (int i = 0; i < n_pairs; ++i) {
+      const PairDev& d = r.pd[(size_t)i];
+      clouds[(size_t)i] = HostCloud{b.mov_xyz.p + 3 * d.mov_off, d.n_mov, d.mov_off};
+    }
+    {
+      StageTimer t(c, &c.tm.grid_mov_ms);
+      grid_build(c, b.gmov, clouds, batch_policy(c), views, centres);
+      t.stop();
+    }
+    for (int i = 0; i < n_pairs; ++i) {
+      r.pd[(size_t)i].gmov = views[(size_t)i];
+      for (int a = 0; a < 3; ++a) r.pd[(size_t)i].cm[a] = centres[(size_t)i * 3 + a];
+    }
   }
   r.no_overlap.assign((size_t)n_pairs, 0);
   c.tm.overlap_ms = 0;
@@ -506,17 +522,28 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
     SICP_CUDA(cudaMemcpyAsync(b.pairs.p, r.pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
     StageTimer t(c, &c.tm.overlap_ms);
     if (map) map_filter(c, b, *map, r);
-    else batch_filter(c, b, r, max_n_fix);
+    else batch_filter(c, b, r, fix_xyz, max_n_fix);
     t.stop();
   }
   SICP_CUDA(cudaMemcpyAsync(b.pairs.p, r.pd.data(), sizeof(PairDev) * (size_t)n_pairs, cudaMemcpyHostToDevice, st));
   if (r.overlap) select_and_normals();
-  // pc_mov.estimate_normals(mov_neighbors) of every pair, in its own movable grid
+  // pc_mov.estimate_normals(mov_neighbors) of every movable cloud, once, in its own grid
   b.mov_attr = rp->mov_neighbors > 0;
   b.mov_cos_max = b.mov_attr ? mov_cos_max_of(rp->max_angle_rad) : -1.0;
   c.tm.mov_normals_ms = 0;
   if (b.mov_attr) {
     b.q_nrm_eff.reserve((size_t)n_pairs * (size_t)r.Kmax);
+    if (r.mov_first.empty()) {
+      b.mov_desc = b.pairs.p;
+      b.n_mov_desc = n_pairs;
+    } else {
+      std::vector<PairDev> desc;
+      for (int i : r.mov_first) desc.push_back(r.pd[(size_t)i]);
+      b.mov_pairs.reserve(desc.size());
+      SICP_CUDA(cudaMemcpyAsync(b.mov_pairs.p, desc.data(), sizeof(PairDev) * desc.size(), cudaMemcpyHostToDevice, st));
+      b.mov_desc = b.mov_pairs.p;
+      b.n_mov_desc = (int)desc.size();
+    }
     StageTimer t(c, &c.tm.mov_normals_ms);
     b.max_n_mov = r.max_n_mov;
     normals_launch(c, &b, true, rp->mov_neighbors);
@@ -566,12 +593,13 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   // what sicp_get_batch_outputs needs of this call (host bookkeeping only)
   b.out_n_pairs = n_pairs;
   b.out_max_iterations = p.max_iterations;
-  b.out_mo = r.mo;
+  b.out_n_mov.resize((size_t)n_pairs);
   b.out_n_kept.resize((size_t)n_pairs);
   b.out_status.resize((size_t)n_pairs);
   b.out_iterations.resize((size_t)n_pairs);
   b.out_mean_std.resize(2 * (size_t)n_pairs);
   for (int i = 0; i < n_pairs; ++i) {
+    b.out_n_mov[(size_t)i] = r.pd[(size_t)i].n_mov;
     b.out_n_kept[(size_t)i] = out[i].n_kept;
     b.out_status[(size_t)i] = out[i].status;
     b.out_iterations[(size_t)i] = out[i].iterations;
@@ -588,23 +616,25 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
 static void get_batch_outputs(Ctx& c, int n_pairs, double* const* mov_xyz_out, double* const* residuals,
                               sicp_iter_record* log, double* T) {
   SICP_REQUIRE(c.batch && c.batch->out_valid, SICP_ERR_STATE,
-               "no batch outputs: no sicp_register_batch / sicp_register_to_map has succeeded since the last "
-               "sicp_set_map");
+               "no batch outputs: no sicp_register_batch / sicp_register_to_map / sicp_register_pairs has "
+               "succeeded since the last sicp_set_map");
   Batch& b = *c.batch;
   SICP_REQUIRE(n_pairs == b.out_n_pairs, SICP_ERR_BAD_ARG,
                "n_pairs must equal the last batched call's (" + std::to_string(b.out_n_pairs) + ")");
   cudaStream_t st = c.stream;
   const int n = n_pairs;
   const auto ok = [&](int i) { return b.out_status[(size_t)i] == SICP_OK; };
-  const auto n_mov = [&](int i) { return b.out_mo[(size_t)i + 1] - b.out_mo[(size_t)i]; };
-  // requested pairs: transforms first, then residual vectors (with their output offsets)
+  const auto n_mov = [&](int i) { return b.out_n_mov[(size_t)i]; };
+  // requested pairs: transforms first, then residual vectors, each with its output offset
   std::vector<int> ids;
   std::vector<long long> off;
-  long long max_n_mov = 0, n_res = 0;
+  long long max_n_mov = 0, n_pts = 0, n_res = 0;
   if (mov_xyz_out)
     for (int i = 0; i < n; ++i)
       if (ok(i) && mov_xyz_out[i]) {
         ids.push_back(i);
+        off.push_back(n_pts);
+        n_pts += n_mov(i);
         max_n_mov = std::max(max_n_mov, n_mov(i));
       }
   const int n_xyz = (int)ids.size();
@@ -618,24 +648,24 @@ static void get_batch_outputs(Ctx& c, int n_pairs, double* const* mov_xyz_out, d
   const int n_rv = (int)ids.size() - n_xyz;
   if (!ids.empty()) {
     b.out_ids.reserve(ids.size());
+    b.out_off.reserve(off.size());
     SICP_CUDA(cudaMemcpyAsync(b.out_ids.p, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, st));
+    SICP_CUDA(cudaMemcpyAsync(b.out_off.p, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice, st));
   }
   if (n_xyz > 0) {
-    b.xyz_out.reserve(3 * (size_t)b.out_mo[(size_t)n]);
-    batch_transform_launch(c, b, b.out_ids.p, n_xyz, max_n_mov, b.xyz_out.p);
+    b.xyz_out.reserve(3 * (size_t)n_pts);
+    batch_transform_launch(c, b, b.out_ids.p, n_xyz, b.out_off.p, max_n_mov, b.xyz_out.p);
     for (int j = 0; j < n_xyz; ++j) {
       const int i = ids[(size_t)j];
-      copy_any(c, mov_xyz_out[i], b.xyz_out.p + 3 * b.out_mo[(size_t)i], sizeof(double) * 3 * (size_t)n_mov(i));
+      copy_any(c, mov_xyz_out[i], b.xyz_out.p + 3 * off[(size_t)j], sizeof(double) * 3 * (size_t)n_mov(i));
     }
   }
   if (n_rv > 0) {
-    b.out_off.reserve(off.size());
     b.resid_out.reserve((size_t)n_res);
-    SICP_CUDA(cudaMemcpyAsync(b.out_off.p, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice, st));
-    batch_residuals_launch(c, b, b.out_ids.p + n_xyz, n_rv, b.out_off.p, b.resid_out.p);
+    batch_residuals_launch(c, b, b.out_ids.p + n_xyz, n_rv, b.out_off.p + n_xyz, b.resid_out.p);
     for (int j = 0; j < n_rv; ++j) {
       const int i = ids[(size_t)(n_xyz + j)];
-      copy_any(c, residuals[i], b.resid_out.p + off[(size_t)j], sizeof(double) * (size_t)b.out_n_kept[(size_t)i]);
+      copy_any(c, residuals[i], b.resid_out.p + off[(size_t)(n_xyz + j)], sizeof(double) * (size_t)b.out_n_kept[(size_t)i]);
     }
   }
   const size_t it_max = (size_t)b.out_max_iterations;
@@ -717,7 +747,8 @@ static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, co
   for (int i = 0; i < n_pairs; ++i) {
     r.pd[(size_t)i].gfix = views[(size_t)i];
     r.pd[(size_t)i].n_fix = n_fix[i];
-    r.pd[(size_t)i].fix_off = fo[(size_t)i];
+    r.pd[(size_t)i].fix_off = r.pd[(size_t)i].flag_off = fo[(size_t)i];
+    r.pd[(size_t)i].mov_off = r.mo[(size_t)i];
   }
   run_pairs(c, b, r, b.fix_xyz.p, nullptr, max_n_fix, out, n_selected);
 }
@@ -779,9 +810,111 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
   for (int i = 0; i < n_scans; ++i) {
     r.pd[(size_t)i].gfix = m.view;
     r.pd[(size_t)i].n_fix = m.n;
-    r.pd[(size_t)i].fix_off = 0;
+    r.pd[(size_t)i].fix_off = r.pd[(size_t)i].flag_off = 0;
+    r.pd[(size_t)i].mov_off = r.mo[(size_t)i];
   }
   run_pairs(c, b, r, m.xyz.p, &m, m.n, out, n_selected);
+}
+
+// sicp_register_pairs: pair i is (cloud fix_id[i], cloud mov_id[i]).  Every referenced cloud is
+// uploaded once into Batch::mov_xyz, which serves as both sides, and gridded once in Batch::gfix:
+// that grid is its fixed grid and its movable grid (a grid depends only on its own cloud, so it is
+// the one sicp_register_batch builds for it on either side).  The movable normals run once per
+// distinct movable cloud.  Each pair has its own keep flags (flag_off) and its own output slices,
+// so pairs that share a cloud never write into a shared slice.  The rest is run_pairs, as for
+// sicp_register_batch on the expanded pairs.
+static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_pairs,
+                           const int32_t* fix_id, const int32_t* mov_id, const sicp_register_params* rp,
+                           const double* observed, sicp_pair_result* out, int64_t* n_selected) {
+  if (c.batch) c.batch->out_valid = false;
+  check_pairs_params(c, n_pairs, xyz && n && fix_id && mov_id && out, rp);
+  SICP_REQUIRE(n_clouds >= 1, SICP_ERR_BAD_ARG, "n_clouds must be >= 1");
+  // role[j]: bit 0 = fixed in some pair, bit 1 = movable in some pair; 0 = not read
+  std::vector<int> role((size_t)n_clouds, 0);
+  for (int i = 0; i < n_pairs; ++i) {
+    SICP_REQUIRE(fix_id[i] >= 0 && fix_id[i] < n_clouds && mov_id[i] >= 0 && mov_id[i] < n_clouds,
+                 SICP_ERR_BAD_ARG, "pair " + std::to_string(i) + ": cloud ids must be in [0, n_clouds)");
+    role[(size_t)fix_id[i]] |= 1;
+    role[(size_t)mov_id[i]] |= 2;
+  }
+  // the referenced clouds' offsets in the store; the store, the overlap flags and their prefix
+  // sums are indexed with 32-bit offsets
+  constexpr long long k32 = 1ll << 32;
+  std::vector<long long> off((size_t)n_clouds, -1);
+  std::vector<int> ref;
+  long long total = 0;
+  for (int j = 0; j < n_clouds; ++j) {
+    if (!role[(size_t)j]) continue;
+    SICP_REQUIRE(xyz[j], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
+    SICP_REQUIRE(n[j] >= 1 && (!(role[(size_t)j] & 1) || n[j] >= rp->neighbors), SICP_ERR_BAD_ARG,
+                 "every fixed cloud needs at least `neighbors` points, every movable cloud one");
+    SICP_REQUIRE(n[j] < k32 - total, SICP_ERR_BAD_ARG, "the points of the referenced clouds must be below 2^32");
+    off[(size_t)j] = total;
+    total += n[j];
+    ref.push_back(j);
+  }
+  PairsRun r;
+  begin_pairs(r, n_pairs, rp, observed);
+  std::vector<long long> fo((size_t)n_pairs + 1, 0);  // the pairs' flag offsets
+  std::vector<char> seen((size_t)n_clouds, 0);
+  long long Kmax = 0, max_n_fix = 0;
+  for (int i = 0; i < n_pairs; ++i) {
+    const long long nf = n[fix_id[i]];
+    add_movable(r, i, n[mov_id[i]]);  // mov_neighbors <= the movable cloud's points
+    fo[(size_t)i + 1] = fo[(size_t)i] + nf;
+    SICP_REQUIRE(fo[(size_t)i + 1] < k32, SICP_ERR_BAD_ARG,
+                 "the fixed points of all pairs must be below 2^32 (32-bit overlap flags and offsets)");
+    Kmax = std::max<long long>(Kmax, std::min<long long>(rp->correspondences, nf));
+    max_n_fix = std::max(max_n_fix, nf);
+    if (!seen[(size_t)mov_id[i]]) {
+      seen[(size_t)mov_id[i]] = 1;
+      r.mov_first.push_back(i);
+    }
+  }
+  if (!c.batch) c.batch = new Batch();
+  Batch& b = *c.batch;
+  r.Kmax = (Kmax + 1) & ~1ll;  // even, as in register_batch
+  b.total_fix = fo[(size_t)n_pairs];
+  b.total_mov = total;
+
+  // ---- each referenced cloud crosses PCIe once, on the context's stream, into the store
+  b.mov_xyz.reserve(3 * (size_t)total);
+  {
+    StageTimer t(c, &c.tm.upload_ms);
+    for (int j : ref)
+      upload_to_device(c, b.mov_xyz.p + 3 * off[(size_t)j], xyz[j], sizeof(double) * 3 * (size_t)n[j]);
+    t.stop();
+  }
+  alloc_pair_buffers(c, b, r);
+
+  // ---- one grid per referenced cloud, for both roles
+  std::vector<HostCloud> clouds;
+  std::vector<int> slot((size_t)n_clouds, -1);
+  for (int j : ref) {
+    slot[(size_t)j] = (int)clouds.size();
+    clouds.push_back(HostCloud{b.mov_xyz.p + 3 * off[(size_t)j], n[j], off[(size_t)j]});
+  }
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  {
+    StageTimer t(c, &c.tm.grid_fix_ms);
+    grid_build(c, b.gfix, clouds, batch_policy(c), views, centres);
+    t.stop();
+  }
+  c.tm.grid_mov_ms = 0;
+  for (int i = 0; i < n_pairs; ++i) {
+    PairDev& d = r.pd[(size_t)i];
+    const int f = slot[(size_t)fix_id[i]], m = slot[(size_t)mov_id[i]];
+    d.gfix = views[(size_t)f];
+    d.n_fix = n[fix_id[i]];
+    d.fix_off = off[(size_t)fix_id[i]];
+    d.flag_off = fo[(size_t)i];
+    d.gmov = views[(size_t)m];
+    d.mov_off = off[(size_t)mov_id[i]];
+    for (int a = 0; a < 3; ++a) d.cm[a] = centres[(size_t)m * 3 + a];
+  }
+  r.mov_built = true;
+  run_pairs(c, b, r, b.mov_xyz.p, nullptr, max_n_fix, out, n_selected);
 }
 
 // The clouds of sicp_map_insert and sicp_map_distances, checked before any device work: their
@@ -1107,6 +1240,13 @@ extern "C" int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const do
                                         const int64_t* n_mov, const sicp_register_params* p,
                                         const double* observed, sicp_pair_result* out, int64_t* n_selected) {
   SICP_BATCH_API(register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected))
+}
+
+extern "C" int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                       int32_t n_pairs, const int32_t* fix_id, const int32_t* mov_id,
+                                       const sicp_register_params* p, const double* observed, sicp_pair_result* out,
+                                       int64_t* n_selected) {
+  SICP_BATCH_API(register_pairs(c, n_clouds, xyz, n, n_pairs, fix_id, mov_id, p, observed, out, n_selected))
 }
 
 extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

@@ -200,7 +200,10 @@ inline float4* mov_attr_eff(Ctx& c) {
 struct PairDev {
   GridView gmov, gfix;
   long long n_fix, n_mov;
-  long long fix_off, mov_off;  // first point of this pair in the concatenated clouds
+  long long fix_off, mov_off;  // first point of this pair's clouds in the concatenated clouds
+  // first overlap keep flag of this pair (Batch::ovl_flag, one per fixed point of the pair): fix_off
+  // when every pair owns its fixed cloud; pairs that share one (sicp_register_pairs) get their own
+  long long flag_off;
   long long K;                 // selected fixed points (<= Kmax)
   long long q_off;             // first entry of this pair in the per-query arrays
   double cm[3];                // centre of the movable grid's box (moment centring)
@@ -211,10 +214,19 @@ struct PairDev {
 
 struct Batch {
   int n_pairs = 0;
-  long long Kmax = 0, total_fix = 0, total_mov = 0, max_n_mov = 0;  // max_n_mov: the largest movable cloud
-  DevBuf<double> fix_xyz, mov_xyz;  // concatenated clouds
+  // total_fix: the fixed points of all pairs (overlap flags); total_mov: the points of mov_xyz;
+  // max_n_mov: the largest movable cloud
+  long long Kmax = 0, total_fix = 0, total_mov = 0, max_n_mov = 0;
+  // concatenated clouds; sicp_register_pairs keeps every referenced cloud once in mov_xyz, which
+  // serves as both sides, and grids it once in gfix
+  DevBuf<double> fix_xyz, mov_xyz;
   GridBufs gfix, gmov;
   DevBuf<PairDev> pairs;
+  // the movable-normals estimate runs over n_mov_desc descriptors: the pairs' own (mov_desc =
+  // pairs), or with shared clouds one per distinct movable cloud (mov_desc = mov_pairs)
+  DevBuf<PairDev> mov_pairs;
+  const PairDev* mov_desc = nullptr;
+  int n_mov_desc = 0;
   // per-query arrays, n_pairs x Kmax
   DevBuf<long long> sel_idx, nn_idx;
   DevBuf<double> q_xyz, dist, m_xyz;
@@ -229,10 +241,11 @@ struct Batch {
   int bin_cap = 0;
   DevBuf<uint32_t> nn_pos;
   DevBuf<uint8_t> keep;
-  // overlap filter, one entry per fixed point of the batch: keep flag, its exclusive prefix sum
-  // (total_fix + 1), the in-cloud indices of the survivors in ascending order per pair
+  // overlap filter, one entry per fixed point of each pair (at PairDev::flag_off): keep flag, its
+  // exclusive prefix sum (total_fix + 1), the in-cloud indices of the survivors in ascending order
+  // per pair
   DevBuf<uint32_t> ovl_flag, ovl_scan, ovl_list, ovl_sums;
-  DevBuf<uint32_t> ovl_bounds;  // n_pairs + 1 prefix values at the pair offsets
+  DevBuf<uint32_t> ovl_bounds;  // n_pairs + 1 prefix values at the pairs' flag offsets
   // per-pair state
   DevBuf<DevState> state;
   DevBuf<unsigned int> lin_hist;       // n_pairs x (LH_BINS + 2)
@@ -246,16 +259,18 @@ struct Batch {
   size_t flags_cap = 0, results_cap = 0;
   unsigned long long* ovl_host = nullptr;    // pinned: what the overlap filters read back
   size_t ovl_host_cap = 0;
-  // What sicp_get_batch_outputs reads of the last sicp_register_batch / sicp_register_to_map.
-  // out_valid is cleared on entry of those two calls and of sicp_set_map, and set only when one of
-  // the two returns successfully; the vectors are per pair of that call.
+  // What sicp_get_batch_outputs reads of the last sicp_register_batch / sicp_register_to_map /
+  // sicp_register_pairs.  out_valid is cleared on entry of those calls and of the calls that
+  // replace the map, and set only when one of the three returns successfully; the vectors are per
+  // pair of that call.
   bool out_valid = false;
   int out_n_pairs = 0, out_max_iterations = 0;
-  std::vector<long long> out_mo, out_n_kept;  // movable point offsets (n_pairs + 1), kept residuals
+  std::vector<long long> out_n_mov, out_n_kept;  // movable points, kept residuals
   std::vector<int> out_status, out_iterations; // sicp_status (SICP_ERR_NO_OVERLAP included), iterations run
   std::vector<double> out_mean_std;            // exact mean / std of the final residuals, 2 per pair
-  // buffers of sicp_get_batch_outputs: transformed clouds (total_mov points, the offsets of
-  // mov_xyz), compacted residuals, the ids and residual offsets of the requested pairs
+  // buffers of sicp_get_batch_outputs: transformed clouds and compacted residuals of the requested
+  // pairs, each pair at its own output offset (pairs may share a movable cloud), the ids and the
+  // output offsets of the requested pairs
   DevBuf<double> xyz_out, resid_out;
   DevBuf<int> out_ids;
   DevBuf<long long> out_off;
@@ -396,9 +411,10 @@ void gather_queries_launch(Ctx& c);
 // fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::fix_xyz or MapStore::xyz)
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
-// PointCloud.select_in_range of every fixed point of the batch under its pair's DevState
-// transform: Batch::ovl_flag[i] = (squared distance to the nearest movable point < r2)
-void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2);
+// PointCloud.select_in_range of every fixed point of every pair under its pair's DevState
+// transform: Batch::ovl_flag[flag_off + i] = (squared distance of fix_xyz[fix_off + i] to the
+// nearest movable point < r2)
+void batch_overlap_launch(Ctx& c, Batch& b, const double* fix_xyz, long long max_n_fix, double r2);
 // Culled overlap filter of sicp_register_to_map: for every scan, the map points inside its
 // MapCull box get the bounded search of batch_overlap_launch (same device code, same flag);
 // survivors set bit i of the scan's row of MapStore::bits (cleared by the caller).
@@ -433,9 +449,10 @@ void map_normals_launch(Ctx& c, const GridView& map, const double* q_xyz, long l
 void batch_rs_launch(Ctx& c, Batch& b, const sicp_run_params& p, int it, bool want_sigma);
 void batch_finish_launch(Ctx& c, Batch& b, int max_iterations);
 // sicp_get_batch_outputs, for the n_ids pairs ids (device) of the last batched run: the movable
-// clouds moved by DevState::T into out at their Batch::mov_xyz offsets, and the final residuals
-// in kept order into out + off[j] (device)
-void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, long long max_n_mov, double* out);
+// clouds moved by DevState::T into out + 3 off[j], and the final residuals in kept order into
+// out + off[j] (off device)
+void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const long long* off, long long max_n_mov,
+                            double* out);
 void batch_residuals_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const long long* off, double* out);
 
 int bin_cap_for(long long K);

@@ -748,7 +748,7 @@ __global__ void __maxnreg__(128) k_match_batch_attr(BatchMatchAttrArgs m) {
 // Overlap filter of a batch (PointCloud.select_in_range, simpleicp.py:158-170): blockIdx.y is the
 // pair, the queries are ALL its fixed points, read in place from the concatenated clouds, and the
 // transform is the pair's DevState (its prior).  Bounded search with unlimited rings, one keep
-// flag per fixed point of the batch.
+// flag per fixed point of each pair, at the pair's own flag offset (pairs may share a fixed cloud).
 template <int MG>
 __global__ void __launch_bounds__(128)
     k_overlap_batch(const PairDev* __restrict__ pairs, const DevState* __restrict__ state,
@@ -757,10 +757,9 @@ __global__ void __launch_bounds__(128)
   const long long n = pd.n_fix;
   const long long gt = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (gt / MG >= n) return;
-  const long long f = pd.fix_off;
   const CorrOut co{nullptr, 0, nullptr, nullptr, 0, 0, nullptr, nullptr, -1.0};
-  match_coop_body<MG, true>(pd.gmov, state + blockIdx.y, fix_xyz + 3 * f, nullptr, nullptr, n, 1 << 30, 0,
-                            nullptr, nullptr, nullptr, nullptr, r2, co, gt, keep + f);
+  match_coop_body<MG, true>(pd.gmov, state + blockIdx.y, fix_xyz + 3 * pd.fix_off, nullptr, nullptr, n, 1 << 30, 0,
+                            nullptr, nullptr, nullptr, nullptr, r2, co, gt, keep + pd.flag_off);
 }
 
 // Culled overlap filter of sicp_register_to_map: blockIdx.y is the scan, blockIdx.x one x-row of
@@ -1368,12 +1367,12 @@ void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool wi
   c.tm.kernel_launches += 1;
 }
 
-void batch_overlap_launch(Ctx& c, Batch& b, long long max_n_fix, double r2) {
+void batch_overlap_launch(Ctx& c, Batch& b, const double* fix_xyz, long long max_n_fix, double r2) {
   const int mg = match_lanes(c, b.total_fix, 4);
   const dim3 grid((unsigned)((max_n_fix * mg + 127) / 128), b.n_pairs);
   with_lanes<4, 8, 16>(mg, [&](auto L) {
     k_overlap_batch<decltype(L)::value>
-        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, b.fix_xyz.p, r2, b.ovl_flag.p);
+        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, fix_xyz, r2, b.ovl_flag.p);
   });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;

@@ -425,11 +425,11 @@ __device__ __forceinline__ void knn_reg_body(const GridView& g, const double* __
 enum class Src {
   One,      // one grid g: q_xyz[n] -> out[n], pos n x k, knn_idx / knn_d2 of option "keep_knn"
   PairFix,  // blockIdx.y = pair: its K selected fixed points at q_off, in its fixed grid
-  PairMov,  // blockIdx.y = pair: its movable points [q0, q0 + n), in its own movable grid
+  PairMov,  // blockIdx.y = movable cloud: its points [q0, q0 + n), in its own grid
 };
 struct KnnQueries {
   GridView g;            // One
-  const PairDev* pairs;  // PairFix, PairMov
+  const PairDev* pairs;  // PairFix: Batch::pairs; PairMov: Batch::mov_desc
   const double* q_xyz;   // One: the queries; PairFix: Batch::q_xyz; PairMov: Batch::mov_xyz
   float4* out;           // One: n entries; PairFix: Batch::q_nrm; PairMov: Batch::mov_nrm
   long long n;           // One: the queries; PairFix, PairMov: pos rows per pair
@@ -572,11 +572,14 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
     knn_pca_launch<Src::PairFix>(c, a, b->Kmax, b->n_pairs, b->Kmax * b->n_pairs);
     return;
   }
-  // every pair's chunk of queries in one launch; the neighbour positions of a launch
-  // (n_pairs x cq x k x 4 bytes) stay within option "normals_scratch_mb"
+  // every movable cloud's chunk of queries in one launch (one descriptor per cloud, Batch::mov_desc);
+  // the neighbour positions of a launch (n_mov_desc x cq x k x 4 bytes) stay within option
+  // "normals_scratch_mb"
+  const int n_desc = b->n_mov_desc;
+  a.pairs = b->mov_desc;
   const long long cq =
-      std::min<long long>(b->max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / b->n_pairs));
-  b->knn_pos.reserve((size_t)b->n_pairs * cq * k);
+      std::min<long long>(b->max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / n_desc));
+  b->knn_pos.reserve((size_t)n_desc * cq * k);
   b->mov_nrm.reserve(std::max<long long>(b->total_mov, 1));
   a.q_xyz = b->mov_xyz.p;
   a.out = b->mov_nrm.p;
@@ -584,7 +587,7 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
   a.pos = b->knn_pos.p;
   for (long long q0 = 0; q0 < b->max_n_mov; q0 += cq) {
     a.q0 = q0;
-    knn_pca_launch<Src::PairMov>(c, a, cq, b->n_pairs, b->total_mov);
+    knn_pca_launch<Src::PairMov>(c, a, cq, n_desc, b->total_mov);
   }
 }
 

@@ -33,28 +33,31 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// sicp_get_batch_outputs: the movable cloud of pair ids[blockIdx.y] moved by its applied transform
-// DevState::T, into the same point offsets of out.  A pair's slice starts at an arbitrary point
-// offset (16-byte aligned only when it is even), so every access is a scalar double.
+// sicp_get_batch_outputs: the movable cloud of pair ids[blockIdx.y] (read at its offset mov_off)
+// moved by its applied transform DevState::T, into out from point off[blockIdx.y] on.  Pairs that
+// share a movable cloud read the same points and write their own slices.  A slice starts at an
+// arbitrary point offset (16-byte aligned only when it is even), so every access is a scalar double.
 __global__ void __launch_bounds__(256)
     k_transform_pairs(const PairDev* __restrict__ pairs, const DevState* __restrict__ state,
-                      const int* __restrict__ ids, const double* __restrict__ in, double* __restrict__ out) {
+                      const int* __restrict__ ids, const long long* __restrict__ off, const double* __restrict__ in,
+                      double* __restrict__ out) {
   const int pair = ids[blockIdx.y];
   const long long n = pairs[pair].n_mov, i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const long long p = 3 * (pairs[pair].mov_off + i);
+  const long long p = 3 * (pairs[pair].mov_off + i), o = 3 * (off[blockIdx.y] + i);
   double x, y, z;
   rigid_apply(state[pair].T, __ldg(in + p + 0), __ldg(in + p + 1), __ldg(in + p + 2), x, y, z);
-  out[p + 0] = x;
-  out[p + 1] = y;
-  out[p + 2] = z;
+  out[o + 0] = x;
+  out[o + 1] = y;
+  out[o + 2] = z;
 }
 
 }  // namespace
 
-void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, long long max_n_mov, double* out) {
+void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const long long* off, long long max_n_mov,
+                            double* out) {
   const long long blocks = std::max<long long>((max_n_mov + 255) / 256, 1);
-  k_transform_pairs<<<dim3((unsigned)blocks, (unsigned)n_ids), 256, 0, c.stream>>>(b.pairs.p, b.state.p, ids,
+  k_transform_pairs<<<dim3((unsigned)blocks, (unsigned)n_ids), 256, 0, c.stream>>>(b.pairs.p, b.state.p, ids, off,
                                                                                  b.mov_xyz.p, out);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;

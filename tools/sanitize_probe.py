@@ -54,6 +54,15 @@ ov = [(p[0][p[0][:, 0] < 20], p[1][p[1][:, 0] > 10]) for p in pairs] + [(pairs[0
 tab_o = sb.simpleicp_batch(ov, engine="batched", correspondences=500, max_overlap_distance=0.5,
                            rbp_observed_values=np.zeros((len(ov), 6)), on_error="nan")
 assert np.isfinite(tab_o[:-1]).all() and tab_o[-1, 16] == -_capi.SICP_ERR_NO_OVERLAP
+# pairs drawn from shared clouds: a self pair, a cloud in both roles, an unreferenced NULL cloud,
+# with the overlap filter and movable normals on (every shared-write hazard of the batch reached)
+with _capi.Engine() as e:
+    prm = e.run_params(0.3, 1.0, 20, e.lsq_params(np.zeros(6), np.zeros(6), np.zeros(6), 1.0))
+    sh = [pairs[0][0], None, pairs[0][1], pairs[1][1]]
+    rs = e.register_pairs(sh, [[0, 0], [0, 2], [2, 3], [3, 0], [2, 0]], 500, 10, prm, max_overlap_distance=0.5,
+                          mov_neighbors=10)
+    outs = e.batch_outputs(rs)
+    assert rs[1].status == 0 and outs[1] is not None
 # map insert: with H (a NaN point, an empty cloud, a cloud at an odd point offset), without H, and
 # one that adds nothing
 with sb.Map(X_fix[:30_000]) as mp:
