@@ -52,27 +52,6 @@ __global__ void k_gather_flags(const DevState* __restrict__ st, int n, int* __re
   flags[2 * i + 1] = st[i].iterations_done;
 }
 
-// Ordered compaction of the overlap filter: with S the exclusive prefix sum of the keep flags of
-// all pairs' fixed points and fo[i] pair i's flag offset, pair i's survivors are the slice
-// [S[fo[i]], S[fo[i+1]]) of the list, in ascending point order; each holds its index inside its
-// own cloud.
-__global__ void __launch_bounds__(256)
-    k_overlap_scatter(const PairDev* __restrict__ pairs, const uint32_t* __restrict__ keep,
-                      const uint32_t* __restrict__ scan, uint32_t* __restrict__ list) {
-  const PairDev& pd = pairs[blockIdx.y];
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= pd.n_fix) return;
-  const long long g = pd.flag_off + i;
-  if (keep[g]) list[scan[g]] = (uint32_t)i;
-}
-
-// bounds[i] = S[fo[i]] for every pair, bounds[n_pairs] = S[total]: the only values the host reads
-__global__ void k_overlap_bounds(const PairDev* __restrict__ pairs, int n_pairs, const uint32_t* __restrict__ scan,
-                                 long long total, uint32_t* __restrict__ bounds) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i <= n_pairs) bounds[i] = scan[i < n_pairs ? pairs[i].flag_off : total];
-}
-
 // sicp_map_insert, one thread per point j of the concatenated clouds (cloud i owns [off[i],
 // off[i + 1])): the point moved by its cloud's transform when there are transforms (T != NULL;
 // rigid_apply as k_transform, in place, scalar accesses since clouds start at any point offset),
@@ -97,31 +76,6 @@ __global__ void __launch_bounds__(256)
     xyz[3 * j + 2] = z = oz;
   }
   fin[j] = (isfinite(x) && isfinite(y) && isfinite(z)) ? 1u : 0u;
-}
-
-// the finite points in ascending j (scan = exclusive prefix sum of fin) with their j
-__global__ void __launch_bounds__(256)
-    k_insert_compact(const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ fin,
-                     const uint32_t* __restrict__ scan, double* __restrict__ fin_xyz, uint32_t* __restrict__ fin_idx) {
-  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (j >= n || !fin[j]) return;
-  const long long f = scan[j];
-  fin_xyz[3 * f + 0] = xyz[3 * j + 0];
-  fin_xyz[3 * f + 1] = xyz[3 * j + 1];
-  fin_xyz[3 * f + 2] = xyz[3 * j + 2];
-  fin_idx[f] = (uint32_t)j;
-}
-
-// the added points in ascending j, written after the map's points (out = the new map + 3 n_map)
-__global__ void __launch_bounds__(256)
-    k_insert_scatter(const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ flag,
-                     const uint32_t* __restrict__ scan, double* __restrict__ out) {
-  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (j >= n || !flag[j]) return;
-  const long long o = scan[j];
-  out[3 * o + 0] = xyz[3 * j + 0];
-  out[3 * o + 1] = xyz[3 * j + 1];
-  out[3 * o + 2] = xyz[3 * j + 2];
 }
 
 // sicp_map_crop, one thread per map point j: keep[j] = 1 iff d2 < r2 for at least one of the n_c
@@ -157,27 +111,6 @@ __global__ void __launch_bounds__(256)
     }
   }
   if (j < n) keep[j] = hit ? 1u : 0u;
-}
-
-// bounds[i] = S[off[i]] for i <= n_clouds (off[n_clouds] = n, S[n] = the total): cloud i added
-// bounds[i + 1] - bounds[i] points
-__global__ void k_insert_bounds(const uint32_t* __restrict__ off, int n_clouds, const uint32_t* __restrict__ scan,
-                                uint32_t* __restrict__ bounds) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i <= n_clouds) bounds[i] = scan[off[i]];
-}
-
-// sicp_map_distances, one thread per point j: the coordinates of its matched map point, at its
-// place among the within points (scan = exclusive prefix sum of the within flags)
-__global__ void __launch_bounds__(256)
-    k_dist_gather(const double* __restrict__ map_xyz, const long long* __restrict__ idx, long long n,
-                  const uint32_t* __restrict__ within, const uint32_t* __restrict__ scan, double* __restrict__ m_xyz) {
-  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (j >= n || !within[j]) return;
-  const long long f = scan[j], m = idx[j];
-  m_xyz[3 * f + 0] = map_xyz[3 * m + 0];
-  m_xyz[3 * f + 1] = map_xyz[3 * m + 1];
-  m_xyz[3 * f + 2] = map_xyz[3 * m + 2];
 }
 
 // the signed distance of point j along its matched map point's normal, plane_distance's expression
@@ -346,28 +279,20 @@ void take_survivors(Ctx& c, Batch& b, PairsRun& r, const uint32_t* bounds) {
 
 // Overlap filter of sicp_register_batch and sicp_register_pairs: bounded search of every fixed
 // point of every pair (coordinates in fix_xyz), one exclusive scan over the keep flags of the whole
-// batch, ordered scatter, and ONE read-back of the pair boundaries.
+// batch, ordered scatter of the flag positions, and ONE read-back of the pair boundaries.
 void batch_filter(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, long long max_n_fix) {
-  cudaStream_t st = c.stream;
-  const int n_pairs = r.n_pairs;
+  CompactScratch& s = c.compact;
   const long long nf = b.total_fix;
-  b.ovl_flag.reserve(nf);
-  b.ovl_scan.reserve(nf + 1);
+  s.flag.reserve(nf);
+  s.scan.reserve(nf + 1);
   b.ovl_list.reserve(std::max<long long>(nf, 1));
-  b.ovl_bounds.reserve((size_t)n_pairs + 1);
   // r2 as sicp_register computes it
   batch_overlap_launch(c, b, fix_xyz, max_n_fix, r.rp->max_overlap_distance * r.rp->max_overlap_distance);
-  scan_u32(c, b.ovl_flag.p, nf, b.ovl_scan.p, b.ovl_sums);
-  k_overlap_scatter<<<dim3((unsigned)((max_n_fix + 255) / 256), n_pairs), 256, 0, st>>>(b.pairs.p, b.ovl_flag.p,
-                                                                                     b.ovl_scan.p, b.ovl_list.p);
-  k_overlap_bounds<<<(n_pairs + 256) / 256, 256, 0, st>>>(b.pairs.p, n_pairs, b.ovl_scan.p, nf, b.ovl_bounds.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 2;
-  pinned_reserve(b.ovl_host, b.ovl_host_cap, (size_t)n_pairs + 1);
-  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.ovl_host);
-  SICP_CUDA(cudaMemcpyAsync(bounds, b.ovl_bounds.p, sizeof(uint32_t) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
-  SICP_CUDA(cudaStreamSynchronize(st));
-  take_survivors(c, b, r, bounds);
+  scan_u32(c, s.flag.p, nf, s.scan.p, s.sums);
+  compact_scatter(c, s.flag.p, nf, s.scan.p, b.ovl_list.p, nullptr, nullptr, nullptr);
+  std::vector<long long> fo((size_t)r.n_pairs + 1, nf);
+  for (int i = 0; i < r.n_pairs; ++i) fo[(size_t)i] = r.pd[(size_t)i].flag_off;
+  take_survivors(c, b, r, compact_bounds(c, s.scan.p, fo));
 }
 
 }  // namespace
@@ -440,28 +365,29 @@ static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
     hint += (long long)(cu[(size_t)i].rows * (cu[(size_t)i].c1[0] - cu[(size_t)i].c0[0] + 1) * c.grid_target_occ);
   }
   const long long words = (m.n + 31) / 32, nw = words * n;
+  CompactScratch& s = c.compact;
   m.culls.reserve(n);
   m.bits.reserve(nw);
-  m.popc.reserve(nw);
-  m.popc_scan.reserve(nw + 1);
+  s.flag.reserve(nw);
+  s.scan.reserve(nw + 1);
   m.n_searched.reserve(1);
   SICP_CUDA(cudaMemcpyAsync(m.culls.p, cu.data(), sizeof(MapCull) * (size_t)n, cudaMemcpyHostToDevice, st));
   SICP_CUDA(cudaMemsetAsync(m.bits.p, 0, sizeof(uint32_t) * (size_t)nw, st));
   SICP_CUDA(cudaMemsetAsync(m.n_searched.p, 0, sizeof(unsigned long long), st));
   if (max_rows > 0) map_overlap_launch(c, b, m, m.culls.p, max_rows, rr * rr, hint);  // r2 as sicp_register computes it
-  map_bits_popc_launch(c, m.bits.p, nw, m.popc.p);
-  scan_u32(c, m.popc.p, nw, m.popc_scan.p, m.sums);
+  map_bits_popc_launch(c, m.bits.p, nw, s.flag.p);
+  scan_u32(c, s.flag.p, nw, s.scan.p, s.sums);
   // n + 1 boundaries, then the count
-  pinned_reserve(b.ovl_host, b.ovl_host_cap, (size_t)n + 2);
-  uint32_t* bounds = reinterpret_cast<uint32_t*>(b.ovl_host);
-  unsigned long long* searched = b.ovl_host + n + 1;
-  SICP_CUDA(cudaMemcpy2DAsync(bounds, sizeof(uint32_t), m.popc_scan.p, sizeof(uint32_t) * (size_t)words,
+  pinned_reserve(s.host, s.host_cap, (size_t)n + 1);
+  uint32_t* bounds = s.host;
+  unsigned long long* searched = reinterpret_cast<unsigned long long*>(c.scal_host);
+  SICP_CUDA(cudaMemcpy2DAsync(bounds, sizeof(uint32_t), s.scan.p, sizeof(uint32_t) * (size_t)words,
                               sizeof(uint32_t), (size_t)n + 1, cudaMemcpyDeviceToHost, st));
   SICP_CUDA(cudaMemcpyAsync(searched, m.n_searched.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   SICP_CUDA(cudaStreamSynchronize(st));
   c.tm.overlap_candidates = (int64_t)*searched;
   b.ovl_list.reserve(std::max<long long>(bounds[n], 1));
-  map_bits_scatter_launch(c, m.bits.p, nw, words, m.popc_scan.p, b.ovl_list.p);
+  map_bits_scatter_launch(c, m.bits.p, nw, words, s.scan.p, b.ovl_list.p);
   take_survivors(c, b, r, bounds);
 }
 
@@ -937,7 +863,8 @@ static std::vector<long long> check_clouds(int n_clouds, const double* const* xy
 }
 
 // The clouds uploaded into MapStore::ins_xyz (off from check_clouds, nt = off[n_clouds] > 0 points)
-// and moved there by k_insert_stage, which also writes fin_flag.
+// and moved there by k_insert_stage, which also writes the finite flags into Ctx::compact.flag
+// (its scan is reserved too: the compactions of both callers take nt flags).
 static void stage_clouds(Ctx& c, MapStore& m, int n_clouds, const double* const* xyz, const int64_t* n,
                          const double* H, const std::vector<long long>& off) {
   cudaStream_t st = c.stream;
@@ -956,8 +883,10 @@ static void stage_clouds(Ctx& c, MapStore& m, int n_clouds, const double* const*
     SICP_CUDA(cudaMemcpyAsync(m.ins_T.p, hT.data(), sizeof(Rigid) * hT.size(), cudaMemcpyHostToDevice, st));
     T = m.ins_T.p;
   }
-  m.fin_flag.reserve((size_t)nt);
-  k_insert_stage<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T, m.fin_flag.p);
+  c.compact.flag.reserve((size_t)nt);
+  c.compact.scan.reserve((size_t)nt + 1);
+  k_insert_stage<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_off.p, n_clouds, T,
+                                                               c.compact.flag.p);
   c.tm.kernel_launches += 1;
 }
 
@@ -1002,49 +931,33 @@ static void map_insert(Ctx& c, int n_clouds, const double* const* xyz, const int
 
   // ---- stage and move the clouds, flag and compact their finite points
   stage_clouds(c, m, n_clouds, xyz, n, H, off);
-  const unsigned blocks = (unsigned)((nt + 255) / 256);
-  m.fin_scan.reserve((size_t)nt + 1);
-  scan_u32(c, m.fin_flag.p, nt, m.fin_scan.p, m.sums);
-  pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
-  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.fin_scan.p + nt, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  SICP_CUDA(cudaStreamSynchronize(st));
-  const long long n_fin = m.bounds_host[0];
+  CompactScratch& s = c.compact;
+  scan_u32(c, s.flag.p, nt, s.scan.p, s.sums);
+  const long long n_fin = compact_bounds(c, s.scan.p, {nt})[0];
   if (n_fin == 0) return;  // nothing finite, nothing added
   m.fin_xyz.reserve(3 * (size_t)n_fin);
   m.fin_idx.reserve((size_t)n_fin);
-  k_insert_compact<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.fin_flag.p, m.fin_scan.p, m.fin_xyz.p, m.fin_idx.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 1;
+  compact_scatter(c, s.flag.p, nt, s.scan.p, m.fin_idx.p, m.ins_xyz.p, nullptr, m.fin_xyz.p);
 
   // ---- the points to add, and how many per cloud (one read-back)
   std::vector<GridView> views;
   std::vector<double> centres;
   grid_build(c, m.gnew, {HostCloud{m.fin_xyz.p, n_fin, 0}}, batch_policy(c), views, centres);
-  m.ins_flag.reserve((size_t)nt);
-  m.ins_scan.reserve((size_t)nt + 1);
-  SICP_CUDA(cudaMemsetAsync(m.ins_flag.p, 0, sizeof(uint32_t) * (size_t)nt, st));
-  map_insert_flags_launch(c, m.view, views[0], m.fin_xyz.p, m.fin_idx.p, n_fin, voxel, m.ins_flag.p);
-  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums);
-  m.ins_bounds.reserve((size_t)n_clouds + 1);
-  k_insert_bounds<<<(n_clouds + 256) / 256, 256, 0, st>>>(m.ins_off.p, n_clouds, m.ins_scan.p, m.ins_bounds.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 1;
-  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_bounds.p, sizeof(uint32_t) * ((size_t)n_clouds + 1),
-                            cudaMemcpyDeviceToHost, st));
-  SICP_CUDA(cudaStreamSynchronize(st));
-  const long long added = m.bounds_host[n_clouds];
+  SICP_CUDA(cudaMemsetAsync(s.flag.p, 0, sizeof(uint32_t) * (size_t)nt, st));
+  map_insert_flags_launch(c, m.view, views[0], m.fin_xyz.p, m.fin_idx.p, n_fin, voxel, s.flag.p);
+  scan_u32(c, s.flag.p, nt, s.scan.p, s.sums);
+  const uint32_t* bounds = compact_bounds(c, s.scan.p, off);
+  const long long added = bounds[n_clouds];
   if (added > 0) {
     // ---- the grown map in fresh buffers, then swapped in (DevBuf::reserve drops what it held)
     const long long n_new = m.n + added;
     m.xyz_next.reserve(3 * (size_t)n_new);
     SICP_CUDA(cudaMemcpyAsync(m.xyz_next.p, m.xyz.p, sizeof(double) * 3 * (size_t)m.n, cudaMemcpyDeviceToDevice, st));
-    k_insert_scatter<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p + 3 * m.n);
-    SICP_CUDA(cudaGetLastError());
-    c.tm.kernel_launches += 1;
+    compact_scatter(c, s.flag.p, nt, s.scan.p, nullptr, m.ins_xyz.p, nullptr, m.xyz_next.p + 3 * m.n);
     swap_in_next_map(c, m, n_new);
   }
   if (n_added)
-    for (int i = 0; i < n_clouds; ++i) n_added[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];
+    for (int i = 0; i < n_clouds; ++i) n_added[i] = (int64_t)bounds[i + 1] - (int64_t)bounds[i];
 }
 
 static void get_map(Ctx& c, double* xyz, int64_t cap, int64_t* n) {
@@ -1059,26 +972,21 @@ static void get_map(Ctx& c, double* xyz, int64_t cap, int64_t* n) {
   }
 }
 
-// The end of sicp_map_crop and sicp_map_thin: the map points whose keep flag (MapStore::ins_flag,
+// The end of sicp_map_crop and sicp_map_thin: the map points whose keep flag (Ctx::compact.flag,
 // one per map point) is set become the new map, in map order.  One scan and one read-back of the
 // kept count; when every point is kept nothing else happens (the map and its grid stay as they
-// are); otherwise k_insert_scatter writes the kept points into xyz_next and swap_in_next_map makes
-// them the map.  A map is never empty: keeping no point is SICP_ERR_NO_OVERLAP with the map
-// unchanged.  Returns the points removed.
+// are); otherwise the kept points are compacted into xyz_next and swap_in_next_map makes them the
+// map.  A map is never empty: keeping no point is SICP_ERR_NO_OVERLAP with the map unchanged.
+// Returns the points removed.
 static long long keep_flagged(Ctx& c, MapStore& m) {
-  cudaStream_t st = c.stream;
+  CompactScratch& s = c.compact;
   const long long n = m.n;
-  scan_u32(c, m.ins_flag.p, n, m.ins_scan.p, m.sums);
-  pinned_reserve(m.bounds_host, m.bounds_cap, 1);
-  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_scan.p + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  SICP_CUDA(cudaStreamSynchronize(st));
-  const long long kept = m.bounds_host[0];
+  scan_u32(c, s.flag.p, n, s.scan.p, s.sums);
+  const long long kept = compact_bounds(c, s.scan.p, {n})[0];
   SICP_REQUIRE(kept > 0, SICP_ERR_NO_OVERLAP, "no map point would be kept (a map is never empty): the map is unchanged");
   if (kept == n) return 0;
   m.xyz_next.reserve(3 * (size_t)kept);
-  k_insert_scatter<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(m.xyz.p, n, m.ins_flag.p, m.ins_scan.p, m.xyz_next.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 1;
+  compact_scatter(c, s.flag.p, n, s.scan.p, nullptr, m.xyz.p, nullptr, m.xyz_next.p);
   swap_in_next_map(c, m, kept);
   return n - kept;
 }
@@ -1097,11 +1005,11 @@ static void map_crop(Ctx& c, int n_centers, const double* centers, double radius
   cudaStream_t st = c.stream;
   m.crop_c.reserve(3 * (size_t)n_centers);
   SICP_CUDA(cudaMemcpyAsync(m.crop_c.p, centers, sizeof(double) * 3 * (size_t)n_centers, cudaMemcpyHostToDevice, st));
-  m.ins_flag.reserve((size_t)m.n);
-  m.ins_scan.reserve((size_t)m.n + 1);
+  c.compact.flag.reserve((size_t)m.n);
+  c.compact.scan.reserve((size_t)m.n + 1);
   // r2 = fl(radius^2), as sicp_select_in_range and sicp_map_distances compute it
   k_map_crop_flags<<<(unsigned)((m.n + 255) / 256), 256, 0, st>>>(m.xyz.p, m.n, m.crop_c.p, n_centers,
-                                                                  radius * radius, m.ins_flag.p);
+                                                                  radius * radius, c.compact.flag.p);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
   const long long removed = keep_flagged(c, m);
@@ -1115,9 +1023,9 @@ static void map_thin(Ctx& c, double voxel, int64_t* n_removed) {
   SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
   MapStore& m = *c.map;
   if (n_removed) *n_removed = 0;
-  m.ins_flag.reserve((size_t)m.n);
-  m.ins_scan.reserve((size_t)m.n + 1);
-  map_thin_flags_launch(c, m.view, m.xyz.p, m.n, voxel, m.ins_flag.p);
+  c.compact.flag.reserve((size_t)m.n);
+  c.compact.scan.reserve((size_t)m.n + 1);
+  map_thin_flags_launch(c, m.view, m.xyz.p, m.n, voxel, c.compact.flag.p);
   const long long removed = keep_flagged(c, m);
   if (n_removed) *n_removed = removed;
 }
@@ -1151,21 +1059,13 @@ static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const 
 
   // ---- nearest map point of every staged point, within flags and their per-cloud counts
   stage_clouds(c, m, n_clouds, xyz, n, H, off);
+  CompactScratch& s = c.compact;
   m.dst_idx.reserve((size_t)nt);
   m.dst_d2.reserve((size_t)nt);
-  m.ins_flag.reserve((size_t)nt);
-  m.ins_scan.reserve((size_t)nt + 1);
-  map_nearest_launch(c, m.view, m.ins_xyz.p, nt, max_distance * max_distance, m.dst_idx.p, m.dst_d2.p, m.ins_flag.p);
-  scan_u32(c, m.ins_flag.p, nt, m.ins_scan.p, m.sums);
-  m.ins_bounds.reserve((size_t)n_clouds + 1);
-  k_insert_bounds<<<(n_clouds + 256) / 256, 256, 0, st>>>(m.ins_off.p, n_clouds, m.ins_scan.p, m.ins_bounds.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 1;
-  pinned_reserve(m.bounds_host, m.bounds_cap, (size_t)n_clouds + 1);
-  SICP_CUDA(cudaMemcpyAsync(m.bounds_host, m.ins_bounds.p, sizeof(uint32_t) * ((size_t)n_clouds + 1),
-                            cudaMemcpyDeviceToHost, st));
-  SICP_CUDA(cudaStreamSynchronize(st));
-  const long long n_in = m.bounds_host[n_clouds];
+  map_nearest_launch(c, m.view, m.ins_xyz.p, nt, max_distance * max_distance, m.dst_idx.p, m.dst_d2.p, s.flag.p);
+  scan_u32(c, s.flag.p, nt, s.scan.p, s.sums);
+  const uint32_t* bounds = compact_bounds(c, s.scan.p, off);
+  const long long n_in = bounds[n_clouds];
 
   // ---- normals of the matched map points and the plane distances
   if (k > 0) {
@@ -1174,12 +1074,10 @@ static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const 
     if (n_in > 0) {
       m.dst_mxyz.reserve(3 * (size_t)n_in);
       m.dst_nrm.reserve((size_t)n_in);
-      k_dist_gather<<<blocks, 256, 0, st>>>(m.xyz.p, m.dst_idx.p, nt, m.ins_flag.p, m.ins_scan.p, m.dst_mxyz.p);
-      SICP_CUDA(cudaGetLastError());
-      c.tm.kernel_launches += 1;
+      compact_scatter(c, s.flag.p, nt, s.scan.p, nullptr, m.xyz.p, m.dst_idx.p, m.dst_mxyz.p);
       map_normals_launch(c, m.view, m.dst_mxyz.p, n_in, k, m.dst_nrm.p, m.dst_pos);
     }
-    k_dist_plane<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, m.ins_flag.p, m.ins_scan.p, m.dst_mxyz.p, m.dst_nrm.p,
+    k_dist_plane<<<blocks, 256, 0, st>>>(m.ins_xyz.p, nt, s.flag.p, s.scan.p, m.dst_mxyz.p, m.dst_nrm.p,
                                          m.dst_plane.p, m.dst_pl.p);
     SICP_CUDA(cudaGetLastError());
     c.tm.kernel_launches += 1;
@@ -1195,7 +1093,7 @@ static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const 
   }
   SICP_CUDA(cudaStreamSynchronize(st));
   if (n_within)
-    for (int i = 0; i < n_clouds; ++i) n_within[i] = (int64_t)m.bounds_host[i + 1] - (int64_t)m.bounds_host[i];
+    for (int i = 0; i < n_clouds; ++i) n_within[i] = (int64_t)bounds[i + 1] - (int64_t)bounds[i];
 }
 
 }  // namespace sicp

@@ -315,6 +315,7 @@ int32_t sicp_destroy(sicp_ctx* ctx) {
   if (c.rec_host) cudaFreeHost(c.rec_host);
   if (c.scal_host) cudaFreeHost(c.scal_host);
   if (c.grid_host) cudaFreeHost(c.grid_host);
+  if (c.compact.host) cudaFreeHost(c.compact.host);
   delete ctx;
   return SICP_OK;
 }
@@ -985,7 +986,8 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
     queue_second_copy();
     mov_normals();  // while the fixed cloud crosses PCIe
     wait_background_upload(c);
-    // PointCloud.select_in_range on all fixed points (simpleicp.py:160-170), compacted on the host
+    // PointCloud.select_in_range on all fixed points (simpleicp.py:160-170), compacted in order
+    // into the selection
     k_iota<<<(unsigned)((n_fix + 255) / 256), 256, 0, c.stream>>>(c.sel_idx.p, n_fix);
     c.K = n_fix;
     gather_queries_launch(c);
@@ -994,21 +996,18 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz, int64_t n_fix, const
     StageTimer t(c, &c.tm.overlap_ms);
     c.dist.reserve(c.K);
     c.keep.reserve(c.K);
+    c.compact.scan.reserve(n_fix + 1);
     match_launch(c, false, c.dist.p, nullptr, true, rp->max_overlap_distance * rp->max_overlap_distance);
     SICP_CUDA(cudaMemsetAsync(c.misc_counters.p + 8, 0, sizeof(unsigned int), c.stream));
     k_range_keep<<<(unsigned)((c.K + 255) / 256), 256, 0, c.stream>>>(
         c.dist.p, c.K, rp->max_overlap_distance * rp->max_overlap_distance, c.keep.p, c.misc_counters.p + 8);
-    std::vector<uint8_t> keep((size_t)n_fix);
-    copy_any(c, keep.data(), c.keep.p, (size_t)n_fix);
+    scan_u32(c, c.keep.p, n_fix, c.compact.scan.p, c.compact.sums);
+    compact_scatter(c, c.keep.p, n_fix, c.compact.scan.p, c.sel_idx.p, nullptr, nullptr);
+    unsigned int cnt = 0;
+    SICP_CUDA(cudaMemcpyAsync(&cnt, c.misc_counters.p + 8, sizeof(cnt), cudaMemcpyDeviceToHost, c.stream));
     t.stop();
-    std::vector<long long> idx;
-    idx.reserve((size_t)n_fix);
-    for (long long i = 0; i < n_fix; ++i)
-      if (keep[(size_t)i]) idx.push_back(i);
-    SICP_REQUIRE(!idx.empty(), SICP_ERR_NO_OVERLAP, "Point clouds do not overlap within max_overlap_distance");
-    copy_any(c, c.sel_idx.p, idx.data(), sizeof(long long) * idx.size());
-    sync(c);  // idx is a local
-    c.K = (long long)idx.size();
+    SICP_REQUIRE(cnt > 0, SICP_ERR_NO_OVERLAP, "Point clouds do not overlap within max_overlap_distance");
+    c.K = cnt;
     build_fix();
   } else {
     build_fix();

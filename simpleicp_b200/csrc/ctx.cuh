@@ -60,6 +60,19 @@ struct SolveWs {
   DevBuf<sicp_iter_record> rec;     // device copy of the per-iteration record ring
 };
 
+// Scratch of the ordered compactions (grid.cu: scan_u32, compact_bounds, compact_scatter) of the
+// overlap filters, the map calls and the residuals.  Calls on one context run one after the other,
+// so they share it; DevBuf::reserve drops what a buffer held, so a call reserves flag and scan
+// before it writes its first flag.
+struct CompactScratch {
+  DevBuf<uint32_t> flag;    // uint32 flags (or counts) of one compaction
+  DevBuf<uint32_t> scan;    // their exclusive prefix sum, n + 1 entries
+  DevBuf<uint32_t> sums;    // the scan's block sums
+  DevBuf<uint32_t> bounds;  // the boundaries picked from the scan
+  uint32_t* host = nullptr; // pinned: the boundaries read back
+  size_t host_cap = 0;
+};
+
 struct Batch;
 struct MapStore;
 
@@ -150,7 +163,7 @@ struct Ctx {
   SolveWs ws;
   DevBuf<DevState> dev_state;
   int rs_parity = 0;
-  DevBuf<unsigned int> compact_sums;
+  CompactScratch compact;
   // grid build scratch (grid.cu: grid_build), kept apart from the select workspace
   DevBuf<unsigned long long> bbox_keys;   // 6 per cloud
   DevBuf<unsigned int> grid_occ;          // occupied cells per cloud
@@ -201,13 +214,14 @@ struct PairDev {
   GridView gmov, gfix;
   long long n_fix, n_mov;
   long long fix_off, mov_off;  // first point of this pair's clouds in the concatenated clouds
-  // first overlap keep flag of this pair (Batch::ovl_flag, one per fixed point of the pair): fix_off
+  // first overlap keep flag of this pair (Ctx::compact.flag, one per fixed point of the pair): fix_off
   // when every pair owns its fixed cloud; pairs that share one (sicp_register_pairs) get their own
   long long flag_off;
   long long K;                 // selected fixed points (<= Kmax)
   long long q_off;             // first entry of this pair in the per-query arrays
   double cm[3];                // centre of the movable grid's box (moment centring)
-  // overlap filter: this pair's survivors are Batch::ovl_list[list_off, list_off + list_len)
+  // overlap filter: this pair's survivors are Batch::ovl_list[list_off, list_off + list_len), each
+  // its fixed point's flag position flag_off + i (i: index in the fixed cloud)
   long long list_off, list_len;
   double obs[6];               // rbp_observed_values of this pair (radians)
 };
@@ -241,11 +255,8 @@ struct Batch {
   int bin_cap = 0;
   DevBuf<uint32_t> nn_pos;
   DevBuf<uint8_t> keep;
-  // overlap filter, one entry per fixed point of each pair (at PairDev::flag_off): keep flag, its
-  // exclusive prefix sum (total_fix + 1), the in-cloud indices of the survivors in ascending order
-  // per pair
-  DevBuf<uint32_t> ovl_flag, ovl_scan, ovl_list, ovl_sums;
-  DevBuf<uint32_t> ovl_bounds;  // n_pairs + 1 prefix values at the pairs' flag offsets
+  // overlap filter: the survivors of every pair in ascending order (PairDev::list_off)
+  DevBuf<uint32_t> ovl_list;
   // per-pair state
   DevBuf<DevState> state;
   DevBuf<unsigned int> lin_hist;       // n_pairs x (LH_BINS + 2)
@@ -257,8 +268,6 @@ struct Batch {
   int* flags_host = nullptr;                 // pinned
   sicp_pair_result* results_host = nullptr;  // pinned
   size_t flags_cap = 0, results_cap = 0;
-  unsigned long long* ovl_host = nullptr;    // pinned: what the overlap filters read back
-  size_t ovl_host_cap = 0;
   // What sicp_get_batch_outputs reads of the last sicp_register_batch / sicp_register_to_map /
   // sicp_register_pairs.  out_valid is cleared on entry of those calls and of the calls that
   // replace the map, and set only when one of the three returns successfully; the vectors are per
@@ -281,7 +290,6 @@ struct Batch {
   ~Batch() {
     if (flags_host) cudaFreeHost(flags_host);
     if (results_host) cudaFreeHost(results_host);
-    if (ovl_host) cudaFreeHost(ovl_host);
     if (rec_host) cudaFreeHost(rec_host);
     if (T_host) cudaFreeHost(T_host);
   }
@@ -304,42 +312,37 @@ struct MapStore {
   GridBufs grid;
   GridView view{};
   long long n = 0;
-  // overlap filter: one bit per (scan, map point), its per-word popcounts and their prefix sum
-  DevBuf<uint32_t> bits, popc, popc_scan, sums;
+  // overlap filter: one bit per (scan, map point); its per-word popcounts and their prefix sum are
+  // a compaction of the context (Ctx::compact)
+  DevBuf<uint32_t> bits;
   DevBuf<unsigned long long> n_searched;  // bounded searches of the last filter
   DevBuf<MapCull> culls;                  // one per scan
   // sicp_map_insert (batch.cu: map_insert): the clouds of one call, moved and concatenated
-  // (ins_xyz), their finite points compacted in order (fin_xyz, with their index in ins_xyz in
-  // fin_idx) and gridded as one cloud (gnew); a keep flag per point of ins_xyz, its prefix sum and
-  // the per-cloud boundaries of that sum.  These staging buffers grow to the largest insert (about
-  // 100 B per point) and stay allocated, also across sicp_set_map, like the batch's buffers.
-  // xyz_next / grid_next receive the grown map, which is then swapped in; they are released after
-  // the swap, so an insert's peak is about two maps and one map stays resident between inserts.
+  // (ins_xyz, cloud i from ins_off[i]), their finite points compacted in order (fin_xyz, with
+  // their index in ins_xyz in fin_idx) and gridded as one cloud (gnew).  The flags of both
+  // compactions are the context's (Ctx::compact).  These staging buffers grow to the largest
+  // insert (about 100 B per point with the compaction scratch) and stay allocated, also across sicp_set_map, like the batch's
+  // buffers.  xyz_next / grid_next receive the grown map, which is then swapped in; they are
+  // released after the swap, so an insert's peak is about two maps and one map stays resident
+  // between inserts.
   DevBuf<double> ins_xyz, fin_xyz, xyz_next;
-  DevBuf<uint32_t> fin_flag, fin_scan, fin_idx, ins_flag, ins_scan, ins_off, ins_bounds;
+  DevBuf<uint32_t> fin_idx, ins_off;
   DevBuf<Rigid> ins_T;
   GridBufs gnew, grid_next;
   // sicp_map_distances (batch.cu: map_distances) stages its clouds in ins_xyz (with ins_off,
-  // ins_T, fin_flag) and takes ins_flag / ins_scan / ins_bounds for its within flags, their prefix
-  // sum and the per-cloud boundaries.  Its own buffers, per staged point: the map index and d2
-  // of the nearest map point, and with normals the plane distance and planarity (28 B); per
-  // within point: the matched map point's coordinates and its (normal, planarity) (40 B); and the
-  // k-NN positions of one chunk of option "normals_scratch_mb".  They stay allocated like the
-  // insert's staging buffers.
+  // ins_T) and compacts its within flags in Ctx::compact.  Its own buffers, per staged point: the
+  // map index and d2 of the nearest map point, and with normals the plane distance and planarity
+  // (28 B); per within point: the matched map point's coordinates and its (normal, planarity)
+  // (40 B); and the k-NN positions of one chunk of option "normals_scratch_mb".  They stay
+  // allocated like the insert's staging buffers.
   DevBuf<long long> dst_idx;
   DevBuf<double> dst_d2, dst_plane, dst_mxyz;
   DevBuf<float> dst_pl;
   DevBuf<float4> dst_nrm;
   DevBuf<uint32_t> dst_pos;
-  // sicp_map_crop / sicp_map_thin (batch.cu: map_crop, map_thin) take ins_flag / ins_scan for a
-  // keep flag per map point and its prefix sum (8 B per map point, kept like the staging buffers),
-  // and write the kept points into xyz_next; crop_c holds the crop's centres.
+  // sicp_map_crop / sicp_map_thin (batch.cu: map_crop, map_thin) compact a keep flag per map
+  // point in Ctx::compact into xyz_next; crop_c holds the crop's centres.
   DevBuf<double> crop_c;
-  uint32_t* bounds_host = nullptr;  // pinned: n_clouds + 1 boundaries
-  size_t bounds_cap = 0;
-  ~MapStore() {
-    if (bounds_host) cudaFreeHost(bounds_host);
-  }
 };
 
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
@@ -355,9 +358,22 @@ void grid_build(Ctx& c, GridBufs& g, const std::vector<HostCloud>& clouds, const
 // one cloud under the one-pair cell policy, into a grid of the one-pair context
 void grid_build_pair(Ctx& c, Grid& g, const double* xyz_dev, long long n);
 void make_float4_copy(Ctx& c);
-// Exclusive prefix sum of n uint32 values (four launches): out[0 .. n], out[n] = the total.
-// block_sums is scratch.
+// Exclusive prefix sum of n uint32 or uint8 values (four launches): out[0 .. n], out[n] = the
+// total.  block_sums is scratch.
 void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums);
+void scan_u32(Ctx& c, const uint8_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums);
+// Ordered compaction of the elements j < n with flag[j] != 0, scan = the flags' exclusive prefix
+// sum (scan_u32), on the scratch Ctx::compact.
+// compact_bounds: scan[off[i]] for every offset (each <= n), read back; the returned pinned array
+// holds them until the next call.
+const uint32_t* compact_bounds(Ctx& c, const uint32_t* scan, const std::vector<long long>& off);
+// compact_scatter: element j goes to o = scan[j]; pos[o] = j, and row o of the output takes row
+// from[j] (row j without from) of the source, rows of 3 doubles for uint32 flags and of 1 double
+// for uint8 flags.  A null pos or output is not written.
+void compact_scatter(Ctx& c, const uint32_t* flag, long long n, const uint32_t* scan, uint32_t* pos,
+                     const double* xyz, const long long* from, double* xyz_out);
+void compact_scatter(Ctx& c, const uint8_t* flag, long long n, const uint32_t* scan, long long* pos,
+                     const double* src, double* out);
 
 // 1-NN of K transformed queries into the movable cloud; fused point-to-plane distance.
 // If out_d2 != nullptr the squared NN distance is written instead of the plane distance epilogue
@@ -412,7 +428,7 @@ void gather_queries_launch(Ctx& c);
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
 // PointCloud.select_in_range of every fixed point of every pair under its pair's DevState
-// transform: Batch::ovl_flag[flag_off + i] = (squared distance of fix_xyz[fix_off + i] to the
+// transform: Ctx::compact.flag[flag_off + i] = (squared distance of fix_xyz[fix_off + i] to the
 // nearest movable point < r2)
 void batch_overlap_launch(Ctx& c, Batch& b, const double* fix_xyz, long long max_n_fix, double r2);
 // Culled overlap filter of sicp_register_to_map: for every scan, the map points inside its

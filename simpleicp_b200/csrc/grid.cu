@@ -23,6 +23,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "ctx.cuh"
 
@@ -97,11 +98,12 @@ __global__ void __launch_bounds__(256) k_cell_count(const CloudPlan* __restrict_
   if (threadIdx.x == 0 && n_first) atomicAdd(&occ[blockIdx.y], (unsigned int)n_first);
 }
 
-// ---- 3-kernel exclusive scan over uint32 ------------------------------------------------------
+// ---- 3-kernel exclusive scan of uint32 or uint8 values ----------------------------------------
 // Any n below 2^32 whose total is below 2^32 (the outputs are uint32): k_scan_blocksums walks the
 // ceil(n / 4096) block sums 1024 at a time with a carry.  tests/test_gpu_scale.py runs it at
 // 2^27 + 4097 elements (a map crop) and at totals of about 3.9e9 (the map filter's survivors).
-__global__ void __launch_bounds__(256) k_scan_reduce(const uint32_t* __restrict__ in, long long n,
+template <typename T>
+__global__ void __launch_bounds__(256) k_scan_reduce(const T* __restrict__ in, long long n,
                                                      uint32_t* __restrict__ block_sums) {
   long long base = (long long)blockIdx.x * kScanItems;
   uint32_t s = 0;
@@ -148,23 +150,26 @@ __global__ void __launch_bounds__(1024) k_scan_blocksums(uint32_t* __restrict__ 
 
 // Exclusive scan of one 4096-item block, fully coalesced: thread t moves uint4 number j*256 + t
 // (j = 0..3), i.e. 16-byte accesses with unit stride across the warp in both directions; the
-// four 256-wide slabs are scanned one after the other with a running carry.
-__global__ void __launch_bounds__(256) k_scan_down(const uint32_t* __restrict__ in, long long n,
+// four 256-wide slabs are scanned one after the other with a running carry.  uint8 inputs are
+// read one value at a time.
+template <typename T>
+__global__ void __launch_bounds__(256) k_scan_down(const T* __restrict__ in, long long n,
                                                    const uint32_t* __restrict__ block_offsets,
                                                    uint32_t* __restrict__ out) {
+  constexpr bool kVec = std::is_same<T, uint32_t>::value;
   const long long base = (long long)blockIdx.x * kScanItems;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   __shared__ uint32_t wsum[8];
   __shared__ uint32_t carry_s;
   uint32_t carry = block_offsets[blockIdx.x];
-  const bool vec_ok = (base + kScanItems <= n) && ((reinterpret_cast<uintptr_t>(in + base) & 15) == 0) &&
+  const bool vec_ok = kVec && (base + kScanItems <= n) && ((reinterpret_cast<uintptr_t>(in + base) & 15) == 0) &&
                       ((reinterpret_cast<uintptr_t>(out + base) & 15) == 0);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const long long i0 = base + 4ll * (j * 256 + threadIdx.x);
     uint4 v = make_uint4(0, 0, 0, 0);
     if (vec_ok) {
-      v = *reinterpret_cast<const uint4*>(in + i0);
+      if constexpr (kVec) v = *reinterpret_cast<const uint4*>(in + i0);
     } else {
       if (i0 + 0 < n) v.x = in[i0 + 0];
       if (i0 + 1 < n) v.y = in[i0 + 1];
@@ -204,10 +209,34 @@ __global__ void __launch_bounds__(256) k_scan_down(const uint32_t* __restrict__ 
   (void)carry_s;
 }
 
-__global__ void k_scan_total(const uint32_t* __restrict__ in, long long n,
-                             uint32_t* __restrict__ out) {
+template <typename T>
+__global__ void k_scan_total(const T* __restrict__ in, long long n, uint32_t* __restrict__ out) {
   // out[n] = out[n-1] + in[n-1]
   if (threadIdx.x == 0 && blockIdx.x == 0) out[n] = (n > 0) ? out[n - 1] + in[n - 1] : 0;
+}
+
+// ---- ordered compaction (compact_bounds, compact_scatter) ---------------------------------------
+// b[i] = scan[b[i]]: the host uploads the offsets into b and reads the boundaries back from it
+__global__ void k_compact_bounds(const uint32_t* __restrict__ scan, int m, uint32_t* __restrict__ b) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) b[i] = scan[b[i]];
+}
+
+// Every j < n with flag[j] != 0 goes to o = scan[j]: pos[o] = j, and the W doubles of row from[j]
+// (row j without from) of src to row o of rows.  A null pos or rows is not written.
+template <typename F, typename I, int W>
+__global__ void __launch_bounds__(256)
+    k_compact(const F* __restrict__ flag, long long n, const uint32_t* __restrict__ scan, I* __restrict__ pos,
+              const double* __restrict__ src, const long long* __restrict__ from, double* __restrict__ rows) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n || !flag[j]) return;
+  const long long o = scan[j];
+  if (pos) pos[o] = (I)j;
+  if (rows) {
+    const long long r = from ? from[j] : j;
+#pragma unroll
+    for (int a = 0; a < W; ++a) rows[W * o + a] = src[W * r + a];
+  }
 }
 
 __global__ void __launch_bounds__(256) k_scatter(const CloudPlan* __restrict__ plans, CloudPlan one,
@@ -274,7 +303,8 @@ inline double host_key_to_f64(unsigned long long k) {
 
 }  // namespace
 
-void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums) {
+template <typename T>
+static void scan_launch(Ctx& c, const T* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums) {
   cudaStream_t st = c.stream;
   const long long nsb = (n + kScanItems - 1) / kScanItems;
   block_sums.reserve(nsb + 1);
@@ -284,6 +314,46 @@ void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uin
   k_scan_total<<<1, 32, 0, st>>>(in, n, out);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 4;
+}
+
+void scan_u32(Ctx& c, const uint32_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums) {
+  scan_launch(c, in, n, out, block_sums);
+}
+
+void scan_u32(Ctx& c, const uint8_t* in, long long n, uint32_t* out, DevBuf<uint32_t>& block_sums) {
+  scan_launch(c, in, n, out, block_sums);
+}
+
+const uint32_t* compact_bounds(Ctx& c, const uint32_t* scan, const std::vector<long long>& off) {
+  CompactScratch& s = c.compact;
+  const int m = (int)off.size();
+  pinned_reserve(s.host, s.host_cap, (size_t)m);
+  s.bounds.reserve((size_t)m);
+  for (int i = 0; i < m; ++i) s.host[i] = (uint32_t)off[(size_t)i];
+  cudaStream_t st = c.stream;
+  SICP_CUDA(cudaMemcpyAsync(s.bounds.p, s.host, sizeof(uint32_t) * (size_t)m, cudaMemcpyHostToDevice, st));
+  k_compact_bounds<<<(m + 255) / 256, 256, 0, st>>>(scan, m, s.bounds.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  SICP_CUDA(cudaMemcpyAsync(s.host, s.bounds.p, sizeof(uint32_t) * (size_t)m, cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  return s.host;
+}
+
+void compact_scatter(Ctx& c, const uint32_t* flag, long long n, const uint32_t* scan, uint32_t* pos,
+                     const double* xyz, const long long* from, double* xyz_out) {
+  k_compact<uint32_t, uint32_t, 3><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(flag, n, scan, pos, xyz, from,
+                                                                                     xyz_out);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void compact_scatter(Ctx& c, const uint8_t* flag, long long n, const uint32_t* scan, long long* pos,
+                     const double* src, double* out) {
+  k_compact<uint8_t, long long, 1><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(flag, n, scan, pos, src,
+                                                                                      nullptr, out);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
 }
 
 void grid_build(Ctx& c, GridBufs& g, const std::vector<HostCloud>& clouds, const CellPolicy& policy,

@@ -1317,8 +1317,8 @@ static void bf_launch(Ctx& c, bool with_distance, double* out, bool whole_set) {
 namespace {
 // per pair: sel[i] = src[rint(linspace(0, m - 1, K))] (PointCloud.select_n_points, k_select_n in
 // capi.cu) and the gather of the selected fixed points, in one launch for the whole batch.  src is
-// the pair's survivor list of the overlap filter (m = its length) or, without a list, the whole
-// cloud (m = n_fix, src = identity).
+// the pair's survivor list of the overlap filter (m = its length; its entries are flag positions
+// flag_off + index) or, without a list, the whole cloud (m = n_fix, src = identity).
 __global__ void __launch_bounds__(256)
     k_select_gather_batch(const PairDev* __restrict__ pairs, const double* __restrict__ fix_xyz,
                           const uint32_t* __restrict__ list, int away, long long* __restrict__ sel,
@@ -1333,7 +1333,7 @@ __global__ void __launch_bounds__(256)
     const double y = (i == n - 1 && n > 1) ? (double)(m - 1) : (double)i * step;
     j = (long long)(away ? round(y) : rint(y));
   }
-  if (list) j = list[pd.list_off + j];
+  if (list) j = (long long)list[pd.list_off + j] - pd.flag_off;
   sel[pd.q_off + i] = j;
   const double* __restrict__ src = fix_xyz + 3 * (pd.fix_off + j);
   double* __restrict__ dst = q_xyz + 3 * (pd.q_off + i);
@@ -1372,7 +1372,7 @@ void batch_overlap_launch(Ctx& c, Batch& b, const double* fix_xyz, long long max
   const dim3 grid((unsigned)((max_n_fix * mg + 127) / 128), b.n_pairs);
   with_lanes<4, 8, 16>(mg, [&](auto L) {
     k_overlap_batch<decltype(L)::value>
-        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, fix_xyz, r2, b.ovl_flag.p);
+        <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, fix_xyz, r2, c.compact.flag.p);
   });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;

@@ -2087,61 +2087,6 @@ __global__ void __launch_bounds__(1024)
   }
 }
 
-// Ordered compaction of the kept residuals (final iteration only): block-level scan, one block
-// per 4096 elements, two kernels.
-__global__ void __launch_bounds__(256)
-    k_compact_count(const uint8_t* __restrict__ keep, long long K, unsigned int* __restrict__ bsum) {
-  const long long base = (long long)blockIdx.x * 4096;
-  unsigned int c = 0;
-  for (int j = threadIdx.x; j < 4096; j += 256)
-    if (base + j < K) c += keep[base + j] ? 1u : 0u;
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  __shared__ unsigned int sh[8];
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned int t = 0;
-    for (int i = 0; i < 8; ++i) t += sh[i];
-    bsum[blockIdx.x] = t;
-  }
-}
-
-__global__ void __launch_bounds__(256)
-    k_compact_write(const uint8_t* __restrict__ keep, const double* __restrict__ resid, long long K,
-                    const unsigned int* __restrict__ bsum, double* __restrict__ out) {
-  // offset of this block = sum of previous block counts (few hundred blocks at most)
-  __shared__ unsigned int boff;
-  __shared__ unsigned int wsum[8];
-  if (threadIdx.x == 0) {
-    unsigned int t = 0;
-    for (unsigned int b = 0; b < blockIdx.x; ++b) t += bsum[b];
-    boff = t;
-  }
-  __syncthreads();
-  const long long base = (long long)blockIdx.x * 4096 + threadIdx.x * 16;
-  unsigned int flags = 0, c = 0;
-#pragma unroll
-  for (int j = 0; j < 16; ++j)
-    if (base + j < K && keep[base + j]) {
-      flags |= 1u << j;
-      ++c;
-    }
-  unsigned int incl = c;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned int t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) wsum[w] = incl;
-  __syncthreads();
-  unsigned int woff = 0;
-  for (int i = 0; i < w; ++i) woff += wsum[i];
-  unsigned int pos = boff + woff + incl - c;
-#pragma unroll
-  for (int j = 0; j < 16; ++j)
-    if (flags & (1u << j)) out[pos++] = resid[base + j];
-}
-
 // The arguments every reject/solve launch takes from the run parameters and the variant /
 // movable-attribute policy: with movable-side attributes the kernels read the match kernels'
 // copy of the normals, whose .w is the signed effective planarity; the linearised variants take
@@ -2371,17 +2316,13 @@ void final_residuals_launch(Ctx& c) {
   c.tm.kernel_launches += 1;
 }
 
+// the kept residuals in correspondence order
 void compact_residuals_launch(Ctx& c) {
   const long long K = c.K;
-  const unsigned int nb = (unsigned int)((K + 4095) / 4096);
-  c.ws.counters.reserve(64);
-  c.compact_sums.reserve(nb + 1);
+  c.compact.scan.reserve(K + 1);
   c.resid_compact.reserve(std::max<long long>(K, 1));
-  k_compact_count<<<nb, 256, 0, c.stream>>>(c.keep.p, K, c.compact_sums.p);
-  k_compact_write<<<nb, 256, 0, c.stream>>>(c.keep.p, c.resid.p, K, c.compact_sums.p,
-                                           c.resid_compact.p);
-  SICP_CUDA(cudaGetLastError());
-  c.tm.kernel_launches += 2;
+  scan_u32(c, c.keep.p, K, c.compact.scan.p, c.compact.sums);
+  compact_scatter(c, c.keep.p, K, c.compact.scan.p, nullptr, c.resid.p, c.resid_compact.p);
 }
 
 }  // namespace sicp

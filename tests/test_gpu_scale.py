@@ -4,10 +4,12 @@ the sizes they are built for, against references that are exact by construction.
 Code that only runs at scale:
   * scan_u32's second level, k_scan_blocksums, walks the block sums 1024 at a time and carries a
     running total between chunks: the carry only runs past 1024 x 4096 = 4 194 304 elements.  Every
-    grid build (cells), the batch overlap filter (fixed points), the map filter (mask words) and
-    the map's insert, crop, thin and distances (points) scan through it;
-  * the per-pair and per-cloud kernels with one thread per pair or cloud (k_overlap_bounds,
-    k_insert_bounds, k_gather_flags, k_bbox_init) use more than one block only past 256, 128 or 42;
+    grid build (cells), the batch overlap filter (fixed points), the map filter (mask words), the
+    map's insert, crop, thin and distances (points), and sicp_register's overlap selection and
+    final residuals (uint8 keep flags) scan through it;
+  * the kernels with one thread per pair or cloud (k_compact_bounds: the boundaries of the batch
+    filter and of the map's insert and distances; k_gather_flags, k_bbox_init) use more than one
+    block only past 256, 128 or 42;
   * the batch match takes 4 lanes once Kmax x n_pairs passes 65 536;
   * the map filter's mask rows, popcount scan and survivor offsets are uint32 up to
     n_scans x n_map < 2^32.
@@ -152,6 +154,65 @@ def test_one_pair_grid_past_the_scan_chunk(gpu, where):
             assert np.array_equal(keep, (off * off).sum(axis=1) <= 2)
 
 
+def _offset_sheet(where, seed):
+    """The 9 M-point sheet (movable) and its points moved by offsets in {-1, 0, 1}^3 units (fixed):
+    fixed point i has movable point i as its nearest, at squared distance |off_i|^2 U^2."""
+    n, SJ = 9_000_001, 3001
+    Mk = sheet_k(np.arange(n), SJ)
+    off = np.random.default_rng(seed).integers(-1, 2, (n, 3))
+    return to_xyz(Mk + off, ORIGINS[where]), to_xyz(Mk, ORIGINS[where]), off
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("where", sorted(ORIGINS))
+def test_register_overlap_selection_past_the_scan_chunk(gpu, where):
+    """sicp_register with max_overlap_distance on a 9 M-point fixed cloud: the keep flags of all
+    its points are compacted into the selection on the device, over more than two scan chunks.
+    With correspondences >= the survivors the selection is the survivors, which the construction
+    gives (|off|^2 <= 2 for r = 1.5 U), and the one call equals the stage-by-stage path
+    (select_in_range, the compaction in NumPy) bit for bit.  The sheet is nearly a plane: the
+    in-plane parameters are fixed, so the solve stays regular."""
+    X_fix, X_mov, off = _offset_sheet(where, 5)
+    want = np.flatnonzero((off * off).sum(axis=1) <= 2)
+    assert want[-1] > 2 * CHUNK
+    kw = dict(correspondences=len(X_fix), max_overlap_distance=1.5 * U, min_planarity=0.0, max_iterations=3,
+              rbp_observation_weights=(0.0, 0.0, np.inf, np.inf, np.inf, 0.0))
+    with _capi.Engine() as e:
+        a = sb.register(X_fix, X_mov, engine=e, want_normals=False, **kw)  # one call
+        b = sb.register(X_fix, X_mov, engine=e, want_normals=True, **kw)   # stage by stage
+    assert np.array_equal(a.idx_selected, want) and np.array_equal(b.idx_selected, want)
+    assert np.array_equal(a.H, b.H) and a.iterations == b.iterations and a.converged == b.converged
+    assert len(a.residuals) > CHUNK and np.array_equal(a.residuals, b.residuals)
+    assert np.array_equal(np.asarray(a.X_mov_transformed), np.asarray(b.X_mov_transformed))
+    for ra, rb in zip(a.records, b.records):
+        assert ra["n_kept"] == rb["n_kept"] and ra["mean_res"] == rb["mean_res"] and ra["std_res"] == rb["std_res"]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("where", sorted(ORIGINS))
+def test_residuals_past_the_scan_chunk(gpu, where):
+    """The ordered compaction of the residuals by 9 M keep flags (more than two scan chunks), more
+    than one chunk of them kept: the offset-sheet queries matched at the identity, normals
+    (0, 0, 1), every seventh planarity below min_planarity, and a solve with all six parameters
+    fixed, whose transform is the identity.  Each residual is then exactly the kept query's match
+    distance, the construction's -off_z U."""
+    X_fix, X_mov, off = _offset_sheet(where, 6)
+    n = len(X_fix)
+    flat = np.arange(n) % 7 != 3
+    with _capi.Engine() as e:
+        e.set_clouds(X_fix, X_mov)
+        e.set_selected(None)
+        z = np.zeros(n, dtype=np.float32)
+        e.set_normals(z, z, np.ones(n, dtype=np.float32), np.where(flat, 0.9, 0.1).astype(np.float32))
+        idx, d = e.match(np.eye(4))
+        assert np.array_equal(idx, np.arange(n)) and np.array_equal(d, -off[:, 2] * U)
+        keep, n_kept, _ = e.reject(0.3)  # |d - median| <= U: only the planarity rejects
+        assert np.array_equal(keep, flat) and n_kept > CHUNK
+        x, _, res, _, _ = e.solve(np.zeros(6), np.zeros(6), np.full(6, np.inf), 1.0, n_kept)
+    assert np.array_equal(x, np.zeros(6))
+    assert np.array_equal(res, d[flat]) and np.array_equal(res, -off[flat, 2] * U)
+
+
 # ------------------------------------------------------------------------------ 2. the map at 9 M points
 N_MAP, SJ_MAP = 3001 * 2999, 2999  # 8 999 999 points: not a multiple of 4096, three scan chunks
 OCC = {"default": None, "occ1": 1.0}
@@ -232,7 +293,7 @@ def test_map_thin_past_the_scan_chunk(gpu, where, occ):
 
 
 def _insert_clouds(where, rng):
-    """4.5 M points in 300 clouds (k_insert_bounds runs two blocks): near the sheet (taken voxels,
+    """4.5 M points in 300 clouds (k_compact_bounds runs two blocks): near the sheet (taken voxels,
     and new ones beyond its edges), far outside with NaN rows, an empty cloud, and 297 pieces lifted
     by 40 units (new voxels, many points per voxel)."""
     o = ORIGINS[where]
@@ -287,7 +348,7 @@ def test_map_distances_past_the_scan_chunk(gpu, where, occ):
             assert np.array_equal(d2[i][:m], o2 * (U * U)), i
             assert n_within[i] == m, i
         assert (idx[3][-307:] == -1).all() and np.isinf(d2[3][-307:-7]).all() and np.isnan(d2[3][-7:]).all()
-        # the first cloud in 300 pieces: the per-cloud counts come from two blocks of k_insert_bounds
+        # the first cloud in 300 pieces: the per-cloud counts come from two blocks of k_compact_bounds
         pieces = np.array_split(clouds[0], 300)
         idx_p, d2_p, _, _, n_p = e.map_distances(pieces, max_distance=r)
         assert np.array_equal(np.concatenate(idx_p), idx[0]) and np.array_equal(np.concatenate(d2_p), d2[0])
