@@ -422,6 +422,50 @@ int32_t sicp_map_crop(sicp_ctx* ctx, int32_t n_centers, const double* centers /*
                       double radius, int64_t* n_removed /*[h] or NULL*/);
 int32_t sicp_map_thin(sicp_ctx* ctx, double voxel_size, int64_t* n_removed /*[h] or NULL*/);
 
+/* ---- carving the map: remove the map points that rays of clouds pass (free space) --------------
+ * sicp_map_carve removes the map points that scans see through: a parked car that has left, a
+ * door that was open.  Cloud i is moved by H[16 i .. 16 i + 15] (row-major 4 x 4, bit for bit what
+ * sicp_transform gives) or, with H NULL, taken as it is.  Every moved point p with three finite
+ * coordinates is a ray from o = origins[3 i .. 3 i + 2] (the map's frame) or, with origins NULL,
+ * from H's translation column (H[16 i + 3], H[16 i + 7], H[16 i + 11], taken as they are): where
+ * a scan given in its sensor frame was taken.  For a map point m and one ray, every operation is
+ * one IEEE double operation rounded on its own, with no fused multiply-add:
+ *   d = p - o, u = m - o (per axis), L2 = (dx dx + dy dy) + dz dz, L = sqrt(L2),
+ *   s = ((ux dx + uy dy) + uz dz) / L, e2 = ((ux ux + uy uy) + uz uz) - s s;
+ *   the ray passes m iff L2 > 0, L2 finite, s > 0, s < L - margin and e2 < fl(radius^2).
+ * passes[m] = the rays of this call that pass m (each ray counts once); m is removed iff
+ * passes[m] >= min_passes.  Nothing is accumulated across calls.
+ *  - margin protects the surfaces the rays end on: a ray meeting a surface at angle a passes within
+ *    radius of it over about radius / sin(a) before its end, so surface points are carved where
+ *    radius / sin(a) > margin.  min_passes > 1 makes one stray ray harmless.
+ *  - The new map is the kept points in their old order; nothing is moved or added.  n_removed (if
+ *    not NULL) = the points removed.  passes (if not NULL, any memory kind) receives the n_map
+ *    counts of the map as it was, on SICP_OK and on SICP_ERR_NO_OVERLAP.
+ *  - When nothing is removed, the map and its grid stay as they are.  Otherwise the grid is
+ *    rebuilt by sicp_set_map's builder, so the carved map registers and gives distances exactly
+ *    as a fresh sicp_set_map of the same points.
+ *  - SICP_ERR_STATE: no map.  SICP_ERR_BAD_ARG, before any device work: n_clouds < 1, a negative
+ *    n[i], a NULL xyz[i] with n[i] > 0 (empty clouds cast no ray), a non-finite H entry, origins
+ *    and H both NULL, a non-finite origin, a radius that is not finite and > 0, a margin that is
+ *    not finite and >= 0, min_passes < 1, or sum n[i] >= 2^32.  SICP_ERR_NO_OVERLAP: the carve
+ *    would remove every point (a map is never empty).
+ *  - The map is replaced only when the new one is complete: after an error it is unchanged.
+ *  - Clears the batch outputs, as sicp_map_crop does; the one-pair state is not touched.
+ *  - Cost: each ray walks the map-grid cells within about radius of its first L - margin, one
+ *    layer of cells along its major axis at a time: about (L / h + 1) (2 radius / h + 2)^2 cells
+ *    for a map cell size h, plus the rebuild when points are removed.
+ *  - Device memory: the staging buffers of sicp_map_distances (about 40 B per point), 4 B of
+ *    passes per map point and 24 B per cloud, all staying on the context; the keep flags and the
+ *    rebuild as for sicp_map_crop (peak about two maps).  Map indices, offsets and counts are
+ *    32-bit: n_map < 2^32 as for sicp_set_map and sum n[i] < 2^32, so no count (at most one per
+ *    ray) can wrap.                                                                              */
+int32_t sicp_map_carve(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                       const int64_t* n /*[h]*/, const double* H /*[h] n_clouds x 16, or NULL*/,
+                       const double* origins /*[h] n_clouds x 3, or NULL: the translation column of H*/,
+                       double radius, double margin, int32_t min_passes,
+                       uint32_t* passes /*[h|d] n_map (the map as it was), or NULL*/,
+                       int64_t* n_removed /*[h] or NULL*/);
+
 /* ---- how well clouds fit the map: cloud-to-map distances --------------------------------------
  * sicp_map_distances gives every point of n_clouds clouds its nearest map point within
  * max_distance, and with neighbors = k > 0 its signed distance along that map point's normal.
@@ -468,9 +512,9 @@ int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const*
  * per-iteration records and the applied transform.  Those two calls only leave these on the
  * device; all the work happens here, and they stay readable (any number of times, same bits)
  * until the next sicp_register_batch, sicp_register_to_map, sicp_register_pairs, sicp_set_map,
- * sicp_map_insert, sicp_map_crop or sicp_map_thin on the context.
- *  - SICP_ERR_STATE: before any such call, after sicp_set_map, sicp_map_insert, sicp_map_crop or
- *    sicp_map_thin, or after a
+ * sicp_map_insert, sicp_map_crop, sicp_map_thin or sicp_map_carve on the context.
+ *  - SICP_ERR_STATE: before any such call, after sicp_set_map, sicp_map_insert, sicp_map_crop,
+ *    sicp_map_thin or sicp_map_carve, or after a
  *    batch / map / pairs call that returned an error (each of these clears the outputs on entry;
  *    only a successful return of the first three makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
  *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose

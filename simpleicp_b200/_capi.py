@@ -42,7 +42,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_get_batch_outputs",
-    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -174,6 +174,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
         "sicp_map_crop": [vp, i32, vp, dbl, C.POINTER(i64)],
         "sicp_map_thin": [vp, dbl, C.POINTER(i64)],
+        "sicp_map_carve": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, vp, dbl, dbl, i32, vp, C.POINTER(i64)],
         "sicp_map_distances": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, i32, C.POINTER(vp), C.POINTER(vp),
                                C.POINTER(vp), C.POINTER(vp), vp],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
@@ -693,6 +694,31 @@ class Engine:
         order.  Returns the points removed."""
         removed = C.c_int64(0)
         self._check(self._lib.sicp_map_thin(self._h, float(voxel_size), C.byref(removed)))
+        self.n_map -= int(removed.value)
+        return int(removed.value)
+
+    def map_carve(self, clouds, H=None, *, origins=None, radius: float, margin: float, min_passes: int = 1,
+                  passes=None) -> int:
+        """sicp_map_carve: remove the map points that at least `min_passes` rays pass, a ray running
+        from cloud i's origin (origins[i], or with origins None H[i]'s translation column) to each
+        finite point of cloud i (moved by H[i] first when `H` (n_clouds x 4 x 4) is given).
+        `passes` is None or a uint32 array / tensor (host or CUDA) of the map's size before the
+        call, which receives every map point's pass count.  Returns the points removed."""
+        n = len(clouds)
+        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
+        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
+        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
+        if H is not None:
+            H = np.ascontiguousarray(H, dtype=np.float64)
+            if H.shape != (n, 4, 4):
+                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
+        if origins is not None:
+            origins = np.ascontiguousarray(origins, dtype=np.float64)
+            if origins.shape != (n, 3):
+                raise ValueError(f"origins must have shape ({n}, 3), got {origins.shape}")
+        removed = C.c_int64(0)
+        self._check(self._lib.sicp_map_carve(self._h, n, ptrs, counts, _ptr(H), _ptr(origins), float(radius),
+                                             float(margin), int(min_passes), _ptr(passes), C.byref(removed)))
         self.n_map -= int(removed.value)
         return int(removed.value)
 

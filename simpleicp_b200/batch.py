@@ -462,6 +462,8 @@ class Map:
     positions (a local map around the sensor, so a loop that keeps inserting stays bounded), and
     ``thin(voxel_size=v)`` to one point per voxel (a dense base map); both keep the points' order
     and leave a map that registers as ``Map(points)`` of the same points would.
+    ``carve(clouds, H, radius=r, margin=e)`` removes what the scans' rays see through (free
+    space), the same way.
     """
 
     def __init__(self, X_map, device: int = 0):
@@ -623,9 +625,66 @@ class Map:
         self.n_points = self._engine.n_map
         return removed
 
+    def carve(self, clouds, H=None, *, origins=None, radius: float, margin: float, min_passes: int = 1,
+              return_passes: bool = False):
+        """Carve free space out of the map on the device (sicp_map_carve): remove the map points
+        that the scans' rays pass, such as a car that has since driven off.
+
+        ``clouds`` and ``H`` are as in ``insert``.  Every finite moved point p of cloud i is a ray
+        from the sensor origin o_i, by default H[i]'s translation column (a scan given in its own
+        sensor frame was taken there); ``origins`` ((n_clouds, 3), the map's frame) gives them
+        explicitly, as clouds already in the map's frame need.  With d = p - o, u = m - o,
+        L = sqrt((dx dx + dy dy) + dz dz), s = ((ux dx + uy dy) + uz dz) / L and
+        e2 = ((ux ux + uy uy) + uz uz) - s s (each operation rounded in double), the ray passes map
+        point m iff L > 0 and finite, 0 < s < L - margin and e2 < radius^2.  A map point that
+        ``min_passes`` or more rays of this call pass is removed; the rest keep their order.
+
+        ``margin`` keeps the rays off the surfaces they end on: a ray that meets a surface at an
+        angle a passes within ``radius`` of it over about radius / sin(a) before its end, so
+        surface points are carved where radius / sin(a) > margin (grazing rays).  ``min_passes`` >
+        1 makes a single stray ray harmless.  Returns the number of points removed, and with
+        ``return_passes=True`` ``(removed, passes)``: the pass count of every point of the map as
+        it was (np.uint32).  A carve that would remove every point raises the library's SicpError
+        (code 2, SICP_ERR_NO_OVERLAP) and leaves the map as it was."""
+        r, mg = float(radius), float(margin)
+        if not (np.isfinite(r) and r > 0):
+            raise ValueError(f"radius must be finite and > 0, got {radius}")
+        if not (np.isfinite(mg) and mg >= 0):
+            raise ValueError(f"margin must be finite and >= 0, got {margin}")
+        if isinstance(min_passes, bool) or int(min_passes) != min_passes or not 1 <= int(min_passes) < (1 << 31):
+            raise ValueError(f"min_passes must be an integer >= 1, got {min_passes}")
+        clouds = list(clouds)
+        if not clouds:
+            raise ValueError("carve needs at least one cloud")
+        for i, X in enumerate(clouds):
+            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
+                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
+        if H is not None:
+            H = np.asarray(H, dtype=np.float64)
+            if H.shape != (len(clouds), 4, 4):
+                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
+            if not np.isfinite(H).all():
+                raise ValueError("H must be finite")
+        if origins is not None:
+            origins = np.asarray(origins, dtype=np.float64)
+            if origins.shape != (len(clouds), 3):
+                raise ValueError(f"origins must have shape ({len(clouds)}, 3), got {origins.shape}")
+            if not np.isfinite(origins).all():
+                raise ValueError("origins must be finite")
+        elif H is None:
+            raise ValueError("carve needs origins, or H whose translations are the sensor origins")
+        import torch
+
+        passes = np.zeros(self.n_points, dtype=np.uint32) if return_passes else None
+        with torch.cuda.device(self.device):
+            removed = self._engine.map_carve(clouds, H, origins=origins, radius=r, margin=mg,
+                                             min_passes=int(min_passes), passes=passes)
+        self.n_points = self._engine.n_map
+        return (removed, passes) if return_passes else removed
+
     def points(self) -> np.ndarray:
         """The map as it stands, (n_points, 3) float64 in map order (a copy): the points it was
-        made of followed by those ``insert`` added, less those ``crop`` and ``thin`` removed.
+        made of followed by those ``insert`` added, less those ``crop``, ``thin`` and ``carve`` removed.
         ``sb.write_xyz(path, m.points())`` saves it."""
         import torch
 

@@ -113,6 +113,13 @@ __global__ void __launch_bounds__(256)
   if (j < n) keep[j] = hit ? 1u : 0u;
 }
 
+// sicp_map_carve's keep flags: keep[j] = passes[j] < min_passes
+__global__ void __launch_bounds__(256)
+    k_carve_keep(const uint32_t* __restrict__ passes, long long n, uint32_t min_passes, uint32_t* __restrict__ keep) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j < n) keep[j] = passes[j] < min_passes ? 1u : 0u;
+}
+
 // the signed distance of point j along its matched map point's normal, plane_distance's expression
 // (nn.cu): ((px - mx) nx + (py - my) ny) + (pz - mz) nz in double, the float32 normal promoted, no
 // fused multiply-add; and that normal's planarity.  NaN for a point without a match.
@@ -1030,6 +1037,54 @@ static void map_thin(Ctx& c, double voxel, int64_t* n_removed) {
   if (n_removed) *n_removed = removed;
 }
 
+// sicp_map_carve: remove the map points that at least min_passes rays of the clouds pass.  The
+// clouds are staged and moved as sicp_map_distances' are; k_map_carve (nn.cu) walks every ray
+// through the map grid and counts the passes per map point; they go to the caller, and the map
+// points with fewer than min_passes are kept through keep_flagged, as by a crop.
+static void map_carve(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
+                      const double* origins, double radius, double margin, int32_t min_passes, uint32_t* passes,
+                      int64_t* n_removed) {
+  if (c.batch) c.batch->out_valid = false;
+  const std::vector<long long> off = check_clouds(n_clouds, xyz, n, H);
+  SICP_REQUIRE(origins || H, SICP_ERR_BAD_ARG, "origins and H are both NULL: a ray needs its origin");
+  std::vector<double> o(3 * (size_t)n_clouds);
+  for (int i = 0; i < n_clouds; ++i)
+    for (int a = 0; a < 3; ++a)  // H's translation column, taken as it is
+      o[3 * (size_t)i + a] = origins ? origins[3 * (size_t)i + a] : H[16 * (size_t)i + 4 * a + 3];
+  for (double v : o) SICP_REQUIRE(std::isfinite(v), SICP_ERR_BAD_ARG, "origins has non-finite coordinates");
+  SICP_REQUIRE(std::isfinite(radius) && radius > 0, SICP_ERR_BAD_ARG, "radius must be finite and > 0");
+  SICP_REQUIRE(std::isfinite(margin) && margin >= 0, SICP_ERR_BAD_ARG, "margin must be finite and >= 0");
+  SICP_REQUIRE(min_passes >= 1, SICP_ERR_BAD_ARG, "min_passes must be >= 1");
+  const long long nt = off[(size_t)n_clouds];
+  SICP_REQUIRE(nt < (1ll << 32), SICP_ERR_BAD_ARG, "the points of the clouds must be below 2^32 (32-bit offsets)");
+  SICP_REQUIRE(c.map && c.map->n > 0, SICP_ERR_STATE, "no map: call sicp_set_map first");
+  MapStore& m = *c.map;
+  if (n_removed) *n_removed = 0;
+  cudaStream_t st = c.stream;
+  // the staging's finite flags, then the keep flags of the map, share the compaction's scratch
+  c.compact.flag.reserve((size_t)std::max(nt, m.n));
+  c.compact.scan.reserve((size_t)std::max(nt, m.n) + 1);
+  m.carve_passes.reserve((size_t)m.n);
+  SICP_CUDA(cudaMemsetAsync(m.carve_passes.p, 0, sizeof(uint32_t) * (size_t)m.n, st));
+  if (nt > 0) {
+    stage_clouds(c, m, n_clouds, xyz, n, H, off);
+    m.carve_o.reserve(o.size());
+    SICP_CUDA(cudaMemcpyAsync(m.carve_o.p, o.data(), sizeof(double) * o.size(), cudaMemcpyHostToDevice, st));
+    // r2 = fl(radius^2), as sicp_map_crop computes it
+    map_carve_launch(c, m.view, m.ins_xyz.p, nt, m.ins_off.p, n_clouds, m.carve_o.p, radius, radius * radius, margin,
+                     m.carve_passes.p);
+  }
+  if (passes) copy_any(c, passes, m.carve_passes.p, sizeof(uint32_t) * (size_t)m.n);
+  k_carve_keep<<<(unsigned)((m.n + 255) / 256), 256, 0, st>>>(m.carve_passes.p, m.n, (uint32_t)min_passes,
+                                                              c.compact.flag.p);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+  // keep_flagged reads its count back (a stream synchronise), so passes is complete when it
+  // returns, also when it throws SICP_ERR_NO_OVERLAP
+  const long long removed = keep_flagged(c, m);
+  if (n_removed) *n_removed = removed;
+}
+
 // sicp_map_distances.  The clouds are staged and moved as sicp_map_insert's are; k_map_nearest
 // finds each point's nearest map point within the bound (nn.cu); one scan over the within flags
 // gives the per-cloud counts (one read-back) and the places of the within points, whose matched
@@ -1163,6 +1218,12 @@ extern "C" int32_t sicp_map_crop(sicp_ctx* ctx, int32_t n_centers, const double*
 
 extern "C" int32_t sicp_map_thin(sicp_ctx* ctx, double voxel_size, int64_t* n_removed) {
   SICP_BATCH_API(map_thin(c, voxel_size, n_removed))
+}
+
+extern "C" int32_t sicp_map_carve(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                  const double* H, const double* origins, double radius, double margin,
+                                  int32_t min_passes, uint32_t* passes, int64_t* n_removed) {
+  SICP_BATCH_API(map_carve(c, n_clouds, xyz, n, H, origins, radius, margin, min_passes, passes, n_removed))
 }
 
 extern "C" int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

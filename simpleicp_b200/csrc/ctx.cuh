@@ -343,6 +343,11 @@ struct MapStore {
   // sicp_map_crop / sicp_map_thin (batch.cu: map_crop, map_thin) compact a keep flag per map
   // point in Ctx::compact into xyz_next; crop_c holds the crop's centres.
   DevBuf<double> crop_c;
+  // sicp_map_carve (batch.cu: map_carve) stages its clouds as sicp_map_distances does; carve_o
+  // holds one origin per cloud and carve_passes one count per map point (4 B); both stay
+  // allocated like the staging buffers, and the keep flags are compacted as the crop's are.
+  DevBuf<double> carve_o;
+  DevBuf<uint32_t> carve_passes;
 };
 
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
@@ -450,6 +455,12 @@ void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh,
 // xyz (gridded in map, in map order) when no map point j' < j has its voxel key floor(p / voxel),
 // else 0
 void map_thin_flags_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double voxel, uint32_t* keep);
+// sicp_map_carve's ray walk (nn.cu: k_map_carve): each finite point j of the n points xyz (cloud i
+// from off[i], n_clouds + 1 offsets) is a ray from origins[3 i]; passes[idx] += 1 for every map
+// record idx the ray passes (radius r, r2 = fl(r r), margin), at most once per ray.  passes is
+// zeroed by the caller.
+void map_carve_launch(Ctx& c, const GridView& map, const double* xyz, long long n, const uint32_t* off, int n_clouds,
+                      const double* origins, double r, double r2, double margin, uint32_t* passes);
 // sicp_map_distances' bounded nearest search (nn.cu: k_map_nearest), one lane group per point j of
 // xyz (n points): the nearest map point (lowest index among ties) when its d2 < cap2 ->
 // idx[j], d2[j], within[j] = 1; else idx -1, within 0 and d2 +inf (finite point) or NaN (a NaN or

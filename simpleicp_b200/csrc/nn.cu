@@ -909,6 +909,119 @@ __global__ void __launch_bounds__(256)
   keep[j] = voxel_taken(map, lo, hi, v, k, j) ? 0u : 1u;
 }
 
+// ---- sicp_map_carve: the map points the rays of clouds pass ---------------------------------
+// Point j of xyz (cloud i = the last with off[i] <= j, finite after the move) is the ray (o, p)
+// from o = origins[i].  For a map record m, with every operation rounded on its own:
+//   d = p - o, u = m - o, L2 = (dx dx + dy dy) + dz dz, L = sqrt(L2),
+//   s = ((ux dx + uy dy) + uz dz) / L, e2 = ((ux ux + uy uy) + uz uz) - s s,
+//   m is passed iff L2 > 0, L2 finite, s > 0, s < L - margin and e2 < r2 (= fl(r r), host).
+// Coverage.  Take the exact segment S from o to o + (L - margin) / L (p - o).  The computed u and
+// d are within u_r |u| and u_r |d| of the exact ones (u_r = 2^-53); the three-term sums, the root
+// and the division add a few u_r each, so s and e2 are within 8 u_r |u| and 8 u_r |u|^2 of the
+// exact projection and squared line distance.  A passed m therefore lies within
+// r + sqrt(8 u_r) |u| + 16 u_r (|u| + L) < r + 4e-8 (L + r) of S (|u| < L + r + tiny for a passed
+// m).  The walk grows that tube to R = r + 1e-6 (L + r) + 1e-12 A, where A bounds the magnitude of
+// every coordinate the walk computes (the endpoints' and the grid box's): each face, end and
+// segment coordinate below is a few rounded operations on such numbers, so it moves by less than
+// 1e-15 A + 1e-15 (L + r), far inside the slack, also at UTM-scale coordinates.
+// Cells are the grid's own cell_coord of the grown faces, monotone and clamping as in voxel_taken,
+// so a record whose coordinate lies between two faces lies in a cell between theirs.
+//  1. Clip: every record lies in the grid's box, so the foot point of a passed m on S lies in that
+//     box grown by R on every axis; S is clipped to it (t in [t0, t1] of o + t d).
+//  2. Layers: on the major axis a of d (|d_a| largest), layer i holds the records with
+//     cell_coord(m_a) = i, whose m_a lies in [g.o_a + i h, g.o_a + (i + 1) h] grown by 1e-12 A
+//     (open below the first layer and above the last, where cell_coord clamps).  A passed m in
+//     layer i has its foot point within R of that slab on axis a: the part of S there is one
+//     t-interval, and its extent on the other two axes grown by R bounds m's cells there.
+//  3. Each cell at most once per ray: layers partition axis a, and a layer's (b, c) box lists
+//     each cell once, walked as contiguous x-rows like voxel_taken.  So passes counts rays.
+// One thread per ray: on the probe of DESIGN §6.8 it was faster than groups of 4 or 8 lanes that
+// split each row's records.
+__global__ void __launch_bounds__(256)
+    k_map_carve(GridView g, const double* __restrict__ xyz, long long n, const uint32_t* __restrict__ off,
+                int n_clouds, const double* __restrict__ origins, double r, double r2, double margin,
+                uint32_t* __restrict__ passes) {
+  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const double p[3] = {xyz[3 * j + 0], xyz[3 * j + 1], xyz[3 * j + 2]};
+  if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]))) return;
+  int lo = 0, hi = n_clouds;  // off[lo] <= j < off[hi], as k_insert_stage
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= (unsigned long long)j) lo = mid;
+    else hi = mid;
+  }
+  const double o[3] = {origins[3 * lo + 0], origins[3 * lo + 1], origins[3 * lo + 2]};
+  const double d[3] = {__dsub_rn(p[0], o[0]), __dsub_rn(p[1], o[1]), __dsub_rn(p[2], o[2])};
+  const double L2 = __dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2]));
+  if (!(L2 > 0.0 && L2 <= DBL_MAX)) return;  // zero-length or overflowing ray
+  const double L = __dsqrt_rn(L2);
+  const double Lm = __dsub_rn(L, margin);
+  if (!(Lm > 0.0)) return;  // s > 0 and s < L - margin cannot both hold
+
+  const double gn[3] = {(double)g.nx, (double)g.ny, (double)g.nz}, go[3] = {g.ox, g.oy, g.oz};
+  double A = 0.0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) A = fmax(A, fabs(o[a]) + fabs(p[a]) + fabs(go[a]) + gn[a] * g.h);
+  const double slack = 1e-12 * A + 1e-300;
+  const double R = r + 1e-6 * (L + r) + slack;
+  // 1. clip S (t in [0, Lm / L]) to the grid's box grown by R
+  double t0 = 0.0, t1 = fmin(1.0, Lm / L);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double blo = go[a] - R, bhi = go[a] + gn[a] * g.h + R;
+    if (d[a] == 0.0) {
+      if (o[a] < blo || o[a] > bhi) return;
+    } else {
+      const double ta = (blo - o[a]) / d[a], tb = (bhi - o[a]) / d[a];
+      t0 = fmax(t0, fmin(ta, tb));
+      t1 = fmin(t1, fmax(ta, tb));
+    }
+  }
+  if (!(t0 <= t1)) return;  // the ray misses the grown box
+  // 2. layers on the major axis (selected without indexing the arrays, which stay in registers)
+  const int a = (fabs(d[1]) > fabs(d[0])) ? ((fabs(d[2]) > fabs(d[1])) ? 2 : 1) : ((fabs(d[2]) > fabs(d[0])) ? 2 : 0);
+  const int gi[3] = {g.nx, g.ny, g.nz};
+  const double oa = (a == 0) ? o[0] : ((a == 1) ? o[1] : o[2]);
+  const double da = (a == 0) ? d[0] : ((a == 1) ? d[1] : d[2]);
+  const double goa = (a == 0) ? go[0] : ((a == 1) ? go[1] : go[2]);
+  const int na = (a == 0) ? gi[0] : ((a == 1) ? gi[1] : gi[2]);
+  const double ida = 1.0 / da;
+  const double sa0 = oa + t0 * da, sa1 = oa + t1 * da;
+  const int i0 = cell_coord(fmin(sa0, sa1) - R, goa, g.inv_h, na);
+  const int i1 = cell_coord(fmax(sa0, sa1) + R, goa, g.inv_h, na);
+  for (int i = i0; i <= i1; ++i) {
+    const double f0 = (i == 0) ? -kInf : goa + i * g.h - slack - R;
+    const double f1 = (i == na - 1) ? kInf : goa + (i + 1) * g.h + slack + R;
+    const double ta = (f0 - oa) * ida, tb = (f1 - oa) * ida;
+    const double tl = fmax(t0, fmin(ta, tb)), th = fmin(t1, fmax(ta, tb));
+    if (!(tl <= th)) continue;
+    int cl[3], ch[3];  // the layer's cell box: [i, i] on axis a, the grown extent of S's part on the others
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const double e0 = o[k] + tl * d[k], e1 = o[k] + th * d[k];
+      cl[k] = (k == a) ? i : cell_coord(fmin(e0, e1) - R, go[k], g.inv_h, gi[k]);
+      ch[k] = (k == a) ? i : cell_coord(fmax(e0, e1) + R, go[k], g.inv_h, gi[k]);
+    }
+    // 3. the layer's cells, as contiguous x-rows
+    for (int z = cl[2]; z <= ch[2]; ++z)
+      for (int y = cl[1]; y <= ch[1]; ++y) {
+        const long long row = ((long long)z * g.ny + y) * g.nx;
+        const uint32_t e = g.cell_start[row + ch[0] + 1];
+        for (uint32_t q = g.cell_start[row + cl[0]]; q < e; ++q) {
+          const Rec m = g.recs[q];
+          const double ux = __dsub_rn(m.x, o[0]), uy = __dsub_rn(m.y, o[1]), uz = __dsub_rn(m.z, o[2]);
+          const double s =
+              __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(ux, d[0]), __dmul_rn(uy, d[1])), __dmul_rn(uz, d[2])), L);
+          if (!(s > 0.0 && s < Lm)) continue;
+          const double e2 = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(ux, ux), __dmul_rn(uy, uy)), __dmul_rn(uz, uz)),
+                                      __dmul_rn(s, s));
+          if (e2 < r2) atomicAdd(&passes[m.idx], 1u);
+        }
+      }
+  }
+}
+
 // ---- sicp_map_distances: the nearest map point of a point, within a bound --------------------
 // MG lanes per point run grid_nn's ring expansion with the rows of each ring dealt over the lanes
 // and reduced after the ring.  guard is the distance from the point to the nearest face behind
@@ -1415,6 +1528,15 @@ void map_insert_flags_launch(Ctx& c, const GridView& map, const GridView& fresh,
 void map_thin_flags_launch(Ctx& c, const GridView& map, const double* xyz, long long n, double voxel, uint32_t* keep) {
   if (n <= 0) return;
   k_map_thin_flags<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(map, xyz, n, voxel, keep);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void map_carve_launch(Ctx& c, const GridView& map, const double* xyz, long long n, const uint32_t* off, int n_clouds,
+                      const double* origins, double r, double r2, double margin, uint32_t* passes) {
+  if (n <= 0) return;
+  k_map_carve<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(map, xyz, n, off, n_clouds, origins, r, r2, margin,
+                                                                 passes);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

@@ -91,5 +91,12 @@ with sb.Map(X_fix[:30_000]) as mp:
         assert err.code == _capi.SICP_ERR_NO_OVERLAP
     t1 = mp.thin(voxel_size=0.1)
     assert c1 > 0 and c2 == 0 and t1 > 0 and mp.n_points == n0 - c1 - t1
+    # map carve: with H and default origins (the NaN point, the empty and odd-offset clouds), and with
+    # explicit origins that remove nothing
+    n1 = mp.n_points
+    org = np.array([[2.0, 2.0, 5.0], [0.0, 0.0, 0.0], [40.0, 60.0, 3.0]])
+    v1 = mp.carve(ins, np.stack([H_true, np.eye(4), H_true]), radius=0.1, margin=0.2)
+    v2, p2 = mp.carve(ins, origins=org, radius=0.3, margin=0.0, min_passes=1000, return_passes=True)
+    assert v2 == 0 and p2.sum() > 0 and mp.n_points == n1 - v1
 print("ok", a.iterations, m.iterations, int(tab[:, 16].sum()), c.iterations, d.iterations, f.iterations, g.iterations, l.iterations,
       float(np.linalg.norm(c.H - H_true)), float(np.linalg.norm(l.T - H_true)))
