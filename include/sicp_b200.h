@@ -285,7 +285,9 @@ int32_t sicp_register(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, 
  * there.
  * n_selected (or NULL) receives the selected fixed points of each pair (sicp_register's value).
  * out[i].status is the sicp_status of pair i (a pair without overlap or without enough
- * correspondences fails alone); the call itself fails only on bad arguments or CUDA errors.     */
+ * correspondences fails alone); the call itself fails only on bad arguments or CUDA errors.
+ * It is sicp_register_pairs over its 2 n_pairs clouds (pair i = clouds 2i and 2i + 1), whose
+ * limits of 2^32 points no input an 80 GB GPU can hold reaches (2^32 points take 103 GB).       */
 typedef struct {
   int32_t status;
   int32_t iterations;
@@ -347,8 +349,10 @@ int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const
  *    mov_neighbors points, sum n over the referenced clouds >= 2^32, or sum over pairs of
  *    n[fix_id[i]] >= 2^32 (the overlap filter's keep flags and their prefix sum are per pair and
  *    32-bit).
- *  - The map (sicp_set_map) is not touched.  sicp_timings: upload_ms is the upload of the clouds,
- *    grid_fix_ms the single grid build, grid_mov_ms 0.
+ *  - The map (sicp_set_map) is not touched.  sicp_timings: upload_ms is the upload of the clouds
+ *    that are fixed in some pair, grid_fix_ms their grid build; the clouds that are only movable
+ *    cross PCIe on a second stream meanwhile, and grid_mov_ms is their grid build (0 without
+ *    them).
  *  - Device memory: the clouds once (24 B per point) and their one grid, plus sicp_register_batch's
  *    per-pair buffers and 4 B of overlap flags per fixed point of each pair.                   */
 int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,

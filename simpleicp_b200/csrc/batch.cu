@@ -6,8 +6,9 @@
 // H100: one match launch has 16 000 threads, one reject/solve launch one block, and the host
 // drives ~30 launches per iteration-loop through a Python thread.  Here every kernel carries a
 // pair dimension instead:
-//   upload        one cudaMemcpyAsync per cloud straight from the caller's (pinned) arrays; the
-//                 movable clouds cross PCIe while the fixed-side work runs
+//   upload        every cloud once into one store (register_pairs): the clouds fixed in some pair
+//                 on the context's stream (upload_to_device), the movable-only ones on the copy
+//                 stream, where they cross PCIe while the fixed-side work runs
 //   grids         segmented counting sort over all clouds of a side (grid.cu: grid_build)
 //   overlap       (max_overlap_distance only) bounded search of every fixed point under its pair's
 //                 prior, one scan + ordered scatter into per-pair survivor lists, one read-back
@@ -27,9 +28,9 @@
 // context (sicp_set_map, MapStore): the fixed side is the map's grid, and the overlap filter only
 // searches the map points inside each scan's box mapped by its prior (map_cull_box, map_filter).
 //
-// sicp_register_pairs runs them too for pairs drawn from one set of clouds: each cloud is
-// uploaded, gridded and (as a movable cloud) given its normals once, whatever number of pairs
-// uses it (register_pairs).
+// sicp_register_pairs runs them for pairs drawn from one set of clouds: each cloud is uploaded,
+// gridded and (as a movable cloud) given its normals once, whatever number of pairs uses it
+// (register_pairs).  sicp_register_batch is register_pairs over its 2 n_pairs clouds.
 //
 // sicp_get_batch_outputs returns what any of these calls left on the device and did not download:
 // transformed clouds, residual vectors, the per-iteration log and the applied transforms.
@@ -145,8 +146,8 @@ __global__ void __launch_bounds__(256)
 // the cell policy of every grid of this file: both sides of a batch, the map and its inserts
 CellPolicy batch_policy(const Ctx& c) { return CellPolicy{CellPolicy::kBatch, c.grid_target_occ}; }
 
-// What the stages shared by sicp_register_batch, sicp_register_to_map and sicp_register_pairs
-// know about one call.
+// What the stages shared by sicp_register_pairs (and through it sicp_register_batch) and
+// sicp_register_to_map know about one call.
 struct PairsRun {
   int n_pairs = 0;
   const sicp_register_params* rp = nullptr;
@@ -155,12 +156,15 @@ struct PairsRun {
   long long Kmax = 0, max_n_mov = 0;
   std::vector<long long> mo;    // prefix sums of the pairs' movable point counts, n_pairs + 1
   std::vector<DevState> hs;     // per-pair start state (the prior)
-  // descriptors; the caller fills gfix, n_fix, fix_off, flag_off and mov_off, and with mov_built
-  // also gmov and cm (the movable grids exist already: run_pairs does not build them)
+  // descriptors; the caller fills gfix, n_fix, fix_off, flag_off and mov_off, and gmov and cm of
+  // the pairs whose movable grid it built (mov_slot[i] < 0)
   std::vector<PairDev> pd;
-  bool mov_built = false;
+  // the movable-only clouds (upload_movable), which run_pairs grids into Batch::gmov once they have
+  // arrived, and each pair's slot in that list (-1: its movable grid is in Batch::gfix)
+  std::vector<HostCloud> mov_clouds;
+  std::vector<int> mov_slot;
   // pairs whose descriptors the movable-normals estimate runs over, one per distinct movable cloud;
-  // empty: every pair's (each owns its movable cloud)
+  // empty or all pairs: every pair's (each has its own movable cloud)
   std::vector<int> mov_first;
   std::vector<char> no_overlap;
 };
@@ -193,23 +197,31 @@ void begin_pairs(PairsRun& r, int n_pairs, const sicp_register_params* rp, const
   r.observed = observed;
   r.overlap = rp->max_overlap_distance > 0 && std::isfinite(rp->max_overlap_distance);
   r.mo.assign((size_t)n_pairs + 1, 0);
+  r.mov_slot.assign((size_t)n_pairs, -1);
+}
+
+void check_movable(const sicp_register_params& rp, int i, int64_t n_mov) {
+  SICP_REQUIRE(n_mov >= rp.mov_neighbors, SICP_ERR_BAD_ARG,
+               "mov_neighbors exceeds the number of points in the movable cloud of pair " + std::to_string(i));
 }
 
 // pair i's movable cloud (checked and counted) and its share of the per-query arrays
 void add_movable(PairsRun& r, int i, int64_t n_mov) {
-  SICP_REQUIRE(n_mov >= r.rp->mov_neighbors, SICP_ERR_BAD_ARG,
-               "mov_neighbors exceeds the number of points in the movable cloud of pair " + std::to_string(i));
+  check_movable(*r.rp, i, n_mov);
   r.max_n_mov = std::max<long long>(r.max_n_mov, n_mov);
   r.mo[(size_t)i + 1] = r.mo[(size_t)i] + n_mov;
 }
 
-// The movable clouds cross PCIe on the copy stream (behind the event the caller recorded on the
-// context's stream after the last use of the buffers); ev_copy marks their arrival.
-void upload_movable(Ctx& c, Batch& b, const PairsRun& r, const double* const* mov_xyz, const int64_t* n_mov) {
-  b.mov_xyz.reserve(3 * (size_t)b.total_mov);
-  for (int i = 0; i < r.n_pairs; ++i)
-    SICP_CUDA(cudaMemcpyAsync(b.mov_xyz.p + 3 * r.mo[(size_t)i], mov_xyz[i], sizeof(double) * 3 * (size_t)n_mov[i],
-                              cudaMemcpyDefault, c.copy_stream));
+// The movable-only clouds xyz[j], j in ids, cross PCIe into the store Batch::xyz at off[j] on the
+// copy stream (behind the event the caller recorded on the context's stream after the last use of
+// the buffers) and join PairsRun::mov_clouds; ev_copy marks their arrival.
+void upload_movable(Ctx& c, Batch& b, PairsRun& r, const std::vector<int>& ids, const double* const* xyz,
+                    const int64_t* n, const std::vector<long long>& off) {
+  for (int j : ids) {
+    double* dst = b.xyz.p + 3 * off[(size_t)j];
+    SICP_CUDA(cudaMemcpyAsync(dst, xyz[j], sizeof(double) * 3 * (size_t)n[j], cudaMemcpyDefault, c.copy_stream));
+    r.mov_clouds.push_back(HostCloud{dst, n[j], off[(size_t)j]});
+  }
   SICP_CUDA(cudaEventRecord(c.ev_copy, c.copy_stream));
 }
 
@@ -398,10 +410,10 @@ static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
   take_survivors(c, b, r, bounds);
 }
 
-// Everything after the fixed side: descriptors, [select + normals], movable grids (unless the
-// caller built them), [overlap filter, select + normals], movable normals, the loop and the
-// results.  fix_xyz holds the fixed coordinates the descriptors' fix_off index; map (or null) is
-// the resident map of sicp_register_to_map, whose filter is the culled one.
+// Everything after the fixed side: descriptors, [select + normals], the grids of the movable-only
+// clouds, [overlap filter, select + normals], movable normals, the loop and the results.  fix_xyz
+// holds the fixed coordinates the descriptors' fix_off index; map (or null) is the resident map of
+// sicp_register_to_map, whose filter is the culled one.
 static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapStore* map, long long max_n_fix,
                       sicp_pair_result* out, int64_t* n_selected) {
   cudaStream_t st = c.stream;
@@ -429,24 +441,22 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
     select_and_normals();
   }
 
-  // ---- movable side
-  if (!r.mov_built) {
+  // ---- movable side: the grids of the movable-only clouds, once they have arrived
+  c.tm.grid_mov_ms = 0;
+  if (!r.mov_clouds.empty()) {
     SICP_CUDA(cudaStreamWaitEvent(st, c.ev_copy, 0));
-    std::vector<HostCloud> clouds((size_t)n_pairs);
     std::vector<GridView> views;
     std::vector<double> centres;
-    for (int i = 0; i < n_pairs; ++i) {
-      const PairDev& d = r.pd[(size_t)i];
-      clouds[(size_t)i] = HostCloud{b.mov_xyz.p + 3 * d.mov_off, d.n_mov, d.mov_off};
-    }
     {
       StageTimer t(c, &c.tm.grid_mov_ms);
-      grid_build(c, b.gmov, clouds, batch_policy(c), views, centres);
+      grid_build(c, b.gmov, r.mov_clouds, batch_policy(c), views, centres);
       t.stop();
     }
     for (int i = 0; i < n_pairs; ++i) {
-      r.pd[(size_t)i].gmov = views[(size_t)i];
-      for (int a = 0; a < 3; ++a) r.pd[(size_t)i].cm[a] = centres[(size_t)i * 3 + a];
+      const int s = r.mov_slot[(size_t)i];
+      if (s < 0) continue;
+      r.pd[(size_t)i].gmov = views[(size_t)s];
+      for (int a = 0; a < 3; ++a) r.pd[(size_t)i].cm[a] = centres[(size_t)s * 3 + a];
     }
   }
   r.no_overlap.assign((size_t)n_pairs, 0);
@@ -466,7 +476,7 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   c.tm.mov_normals_ms = 0;
   if (b.mov_attr) {
     b.q_nrm_eff.reserve((size_t)n_pairs * (size_t)r.Kmax);
-    if (r.mov_first.empty()) {
+    if (r.mov_first.empty() || r.mov_first.size() == (size_t)n_pairs) {
       b.mov_desc = b.pairs.p;
       b.n_mov_desc = n_pairs;
     } else {
@@ -630,62 +640,6 @@ static void get_batch_outputs(Ctx& c, int n_pairs, double* const* mov_xyz_out, d
   }
 }
 
-static void register_batch(Ctx& c, int n_pairs, const double* const* fix_xyz, const int64_t* n_fix,
-                           const double* const* mov_xyz, const int64_t* n_mov,
-                           const sicp_register_params* rp, const double* observed, sicp_pair_result* out,
-                           int64_t* n_selected) {
-  if (c.batch) c.batch->out_valid = false;
-  check_pairs_params(c, n_pairs, fix_xyz && n_fix && mov_xyz && n_mov && out, rp);
-  PairsRun r;
-  begin_pairs(r, n_pairs, rp, observed);
-  std::vector<long long> fo((size_t)n_pairs + 1, 0);
-  long long Kmax = 0, max_n_fix = 0;
-  for (int i = 0; i < n_pairs; ++i) {
-    SICP_REQUIRE(fix_xyz[i] && mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
-    SICP_REQUIRE(n_fix[i] >= rp->neighbors && n_mov[i] >= 1, SICP_ERR_BAD_ARG,
-                 "every fixed cloud needs at least `neighbors` points, every movable cloud one");
-    add_movable(r, i, n_mov[i]);
-    fo[(size_t)i + 1] = fo[(size_t)i] + n_fix[i];
-    Kmax = std::max<long long>(Kmax, std::min<long long>(rp->correspondences, n_fix[i]));
-    max_n_fix = std::max<long long>(max_n_fix, n_fix[i]);
-  }
-  if (!c.batch) c.batch = new Batch();
-  Batch& b = *c.batch;
-  r.Kmax = (Kmax + 1) & ~1ll;  // even: every pair's slice of the per-query arrays starts 16-byte aligned
-  b.total_fix = fo[(size_t)n_pairs];
-  b.total_mov = r.mo[(size_t)n_pairs];
-  cudaStream_t st = c.stream;
-
-  // ---- uploads: fixed clouds on the context's stream, movable ones behind them on the copy stream
-  b.fix_xyz.reserve(3 * (size_t)b.total_fix);
-  SICP_CUDA(cudaEventRecord(c.ev_user, st));
-  SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
-  for (int i = 0; i < n_pairs; ++i)
-    SICP_CUDA(cudaMemcpyAsync(b.fix_xyz.p + 3 * fo[(size_t)i], fix_xyz[i], sizeof(double) * 3 * (size_t)n_fix[i],
-                              cudaMemcpyDefault, st));
-  upload_movable(c, b, r, mov_xyz, n_mov);
-  alloc_pair_buffers(c, b, r);
-  SICP_CUDA(cudaStreamSynchronize(st));  // the fixed clouds have arrived
-
-  // ---- fixed side: grids (the movable clouds are still in flight)
-  std::vector<HostCloud> clouds((size_t)n_pairs);
-  std::vector<GridView> views;
-  std::vector<double> centres;
-  for (int i = 0; i < n_pairs; ++i) clouds[(size_t)i] = HostCloud{b.fix_xyz.p + 3 * fo[(size_t)i], n_fix[i], fo[(size_t)i]};
-  {
-    StageTimer t(c, &c.tm.grid_fix_ms);
-    grid_build(c, b.gfix, clouds, batch_policy(c), views, centres);
-    t.stop();
-  }
-  for (int i = 0; i < n_pairs; ++i) {
-    r.pd[(size_t)i].gfix = views[(size_t)i];
-    r.pd[(size_t)i].n_fix = n_fix[i];
-    r.pd[(size_t)i].fix_off = r.pd[(size_t)i].flag_off = fo[(size_t)i];
-    r.pd[(size_t)i].mov_off = r.mo[(size_t)i];
-  }
-  run_pairs(c, b, r, b.fix_xyz.p, nullptr, max_n_fix, out, n_selected);
-}
-
 static void set_map(Ctx& c, const double* map_xyz, int64_t n_map) {
   if (c.batch) c.batch->out_valid = false;
   if (map_xyz == nullptr || n_map == 0) {
@@ -736,26 +690,29 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
   r.Kmax = (std::min<long long>(rp->correspondences, m.n) + 1) & ~1ll;
   b.total_mov = r.mo[(size_t)n_scans];
   c.tm.overlap_candidates = 0;
+  b.xyz.reserve(3 * (size_t)b.total_mov);
   SICP_CUDA(cudaEventRecord(c.ev_user, c.stream));
   SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
-  upload_movable(c, b, r, mov_xyz, n_mov);
+  std::vector<int> scans((size_t)n_scans);
+  for (int i = 0; i < n_scans; ++i) scans[(size_t)i] = i;
+  upload_movable(c, b, r, scans, mov_xyz, n_mov, r.mo);
   alloc_pair_buffers(c, b, r);
   for (int i = 0; i < n_scans; ++i) {
     r.pd[(size_t)i].gfix = m.view;
     r.pd[(size_t)i].n_fix = m.n;
     r.pd[(size_t)i].fix_off = r.pd[(size_t)i].flag_off = 0;
     r.pd[(size_t)i].mov_off = r.mo[(size_t)i];
+    r.mov_slot[(size_t)i] = i;
   }
   run_pairs(c, b, r, m.xyz.p, &m, m.n, out, n_selected);
 }
 
 // sicp_register_pairs: pair i is (cloud fix_id[i], cloud mov_id[i]).  Every referenced cloud is
-// uploaded once into Batch::mov_xyz, which serves as both sides, and gridded once in Batch::gfix:
-// that grid is its fixed grid and its movable grid (a grid depends only on its own cloud, so it is
-// the one sicp_register_batch builds for it on either side).  The movable normals run once per
-// distinct movable cloud.  Each pair has its own keep flags (flag_off) and its own output slices,
-// so pairs that share a cloud never write into a shared slice.  The rest is run_pairs, as for
-// sicp_register_batch on the expanded pairs.
+// uploaded once into the store Batch::xyz and gridded once: in Batch::gfix if it is fixed in some
+// pair (that grid is also its movable grid), else in Batch::gmov by run_pairs (a grid depends only
+// on its own cloud).  The movable normals run once per distinct movable cloud.  Each pair has its
+// own keep flags (flag_off) and its own output slices, so pairs that share a cloud never write
+// into a shared slice.
 static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_pairs,
                            const int32_t* fix_id, const int32_t* mov_id, const sicp_register_params* rp,
                            const double* observed, sicp_pair_result* out, int64_t* n_selected) {
@@ -770,11 +727,8 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
     role[(size_t)fix_id[i]] |= 1;
     role[(size_t)mov_id[i]] |= 2;
   }
-  // the referenced clouds' offsets in the store; the store, the overlap flags and their prefix
-  // sums are indexed with 32-bit offsets
+  // the store, the overlap flags and their prefix sums are indexed with 32-bit offsets
   constexpr long long k32 = 1ll << 32;
-  std::vector<long long> off((size_t)n_clouds, -1);
-  std::vector<int> ref;
   long long total = 0;
   for (int j = 0; j < n_clouds; ++j) {
     if (!role[(size_t)j]) continue;
@@ -782,9 +736,25 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
     SICP_REQUIRE(n[j] >= 1 && (!(role[(size_t)j] & 1) || n[j] >= rp->neighbors), SICP_ERR_BAD_ARG,
                  "every fixed cloud needs at least `neighbors` points, every movable cloud one");
     SICP_REQUIRE(n[j] < k32 - total, SICP_ERR_BAD_ARG, "the points of the referenced clouds must be below 2^32");
-    off[(size_t)j] = total;
     total += n[j];
-    ref.push_back(j);
+  }
+  // the store holds the movable-only clouds, then the clouds in both roles, then the fixed-only
+  // ones: the movable clouds are its prefix [0, total_mov), the fixed-role ones its suffix from
+  // fix0; slot[j] is cloud j's place in mov_only or in fixed
+  std::vector<long long> off((size_t)n_clouds, -1);
+  std::vector<int> mov_only, fixed, slot((size_t)n_clouds, -1);
+  long long at = 0, fix0 = 0, total_mov = 0;
+  for (int rl : {2, 3, 1}) {
+    if (rl == 3) fix0 = at;
+    if (rl == 1) total_mov = at;
+    for (int j = 0; j < n_clouds; ++j) {
+      if (role[(size_t)j] != rl) continue;
+      off[(size_t)j] = at;
+      at += n[j];
+      std::vector<int>& list = rl == 2 ? mov_only : fixed;
+      slot[(size_t)j] = (int)list.size();
+      list.push_back(j);
+    }
   }
   PairsRun r;
   begin_pairs(r, n_pairs, rp, observed);
@@ -806,27 +776,28 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
   }
   if (!c.batch) c.batch = new Batch();
   Batch& b = *c.batch;
-  r.Kmax = (Kmax + 1) & ~1ll;  // even, as in register_batch
+  r.Kmax = (Kmax + 1) & ~1ll;  // even: every pair's slice of the per-query arrays starts 16-byte aligned
   b.total_fix = fo[(size_t)n_pairs];
-  b.total_mov = total;
+  b.total_mov = total_mov;
 
-  // ---- each referenced cloud crosses PCIe once, on the context's stream, into the store
-  b.mov_xyz.reserve(3 * (size_t)total);
+  // ---- uploads: the fixed-role clouds on the context's stream, the movable-only ones behind them
+  // on the copy stream, where they go on arriving while the fixed side computes
+  b.xyz.reserve(3 * (size_t)total);
+  SICP_CUDA(cudaStreamWaitEvent(c.stream, c.ev_copy, 0));  // copies into the store a failed call left in flight
+  SICP_CUDA(cudaEventRecord(c.ev_user, c.stream));
+  SICP_CUDA(cudaStreamWaitEvent(c.copy_stream, c.ev_user, 0));  // buffers of an earlier call are free
   {
     StageTimer t(c, &c.tm.upload_ms);
-    for (int j : ref)
-      upload_to_device(c, b.mov_xyz.p + 3 * off[(size_t)j], xyz[j], sizeof(double) * 3 * (size_t)n[j]);
-    t.stop();
+    for (int j : fixed)
+      upload_to_device(c, b.xyz.p + 3 * off[(size_t)j], xyz[j], sizeof(double) * 3 * (size_t)n[j]);
+    upload_movable(c, b, r, mov_only, xyz, n, off);
+    alloc_pair_buffers(c, b, r);  // queued while the clouds cross PCIe
+    t.stop();  // the fixed-role clouds have arrived
   }
-  alloc_pair_buffers(c, b, r);
 
-  // ---- one grid per referenced cloud, for both roles
+  // ---- the grids of the fixed-role clouds (the movable-only clouds are still in flight)
   std::vector<HostCloud> clouds;
-  std::vector<int> slot((size_t)n_clouds, -1);
-  for (int j : ref) {
-    slot[(size_t)j] = (int)clouds.size();
-    clouds.push_back(HostCloud{b.mov_xyz.p + 3 * off[(size_t)j], n[j], off[(size_t)j]});
-  }
+  for (int j : fixed) clouds.push_back(HostCloud{b.xyz.p + 3 * off[(size_t)j], n[j], off[(size_t)j] - fix0});
   std::vector<GridView> views;
   std::vector<double> centres;
   {
@@ -834,7 +805,6 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
     grid_build(c, b.gfix, clouds, batch_policy(c), views, centres);
     t.stop();
   }
-  c.tm.grid_mov_ms = 0;
   for (int i = 0; i < n_pairs; ++i) {
     PairDev& d = r.pd[(size_t)i];
     const int f = slot[(size_t)fix_id[i]], m = slot[(size_t)mov_id[i]];
@@ -842,12 +812,41 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
     d.n_fix = n[fix_id[i]];
     d.fix_off = off[(size_t)fix_id[i]];
     d.flag_off = fo[(size_t)i];
-    d.gmov = views[(size_t)m];
     d.mov_off = off[(size_t)mov_id[i]];
+    if (role[(size_t)mov_id[i]] == 2) {
+      r.mov_slot[(size_t)i] = m;
+      continue;
+    }
+    d.gmov = views[(size_t)m];
     for (int a = 0; a < 3; ++a) d.cm[a] = centres[(size_t)m * 3 + a];
   }
-  r.mov_built = true;
-  run_pairs(c, b, r, b.mov_xyz.p, nullptr, max_n_fix, out, n_selected);
+  run_pairs(c, b, r, b.xyz.p, nullptr, max_n_fix, out, n_selected);
+}
+
+// sicp_register_batch: sicp_register_pairs over its 2 n_pairs clouds, pair i = (cloud 2i, cloud
+// 2i + 1).  Its own checks come first, in the order and with the messages they have always had.
+static void batch_to_pairs(Ctx& c, int n_pairs, const double* const* fix_xyz, const int64_t* n_fix,
+                           const double* const* mov_xyz, const int64_t* n_mov, const sicp_register_params* rp,
+                           const double* observed, sicp_pair_result* out, int64_t* n_selected) {
+  if (c.batch) c.batch->out_valid = false;
+  check_pairs_params(c, n_pairs, fix_xyz && n_fix && mov_xyz && n_mov && out, rp);
+  std::vector<const double*> xyz(2 * (size_t)n_pairs);
+  std::vector<int64_t> n(2 * (size_t)n_pairs);
+  std::vector<int32_t> fix_id((size_t)n_pairs), mov_id((size_t)n_pairs);
+  for (int i = 0; i < n_pairs; ++i) {
+    SICP_REQUIRE(fix_xyz[i] && mov_xyz[i], SICP_ERR_BAD_ARG, "cloud pointer is NULL");
+    SICP_REQUIRE(n_fix[i] >= rp->neighbors && n_mov[i] >= 1, SICP_ERR_BAD_ARG,
+                 "every fixed cloud needs at least `neighbors` points, every movable cloud one");
+    check_movable(*rp, i, n_mov[i]);
+    xyz[2 * (size_t)i] = fix_xyz[i];
+    xyz[2 * (size_t)i + 1] = mov_xyz[i];
+    n[2 * (size_t)i] = n_fix[i];
+    n[2 * (size_t)i + 1] = n_mov[i];
+    fix_id[(size_t)i] = 2 * i;
+    mov_id[(size_t)i] = 2 * i + 1;
+  }
+  register_pairs(c, 2 * n_pairs, xyz.data(), n.data(), n_pairs, fix_id.data(), mov_id.data(), rp, observed, out,
+                 n_selected);
 }
 
 // The clouds of sicp_map_insert and sicp_map_distances, checked before any device work: their
@@ -1182,7 +1181,7 @@ extern "C" int32_t sicp_register_batch(sicp_ctx* ctx, int32_t n_pairs, const dou
                                        const int64_t* n_fix, const double* const* mov_xyz,
                                        const int64_t* n_mov, const sicp_register_params* p,
                                        const double* observed, sicp_pair_result* out, int64_t* n_selected) {
-  SICP_BATCH_API(register_batch(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected))
+  SICP_BATCH_API(batch_to_pairs(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected))
 }
 
 extern "C" int32_t sicp_set_map(sicp_ctx* ctx, const double* map_xyz, int64_t n_map) {

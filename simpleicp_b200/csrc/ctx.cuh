@@ -214,8 +214,8 @@ struct PairDev {
   GridView gmov, gfix;
   long long n_fix, n_mov;
   long long fix_off, mov_off;  // first point of this pair's clouds in the concatenated clouds
-  // first overlap keep flag of this pair (Ctx::compact.flag, one per fixed point of the pair): fix_off
-  // when every pair owns its fixed cloud; pairs that share one (sicp_register_pairs) get their own
+  // first overlap keep flag of this pair (Ctx::compact.flag, one per fixed point of the pair): the
+  // fixed points of the pairs before it (0 on the map path, whose filter has its own bit rows)
   long long flag_off;
   long long K;                 // selected fixed points (<= Kmax)
   long long q_off;             // first entry of this pair in the per-query arrays
@@ -228,12 +228,12 @@ struct PairDev {
 
 struct Batch {
   int n_pairs = 0;
-  // total_fix: the fixed points of all pairs (overlap flags); total_mov: the points of mov_xyz;
-  // max_n_mov: the largest movable cloud
+  // total_fix: the fixed points of all pairs (overlap flags); total_mov: the points of the movable
+  // clouds, the prefix of xyz; max_n_mov: the largest movable cloud
   long long Kmax = 0, total_fix = 0, total_mov = 0, max_n_mov = 0;
-  // concatenated clouds; sicp_register_pairs keeps every referenced cloud once in mov_xyz, which
-  // serves as both sides, and grids it once in gfix
-  DevBuf<double> fix_xyz, mov_xyz;
+  // every cloud of the call once (batch.cu: register_pairs); gfix holds the grids of the clouds
+  // fixed in some pair, which serve both roles, gmov those of the movable-only clouds
+  DevBuf<double> xyz;
   GridBufs gfix, gmov;
   DevBuf<PairDev> pairs;
   // the movable-normals estimate runs over n_mov_desc descriptors: the pairs' own (mov_desc =
@@ -413,7 +413,7 @@ void set_state_transform(Ctx& c, const double x[6], const Rigid* T_or_null, bool
 // b == nullptr, the one-pair context: the fixed side (c.gfix, c.q_xyz, c.K -> c.q_nrm, the lists
 // kept under option "keep_knn") or the movable side (c.gmov, c.mov_xyz, c.n_mov -> c.mov_nrm).
 // b != nullptr, a batch: every pair's selected fixed points in its fixed grid (Batch::q_xyz ->
-// Batch::q_nrm) or its movable points in its own movable grid (Batch::mov_xyz -> Batch::mov_nrm).
+// Batch::q_nrm) or its movable points in its own movable grid (Batch::xyz -> Batch::mov_nrm).
 // The movable side is chunked: as many queries per launch as option "normals_scratch_mb" holds at
 // k x 4 bytes of neighbour positions each.
 void normals_launch(Ctx& c, Batch* b, bool movable, int k);
@@ -429,7 +429,7 @@ void gather_queries_launch(Ctx& c);
 
 // batched launches
 // with_list: pick from each pair's survivor list (Batch::ovl_list) instead of its whole cloud;
-// fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::fix_xyz or MapStore::xyz)
+// fix_xyz: the fixed coordinates the descriptors' fix_off index (Batch::xyz or MapStore::xyz)
 void batch_select_gather_launch(Ctx& c, Batch& b, const double* fix_xyz, bool with_list, int round_away);
 void batch_match_launch(Ctx& c, Batch& b, bool warm);
 // PointCloud.select_in_range of every fixed point of every pair under its pair's DevState

@@ -430,7 +430,7 @@ enum class Src {
 struct KnnQueries {
   GridView g;            // One
   const PairDev* pairs;  // PairFix: Batch::pairs; PairMov: Batch::mov_desc
-  const double* q_xyz;   // One: the queries; PairFix: Batch::q_xyz; PairMov: Batch::mov_xyz
+  const double* q_xyz;   // One: the queries; PairFix: Batch::q_xyz; PairMov: Batch::xyz
   float4* out;           // One: n entries; PairFix: Batch::q_nrm; PairMov: Batch::mov_nrm
   long long n;           // One: the queries; PairFix, PairMov: pos rows per pair
   long long q0;          // PairMov: first movable point of the chunk
@@ -581,7 +581,7 @@ void normals_launch(Ctx& c, Batch* b, bool movable, int k) {
       std::min<long long>(b->max_n_mov, std::max<long long>(128, normals_chunk_queries(c, k) / n_desc));
   b->knn_pos.reserve((size_t)n_desc * cq * k);
   b->mov_nrm.reserve(std::max<long long>(b->total_mov, 1));
-  a.q_xyz = b->mov_xyz.p;
+  a.q_xyz = b->xyz.p;
   a.out = b->mov_nrm.p;
   a.n = cq;
   a.pos = b->knn_pos.p;

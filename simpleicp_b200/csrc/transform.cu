@@ -58,7 +58,7 @@ void batch_transform_launch(Ctx& c, Batch& b, const int* ids, int n_ids, const l
                             double* out) {
   const long long blocks = std::max<long long>((max_n_mov + 255) / 256, 1);
   k_transform_pairs<<<dim3((unsigned)blocks, (unsigned)n_ids), 256, 0, c.stream>>>(b.pairs.p, b.state.p, ids, off,
-                                                                                 b.mov_xyz.p, out);
+                                                                                 b.xyz.p, out);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }

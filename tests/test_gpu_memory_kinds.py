@@ -377,6 +377,27 @@ def test_register_batch_mixed_kinds(eng, opts):
     _same_all(_pair_table(eng.register_batch(pairs, 1000, 10, params, **opts)), base, f"batch {opts}")
 
 
+@pytest.mark.parametrize("opts", [dict(), dict(max_overlap_distance=1.0, mov_neighbors=10)], ids=["plain", "filter_mov"])
+def test_register_pairs_movable_only_kinds(eng, opts):
+    """register_pairs on 8 C5 pairs and one more: pair i (i < 8) is (fixed cloud i, movable cloud
+    8 + i), the movable cloud in kind i, so the movable-only clouds, which cross PCIe on the copy
+    stream, take every kind; pair 8 is (fixed cloud 1, fixed cloud 0), so cloud 0 is in both roles
+    and clouds 1-7 are fixed only.  The fixed clouds are pageable."""
+    raw = [synthetic.c5_pair(i)[:2] for i in range(8)]
+    clouds, values = [Xf for Xf, _ in raw], [Xf for Xf, _ in raw]
+    for i, (_, Xm) in enumerate(raw):
+        m, Vm = _cloud(CLOUD_KINDS[i], Xm)
+        clouds.append(m)
+        values.append(Vm)
+    edges = [(i, 8 + i) for i in range(8)] + [(1, 0)]
+    params = eng.run_params(0.3, 1.0, 100, eng.lsq_params(np.zeros(6), np.zeros(6), np.zeros(6), 1.0))
+    _options(eng, threads=0)
+    base = _pair_table(eng.register_pairs([V.copy() for V in values], edges, 1000, 10, params, **opts))
+    _options(eng)
+    assert all(base[f"pair {i} status"] == 0 for i in range(len(edges)))
+    _same_all(_pair_table(eng.register_pairs(clouds, edges, 1000, 10, params, **opts)), base, f"pairs {opts}")
+
+
 _MAP = {}
 
 
