@@ -363,6 +363,47 @@ int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const
                             sicp_pair_result* out /*[h] n_pairs*/,
                             int64_t* n_selected /*[h] n_pairs or NULL*/);
 
+/* ---- many clouds registered JOINTLY (multi-scan ICP, linearised) ---------------------------------
+ * sicp_register_joint estimates one pose T_c (world <- cloud, row-major 4 x 4) per cloud from the
+ * edges (fix_id[e], mov_id[e]): per iteration every edge is matched and rejected as pair
+ * (a, b) of sicp_register_pairs under SICP_VARIANT_LINEARIZED from R_e = T_a^-1 T_b, and ONE least-
+ * squares problem over the kept rows of all edges gives a linearised increment x_c per free cloud;
+ * T_c <- dH(x_c) T_c.  DESIGN.md §6.9 states the rule.
+ *  - Rules: always the linearised ones, whatever the context's "variant" option.  p is read as
+ *    sicp_register_pairs reads it (correspondences, neighbors, max_overlap_distance,
+ *    run.min_planarity, run.min_change, run.max_iterations).
+ *  - Reduction: with two clouds, one edge (0, 1), cloud 0 fixed with T_0 = I and H0[1] = H(x0), the
+ *    result equals sicp_register_pairs' under SICP_VARIANT_LINEARIZED with observed row x0 up to
+ *    rounding.
+ *  - SICP_ERR_BAD_ARG, before any device work: every check of sicp_register_pairs under a
+ *    linearised variant (n_edges in [1, 65535], correspondences <= 4096, zero observation weights,
+ *    ...), mov_neighbors != 0, a self edge, a non-finite H0 entry, no free cloud or more than 256
+ *    free clouds among the referenced ones, or a free cloud whose component of the edge graph holds
+ *    no fixed cloud.  A cloud no edge references is not read (its pointer may be NULL).
+ *  - Outputs: H_out[c] = the final T_c; fixed and unreferenced clouds get H0 (identity for a NULL
+ *    H0) bit for bit.  out[e]: status, the call's iterations and convergence, the edge's last
+ *    n_kept, H = final T_a^-1 T_b, x = the edge's last increment in frame a, mean_res / std_res of
+ *    the final linear-model residuals (two-pass), sigma NaN.  Converged when at an iteration i > 0
+ *    every edge with >= 6 kept rows meets the stop rule.
+ *  - Failures: an edge without overlap under R_e gets SICP_ERR_NO_OVERLAP and takes no part (the
+ *    call returns SICP_ERR_NO_OVERLAP if that leaves a free cloud without a path to a fixed one);
+ *    an edge with < 6 kept rows contributes nothing to that iteration, and reports
+ *    SICP_ERR_TOO_FEW_CORR if that was its last; a joint normal matrix that is not positive
+ *    definite returns SICP_ERR_SINGULAR.  On any error H_out is not written.
+ *  - After SICP_OK, sicp_get_batch_outputs (n_pairs = n_edges) returns per edge cloud b moved by the
+ *    final T_a^-1 T_b, the final linear-model residuals in kept order, the log and T = that
+ *    transform.  The map and the one-pair state are not touched.  sicp_timings: match_ms,
+ *    reject_solve_ms and transform_ms are the loop's match, reject-and-blocks and joint solve +
+ *    update times (device events, summed over the iterations run).                             */
+int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                            const int64_t* n /*[h]*/, int32_t n_edges,
+                            const int32_t* fix_id, const int32_t* mov_id /*[h] n_edges*/,
+                            const int32_t* is_fixed /*[h] n_clouds, nonzero: pose held*/,
+                            const double* H0 /*[h] n_clouds x 16 row-major, or NULL: identity*/,
+                            const sicp_register_params* p,
+                            double* H_out /*[h] n_clouds x 16*/,
+                            sicp_pair_result* out /*[h] n_edges*/, int64_t* n_selected /*[h] or NULL*/);
+
 /* ---- growing the map and reading it back -------------------------------------------------------
  * sicp_map_insert appends to the map, for every voxel of size voxel_size it does not occupy, the
  * first new point that falls into it.  C is the concatenation of the n_clouds clouds in call
@@ -509,18 +550,18 @@ int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const*
                            int64_t* n_within          /*[h] n_clouds, or NULL*/);
 
 /* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
- * sicp_register_batch, sicp_register_to_map and sicp_register_pairs report per pair only the
+ * sicp_register_batch, sicp_register_to_map, sicp_register_pairs and sicp_register_joint report per pair only the
  * record above.  This call returns what else sicp_register returns, for every pair of the LAST
  * successful call of any of them on this context: X_mov_transformed (transform_by_H, pointcloud.py:205-217, as at
  * simpleicp.py:316), the final distance residuals (simpleicp.py:324, 4th return value), the
  * per-iteration records and the applied transform.  Those two calls only leave these on the
  * device; all the work happens here, and they stay readable (any number of times, same bits)
- * until the next sicp_register_batch, sicp_register_to_map, sicp_register_pairs, sicp_set_map,
+ * until the next sicp_register_batch, sicp_register_to_map, sicp_register_pairs, sicp_register_joint, sicp_set_map,
  * sicp_map_insert, sicp_map_crop, sicp_map_thin or sicp_map_carve on the context.
  *  - SICP_ERR_STATE: before any such call, after sicp_set_map, sicp_map_insert, sicp_map_crop,
  *    sicp_map_thin or sicp_map_carve, or after a
- *    batch / map / pairs call that returned an error (each of these clears the outputs on entry;
- *    only a successful return of the first three makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
+ *    batch / map / pairs / joint call that returned an error (each of these clears the outputs on
+ *    entry; only a successful return of the first four makes them valid).  SICP_ERR_BAD_ARG: n_pairs differs from that call's.
  *  - A NULL array skips that output, a NULL entry skips that pair.  Nothing of a pair whose
  *    status was not SICP_OK (SICP_ERR_NO_OVERLAP included) is ever written.
  *  - mov_xyz_out[i]: pair i's movable cloud (n_mov[i] x 3) moved by the transform the run applied,

@@ -20,7 +20,7 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 OBJ = PKG / "_build"
 LIB = PKG / "libsicp_b200.so"
-SOURCES = ["capi.cu", "batch.cu", "grid.cu", "nn.cu", "normals.cu", "reject_solve.cu", "transform.cu", "upload.cu", "io.cpp"]
+SOURCES = ["capi.cu", "batch.cu", "grid.cu", "joint.cu", "nn.cu", "normals.cu", "reject_solve.cu", "transform.cu", "upload.cu", "io.cpp"]
 CLI_SRC = PKG.parent / "cli" / "sicp_cli.cpp"
 CLI_BIN = PKG / "sicp_cli"
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

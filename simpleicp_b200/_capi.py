@@ -41,7 +41,7 @@ SYMBOLS = (
     "sicp_set_normals", "sicp_set_mov_normals", "sicp_get_knn", "sicp_match", "sicp_reject", "sicp_solve",
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
-    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_get_batch_outputs",
+    "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_register_joint", "sicp_get_batch_outputs",
     "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
@@ -169,6 +169,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
                                  C.POINTER(PairResult), vp],
         "sicp_register_pairs": [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i32), C.POINTER(i32),
                                 C.POINTER(RegisterParams), vp, C.POINTER(PairResult), vp],
+        "sicp_register_joint": [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i32), C.POINTER(i32),
+                                C.POINTER(i32), vp, C.POINTER(RegisterParams), vp, C.POINTER(PairResult), vp],
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
@@ -622,6 +624,43 @@ class Engine:
         # an id out of range was refused above
         out.n_mov, out.max_iterations = np.array([counts[j] for j in mov], dtype=np.int64), int(params.max_iterations)
         return out
+
+    def register_joint(self, clouds, edges, fixed, H0, correspondences, neighbors, params: RunParams,
+                       max_overlap_distance: float = -1.0):
+        """sicp_register_joint: one pose per cloud from the edges (n_edges, 2) of (fixed side,
+        movable side) indices into `clouds` (NumPy arrays or CUDA tensors, None for a cloud no edge
+        uses), `fixed` a boolean mask of the clouds whose pose is held, `H0` (n_clouds, 4, 4) or
+        None (identity) the start poses, world <- cloud.  Always the linearised rules; the lsq part
+        of `params` is not read beyond its checks.  Returns (H, out): the final poses (n_clouds, 4,
+        4) and the PairResult array per edge (H = final T_a^-1 T_b), which batch_outputs reads."""
+        ids = np.asarray(edges)
+        if ids.ndim != 2 or ids.shape[1] != 2 or ids.shape[0] < 1 or not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError(f"edges must be integers of shape (n_edges, 2) with n_edges >= 1, got {ids.dtype} "
+                             f"of shape {ids.shape}")
+        if ids.min() < -(1 << 31) or ids.max() >= (1 << 31):
+            raise ValueError("cloud ids must fit in int32")  # the library checks [0, n_clouds)
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        n, m = ids.shape[0], len(clouds)
+        keep = [None if X is None else _as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
+        ptrs = (C.c_void_p * m)(*[_ptr(X) for X in keep])
+        counts = (C.c_int64 * m)(*[0 if X is None else int(X.shape[0]) for X in keep])
+        fix, mov = np.ascontiguousarray(ids[:, 0]), np.ascontiguousarray(ids[:, 1])
+        is_fixed = np.ascontiguousarray(np.asarray(fixed, dtype=bool).reshape(m), dtype=np.int32)
+        if H0 is not None:
+            H0 = np.ascontiguousarray(H0, dtype=np.float64)
+            if H0.shape != (m, 4, 4):
+                raise ValueError(f"H0 must have shape ({m}, 4, 4), got {H0.shape}")
+        rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, 0, -1.0)
+        H = np.zeros((m, 4, 4))
+        out = (PairResult * n)()
+        n_selected = np.zeros(n, dtype=np.int64)
+        i32p = C.POINTER(C.c_int32)
+        self._check(self._lib.sicp_register_joint(
+            self._h, m, ptrs, counts, n, fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p),
+            is_fixed.ctypes.data_as(i32p), _ptr(H0), C.byref(rp), _ptr(H), out, _ptr(n_selected)))
+        out.n_selected = n_selected
+        out.n_mov, out.max_iterations = np.array([counts[j] for j in mov], dtype=np.int64), int(params.max_iterations)
+        return H, out
 
     def map_insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
         """sicp_map_insert: append to the resident map, per voxel of `voxel_size` it does not

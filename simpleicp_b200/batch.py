@@ -290,6 +290,119 @@ def simpleicp_edges(clouds: Sequence, edges, *, rank: int = 0, world_size: int =
     return _gather_share(local, found, mine, n, rank, world_size, dist, device, on_error, full_output, messages)
 
 
+# run() arguments simpleicp_joint serves (sicp_register_joint, always the linearised rules)
+_JOINT_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations", "max_overlap_distance"}
+
+
+class JointResult:
+    """simpleicp_joint's return value: H (n_clouds, 4, 4) final poses, world <- cloud; table the
+    (n_edges, 20) record table of simpleicp_edges with H = the final T_a^-1 T_b of each edge;
+    iterations and converged of the call; results (full_output) the per-edge result objects."""
+
+    def __init__(self, H, table, iterations, converged, results=None):
+        self.H, self.table, self.iterations, self.converged, self.results = H, table, iterations, converged, results
+
+
+def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
+                    full_output: bool = False, **run_kwargs) -> JointResult:
+    """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
+    (a, b) of `edges` -- scan-to-scan pairs such as (i, i + 1), (i, i + 2) and loop closures -- is
+    registered consistently.  Each iteration matches every edge as simpleicp_edges would under the
+    linearised rules (median / MAD of all distances, sigma = 1.4826 MAD, point-to-plane rows of the
+    C++ driver) and solves ONE least-squares problem for the increments of all free clouds; the
+    clouds listed in `fixed` (indices, at least one) hold their pose.  `H0` (n_clouds, 4, 4) are
+    the start poses (None: identity), world <- cloud.
+
+    The run() arguments served are correspondences (<= 4096), neighbors, min_planarity,
+    min_change, max_iterations and max_overlap_distance; anything else is a TypeError.  Every free
+    cloud an edge references must be connected to a fixed cloud through the edges, and there may be
+    at most 256 of them.  A cloud no edge references may be None; it keeps its H0.  One library call
+    on one device (sicp_register_joint).  `on_error` and `full_output` are as in simpleicp_edges:
+    an edge that failed (no overlap, too few correspondences) has its status in the table and raises
+    BatchError under "raise"; a failure of the whole call (SICP_ERR_SINGULAR, or a free cloud left
+    without a path to a fixed one by the edges without overlap) raises SicpError."""
+    from . import _capi
+
+    unknown = set(run_kwargs) - _JOINT_KEYS
+    if unknown:
+        raise TypeError(f"simpleicp_joint() got unsupported arguments {sorted(unknown)}")
+    if int(run_kwargs.get("correspondences", 1000)) > 4096:
+        raise ValueError("simpleicp_joint runs one block per edge: correspondences must be <= 4096")
+    n_clouds = len(clouds)
+    e = _check_edges(edges, n_clouds)
+    if e.shape[0] < 1:
+        raise ValueError("simpleicp_joint needs at least one edge")
+    if np.any(e[:, 0] == e[:, 1]):
+        raise ValueError(f"edges must not be self edges: edge {int(np.flatnonzero(e[:, 0] == e[:, 1])[0])}")
+    fx = np.asarray(fixed)
+    if fx.ndim != 1 or fx.size < 1 or not np.issubdtype(fx.dtype, np.integer):
+        raise ValueError("fixed must be a sequence of at least one integer cloud index")
+    if fx.min() < 0 or fx.max() >= n_clouds:
+        raise ValueError(f"fixed must index the {n_clouds} clouds")
+    is_fixed = np.zeros(n_clouds, dtype=bool)
+    is_fixed[fx] = True
+    if H0 is not None:
+        H0 = np.asarray(H0, dtype=np.float64)
+        if H0.shape != (n_clouds, 4, 4):
+            raise ValueError(f"H0 must have shape ({n_clouds}, 4, 4), got {H0.shape}")
+        if not np.isfinite(H0).all():
+            raise ValueError("H0 must be finite")
+    used = np.zeros(n_clouds, dtype=bool)
+    used[e.ravel()] = True
+    free = used & ~is_fixed
+    if not 1 <= int(free.sum()) <= 256:
+        raise ValueError(f"the edges must reference between 1 and 256 free clouds, got {int(free.sum())}")
+    up = list(range(n_clouds))
+
+    def root(i):
+        while up[i] != i:
+            up[i] = up[up[i]]
+            i = up[i]
+        return i
+
+    for a, b in e:
+        up[root(int(a))] = root(int(b))
+    anchored = {root(i) for i in np.flatnonzero(is_fixed)}
+    lost = [i for i in np.flatnonzero(free) if root(int(i)) not in anchored]
+    if lost:
+        raise ValueError(f"free cloud {int(lost[0])} has no path to a fixed cloud over the edges")
+    for i in np.flatnonzero(used):
+        if clouds[i] is None:
+            raise ValueError(f"cloud {int(i)} is referenced by an edge but is None")
+    import torch
+
+    with torch.cuda.device(device):
+        eng = _BATCH_ENGINES.get(int(device))
+        if eng is None or not eng.alive:
+            eng = _BATCH_ENGINES[int(device)] = _capi.Engine(int(device))
+        lsq = eng.lsq_params((0.0,) * 6, (0.0,) * 6, [0.0] * 6, 1)
+        params = eng.run_params(run_kwargs.get("min_planarity", 0.3), run_kwargs.get("min_change", 1.0),
+                                run_kwargs.get("max_iterations", 100), lsq)
+        mod = float(run_kwargs.get("max_overlap_distance", np.inf))
+        H, res = eng.register_joint(list(clouds), e, is_fixed, H0, run_kwargs.get("correspondences", 1000),
+                                    run_kwargs.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0)
+        n = e.shape[0]
+        table = np.zeros((n, RECORD_LEN))
+        messages: List[str] = []
+        for j, r in enumerate(res):
+            if r.status == 0:
+                table[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)
+            else:
+                messages.append(f"edge {j}: library status {r.status}")
+                table[j] = pack_record(np.full((4, 4), np.nan), -int(r.status), 0, np.nan, np.nan)
+        results = None
+        if full_output:
+            results = [None if o is None else _batch_result(r, o, np.zeros(6), (0.0,) * 6)
+                       for r, o in zip(res, eng.batch_outputs(res))]
+    ok = [r for r in res if r.status == 0]
+    out = JointResult(H, table, max((int(r.iterations) for r in ok), default=0),
+                      bool(ok) and all(bool(r.converged) for r in ok), results)
+    failed = np.flatnonzero(table[:, 16] < 0)
+    if failed.size and on_error == "raise":
+        raise BatchError(table, failed, messages, results)
+    return out
+
+
 def _check_edges(edges, n_clouds: int) -> np.ndarray:
     """edges as an (n_edges, 2) int64 array of indices into n_clouds clouds, or ValueError."""
     e = np.asarray(edges)

@@ -44,6 +44,8 @@
 
 namespace sicp {
 
+struct JointRun;
+
 namespace {
 
 __global__ void k_gather_flags(const DevState* __restrict__ st, int n, int* __restrict__ flags) {
@@ -167,6 +169,10 @@ struct PairsRun {
   // empty or all pairs: every pair's (each has its own movable cloud)
   std::vector<int> mov_first;
   std::vector<char> no_overlap;
+  // sicp_register_joint: each pair's start transform (instead of rigid_from_x of its x0), and the
+  // joint problem whose loop replaces the per-pair one
+  const Rigid* prior = nullptr;
+  JointRun* joint = nullptr;
 };
 
 // Argument checks of both entry points that need no cloud (the clouds are checked per pair by
@@ -265,7 +271,7 @@ void alloc_pair_buffers(Ctx& c, Batch& b, PairsRun& r) {
     DevState& h = r.hs[(size_t)i];
     std::memset(&h, 0, sizeof(h));
     for (int j = 0; j < 6; ++j) h.x[j] = r.observed ? r.observed[6 * i + j] : p.lsq.x0[j];
-    h.T = rigid_from_x(h.x);
+    h.T = r.prior ? r.prior[i] : rigid_from_x(h.x);
     h.Tinv = rigid_inverse(h.T);
     h.T_res = h.T;
     h.H_rep = h.T;
@@ -410,6 +416,185 @@ static void map_filter(Ctx& c, Batch& b, MapStore& m, PairsRun& r) {
   take_survivors(c, b, r, bounds);
 }
 
+// What sicp_register_joint knows of its problem on the host: the edges, every cloud's pose and
+// role, and (after the loop) the final poses.
+struct JointRun {
+  int n_clouds = 0, n_edges = 0, F = 0;
+  const int32_t* fix_id = nullptr;
+  const int32_t* mov_id = nullptr;
+  std::vector<char> fixed;      // per cloud: pose held
+  std::vector<Rigid> pose;      // per cloud, world <- cloud
+  std::vector<Rigid> prior;     // per edge: T_a^-1 T_b
+  std::vector<int> free_of, free_ids;
+};
+
+// Union-find of the clouds over the edges with use[e] != 0; SICP_REQUIRE fails with `code` when a
+// cloud some edge references shares its component with no fixed cloud.
+static void check_anchored(const JointRun& j, const std::vector<char>& use, int code, const char* msg) {
+  std::vector<int> up((size_t)j.n_clouds);
+  for (int i = 0; i < j.n_clouds; ++i) up[(size_t)i] = i;
+  auto root = [&](int i) {
+    while (up[(size_t)i] != i) i = up[(size_t)i] = up[(size_t)up[(size_t)i]];
+    return i;
+  };
+  for (int e = 0; e < j.n_edges; ++e)
+    if (use[(size_t)e]) up[(size_t)root(j.fix_id[e])] = root(j.mov_id[e]);
+  std::vector<char> anchored((size_t)j.n_clouds, 0);
+  for (int i = 0; i < j.n_clouds; ++i)
+    if (j.fixed[(size_t)i]) anchored[(size_t)root(i)] = 1;
+  for (int e = 0; e < j.n_edges; ++e)
+    for (int k = 0; k < 2; ++k) {
+      const int cl = k ? j.mov_id[e] : j.fix_id[e];
+      SICP_REQUIRE(anchored[(size_t)root(cl)], code, std::string(msg) + " (cloud " + std::to_string(cl) + ")");
+    }
+}
+
+// The loop of sicp_register_joint, in place of run_pairs' per-pair loop: per iteration the match of
+// every edge, k_joint_reject and k_joint_solve (joint.cu), and the read of the stop flag every
+// host_sync_every iterations.  The edges without overlap (parked by the filter) take no part.
+static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
+  JointRun& j = *r.joint;
+  cudaStream_t st = c.stream;
+  const int n_edges = r.n_pairs;
+  std::vector<char> live((size_t)n_edges);
+  for (int e = 0; e < n_edges; ++e) live[(size_t)e] = !r.no_overlap[(size_t)e];
+  check_anchored(j, live, SICP_ERR_NO_OVERLAP, "a free cloud has no path to a fixed cloud over edges with overlap");
+  // the common centre: the box centre of the first live edge's movable cloud, in the world
+  int e0 = 0;
+  while (!live[(size_t)e0]) ++e0;
+  double cw[3];
+  const double* cm = r.pd[(size_t)e0].cm;
+  rigid_apply(j.pose[(size_t)j.mov_id[e0]], cm[0], cm[1], cm[2], cw[0], cw[1], cw[2]);
+  // the lower blocks every live edge touches, its edges in ascending order
+  const int F = j.F;
+  std::vector<std::vector<int>> lists;
+  std::vector<int> blk_of((size_t)F * F, -1);
+  auto add = [&](int p, int q, int v) {
+    int& bi = blk_of[(size_t)p * F + q];
+    if (bi < 0) {
+      bi = (int)lists.size();
+      lists.emplace_back();
+    }
+    lists[(size_t)bi].push_back(v);
+  };
+  for (int e = 0; e < n_edges; ++e) {
+    if (!live[(size_t)e]) continue;
+    const int fa = j.free_of[(size_t)j.fix_id[e]], fb = j.free_of[(size_t)j.mov_id[e]];
+    if (fa >= 0) add(fa, fa, 2 * e + 1);
+    if (fb >= 0) add(fb, fb, 2 * e);
+    if (fa >= 0 && fb >= 0) add(std::max(fa, fb), std::min(fa, fb), 2 * e);
+  }
+  std::vector<int> ids;
+  ids.insert(ids.end(), j.fix_id, j.fix_id + n_edges);
+  ids.insert(ids.end(), j.mov_id, j.mov_id + n_edges);
+  ids.insert(ids.end(), j.free_of.begin(), j.free_of.end());
+  ids.insert(ids.end(), j.free_ids.begin(), j.free_ids.end());
+  ids.insert(ids.end(), blk_of.begin(), blk_of.end());
+  const size_t o_off = ids.size();
+  int at = 0;
+  for (const auto& l : lists) {
+    ids.push_back(at);
+    at += (int)l.size();
+  }
+  ids.push_back(at);
+  const size_t o_edge = ids.size();
+  for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+
+  JointStore& js = b.joint;
+  const int npad = (6 * F + 1 + 31) / 32 * 32;
+  js.edges.reserve(n_edges);
+  js.flags.reserve(1);
+  js.pose.reserve(j.n_clouds);
+  js.ids.reserve(ids.size());
+  js.A.reserve((size_t)npad * npad);
+  js.bar.reserve(2);
+  if (!js.flags_host) SICP_CUDA(cudaMallocHost(&js.flags_host, sizeof(JointFlags)));
+  SICP_CUDA(cudaMemsetAsync(js.edges.p, 0, sizeof(JointEdge) * (size_t)n_edges, st));
+  SICP_CUDA(cudaMemsetAsync(js.flags.p, 0, sizeof(JointFlags), st));
+  SICP_CUDA(cudaMemsetAsync(js.bar.p, 0, 2 * sizeof(unsigned int), st));
+  SICP_CUDA(cudaMemcpyAsync(js.pose.p, j.pose.data(), sizeof(Rigid) * j.pose.size(), cudaMemcpyHostToDevice, st));
+  SICP_CUDA(cudaMemcpyAsync(js.ids.p, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, st));
+
+  const sicp_run_params& p = r.rp->run;
+  JointArgs a{};
+  a.pairs = b.pairs.p;
+  a.state = b.state.p;
+  a.edges = js.edges.p;
+  a.flags = js.flags.p;
+  a.dist = b.dist.p;
+  a.q_nrm = b.q_nrm.p;
+  a.m_xyz = b.m_xyz.p;
+  a.keep = b.keep.p;
+  a.rec = b.rec.p;
+  a.rec_stride = p.max_iterations;
+  a.pose = js.pose.p;
+  a.fix_id = js.ids.p;
+  a.mov_id = js.ids.p + n_edges;
+  a.free_of = js.ids.p + 2 * n_edges;
+  a.free_ids = a.free_of + j.n_clouds;
+  a.blk_of = a.free_ids + F;
+  a.blk_off = js.ids.p + o_off;
+  a.blk_edge = js.ids.p + o_edge;
+  a.F = F;
+  a.n_edges = n_edges;
+  a.npad = npad;
+  a.A = js.A.p;
+  a.bar = js.bar.p;
+  for (int k = 0; k < 3; ++k) a.cw[k] = cw[k];
+  a.min_planarity = p.min_planarity;
+  a.min_change = p.min_change;
+
+  // device events around the three stages of the iterations queued since the last host read (match,
+  // reject + blocks, solve + update: sicp_timings), read at each host read.  The host reads at
+  // iteration 1 and then every `every` iterations, so every + 1 sets suffice; they are created once
+  // per call and destroyed on every way out.
+  struct Events {
+    std::vector<cudaEvent_t> ev;
+    ~Events() {
+      for (cudaEvent_t e : ev)
+        if (e) cudaEventDestroy(e);
+    }
+  } evs;
+  const int every = std::max(1, c.host_sync_every);
+  evs.ev.assign(4 * (size_t)(every + 1), nullptr);
+  for (cudaEvent_t& e : evs.ev) SICP_CUDA(cudaEventCreate(&e));
+  int queued = 0;
+  double t3[3] = {0, 0, 0};
+  int next_sync = 1;
+  for (int it = 0; it < p.max_iterations; ++it) {
+    a.it = it;
+    a.last = it + 1 == p.max_iterations;
+    cudaEvent_t* e = evs.ev.data() + 4 * queued++;
+    SICP_CUDA(cudaEventRecord(e[0], st));
+    batch_match_launch(c, b, c.warm_start && it > 0);
+    SICP_CUDA(cudaEventRecord(e[1], st));
+    joint_reject_launch(c, a, n_edges);
+    SICP_CUDA(cudaEventRecord(e[2], st));
+    joint_solve_launch(c, a);
+    SICP_CUDA(cudaEventRecord(e[3], st));
+    if (it >= next_sync || a.last) {
+      next_sync = it + every;
+      SICP_CUDA(cudaMemcpyAsync(js.flags_host, js.flags.p, sizeof(JointFlags), cudaMemcpyDeviceToHost, st));
+      SICP_CUDA(cudaStreamSynchronize(st));
+      for (int q = 0; q < queued; ++q)
+        for (int k = 0; k < 3; ++k) {
+          float ms = 0;
+          SICP_CUDA(cudaEventElapsedTime(&ms, evs.ev[4 * (size_t)q + k], evs.ev[4 * (size_t)q + k + 1]));
+          t3[k] += ms;
+        }
+      queued = 0;
+      if (js.flags_host->done) break;
+    }
+  }
+  c.tm.match_ms = t3[0];
+  c.tm.reject_solve_ms = t3[1];
+  c.tm.transform_ms = t3[2];
+  SICP_REQUIRE(!js.flags_host->singular, SICP_ERR_SINGULAR,
+               "the joint normal matrix is not positive definite (a free cloud is not constrained in all six "
+               "degrees of freedom)");
+  SICP_CUDA(cudaMemcpy(j.pose.data(), js.pose.p, sizeof(Rigid) * j.pose.size(), cudaMemcpyDeviceToHost));
+}
+
 // Everything after the fixed side: descriptors, [select + normals], the grids of the movable-only
 // clouds, [overlap filter, select + normals], movable normals, the loop and the results.  fix_xyz
 // holds the fixed coordinates the descriptors' fix_off index; map (or null) is the resident map of
@@ -500,7 +685,8 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   SICP_CUDA(cudaEventRecord(e0, st));
   const int every = std::max(1, c.host_sync_every);
   int next_sync = 1;
-  for (int it = 0; it < p.max_iterations; ++it) {
+  if (r.joint) joint_loop(c, b, r);
+  for (int it = 0; !r.joint && it < p.max_iterations; ++it) {
     batch_match_launch(c, b, c.warm_start && it > 0);
     batch_rs_launch(c, b, p, it, it + 1 == p.max_iterations);
     if (it >= next_sync || it + 1 == p.max_iterations) {
@@ -527,7 +713,7 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   cudaEventElapsedTime(&ms, e0, e1);
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  c.tm.reject_solve_ms = ms;
+  if (!r.joint) c.tm.reject_solve_ms = ms;
   std::memcpy(out, b.results_host, sizeof(sicp_pair_result) * (size_t)n_pairs);
   for (int i = 0; i < n_pairs; ++i) {
     if (r.no_overlap[(size_t)i]) out[i].status = SICP_ERR_NO_OVERLAP;
@@ -715,7 +901,8 @@ static void register_to_map(Ctx& c, int n_scans, const double* const* mov_xyz, c
 // into a shared slice.
 static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_pairs,
                            const int32_t* fix_id, const int32_t* mov_id, const sicp_register_params* rp,
-                           const double* observed, sicp_pair_result* out, int64_t* n_selected) {
+                           const double* observed, sicp_pair_result* out, int64_t* n_selected,
+                           JointRun* joint = nullptr) {
   if (c.batch) c.batch->out_valid = false;
   check_pairs_params(c, n_pairs, xyz && n && fix_id && mov_id && out, rp);
   SICP_REQUIRE(n_clouds >= 1, SICP_ERR_BAD_ARG, "n_clouds must be >= 1");
@@ -758,6 +945,10 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
   }
   PairsRun r;
   begin_pairs(r, n_pairs, rp, observed);
+  if (joint) {
+    r.joint = joint;
+    r.prior = joint->prior.data();
+  }
   std::vector<long long> fo((size_t)n_pairs + 1, 0);  // the pairs' flag offsets
   std::vector<char> seen((size_t)n_clouds, 0);
   long long Kmax = 0, max_n_fix = 0;
@@ -821,6 +1012,68 @@ static void register_pairs(Ctx& c, int n_clouds, const double* const* xyz, const
     for (int a = 0; a < 3; ++a) d.cm[a] = centres[(size_t)m * 3 + a];
   }
   run_pairs(c, b, r, b.xyz.p, nullptr, max_n_fix, out, n_selected);
+}
+
+// The variant of the context for the length of one call.
+struct VariantScope {
+  Ctx& c;
+  int saved;
+  VariantScope(Ctx& c_, int v) : c(c_), saved(c_.variant) { c.variant = v; }
+  ~VariantScope() { c.variant = saved; }
+};
+
+// sicp_register_joint: sicp_register_pairs' stages under the linearised rules, edge e = pair
+// (fix_id[e], mov_id[e]) starting from T_a^-1 T_b, with joint_loop in place of the per-pair loop.
+static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_edges,
+                           const int32_t* fix_id, const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
+                           const sicp_register_params* rp, double* H_out, sicp_pair_result* out,
+                           int64_t* n_selected) {
+  if (c.batch) c.batch->out_valid = false;
+  VariantScope linearised(c, SICP_VARIANT_LINEARIZED);
+  check_pairs_params(c, n_edges, xyz && n && fix_id && mov_id && is_fixed && H_out && out, rp);
+  SICP_REQUIRE(rp->mov_neighbors == 0, SICP_ERR_BAD_ARG, "the joint registration has no movable-side normals");
+  SICP_REQUIRE(n_clouds >= 1, SICP_ERR_BAD_ARG, "n_clouds must be >= 1");
+  JointRun j;
+  j.n_clouds = n_clouds;
+  j.n_edges = n_edges;
+  j.fix_id = fix_id;
+  j.mov_id = mov_id;
+  std::vector<char> used((size_t)n_clouds, 0);
+  for (int e = 0; e < n_edges; ++e) {
+    SICP_REQUIRE(fix_id[e] >= 0 && fix_id[e] < n_clouds && mov_id[e] >= 0 && mov_id[e] < n_clouds,
+                 SICP_ERR_BAD_ARG, "edge " + std::to_string(e) + ": cloud ids must be in [0, n_clouds)");
+    SICP_REQUIRE(fix_id[e] != mov_id[e], SICP_ERR_BAD_ARG, "edge " + std::to_string(e) + " is a self edge");
+    used[(size_t)fix_id[e]] = used[(size_t)mov_id[e]] = 1;
+  }
+  if (H0)
+    for (long long k = 0; k < 16ll * n_clouds; ++k)
+      SICP_REQUIRE(std::isfinite(H0[k]), SICP_ERR_BAD_ARG, "H0 has non-finite entries");
+  j.fixed.assign((size_t)n_clouds, 0);
+  j.free_of.assign((size_t)n_clouds, -1);
+  j.pose.resize((size_t)n_clouds);
+  const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  for (int i = 0; i < n_clouds; ++i) {
+    j.fixed[(size_t)i] = is_fixed[i] != 0;
+    j.pose[(size_t)i] = rigid_from_H(H0 ? H0 + 16 * (size_t)i : I);
+    if (used[(size_t)i] && !j.fixed[(size_t)i]) {
+      j.free_of[(size_t)i] = (int)j.free_ids.size();
+      j.free_ids.push_back(i);
+    }
+  }
+  j.F = (int)j.free_ids.size();
+  SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_MAX_FREE, SICP_ERR_BAD_ARG,
+               "the edges must reference between 1 and 256 free clouds (got " + std::to_string(j.F) + ")");
+  check_anchored(j, std::vector<char>((size_t)n_edges, 1), SICP_ERR_BAD_ARG,
+                 "a free cloud is in a component of the edge graph without a fixed cloud");
+  j.prior.resize((size_t)n_edges);
+  for (int e = 0; e < n_edges; ++e)
+    j.prior[(size_t)e] = rigid_compose(rigid_inverse(j.pose[(size_t)fix_id[e]]), j.pose[(size_t)mov_id[e]]);
+  register_pairs(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, rp, nullptr, out, n_selected, &j);
+  for (int i = 0; i < n_clouds; ++i) {
+    double* dst = H_out + 16 * (size_t)i;
+    if (j.free_of[(size_t)i] >= 0) H_from_rigid(j.pose[(size_t)i], dst);
+    else std::memcpy(dst, H0 ? H0 + 16 * (size_t)i : I, sizeof(double) * 16);
+  }
 }
 
 // sicp_register_batch: sicp_register_pairs over its 2 n_pairs clouds, pair i = (cloud 2i, cloud
@@ -1199,6 +1452,13 @@ extern "C" int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const do
                                        const sicp_register_params* p, const double* observed, sicp_pair_result* out,
                                        int64_t* n_selected) {
   SICP_BATCH_API(register_pairs(c, n_clouds, xyz, n, n_pairs, fix_id, mov_id, p, observed, out, n_selected))
+}
+
+extern "C" int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                       int32_t n_edges, const int32_t* fix_id, const int32_t* mov_id,
+                                       const int32_t* is_fixed, const double* H0, const sicp_register_params* p,
+                                       double* H_out, sicp_pair_result* out, int64_t* n_selected) {
+  SICP_BATCH_API(register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, p, H_out, out, n_selected))
 }
 
 extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

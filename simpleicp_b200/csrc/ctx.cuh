@@ -226,6 +226,70 @@ struct PairDev {
   double obs[6];               // rbp_observed_values of this pair (radians)
 };
 
+// ---- sicp_register_joint (joint.cu): one edge of the joint problem per pair of the batch ----
+constexpr int JE_NSUM = 36;  // N (21, packed lower), sum a d (6), sum a (6), sum d, sum d^2, count
+constexpr int JOINT_MAX_FREE = 256;
+constexpr int JOINT_MAX_PAD = 1568;  // 6 JOINT_MAX_FREE + 1 rounded up to the 32-wide tiles
+// What k_joint_reject leaves of edge e = (a, b) for the solve and the update: the sums of its
+// kept rows a = [w x n, n] (centred about c_f in frame a), its world block Nw = Ad^T N Ad and
+// right-hand side gw = -Ad^T h, and Ad's inputs (cloud a's rotation, v = T_a c_f - c_w).
+struct JointEdge {
+  double N[21], h[6], s[6], sd, sd2;
+  double Nw[36], gw[6];
+  double Ra[9], v[3], cf[3];
+  long long n;
+  int part;  // >= 6 kept rows this iteration: the edge enters the joint system
+  int pad;
+};
+struct JointFlags {
+  int done;       // converged, last iteration or singular: every later queued kernel returns
+  int converged;
+  int singular;
+  int pad;
+};
+struct JointArgs {
+  const PairDev* pairs;
+  DevState* state;  // per edge: R_e = T_a^-1 T_b in T / Tinv, the record state
+  JointEdge* edges;
+  JointFlags* flags;
+  const double* dist;
+  const float4* q_nrm;
+  const double* m_xyz;
+  uint8_t* keep;
+  sicp_iter_record* rec;  // n_edges x rec_stride
+  int rec_stride;
+  int it, last;
+  Rigid* pose;             // per cloud, world <- cloud
+  const int* fix_id;       // per edge: cloud a
+  const int* mov_id;       // per edge: cloud b
+  const int* free_of;      // per cloud: index among the free clouds, -1
+  const int* free_ids;     // per free cloud: its cloud
+  // lower blocks (p >= q) of the joint matrix that some edge touches: blk_of[p F + q] indexes
+  // blk_off; blk_edge[blk_off[b] ..] lists its edges ascending as 2 e + (1: cloud p is the edge's a)
+  const int* blk_of;
+  const int* blk_off;
+  const int* blk_edge;
+  int F, n_edges, npad;
+  double* A;               // npad x npad, row-major, the lower triangle is used
+  unsigned int* bar;       // grid barrier of k_joint_solve, {0, any} between launches
+  double cw[3];            // the common world centre of the increments
+  double min_planarity, min_change;
+};
+struct JointStore {
+  DevBuf<JointEdge> edges;
+  DevBuf<JointFlags> flags;
+  DevBuf<Rigid> pose;
+  DevBuf<int> ids;  // fix_id, mov_id, free_of, free_ids, blk_of, blk_off, blk_edge
+  DevBuf<double> A;
+  DevBuf<unsigned int> bar;
+  JointFlags* flags_host = nullptr;  // pinned
+  ~JointStore() {
+    if (flags_host) cudaFreeHost(flags_host);
+  }
+};
+void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges);
+void joint_solve_launch(Ctx& c, const JointArgs& a);
+
 struct Batch {
   int n_pairs = 0;
   // total_fix: the fixed points of all pairs (overlap flags); total_mov: the points of the movable
@@ -287,6 +351,7 @@ struct Batch {
   size_t rec_cap = 0;
   Rigid* T_host = nullptr;                   // pinned: DevState::T of every pair
   size_t T_cap = 0;
+  JointStore joint;                          // sicp_register_joint's buffers
   ~Batch() {
     if (flags_host) cudaFreeHost(flags_host);
     if (results_host) cudaFreeHost(results_host);

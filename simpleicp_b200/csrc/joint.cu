@@ -1,0 +1,456 @@
+// joint.cu — the device work of sicp_register_joint per iteration, after the batched match of
+// every edge (batch_match_launch, unchanged):
+//
+//   k_joint_reject   one block per edge: median / MAD of all distances (upper middle elements, by a
+//                    bitonic sort of the order-preserving keys in shared memory), the linearised
+//                    keep rule, the edge's point-to-plane normal equations N, h = sum a d from the
+//                    kept rows a = [w x n, n] with w = R_e (p - c_m) (centred about the edge's movable
+//                    centre c_f = R_e c_m in frame a), and the edge's 6 x 6 block Ad^T N Ad and
+//                    right-hand side -Ad^T h in the common world parameterisation
+//   k_joint_solve    one cooperative launch: assembly of the dense 6F x 6F normal matrix, augmented
+//                    by the right-hand side as one more row, from the edge blocks in ascending edge
+//                    order; right-looking tiled Cholesky (the augmented row leaves L^-1 b behind);
+//                    back substitution; the pose update of every free cloud, each edge's new
+//                    relative transform, increment, residual statistics, record and stop rule
+//
+// DESIGN.md §6.9 gives the rule, the Ad mapping and the centring.  Every sum runs in a fixed
+// order (no atomics), so repeated calls give the same bits.
+#include "ctx.cuh"
+
+namespace sicp {
+
+namespace {
+
+constexpr int JR_THREADS = 512;
+constexpr int JR_WARPS = JR_THREADS / 32;
+constexpr int JR_CAP = 4096;  // correspondences per edge (sicp_register_pairs' limit)
+constexpr int JS_THREADS = 256;
+constexpr int TS = 32;        // Cholesky tile
+
+// Ascending bitonic sort of P (a power of two) keys in shared memory by the whole block.
+__device__ void bitonic_sort(unsigned long long* k, int P) {
+  for (int size = 2; size <= P; size <<= 1)
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      __syncthreads();
+      for (int t = threadIdx.x; t < P / 2; t += blockDim.x) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        const bool up = (lo & size) == 0;
+        const unsigned long long x = k[lo], y = k[hi];
+        if ((x > y) == up) {
+          k[lo] = y;
+          k[hi] = x;
+        }
+      }
+    }
+  __syncthreads();
+}
+
+// xi = Ad y: a world-frame increment y = (omega, t') about the world centre c_w, carried into
+// frame a about the edge centre c_f (Ra: rotation of the pose of cloud a, v = T_a c_f - c_w):
+// alpha = Ra^T omega, t_c = Ra^T (t' - v x omega).
+__device__ __forceinline__ void ad_apply(const double* Ra, const double* v, const double* y, double* xi) {
+  const double w0 = y[0], w1 = y[1], w2 = y[2];
+  const double u0 = y[3] - (v[1] * w2 - v[2] * w1), u1 = y[4] - (v[2] * w0 - v[0] * w2),
+               u2 = y[5] - (v[0] * w1 - v[1] * w0);
+  for (int r = 0; r < 3; ++r) {
+    xi[r] = Ra[0 * 3 + r] * w0 + Ra[1 * 3 + r] * w1 + Ra[2 * 3 + r] * w2;
+    xi[3 + r] = Ra[0 * 3 + r] * u0 + Ra[1 * 3 + r] * u1 + Ra[2 * 3 + r] * u2;
+  }
+}
+
+__device__ __forceinline__ int tri(int r, int c) { return r * (r + 1) / 2 + c; }  // c <= r
+
+__global__ void __launch_bounds__(JR_THREADS) k_joint_reject(const JointArgs a) {
+  __shared__ unsigned long long key[JR_CAP];
+  __shared__ double red[JR_WARPS][JE_NSUM];
+  __shared__ double tot[JE_NSUM];
+  const int e = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (a.flags->done) return;
+  DevState* st = a.state + e;
+  if (st->stop) return;  // no overlap: the edge takes no part
+  const PairDev& pd = a.pairs[e];
+  const long long q = pd.q_off;
+  const int K = (int)pd.K;
+  int P = 1;
+  while (P < K) P <<= 1;
+  // median and MAD over every distance: the element at K / 2 of the sorted keys
+  for (int i = tid; i < P; i += JR_THREADS) key[i] = (i < K) ? f64_to_key(a.dist[q + i]) : ~0ull;
+  bitonic_sort(key, P);
+  const double med = key_to_f64(key[K >> 1]);
+  __syncthreads();
+  for (int i = tid; i < P; i += JR_THREADS) key[i] = (i < K) ? f64_to_key(fabs(a.dist[q + i] - med)) : ~0ull;
+  bitonic_sort(key, P);
+  const double mad = key_to_f64(key[K >> 1]);
+  const double lim = 3.0 * (1.4826 * mad);
+
+  const Rigid R = st->T;
+  const double cm0 = pd.cm[0], cm1 = pd.cm[1], cm2 = pd.cm[2];
+  double acc[JE_NSUM];
+#pragma unroll
+  for (int j = 0; j < JE_NSUM; ++j) acc[j] = 0.0;
+  for (int i = tid; i < K; i += JR_THREADS) {
+    const float4 nr = a.q_nrm[q + i];
+    const double d = a.dist[q + i];
+    const bool kp = (double)nr.w >= a.min_planarity && fabs(d - med) <= lim;
+    a.keep[q + i] = kp ? 1 : 0;
+    if (!kp) continue;
+    const double u0 = a.m_xyz[3 * (q + i) + 0] - cm0, u1 = a.m_xyz[3 * (q + i) + 1] - cm1,
+                 u2 = a.m_xyz[3 * (q + i) + 2] - cm2;
+    const double w0 = R.r[0] * u0 + R.r[1] * u1 + R.r[2] * u2;
+    const double w1 = R.r[3] * u0 + R.r[4] * u1 + R.r[5] * u2;
+    const double w2 = R.r[6] * u0 + R.r[7] * u1 + R.r[8] * u2;
+    const double n0 = (double)nr.x, n1 = (double)nr.y, n2 = (double)nr.z;
+    const double row[6] = {w1 * n2 - w2 * n1, w2 * n0 - w0 * n2, w0 * n1 - w1 * n0, n0, n1, n2};
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+#pragma unroll
+      for (int c = 0; c <= r; ++c) acc[tri(r, c)] = fma(row[r], row[c], acc[tri(r, c)]);
+      acc[21 + r] = fma(row[r], d, acc[21 + r]);
+      acc[27 + r] += row[r];
+    }
+    acc[33] += d;
+    acc[34] = fma(d, d, acc[34]);
+    acc[35] += 1.0;
+  }
+#pragma unroll
+  for (int j = 0; j < JE_NSUM; ++j) {
+    const double v = warp_sum(acc[j]);
+    if (lane == 0) red[warp][j] = v;
+  }
+  __syncthreads();
+  if (tid < JE_NSUM) {
+    double v = 0.0;
+    for (int w = 0; w < JR_WARPS; ++w) v += red[w][tid];
+    tot[tid] = v;
+  }
+  __syncthreads();
+  if (tid != 0) return;
+
+  JointEdge& je = a.edges[e];
+  const long long n = (long long)(tot[35] + 0.5);
+  const double mean_d = n > 0 ? tot[33] / (double)n : nan("");
+  const double var_d1 = n > 1 ? fmax(tot[34] - (double)n * mean_d * mean_d, 0.0) / (double)(n - 1) : nan("");
+  sicp_iter_record* rec = a.rec + (size_t)e * a.rec_stride + a.it;
+  rec->n_kept = n;
+  rec->median = med;
+  rec->mad = mad;
+  rec->mean_dist = mean_d;
+  rec->std_dist = sqrt(var_d1);
+  rec->distance_weight = 1.0;
+  rec->lm_iterations = n >= 6 ? 1 : 0;
+  rec->n_bruteforce = 0;
+  je.part = n >= 6 ? 1 : 0;
+  je.n = n;
+  for (int j = 0; j < 21; ++j) je.N[j] = tot[j];
+  for (int j = 0; j < 6; ++j) {
+    je.h[j] = tot[21 + j];
+    je.s[j] = tot[27 + j];
+  }
+  je.sd = tot[33];
+  je.sd2 = tot[34];
+  // the edge centre in frame a and in the world, and the rotation of cloud a's pose: Ad
+  double cf[3], wc[3];
+  rigid_apply(R, cm0, cm1, cm2, cf[0], cf[1], cf[2]);
+  const Rigid& Ta = a.pose[a.fix_id[e]];
+  rigid_apply(Ta, cf[0], cf[1], cf[2], wc[0], wc[1], wc[2]);
+  for (int j = 0; j < 3; ++j) {
+    je.cf[j] = cf[j];
+    je.v[j] = wc[j] - a.cw[j];
+  }
+  for (int j = 0; j < 9; ++j) je.Ra[j] = Ta.r[j];
+  // columns of Ad: Ad e_k, then N Ad and Ad^T N Ad, Ad^T (-h)
+  double Ad[6][6], NA[6][6];
+  for (int k = 0; k < 6; ++k) {
+    double y[6] = {0, 0, 0, 0, 0, 0}, col[6];
+    y[k] = 1.0;
+    ad_apply(je.Ra, je.v, y, col);
+    for (int r = 0; r < 6; ++r) Ad[r][k] = col[r];
+  }
+  for (int r = 0; r < 6; ++r)
+    for (int k = 0; k < 6; ++k) {
+      double v = 0.0;
+      for (int m = 0; m < 6; ++m) v = fma(je.N[r >= m ? tri(r, m) : tri(m, r)], Ad[m][k], v);
+      NA[r][k] = v;
+    }
+  for (int r = 0; r < 6; ++r) {
+    for (int k = 0; k <= r; ++k) {
+      double v = 0.0;
+      for (int m = 0; m < 6; ++m) v = fma(Ad[m][r], NA[m][k], v);
+      je.Nw[r * 6 + k] = v;
+      je.Nw[k * 6 + r] = v;
+    }
+    double g = 0.0;
+    for (int m = 0; m < 6; ++m) g = fma(Ad[m][r], -je.h[m], g);
+    je.gw[r] = g;
+  }
+}
+
+// Grid barrier of the cooperative k_joint_solve (every block resident): bar[0] arrivals, bar[1]
+// generation; the fences make the tiles other blocks wrote visible after it.
+__device__ void joint_grid_sync(unsigned int* bar) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned int gen = *(volatile unsigned int*)(bar + 1);
+    if (atomicAdd(bar, 1u) == gridDim.x - 1u) {
+      *(volatile unsigned int*)bar = 0u;
+      __threadfence();
+      atomicAdd(bar + 1, 1u);
+    } else {
+      while (*(volatile unsigned int*)(bar + 1) == gen) __nanosleep(64);
+    }
+    __threadfence();
+  }
+  __syncthreads();
+}
+
+struct SolveSmem {
+  double t0[TS][TS + 1];
+  double t1[TS][TS + 1];
+  double xs[JOINT_MAX_PAD];
+  int bad;
+  int conv;
+};
+
+__device__ void load_tile(double (&t)[TS][TS + 1], const double* A, int npad, int ti, int tj) {
+  for (int e = threadIdx.x; e < TS * TS; e += JS_THREADS)
+    t[e / TS][e % TS] = __ldcg(&A[(size_t)(ti * TS + e / TS) * npad + tj * TS + e % TS]);
+}
+__device__ void store_tile(const double (&t)[TS][TS + 1], double* A, int npad, int ti, int tj) {
+  for (int e = threadIdx.x; e < TS * TS; e += JS_THREADS)
+    __stcg(&A[(size_t)(ti * TS + e / TS) * npad + tj * TS + e % TS], t[e / TS][e % TS]);
+}
+
+__device__ __forceinline__ double change_pct(double v, double v0) {
+  return (v0 == 0.0) ? ((v == 0.0) ? 0.0 : kInf) : fabs((v - v0) / v0 * 100.0);
+}
+
+__global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
+  __shared__ SolveSmem sm;
+  const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
+  if (a.flags->done) return;  // uniform: only block 0 writes it, at the very end of this launch
+  const int n = 6 * a.F, npad = a.npad, KT = npad / TS;
+  double* A = a.A;
+
+  // ---- assembly of the lower triangle: edge blocks in ascending edge order, the right-hand side
+  // as row n, identity padding
+  for (long long idx = (long long)bid * JS_THREADS + tid; idx < (long long)npad * npad; idx += (long long)G * JS_THREADS) {
+    const int i = (int)(idx / npad), j = (int)(idx % npad);
+    if (j > i) continue;
+    double v = 0.0;
+    if (i < n) {
+      const int p = i / 6, qq = j / 6, ri = i % 6, cj = j % 6;
+      const int b = a.blk_of[p * a.F + qq];
+      if (b >= 0)
+        for (int l = a.blk_off[b]; l < a.blk_off[b + 1]; ++l) {
+          const JointEdge& je = a.edges[a.blk_edge[l] >> 1];
+          if (je.part) v += (p == qq) ? je.Nw[ri * 6 + cj] : -je.Nw[ri * 6 + cj];
+        }
+    } else if (i == n && j < n) {
+      const int p = j / 6, b = a.blk_of[p * a.F + p];
+      for (int l = a.blk_off[b]; l < a.blk_off[b + 1]; ++l) {
+        const JointEdge& je = a.edges[a.blk_edge[l] >> 1];
+        if (je.part) v += (a.blk_edge[l] & 1) ? -je.gw[j % 6] : je.gw[j % 6];
+      }
+    } else if (i == j) {
+      v = 1.0;
+    }
+    __stcg(&A[(size_t)i * npad + j], v);
+  }
+  if (tid == 0) sm.bad = 0;
+  joint_grid_sync(a.bar);
+
+  // ---- right-looking tiled Cholesky of the augmented matrix
+  for (int k = 0; k < KT; ++k) {
+    if (bid == 0) {
+      load_tile(sm.t0, A, npad, k, k);
+      __syncthreads();
+      for (int j = 0; j < TS; ++j) {
+        const int gj = k * TS + j;
+        if (tid == 0) {
+          double d = sm.t0[j][j];
+          if (gj < n) {
+            if (!(d > 0.0) || !isfinite(d)) sm.bad = 1;
+          } else {
+            d = 1.0;  // the right-hand side's row and the padding
+          }
+          sm.t0[j][j] = sqrt(d);
+        }
+        __syncthreads();
+        if (tid > j && tid < TS) sm.t0[tid][j] /= sm.t0[j][j];
+        __syncthreads();
+        for (int e = tid; e < TS * TS; e += JS_THREADS) {
+          const int r = e / TS, c = e % TS;
+          if (c > j && r >= c) sm.t0[r][c] = fma(-sm.t0[r][j], sm.t0[c][j], sm.t0[r][c]);
+        }
+        __syncthreads();
+      }
+      store_tile(sm.t0, A, npad, k, k);
+    }
+    joint_grid_sync(a.bar);
+    // panel: X L_kk^T = A_ik for every tile below the diagonal tile
+    for (int i = k + 1 + bid; i < KT; i += G) {
+      load_tile(sm.t0, A, npad, k, k);
+      load_tile(sm.t1, A, npad, i, k);
+      __syncthreads();
+      if (tid < TS)
+        for (int j = 0; j < TS; ++j) {
+          double v = sm.t1[tid][j];
+          for (int m = 0; m < j; ++m) v = fma(-sm.t1[tid][m], sm.t0[j][m], v);
+          sm.t1[tid][j] = v / sm.t0[j][j];
+        }
+      __syncthreads();
+      store_tile(sm.t1, A, npad, i, k);
+      __syncthreads();
+    }
+    joint_grid_sync(a.bar);
+    // trailing update A_ij -= L_ik L_jk^T, k < j <= i
+    const int m = KT - k - 1;
+    for (int t = bid; t < m * (m + 1) / 2; t += G) {
+      int ii = 0;
+      while ((ii + 1) * (ii + 2) / 2 <= t) ++ii;
+      const int jj = t - ii * (ii + 1) / 2, ti = k + 1 + ii, tj = k + 1 + jj;
+      load_tile(sm.t0, A, npad, ti, k);
+      load_tile(sm.t1, A, npad, tj, k);
+      __syncthreads();
+      for (int e = tid; e < TS * TS; e += JS_THREADS) {
+        const int r = e / TS, c = e % TS;
+        double s = 0.0;
+        for (int mm = 0; mm < TS; ++mm) s = fma(sm.t0[r][mm], sm.t1[c][mm], s);
+        double* dst = &A[(size_t)(ti * TS + r) * npad + tj * TS + c];
+        __stcg(dst, __ldcg(dst) - s);
+      }
+      __syncthreads();
+    }
+    joint_grid_sync(a.bar);
+  }
+  if (bid != 0) return;
+
+  // ---- back substitution L^T y = L^-1 b (row n of the factor), block 0
+  for (int i = tid; i < n; i += JS_THREADS) sm.xs[i] = __ldcg(&A[(size_t)n * npad + i]);
+  __syncthreads();
+  if (sm.bad) {
+    if (tid == 0) {
+      a.flags->singular = 1;
+      a.flags->done = 1;
+    }
+    return;
+  }
+  for (int k = (n - 1) / TS; k >= 0; --k) {
+    const int lo = k * TS, hi = min(lo + TS, n);
+    if (tid < 32) {
+      for (int r = hi - 1; r >= lo; --r) {
+        const double xr = sm.xs[r] / __ldcg(&A[(size_t)r * npad + r]);
+        __syncwarp();
+        if (lo + tid < r) sm.xs[lo + tid] = fma(-__ldcg(&A[(size_t)r * npad + lo + tid]), xr, sm.xs[lo + tid]);
+        if (tid == 0) sm.xs[r] = xr;
+        __syncwarp();
+      }
+    }
+    __syncthreads();
+    for (int mcol = tid; mcol < lo; mcol += JS_THREADS) {
+      double v = sm.xs[mcol];
+      for (int r = lo; r < hi; ++r) v = fma(-__ldcg(&A[(size_t)r * npad + mcol]), sm.xs[r], v);
+      sm.xs[mcol] = v;
+    }
+    __syncthreads();
+  }
+
+  // ---- poses: T_c <- dH(x_c) T_c, x_c = (omega, t' - omega x c_w)
+  for (int f = tid; f < a.F; f += JS_THREADS) {
+    const double* y = sm.xs + 6 * f;
+    const double x[6] = {y[0], y[1], y[2], y[3] - (y[1] * a.cw[2] - y[2] * a.cw[1]),
+                         y[4] - (y[2] * a.cw[0] - y[0] * a.cw[2]), y[5] - (y[0] * a.cw[1] - y[1] * a.cw[0])};
+    Rigid& T = a.pose[a.free_ids[f]];
+    T = rigid_compose(rigid_from_x(x), T);
+  }
+  __syncthreads();
+
+  // ---- edges: new relative transform, increment, residual statistics, record, stop rule
+  int conv = a.it > 0 ? 1 : 0;
+  for (int e = tid; e < a.n_edges; e += JS_THREADS) {
+    DevState& st = a.state[e];
+    if (st.stop) continue;
+    const JointEdge& je = a.edges[e];
+    const int ca = a.fix_id[e], cb = a.mov_id[e];
+    const Rigid Rold = st.T;
+    const Rigid Rn = rigid_compose(rigid_inverse(a.pose[ca]), a.pose[cb]);
+    st.T = Rn;
+    st.Tinv = rigid_inverse(Rn);
+    st.H_rep = Rn;
+    st.T_new = Rn;
+    st.T_res = Rn;
+    st.n_kept = je.n;
+    st.iterations_done = a.it + 1;
+    st.lm_ok = 1;
+    for (int j = 0; j < 6; ++j) st.sigma[j] = nan("");
+    if (!je.part) continue;
+    const int fa = a.free_of[ca], fb = a.free_of[cb];
+    double y[6], xi[6];
+    for (int j = 0; j < 6; ++j) y[j] = (fb >= 0 ? sm.xs[6 * fb + j] : 0.0) - (fa >= 0 ? sm.xs[6 * fa + j] : 0.0);
+    ad_apply(je.Ra, je.v, y, xi);
+    // residuals a . xi + d of the kept rows: their sum and sum of squares from the sums
+    double sr = je.sd, quad = 0.0, lin = 0.0;
+    for (int r = 0; r < 6; ++r) {
+      sr = fma(je.s[r], xi[r], sr);
+      lin = fma(je.h[r], xi[r], lin);
+      double row = 0.0;
+      for (int c = 0; c < 6; ++c) row = fma(je.N[r >= c ? tri(r, c) : tri(c, r)], xi[c], row);
+      quad = fma(row, xi[r], quad);
+    }
+    const double nn = (double)je.n;
+    const double mean = sr / nn;
+    const double sr2 = quad + 2.0 * lin + je.sd2;
+    const double sd = sqrt(fmax(sr2 - nn * mean * mean, 0.0) / (nn - 1.0));
+    // the origin-based increment of frame a: t = t_c - alpha x c_f
+    const double ex[6] = {xi[0], xi[1], xi[2], xi[3] - (xi[1] * je.cf[2] - xi[2] * je.cf[1]),
+                          xi[4] - (xi[2] * je.cf[0] - xi[0] * je.cf[2]), xi[5] - (xi[0] * je.cf[1] - xi[1] * je.cf[0])};
+    Rigid L;
+    L.r[0] = 1.0; L.r[1] = -ex[2]; L.r[2] = ex[1];
+    L.r[3] = ex[2]; L.r[4] = 1.0; L.r[5] = -ex[0];
+    L.r[6] = -ex[1]; L.r[7] = ex[0]; L.r[8] = 1.0;
+    L.t[0] = ex[3]; L.t[1] = ex[4]; L.t[2] = ex[5];
+    st.T_res = rigid_compose(L, Rold);
+    sicp_iter_record* rec = a.rec + (size_t)e * a.rec_stride + a.it;
+    for (int j = 0; j < 6; ++j) {
+      rec->x[j] = ex[j];
+      st.x_new[j] = ex[j];
+    }
+    rec->mean_res = mean;
+    rec->std_res = sd;
+    const bool stop = change_pct(mean, st.prev_mean) < a.min_change && change_pct(sd, st.prev_std) < a.min_change;
+    if (!stop) conv = 0;
+    st.prev_mean = mean;
+    st.prev_std = sd;
+  }
+  conv = __syncthreads_and(conv);
+  const bool finish = conv || a.last;
+  if (finish)
+    for (int e = tid; e < a.n_edges; e += JS_THREADS) {
+      DevState& st = a.state[e];
+      if (st.stop) continue;
+      st.converged = conv;
+      st.stop = a.edges[e].part ? (conv ? 1 : 0) : 2;
+    }
+  if (tid == 0) {
+    a.flags->converged = conv;
+    a.flags->done = finish ? 1 : 0;
+  }
+}
+
+}  // namespace
+
+void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges) {
+  k_joint_reject<<<n_edges, JR_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void joint_solve_launch(Ctx& c, const JointArgs& a) {
+  JointArgs args = a;
+  void* p[] = {&args};
+  SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_solve, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
+  c.tm.kernel_launches += 1;
+}
+
+}  // namespace sicp
