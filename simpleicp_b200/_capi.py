@@ -275,6 +275,40 @@ def _as_f64_xyz(X):
     return X.to(torch.float64).contiguous()
 
 
+def _clouds_arg(clouds, allow_none: bool = False):
+    """A cloud sequence as the C calls take it: (keep, ptrs, counts) -- every cloud through
+    _as_f64_xyz, their addresses and their point counts; with `allow_none` a None entry passes
+    NULL and 0.  The library reads the arrays in `keep`, which may be copies made here: the caller
+    holds `keep` until the call has returned."""
+    keep = [None if X is None and allow_none else _as_f64_xyz(X) for X in clouds]
+    ptrs = (C.c_void_p * len(keep))(*[_ptr(X) for X in keep])
+    counts = (C.c_int64 * len(keep))(*[0 if X is None else int(X.shape[0]) for X in keep])
+    return keep, ptrs, counts
+
+
+def _shaped_arg(a, name: str, shape: tuple):
+    """None, or `a` as a C-contiguous float64 array of `shape` (else ValueError)."""
+    if a is None:
+        return None
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    if a.shape != shape:
+        raise ValueError(f"{name} must have shape {shape}, got {a.shape}")
+    return a
+
+
+def _ids_arg(ids, name: str):
+    """(n, 2) integer cloud ids, n >= 1, as their two columns in contiguous int32 arrays (else
+    ValueError); `name` is "pairs" or "edges".  The library checks them against [0, n_clouds)."""
+    ids = np.asarray(ids)
+    if ids.ndim != 2 or ids.shape[1] != 2 or ids.shape[0] < 1 or not np.issubdtype(ids.dtype, np.integer):
+        raise ValueError(f"{name} must be integers of shape (n_{name}, 2) with n_{name} >= 1, got {ids.dtype} "
+                         f"of shape {ids.shape}")
+    if ids.min() < -(1 << 31) or ids.max() >= (1 << 31):
+        raise ValueError("cloud ids must fit in int32")
+    ids = np.ascontiguousarray(ids, dtype=np.int32)
+    return np.ascontiguousarray(ids[:, 0]), np.ascontiguousarray(ids[:, 1])
+
+
 def _d6(v: Sequence[float]):
     return (C.c_double * 6)(*[float(x) for x in v])
 
@@ -504,13 +538,8 @@ class Engine:
         by the angle between the normals."""
         Xf, Xm = _as_f64_xyz(X_fix), _as_f64_xyz(X_mov)
         self.n_fix, self.n_mov = int(Xf.shape[0]), int(Xm.shape[0])
-        rp = RegisterParams()
-        rp.correspondences = int(correspondences)
-        rp.neighbors = int(neighbors)
-        rp.max_overlap_distance = float(max_overlap_distance)
-        rp.run = params
-        rp.mov_neighbors = int(mov_neighbors)
-        rp.max_angle_rad = float(max_angle_rad)
+        rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
+                                   max_angle_rad)
         out = RunResult()
         log = (IterRecord * int(params.max_iterations))()
         if transform_out is None:
@@ -537,23 +566,14 @@ class Engine:
         of `params`).  `mov_neighbors` / `max_angle_rad` as in register_fused, for every pair's
         movable cloud.  Returns the ctypes array of PairResult (status per pair); its attribute
         `n_selected` holds the selected fixed points of each pair (int64)."""
-        n = len(pairs)
-        keep = [(_as_f64_xyz(a), _as_f64_xyz(b)) for a, b in pairs]  # keeps converted copies alive
-        fp = (C.c_void_p * n)(*[_ptr(a) for a, _ in keep])
-        mp = (C.c_void_p * n)(*[_ptr(b) for _, b in keep])
-        nf = (C.c_int64 * n)(*[int(a.shape[0]) for a, _ in keep])
-        nm = (C.c_int64 * n)(*[int(b.shape[0]) for _, b in keep])
-        observed = self._observed_rows(observed, n)
+        keep_f, fp, nf = _clouds_arg([a for a, _ in pairs])
+        keep_m, mp, nm = _clouds_arg([b for _, b in pairs])
+        n = len(nm)
+        observed = _shaped_arg(observed, "observed", (n, 6))
         rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
                                    max_angle_rad)
-        out = (PairResult * n)()
-        n_selected = np.zeros(n, dtype=np.int64)
-        self._check(self._lib.sicp_register_batch(self._h, n, fp, nf, mp, nm, C.byref(rp),
-                                                  None if observed is None else _ptr(observed), out,
-                                                  _ptr(n_selected)))
-        out.n_selected = n_selected
-        out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
-        return out
+        return self._batched(self._lib.sicp_register_batch, params, nm, None, n, fp, nf, mp, nm, C.byref(rp),
+                             _ptr(observed))
 
     def set_map(self, X_map):
         """sicp_set_map: upload a fixed cloud and build its grid once; it stays on this engine
@@ -573,21 +593,12 @@ class Engine:
         of every scan, which is neither uploaded nor gridded again, and with an overlap filter
         that only searches the map points near each scan.  Same arguments and result as
         register_batch, with the movable clouds `scans` in place of the pairs."""
-        n = len(scans)
-        keep = [_as_f64_xyz(X) for X in scans]  # keeps converted copies alive
-        mp = (C.c_void_p * n)(*[_ptr(X) for X in keep])
-        nm = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
-        observed = self._observed_rows(observed, n)
+        keep, mp, nm = _clouds_arg(scans)
+        n = len(nm)
+        observed = _shaped_arg(observed, "observed", (n, 6))
         rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
                                    max_angle_rad)
-        out = (PairResult * n)()
-        n_selected = np.zeros(n, dtype=np.int64)
-        self._check(self._lib.sicp_register_to_map(self._h, n, mp, nm, C.byref(rp),
-                                                   None if observed is None else _ptr(observed), out,
-                                                   _ptr(n_selected)))
-        out.n_selected = n_selected
-        out.n_mov, out.max_iterations = np.array(nm, dtype=np.int64), int(params.max_iterations)
-        return out
+        return self._batched(self._lib.sicp_register_to_map, params, nm, None, n, mp, nm, C.byref(rp), _ptr(observed))
 
     def register_pairs(self, clouds, pairs, correspondences, neighbors, params: RunParams,
                        max_overlap_distance: float = -1.0, observed=None, mov_neighbors: int = 0,
@@ -599,31 +610,15 @@ class Engine:
         result equals, bit for bit, register_batch's for (clouds[pairs[i, 0]], clouds[pairs[i, 1]]).
         Same other arguments and result as register_batch (`n_mov` is the size of each pair's
         movable cloud), so batch_outputs works on it."""
-        ids = np.asarray(pairs)
-        if ids.ndim != 2 or ids.shape[1] != 2 or ids.shape[0] < 1 or not np.issubdtype(ids.dtype, np.integer):
-            raise ValueError(f"pairs must be integers of shape (n_pairs, 2) with n_pairs >= 1, got {ids.dtype} "
-                             f"of shape {ids.shape}")
-        if ids.min() < -(1 << 31) or ids.max() >= (1 << 31):
-            raise ValueError("cloud ids must fit in int32")  # the library checks [0, n_clouds)
-        ids = np.ascontiguousarray(ids, dtype=np.int32)
-        n, m = ids.shape[0], len(clouds)
-        keep = [None if X is None else _as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
-        ptrs = (C.c_void_p * m)(*[_ptr(X) for X in keep])
-        counts = (C.c_int64 * m)(*[0 if X is None else int(X.shape[0]) for X in keep])
-        fix, mov = np.ascontiguousarray(ids[:, 0]), np.ascontiguousarray(ids[:, 1])
-        observed = self._observed_rows(observed, n)
+        fix, mov = _ids_arg(pairs, "pairs")
+        keep, ptrs, counts = _clouds_arg(clouds, allow_none=True)
+        n = len(fix)
+        observed = _shaped_arg(observed, "observed", (n, 6))
         rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, mov_neighbors,
                                    max_angle_rad)
-        out = (PairResult * n)()
-        n_selected = np.zeros(n, dtype=np.int64)
-        self._check(self._lib.sicp_register_pairs(
-            self._h, m, ptrs, counts, n, fix.ctypes.data_as(C.POINTER(C.c_int32)),
-            mov.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(rp), None if observed is None else _ptr(observed), out,
-            _ptr(n_selected)))
-        out.n_selected = n_selected
-        # an id out of range was refused above
-        out.n_mov, out.max_iterations = np.array([counts[j] for j in mov], dtype=np.int64), int(params.max_iterations)
-        return out
+        i32p = C.POINTER(C.c_int32)
+        return self._batched(self._lib.sicp_register_pairs, params, counts, mov, len(counts), ptrs, counts, n,
+                             fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p), C.byref(rp), _ptr(observed))
 
     def register_joint(self, clouds, edges, fixed, H0, correspondences, neighbors, params: RunParams,
                        max_overlap_distance: float = -1.0):
@@ -633,48 +628,43 @@ class Engine:
         None (identity) the start poses, world <- cloud.  Always the linearised rules; the lsq part
         of `params` is not read beyond its checks.  Returns (H, out): the final poses (n_clouds, 4,
         4) and the PairResult array per edge (H = final T_a^-1 T_b), which batch_outputs reads."""
-        ids = np.asarray(edges)
-        if ids.ndim != 2 or ids.shape[1] != 2 or ids.shape[0] < 1 or not np.issubdtype(ids.dtype, np.integer):
-            raise ValueError(f"edges must be integers of shape (n_edges, 2) with n_edges >= 1, got {ids.dtype} "
-                             f"of shape {ids.shape}")
-        if ids.min() < -(1 << 31) or ids.max() >= (1 << 31):
-            raise ValueError("cloud ids must fit in int32")  # the library checks [0, n_clouds)
-        ids = np.ascontiguousarray(ids, dtype=np.int32)
-        n, m = ids.shape[0], len(clouds)
-        keep = [None if X is None else _as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
-        ptrs = (C.c_void_p * m)(*[_ptr(X) for X in keep])
-        counts = (C.c_int64 * m)(*[0 if X is None else int(X.shape[0]) for X in keep])
-        fix, mov = np.ascontiguousarray(ids[:, 0]), np.ascontiguousarray(ids[:, 1])
+        fix, mov = _ids_arg(edges, "edges")
+        keep, ptrs, counts = _clouds_arg(clouds, allow_none=True)
+        n, m = len(fix), len(counts)
         is_fixed = np.ascontiguousarray(np.asarray(fixed, dtype=bool).reshape(m), dtype=np.int32)
-        if H0 is not None:
-            H0 = np.ascontiguousarray(H0, dtype=np.float64)
-            if H0.shape != (m, 4, 4):
-                raise ValueError(f"H0 must have shape ({m}, 4, 4), got {H0.shape}")
+        H0 = _shaped_arg(H0, "H0", (m, 4, 4))
         rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, 0, -1.0)
         H = np.zeros((m, 4, 4))
+        i32p = C.POINTER(C.c_int32)
+        out = self._batched(self._lib.sicp_register_joint, params, counts, mov, m, ptrs, counts, n,
+                            fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p), is_fixed.ctypes.data_as(i32p),
+                            _ptr(H0), C.byref(rp), _ptr(H))
+        return H, out
+
+    def _batched(self, fn, params: RunParams, counts, mov, *args):
+        """The end of the batched register_* calls: fn(ctx, *args, out, n_selected) with `out` one
+        PairResult per pair, returned with its attributes `n_selected`, `n_mov` (the movable point
+        counts, which batch_outputs sizes its clouds by) and `max_iterations`.  Pair i's movable
+        cloud has counts[i] points, or counts[mov[i]] given the movable cloud ids `mov`, which are
+        read only after the library has accepted them."""
+        n = len(counts) if mov is None else len(mov)
         out = (PairResult * n)()
         n_selected = np.zeros(n, dtype=np.int64)
-        i32p = C.POINTER(C.c_int32)
-        self._check(self._lib.sicp_register_joint(
-            self._h, m, ptrs, counts, n, fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p),
-            is_fixed.ctypes.data_as(i32p), _ptr(H0), C.byref(rp), _ptr(H), out, _ptr(n_selected)))
+        self._check(fn(self._h, *args, out, _ptr(n_selected)))
+        n_mov = np.array(counts, dtype=np.int64)
         out.n_selected = n_selected
-        out.n_mov, out.max_iterations = np.array([counts[j] for j in mov], dtype=np.int64), int(params.max_iterations)
-        return H, out
+        out.n_mov = n_mov if mov is None else n_mov[mov]
+        out.max_iterations = int(params.max_iterations)
+        return out
 
     def map_insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
         """sicp_map_insert: append to the resident map, per voxel of `voxel_size` it does not
         occupy, the first finite point of `clouds` (in order) falling into it, cloud i moved by
         H[i] first when `H` (n_clouds x 4 x 4) is given.  Returns the points each cloud added
         (int64)."""
-        n = len(clouds)
-        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
-        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
-        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
-        if H is not None:
-            H = np.ascontiguousarray(H, dtype=np.float64)
-            if H.shape != (n, 4, 4):
-                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
+        keep, ptrs, counts = _clouds_arg(clouds)
+        n = len(counts)
+        H = _shaped_arg(H, "H", (n, 4, 4))
         added = np.zeros(n, dtype=np.int64)
         self._check(self._lib.sicp_map_insert(self._h, n, ptrs, counts, _ptr(H), float(voxel_size), _ptr(added)))
         self.n_map += int(added.sum())
@@ -688,14 +678,9 @@ class Engine:
         for a non-finite point); with `neighbors` = k > 0 per cloud the signed distance along the
         matched map point's normal (float64) and its planarity (float32), both NaN where idx is -1,
         else None; and the within points of each cloud (int64)."""
-        n = len(clouds)
-        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
-        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
-        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
-        if H is not None:
-            H = np.ascontiguousarray(H, dtype=np.float64)
-            if H.shape != (n, 4, 4):
-                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
+        keep, ptrs, counts = _clouds_arg(clouds)
+        n = len(counts)
+        H = _shaped_arg(H, "H", (n, 4, 4))
         k = int(neighbors)
         sizes = [int(c) for c in counts]
         idx = [np.empty(m, dtype=np.int64) for m in sizes]
@@ -743,18 +728,10 @@ class Engine:
         finite point of cloud i (moved by H[i] first when `H` (n_clouds x 4 x 4) is given).
         `passes` is None or a uint32 array / tensor (host or CUDA) of the map's size before the
         call, which receives every map point's pass count.  Returns the points removed."""
-        n = len(clouds)
-        keep = [_as_f64_xyz(X) for X in clouds]  # keeps converted copies alive
-        ptrs = (C.c_void_p * n)(*[_ptr(X) for X in keep])
-        counts = (C.c_int64 * n)(*[int(X.shape[0]) for X in keep])
-        if H is not None:
-            H = np.ascontiguousarray(H, dtype=np.float64)
-            if H.shape != (n, 4, 4):
-                raise ValueError(f"H must have shape ({n}, 4, 4), got {H.shape}")
-        if origins is not None:
-            origins = np.ascontiguousarray(origins, dtype=np.float64)
-            if origins.shape != (n, 3):
-                raise ValueError(f"origins must have shape ({n}, 3), got {origins.shape}")
+        keep, ptrs, counts = _clouds_arg(clouds)
+        n = len(counts)
+        H = _shaped_arg(H, "H", (n, 4, 4))
+        origins = _shaped_arg(origins, "origins", (n, 3))
         removed = C.c_int64(0)
         self._check(self._lib.sicp_map_carve(self._h, n, ptrs, counts, _ptr(H), _ptr(origins), float(radius),
                                              float(margin), int(min_passes), _ptr(passes), C.byref(removed)))
@@ -778,15 +755,6 @@ class Engine:
             T.ctypes.data_as(C.POINTER(C.c_double))))
         return [(X[i], R[i], [log[i * it + j] for j in range(result[i].iterations)], T[i].reshape(4, 4))
                 if ok[i] else None for i in range(n)]
-
-    @staticmethod
-    def _observed_rows(observed, n: int):
-        if observed is None:
-            return None
-        observed = np.ascontiguousarray(observed, dtype=np.float64)
-        if observed.shape != (n, 6):
-            raise ValueError(f"observed must have shape ({n}, 6), got {observed.shape}")
-        return observed
 
     @staticmethod
     def _register_params(correspondences, neighbors, params: RunParams, max_overlap_distance, mov_neighbors,

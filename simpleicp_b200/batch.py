@@ -29,6 +29,27 @@ def pack_record(H: np.ndarray, iterations: int, n_kept: int, mean: float, std: f
     return r
 
 
+def _failed_record(code: int) -> np.ndarray:
+    """The record of a pair that could not be registered: NaN, iterations = -code."""
+    return pack_record(np.full((4, 4), np.nan), -int(code), 0, np.nan, np.nan)
+
+
+def _pair_record(r, kind: str, number: int, messages: List[str]) -> np.ndarray:
+    """The record of PairResult `r`, pair or edge `number` of the call; for one that failed the
+    library's status also goes to `messages`."""
+    if r.status == 0:
+        return pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)
+    messages.append(f"{kind} {number}: library status {r.status}")
+    return _failed_record(r.status)
+
+
+def _raise_failed(table: np.ndarray, on_error: str, messages: List[str], results=None) -> None:
+    """BatchError when rows of `table` failed (iterations < 0) and `on_error` is "raise"."""
+    failed = np.flatnonzero(table[:, 16] < 0)
+    if failed.size and on_error == "raise":
+        raise BatchError(table, failed, messages, results)
+
+
 def gather_records(local: np.ndarray, n_pairs: int, world_size: int, rank: int, dist=None,
                    device=None) -> np.ndarray:
     """All-gather the per-pair records.  `local` is (len(shard), RECORD_LEN) in shard order;
@@ -183,7 +204,7 @@ def simpleicp_batch(
             if code is None:
                 code = 2 if "overlap" in msg else (3 if "correspondences" in msg else 99)
             messages.append(msg)
-            return pack_record(np.full((4, 4), np.nan), -int(code), 0, np.nan, np.nan)
+            return _failed_record(code)
 
     messages: List[str] = []
     if register_fn is not None:
@@ -229,7 +250,7 @@ def simpleicp_batch(
         if errors:  # not a per-pair outcome (bad generator, lost device): NaN for what is missing
             messages.append(repr(errors[0]))
             done = np.isfinite(local[:, 16]) & (local[:, 16] != 0)
-            local[~done] = pack_record(np.full((4, 4), np.nan), -99, 0, np.nan, np.nan)
+            local[~done] = _failed_record(99)
     return _gather_share(local, found, mine, n_pairs, rank, world_size, dist, device, on_error, full_output, messages)
 
 
@@ -248,9 +269,7 @@ def _gather_share(local, found, mine, n_pairs, rank, world_size, dist, device, o
         results = [None] * n_pairs
         for j, i in enumerate(mine):
             results[i] = found[j]
-    failed = np.flatnonzero(table[:, 16] < 0)
-    if failed.size and on_error == "raise":
-        raise BatchError(table, failed, messages, results)
+    _raise_failed(table, on_error, messages, results)
     return (table, results) if full_output else table
 
 
@@ -272,11 +291,7 @@ def simpleicp_edges(clouds: Sequence, edges, *, rank: int = 0, world_size: int =
     edge's prior.  The run() arguments served are those of the batched engine without
     ``want_normals`` (at most 4096 correspondences); anything else is a TypeError.  `on_error`,
     `full_output` and BatchError are as in simpleicp_batch."""
-    unknown = set(run_kwargs) - _EDGE_KEYS
-    if unknown:
-        raise TypeError(f"simpleicp_edges() got unsupported arguments {sorted(unknown)}")
-    if int(run_kwargs.get("correspondences", 1000)) > 4096:
-        raise ValueError("simpleicp_edges runs one block per edge: correspondences must be <= 4096")
+    _check_run_keys(run_kwargs, _EDGE_KEYS, "simpleicp_edges", "edge")
     e = _check_edges(edges, len(clouds))
     n = e.shape[0]
     rows = _per_pair_observed(run_kwargs, n)
@@ -321,13 +336,7 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     an edge that failed (no overlap, too few correspondences) has its status in the table and raises
     BatchError under "raise"; a failure of the whole call (SICP_ERR_SINGULAR, or a free cloud left
     without a path to a fixed one by the edges without overlap) raises SicpError."""
-    from . import _capi
-
-    unknown = set(run_kwargs) - _JOINT_KEYS
-    if unknown:
-        raise TypeError(f"simpleicp_joint() got unsupported arguments {sorted(unknown)}")
-    if int(run_kwargs.get("correspondences", 1000)) > 4096:
-        raise ValueError("simpleicp_joint runs one block per edge: correspondences must be <= 4096")
+    _check_run_keys(run_kwargs, _JOINT_KEYS, "simpleicp_joint", "edge")
     n_clouds = len(clouds)
     e = _check_edges(edges, n_clouds)
     if e.shape[0] < 1:
@@ -342,11 +351,7 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     is_fixed = np.zeros(n_clouds, dtype=bool)
     is_fixed[fx] = True
     if H0 is not None:
-        H0 = np.asarray(H0, dtype=np.float64)
-        if H0.shape != (n_clouds, 4, 4):
-            raise ValueError(f"H0 must have shape ({n_clouds}, 4, 4), got {H0.shape}")
-        if not np.isfinite(H0).all():
-            raise ValueError("H0 must be finite")
+        H0 = _finite_array(H0, "H0", (n_clouds, 4, 4))
     used = np.zeros(n_clouds, dtype=bool)
     used[e.ravel()] = True
     free = used & ~is_fixed
@@ -372,9 +377,7 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     import torch
 
     with torch.cuda.device(device):
-        eng = _BATCH_ENGINES.get(int(device))
-        if eng is None or not eng.alive:
-            eng = _BATCH_ENGINES[int(device)] = _capi.Engine(int(device))
+        eng = _batch_engine(device)
         lsq = eng.lsq_params((0.0,) * 6, (0.0,) * 6, [0.0] * 6, 1)
         params = eng.run_params(run_kwargs.get("min_planarity", 0.3), run_kwargs.get("min_change", 1.0),
                                 run_kwargs.get("max_iterations", 100), lsq)
@@ -385,11 +388,7 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         table = np.zeros((n, RECORD_LEN))
         messages: List[str] = []
         for j, r in enumerate(res):
-            if r.status == 0:
-                table[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)
-            else:
-                messages.append(f"edge {j}: library status {r.status}")
-                table[j] = pack_record(np.full((4, 4), np.nan), -int(r.status), 0, np.nan, np.nan)
+            table[j] = _pair_record(r, "edge", j, messages)
         results = None
         if full_output:
             results = [None if o is None else _batch_result(r, o, np.zeros(6), (0.0,) * 6)
@@ -397,9 +396,7 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     ok = [r for r in res if r.status == 0]
     out = JointResult(H, table, max((int(r.iterations) for r in ok), default=0),
                       bool(ok) and all(bool(r.converged) for r in ok), results)
-    failed = np.flatnonzero(table[:, 16] < 0)
-    if failed.size and on_error == "raise":
-        raise BatchError(table, failed, messages, results)
+    _raise_failed(table, on_error, messages, results)
     return out
 
 
@@ -434,17 +431,29 @@ def edge_chunks(edges: np.ndarray, mine: Sequence[int], batch_size: int):
 _BATCH_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations",
                "distance_weights", "rbp_observed_values", "rbp_observation_weights", "max_overlap_distance",
                "want_normals", "mov_neighbors", "max_angle_between_normals"}
-# run() arguments simpleicp_edges serves (sicp_register_pairs): the batched engine's, without the
-# debug output
-_EDGE_KEYS = _BATCH_KEYS - {"want_normals"}
+# run() arguments simpleicp_edges (sicp_register_pairs) and Map.register (sicp_register_to_map)
+# serve: the batched engine's, without the debug output
+_EDGE_KEYS = _MAP_KEYS = _BATCH_KEYS - {"want_normals"}
+# the batched engines run one block per pair, which holds at most this many correspondences
+_MAX_CORRESPONDENCES = 4096
 
 
 def _batchable(kw) -> bool:
-    """Can the batched engine serve these run() arguments?  (One block per pair: at most 4096
-    correspondences; nothing that needs per-pair host interaction.)"""
+    """Can the batched engine serve these run() arguments?  (One block per pair: at most
+    _MAX_CORRESPONDENCES; nothing that needs per-pair host interaction.)"""
     if set(kw) - _BATCH_KEYS:
         return False
-    return int(kw.get("correspondences", 1000)) <= 4096 and not kw.get("want_normals", False)
+    return int(kw.get("correspondences", 1000)) <= _MAX_CORRESPONDENCES and not kw.get("want_normals", False)
+
+
+def _check_run_keys(kw, allowed, caller: str, unit: str) -> None:
+    """The run() arguments of `caller`, which runs one block per `unit` (edge, scan): a key
+    outside `allowed` is a TypeError, more than _MAX_CORRESPONDENCES a ValueError."""
+    unknown = set(kw) - allowed
+    if unknown:
+        raise TypeError(f"{caller}() got unsupported arguments {sorted(unknown)}")
+    if int(kw.get("correspondences", 1000)) > _MAX_CORRESPONDENCES:
+        raise ValueError(f"{caller} runs one block per {unit}: correspondences must be <= {_MAX_CORRESPONDENCES}")
 
 
 def _check_mov_kwargs(kw) -> None:
@@ -481,6 +490,17 @@ def _per_pair_observed(kw, n_pairs: int):
 _BATCH_ENGINES: dict = {}
 
 
+def _batch_engine(device: int):
+    """The batched engine kept for `device` in _BATCH_ENGINES, created when missing or closed;
+    called under torch.cuda.device(device)."""
+    from . import _capi
+
+    eng = _BATCH_ENGINES.get(int(device))
+    if eng is None or not eng.alive:
+        eng = _BATCH_ENGINES[int(device)] = _capi.Engine(int(device))
+    return eng
+
+
 def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, map_engine=None, results=None,
                  edges=None):
     """The rank's share `mine` through the batched engine, `batch_size` pairs per call, records into
@@ -492,7 +512,6 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, 
     (sicp_get_batch_outputs) because the next one reuses the library's buffers."""
     import torch
 
-    from . import _capi
     from .simpleicp import _check_arguments, _observed_in_radians
 
     dw = kw.get("distance_weights", 1)
@@ -507,9 +526,8 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, 
     k_mov = kw.get("mov_neighbors")
     ang = kw.get("max_angle_between_normals")
     with torch.cuda.device(device):
-        eng = map_engine if map_engine is not None else _BATCH_ENGINES.get(int(device))
-        if eng is None or not eng.alive:
-            eng = _BATCH_ENGINES[int(device)] = _capi.Engine(int(device))
+        # a closed map's engine is replaced too: the call then reports that there is no map
+        eng = map_engine if map_engine is not None and map_engine.alive else _batch_engine(device)
         register = eng.register_to_map if map_engine is not None else eng.register_batch
         lsq = eng.lsq_params(obs, obs, [float(w) for w in obs_w], dw)
         params = eng.run_params(kw.get("min_planarity", 0.3), kw.get("min_change", 1.0),
@@ -526,11 +544,7 @@ def _run_batched(get, mine, local, device, batch_size, kw, messages, rows=None, 
             else:
                 res = eng.register_pairs([get(int(c)) for c in cloud_ids], local_edges, *args)
             for j, r in zip(ids, res):
-                if r.status == 0:
-                    local[j] = pack_record(np.array(r.H).reshape(4, 4), r.iterations, r.n_kept, r.mean_res, r.std_res)
-                else:
-                    messages.append(f"pair {mine[j]}: library status {r.status}")
-                    local[j] = pack_record(np.full((4, 4), np.nan), -int(r.status), 0, np.nan, np.nan)
+                local[j] = _pair_record(r, "pair", mine[j], messages)
             if results is not None:
                 for k, (j, r, o) in enumerate(zip(ids, res, eng.batch_outputs(res))):
                     if o is not None:
@@ -553,8 +567,27 @@ def _batch_result(r, outputs, obs, rbp_observation_weights):
     return res
 
 
-# run() arguments Map.register serves: those of the batched engine, without the debug output
-_MAP_KEYS = _BATCH_KEYS - {"want_normals"}
+def _finite_array(a, name: str, shape: tuple) -> np.ndarray:
+    """`a` as a float64 array of `shape` with only finite entries, or ValueError."""
+    a = np.asarray(a, dtype=np.float64)
+    if a.shape != shape:
+        raise ValueError(f"{name} must have shape {shape}, got {a.shape}")
+    if not np.isfinite(a).all():
+        raise ValueError(f"{name} must be finite")
+    return a
+
+
+def _map_clouds(method: str, clouds, H):
+    """The `clouds` and `H` of Map.insert / distances / carve checked: at least one cloud, each
+    (n, 3), and H None or finite of shape (n_clouds, 4, 4).  Returns (list of clouds, H as
+    float64); ValueError otherwise."""
+    clouds = list(clouds)
+    if not clouds:
+        raise ValueError(f"{method} needs at least one cloud")
+    for i, X in enumerate(clouds):
+        if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
+            raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
+    return clouds, None if H is None else _finite_array(H, "H", (len(clouds), 4, 4))
 
 
 class Map:
@@ -602,11 +635,7 @@ class Map:
         as simpleicp_batch does: ``results[i]`` is register()'s result object for scan i
         (``X_mov_transformed`` in the map's frame, residuals, records, uncertainties), None for
         a scan that failed."""
-        unknown = set(run_kwargs) - _MAP_KEYS
-        if unknown:
-            raise TypeError(f"Map.register() got unsupported arguments {sorted(unknown)}")
-        if int(run_kwargs.get("correspondences", 1000)) > 4096:
-            raise ValueError("Map.register runs one block per scan: correspondences must be <= 4096")
+        _check_run_keys(run_kwargs, _MAP_KEYS, "Map.register", "scan")
         n = len(scans)
         rows = _per_pair_observed(run_kwargs, n)
         _check_mov_kwargs(run_kwargs)
@@ -617,9 +646,7 @@ class Map:
         per_call = max(1, min(int(batch_size), ((1 << 32) - 1) // max(self.n_points, 1)))
         _run_batched(lambda i: scans[i], list(range(n)), local, self.device, per_call, run_kwargs, messages, rows,
                      map_engine=self._engine, **({"results": results} if full_output else {}))
-        failed = np.flatnonzero(local[:, 16] < 0)
-        if failed.size and on_error == "raise":
-            raise BatchError(local, failed, messages, results)
+        _raise_failed(local, on_error, messages, results)
         return (local, results) if full_output else local
 
     def insert(self, clouds, H=None, *, voxel_size: float) -> np.ndarray:
@@ -636,18 +663,7 @@ class Map:
         v = float(voxel_size)
         if not (np.isfinite(v) and v > 0):
             raise ValueError(f"voxel_size must be finite and > 0, got {voxel_size}")
-        clouds = list(clouds)
-        if not clouds:
-            raise ValueError("insert needs at least one cloud")
-        for i, X in enumerate(clouds):
-            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
-                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
-        if H is not None:
-            H = np.asarray(H, dtype=np.float64)
-            if H.shape != (len(clouds), 4, 4):
-                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
-            if not np.isfinite(H).all():
-                raise ValueError("H must be finite")
+        clouds, H = _map_clouds("insert", clouds, H)
         import torch
 
         with torch.cuda.device(self.device):
@@ -677,18 +693,7 @@ class Map:
         if neighbors is not None and not (2 <= k <= 64 and k <= self.n_points):
             raise ValueError(f"neighbors must be between 2 and 64 and at most the map's {self.n_points} points, "
                              f"got {neighbors}")
-        clouds = list(clouds)
-        if not clouds:
-            raise ValueError("distances needs at least one cloud")
-        for i, X in enumerate(clouds):
-            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
-                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
-        if H is not None:
-            H = np.asarray(H, dtype=np.float64)
-            if H.shape != (len(clouds), 4, 4):
-                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
-            if not np.isfinite(H).all():
-                raise ValueError("H must be finite")
+        clouds, H = _map_clouds("distances", clouds, H)
         import torch
 
         with torch.cuda.device(self.device):
@@ -766,24 +771,9 @@ class Map:
             raise ValueError(f"margin must be finite and >= 0, got {margin}")
         if isinstance(min_passes, bool) or int(min_passes) != min_passes or not 1 <= int(min_passes) < (1 << 31):
             raise ValueError(f"min_passes must be an integer >= 1, got {min_passes}")
-        clouds = list(clouds)
-        if not clouds:
-            raise ValueError("carve needs at least one cloud")
-        for i, X in enumerate(clouds):
-            if len(getattr(X, "shape", ())) != 2 or X.shape[1] != 3:
-                raise ValueError(f"cloud {i} must have shape (n, 3), got {tuple(getattr(X, 'shape', ()))}")
-        if H is not None:
-            H = np.asarray(H, dtype=np.float64)
-            if H.shape != (len(clouds), 4, 4):
-                raise ValueError(f"H must have shape ({len(clouds)}, 4, 4), got {H.shape}")
-            if not np.isfinite(H).all():
-                raise ValueError("H must be finite")
+        clouds, H = _map_clouds("carve", clouds, H)
         if origins is not None:
-            origins = np.asarray(origins, dtype=np.float64)
-            if origins.shape != (len(clouds), 3):
-                raise ValueError(f"origins must have shape ({len(clouds)}, 3), got {origins.shape}")
-            if not np.isfinite(origins).all():
-                raise ValueError("origins must be finite")
+            origins = _finite_array(origins, "origins", (len(clouds), 3))
         elif H is None:
             raise ValueError("carve needs origins, or H whose translations are the sensor origins")
         import torch

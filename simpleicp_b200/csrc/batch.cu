@@ -1407,93 +1407,93 @@ static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const 
 
 using namespace sicp;
 
-#define SICP_BATCH_API(body)                 \
-  if (!ctx) {                                \
-    sicp::set_thread_error("sicp_ctx is NULL"); \
-    return SICP_ERR_BAD_ARG;                 \
-  }                                          \
-  Ctx& c = ctx->c;                           \
-  try {                                      \
-    SICP_CUDA(cudaSetDevice(c.device));      \
-    body;                                    \
-  } catch (const sicp::Error& e) {           \
-    c.up.cancel();                           \
-    c.err = e.msg;                           \
-    sicp::set_thread_error(e.msg);           \
-    if (e.code == SICP_ERR_CUDA) cudaGetLastError(); \
-    return e.code;                           \
-  } catch (const std::exception& e) {        \
-    c.up.cancel();                           \
-    c.err = e.what();                        \
-    sicp::set_thread_error(c.err);           \
-    return SICP_ERR_CUDA;                    \
-  }                                          \
-  return SICP_OK;
-
 extern "C" int32_t sicp_register_batch(sicp_ctx* ctx, int32_t n_pairs, const double* const* fix_xyz,
                                        const int64_t* n_fix, const double* const* mov_xyz,
                                        const int64_t* n_mov, const sicp_register_params* p,
                                        const double* observed, sicp_pair_result* out, int64_t* n_selected) {
-  SICP_BATCH_API(batch_to_pairs(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected))
+  API_BEGIN(ctx)
+  batch_to_pairs(c, n_pairs, fix_xyz, n_fix, mov_xyz, n_mov, p, observed, out, n_selected);
+  API_END
 }
 
 extern "C" int32_t sicp_set_map(sicp_ctx* ctx, const double* map_xyz, int64_t n_map) {
-  SICP_BATCH_API(set_map(c, map_xyz, n_map))
+  API_BEGIN(ctx)
+  set_map(c, map_xyz, n_map);
+  API_END
 }
 
 extern "C" int32_t sicp_register_to_map(sicp_ctx* ctx, int32_t n_scans, const double* const* mov_xyz,
                                         const int64_t* n_mov, const sicp_register_params* p,
                                         const double* observed, sicp_pair_result* out, int64_t* n_selected) {
-  SICP_BATCH_API(register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected))
+  API_BEGIN(ctx)
+  register_to_map(c, n_scans, mov_xyz, n_mov, p, observed, out, n_selected);
+  API_END
 }
 
 extern "C" int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                        int32_t n_pairs, const int32_t* fix_id, const int32_t* mov_id,
                                        const sicp_register_params* p, const double* observed, sicp_pair_result* out,
                                        int64_t* n_selected) {
-  SICP_BATCH_API(register_pairs(c, n_clouds, xyz, n, n_pairs, fix_id, mov_id, p, observed, out, n_selected))
+  API_BEGIN(ctx)
+  register_pairs(c, n_clouds, xyz, n, n_pairs, fix_id, mov_id, p, observed, out, n_selected);
+  API_END
 }
 
 extern "C" int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                        int32_t n_edges, const int32_t* fix_id, const int32_t* mov_id,
                                        const int32_t* is_fixed, const double* H0, const sicp_register_params* p,
                                        double* H_out, sicp_pair_result* out, int64_t* n_selected) {
-  SICP_BATCH_API(register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, p, H_out, out, n_selected))
+  API_BEGIN(ctx)
+  register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, p, H_out, out, n_selected);
+  API_END
 }
 
 extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                    const double* H, double voxel_size, int64_t* n_added) {
-  SICP_BATCH_API(map_insert(c, n_clouds, xyz, n, H, voxel_size, n_added))
+  API_BEGIN(ctx)
+  map_insert(c, n_clouds, xyz, n, H, voxel_size, n_added);
+  API_END
 }
 
 extern "C" int32_t sicp_get_map(sicp_ctx* ctx, double* xyz, int64_t cap, int64_t* n) {
-  SICP_BATCH_API(get_map(c, xyz, cap, n))
+  API_BEGIN(ctx)
+  get_map(c, xyz, cap, n);
+  API_END
 }
 
 extern "C" int32_t sicp_map_crop(sicp_ctx* ctx, int32_t n_centers, const double* centers, double radius,
                                  int64_t* n_removed) {
-  SICP_BATCH_API(map_crop(c, n_centers, centers, radius, n_removed))
+  API_BEGIN(ctx)
+  map_crop(c, n_centers, centers, radius, n_removed);
+  API_END
 }
 
 extern "C" int32_t sicp_map_thin(sicp_ctx* ctx, double voxel_size, int64_t* n_removed) {
-  SICP_BATCH_API(map_thin(c, voxel_size, n_removed))
+  API_BEGIN(ctx)
+  map_thin(c, voxel_size, n_removed);
+  API_END
 }
 
 extern "C" int32_t sicp_map_carve(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                   const double* H, const double* origins, double radius, double margin,
                                   int32_t min_passes, uint32_t* passes, int64_t* n_removed) {
-  SICP_BATCH_API(map_carve(c, n_clouds, xyz, n, H, origins, radius, margin, min_passes, passes, n_removed))
+  API_BEGIN(ctx)
+  map_carve(c, n_clouds, xyz, n, H, origins, radius, margin, min_passes, passes, n_removed);
+  API_END
 }
 
 extern "C" int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                       const double* H, double max_distance, int32_t neighbors, int64_t* const* idx,
                                       double* const* dist2, double* const* plane_dist, float* const* planarity,
                                       int64_t* n_within) {
-  SICP_BATCH_API(map_distances(c, n_clouds, xyz, n, H, max_distance, neighbors, idx, dist2, plane_dist, planarity,
-                               n_within))
+  API_BEGIN(ctx)
+  map_distances(c, n_clouds, xyz, n, H, max_distance, neighbors, idx, dist2, plane_dist, planarity, n_within);
+  API_END
 }
 
 extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double* const* mov_xyz_out,
                                           double* const* residuals, sicp_iter_record* log, double* T) {
-  SICP_BATCH_API(get_batch_outputs(c, n_pairs, mov_xyz_out, residuals, log, T))
+  API_BEGIN(ctx)
+  get_batch_outputs(c, n_pairs, mov_xyz_out, residuals, log, T);
+  API_END
 }

@@ -209,32 +209,6 @@ void upload_to_device(Ctx& c, void* dst, const void* src, size_t bytes) { upload
 
 using namespace sicp;
 
-#define API_BEGIN(ctxptr)                                    \
-  if (!(ctxptr)) {                                           \
-    sicp::set_thread_error("sicp_ctx is NULL");              \
-    return SICP_ERR_BAD_ARG;                                 \
-  }                                                          \
-  Ctx& c = (ctxptr)->c;                                      \
-  try {                                                      \
-    SICP_CUDA(cudaSetDevice(c.device));
-
-#define API_END                                              \
-  }                                                          \
-  catch (const sicp::Error& e) {                             \
-    c.up.cancel();                                           \
-    c.err = e.msg;                                           \
-    sicp::set_thread_error(e.msg);                           \
-    if (e.code == SICP_ERR_CUDA) cudaGetLastError();         \
-    return e.code;                                           \
-  }                                                          \
-  catch (const std::exception& e) {                          \
-    c.up.cancel();                                           \
-    c.err = e.what();                                        \
-    sicp::set_thread_error(c.err);                           \
-    return SICP_ERR_CUDA;                                    \
-  }                                                          \
-  return SICP_OK;
-
 extern "C" {
 
 int32_t sicp_abi_version(void) { return SICP_ABI_VERSION; }

@@ -582,3 +582,32 @@ struct sicp_ctx {
   sicp::Ctx c;
   int it_counter = 0;
 };
+
+// Body of every entry point that takes a context: API_BEGIN(ctx) binds `c` to it and makes its
+// device current, API_END turns what the body throws into the return code, the context's and the
+// thread's message, and cancels pending staged uploads.
+#define API_BEGIN(ctxptr)                                    \
+  if (!(ctxptr)) {                                           \
+    sicp::set_thread_error("sicp_ctx is NULL");              \
+    return SICP_ERR_BAD_ARG;                                 \
+  }                                                          \
+  sicp::Ctx& c = (ctxptr)->c;                                \
+  try {                                                      \
+    SICP_CUDA(cudaSetDevice(c.device));
+
+#define API_END                                              \
+  }                                                          \
+  catch (const sicp::Error& e) {                             \
+    c.up.cancel();                                           \
+    c.err = e.msg;                                           \
+    sicp::set_thread_error(e.msg);                           \
+    if (e.code == SICP_ERR_CUDA) cudaGetLastError();         \
+    return e.code;                                           \
+  }                                                          \
+  catch (const std::exception& e) {                          \
+    c.up.cancel();                                           \
+    c.err = e.what();                                        \
+    sicp::set_thread_error(c.err);                           \
+    return SICP_ERR_CUDA;                                    \
+  }                                                          \
+  return SICP_OK;
