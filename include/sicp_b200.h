@@ -383,7 +383,8 @@ int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const
  *  - Outputs: H_out[c] = the final T_c; fixed and unreferenced clouds get H0 (identity for a NULL
  *    H0) bit for bit.  out[e]: status, the call's iterations and convergence, the edge's last
  *    n_kept, H = final T_a^-1 T_b, x = the edge's last increment in frame a, mean_res / std_res of
- *    the final linear-model residuals (two-pass), sigma NaN.  Converged when at an iteration i > 0
+ *    the final linear-model residuals (two-pass), sigma NaN (the a-posteriori covariances of every
+ *    pose and every edge come from sicp_get_joint_covariances).  Converged when at an iteration i > 0
  *    every edge with >= 6 kept rows meets the stop rule.
  *  - Failures: an edge without overlap under R_e gets SICP_ERR_NO_OVERLAP and takes no part (the
  *    call returns SICP_ERR_NO_OVERLAP if that leaves a free cloud without a path to a fixed one);
@@ -579,6 +580,35 @@ int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
                                double* const* residuals   /*[h|d] per pair out[i].n_kept, or NULL*/,
                                sicp_iter_record* log      /*[h] n_pairs x max_iterations, or NULL*/,
                                double* T                  /*[h] n_pairs x 16, or NULL*/);
+
+/* ---- a-posteriori covariances of a joint registration (DESIGN.md §6.9) ------------------------
+ * sicp_get_joint_covariances returns, for the LAST sicp_register_joint on this context, the
+ * covariance of every cloud's pose and of every edge's relative pose, all from its final iteration
+ * (the last one whose solve ran; its increments gave the returned poses):
+ *  - N is that iteration's joint normal matrix over the edges with >= 6 kept rows, unweighted.
+ *    s0^2 = sum_e sum_i r_ei^2 / (sum_e n_e - 6 F) over those edges, r_ei the final residuals that
+ *    sicp_get_batch_outputs returns and n_e = out[e].n_kept; a denominator <= 0 makes s0 and every
+ *    covariance NaN.
+ *  - cloud_cov[c] = Cov(u_c), u_c = (omega_c, do_c): the world-frame rotation increment (radians)
+ *    and the world displacement of the cloud's origin o_c (the translation of the returned T_c), at
+ *    the returned poses.  With y_c the centred unknowns of N (DESIGN.md §6.9) u_c = J_c y_c,
+ *    J_c = [[I, 0], [-[o_c - c_w]x, I]] and C_c = s0^2 J_c (N^-1)_cc J_c^T.  A fixed cloud some edge
+ *    references gets exact zeros, a cloud no edge references NaN.
+ *  - edge_cov[e] = Cov(u_e) for e = (a, b), u_e = (alpha_e, dq_e): the rotation increment of
+ *    T_a^-1 T_b in frame-a axes and the displacement of o_b expressed in frame a.  u_e = G_b u_b -
+ *    G_a u_a with G_b = diag(R_a^T, R_a^T), G_a = [[R_a^T, 0], [-R_a^T [o_b - o_a]x, R_a^T]], so C_e =
+ *    G_b C_bb G_b^T + G_a C_aa G_a^T - G_b C_ba G_a^T - G_a C_ab G_b^T with the cross-covariances
+ *    of the two clouds.  Defined for every edge, also one that took no part in the final iteration.
+ *  - Row-major 6 x 6 blocks in the variable order above.  The per-edge sigma of out[] stays NaN.
+ *  - The first request after the call computes them on the device (sicp_register_joint itself does
+ *    no extra work and its timings do not include it); every later one returns the same bits.
+ *  - SICP_ERR_STATE whenever sicp_get_batch_outputs would return it, and when the last batched
+ *    call was not a sicp_register_joint.  SICP_ERR_BAD_ARG: n_clouds or n_edges differs from that
+ *    call's.  A NULL output is skipped.  Nothing else changes: the batch outputs, the map and the
+ *    one-pair state.                                                                             */
+int32_t sicp_get_joint_covariances(sicp_ctx* ctx, int32_t n_clouds,
+                                   double* cloud_cov /*[h] n_clouds x 36, or NULL*/, int32_t n_edges,
+                                   double* edge_cov /*[h] n_edges x 36, or NULL*/, double* s0 /*[h] or NULL*/);
 
 /* ---- PointCloud.transform_by_H (pointcloud.py:205-217), final application simpleicp.py:316 -- */
 int32_t sicp_transform(sicp_ctx* ctx, const double H[16], double* mov_xyz_out /*[h|d] n_mov x 3*/);

@@ -312,14 +312,17 @@ _JOINT_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "m
 class JointResult:
     """simpleicp_joint's return value: H (n_clouds, 4, 4) final poses, world <- cloud; table the
     (n_edges, 20) record table of simpleicp_edges with H = the final T_a^-1 T_b of each edge;
-    iterations and converged of the call; results (full_output) the per-edge result objects."""
+    iterations and converged of the call; results (full_output) the per-edge result objects; with
+    covariances=True cov (n_clouds, 6, 6), edge_cov (n_edges, 6, 6) and s0, the a-posteriori
+    covariances of sicp_get_joint_covariances (else None)."""
 
-    def __init__(self, H, table, iterations, converged, results=None):
+    def __init__(self, H, table, iterations, converged, results=None, cov=None, edge_cov=None, s0=None):
         self.H, self.table, self.iterations, self.converged, self.results = H, table, iterations, converged, results
+        self.cov, self.edge_cov, self.s0 = cov, edge_cov, s0
 
 
 def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
-                    full_output: bool = False, **run_kwargs) -> JointResult:
+                    full_output: bool = False, covariances: bool = False, **run_kwargs) -> JointResult:
     """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
     (a, b) of `edges` -- scan-to-scan pairs such as (i, i + 1), (i, i + 2) and loop closures -- is
     registered consistently.  Each iteration matches every edge as simpleicp_edges would under the
@@ -335,7 +338,15 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     on one device (sicp_register_joint).  `on_error` and `full_output` are as in simpleicp_edges:
     an edge that failed (no overlap, too few correspondences) has its status in the table and raises
     BatchError under "raise"; a failure of the whole call (SICP_ERR_SINGULAR, or a free cloud left
-    without a path to a fixed one by the edges without overlap) raises SicpError."""
+    without a path to a fixed one by the edges without overlap) raises SicpError.
+
+    `covariances=True` also returns the a-posteriori covariances of the final iteration
+    (sicp_get_joint_covariances, DESIGN.md §6.9): cov[c] of cloud c's (rotation increment, origin
+    displacement) in the world frame, zeros for a fixed cloud and NaN for a cloud no edge
+    references; edge_cov[e] of edge (a, b)'s (rotation increment, displacement of b's origin) in
+    frame a; s0 the a-posteriori standard deviation of unit weight."""
+    if not isinstance(covariances, (bool, np.bool_)):
+        raise TypeError(f"covariances must be True or False, got {covariances!r}")
     _check_run_keys(run_kwargs, _JOINT_KEYS, "simpleicp_joint", "edge")
     n_clouds = len(clouds)
     e = _check_edges(edges, n_clouds)
@@ -393,9 +404,10 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         if full_output:
             results = [None if o is None else _batch_result(r, o, np.zeros(6), (0.0,) * 6)
                        for r, o in zip(res, eng.batch_outputs(res))]
+        cov = eng.joint_covariances(n_clouds, n) if covariances else (None, None, None)
     ok = [r for r in res if r.status == 0]
     out = JointResult(H, table, max((int(r.iterations) for r in ok), default=0),
-                      bool(ok) and all(bool(r.converged) for r in ok), results)
+                      bool(ok) and all(bool(r.converged) for r in ok), results, *cov)
     _raise_failed(table, on_error, messages, results)
     return out
 

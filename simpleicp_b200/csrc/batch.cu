@@ -502,6 +502,15 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
 
   JointStore& js = b.joint;
   const int npad = (6 * F + 1 + 31) / 32 * 32;
+  js.n_clouds = j.n_clouds;
+  js.n_edges = n_edges;
+  js.F = F;
+  js.npad = npad;
+  for (int k = 0; k < 3; ++k) js.cw[k] = cw[k];
+  js.role.assign((size_t)j.n_clouds, 0);
+  for (int e = 0; e < n_edges; ++e)
+    for (int cl : {j.fix_id[e], j.mov_id[e]}) js.role[(size_t)cl] = j.free_of[(size_t)cl] >= 0 ? 2 : 1;
+  js.cov_done = false;
   js.edges.reserve(n_edges);
   js.flags.reserve(1);
   js.pose.reserve(j.n_clouds);
@@ -736,6 +745,68 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
     b.out_mean_std[2 * (size_t)i + 1] = out[i].std_res;
   }
   b.out_valid = true;
+  b.out_joint = r.joint != nullptr;
+}
+
+// sicp_get_joint_covariances: the first request after a sicp_register_joint runs joint_cov_launch
+// on what its final iteration left and keeps the result on the host; every later one copies it.
+static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n_edges, double* edge_cov,
+                                  double* s0) {
+  SICP_REQUIRE(c.batch && c.batch->out_valid && c.batch->out_joint, SICP_ERR_STATE,
+               "no joint covariances: the last batched call on this context was not a successful "
+               "sicp_register_joint, or a later call cleared its outputs");
+  Batch& b = *c.batch;
+  JointStore& js = b.joint;
+  SICP_REQUIRE(n_clouds == js.n_clouds && n_edges == js.n_edges, SICP_ERR_BAD_ARG,
+               "n_clouds and n_edges must equal the last sicp_register_joint's (" + std::to_string(js.n_clouds) +
+                   ", " + std::to_string(js.n_edges) + ")");
+  if (!js.cov_done) {
+    const int F = js.F, ne = js.n_edges;
+    js.Z.reserve((size_t)js.npad * js.npad);
+    js.cov.reserve((size_t)ne + 1 + 36 * ((size_t)F + ne));
+    JointCovArgs a{};
+    a.pairs = b.pairs.p;
+    a.state = b.state.p;
+    a.keep = b.keep.p;
+    a.m_xyz = b.m_xyz.p;
+    a.q_xyz = b.q_xyz.p;
+    a.q_nrm = b.q_nrm.p;
+    a.edges = js.edges.p;
+    a.pose = js.pose.p;
+    a.fix_id = js.ids.p;
+    a.mov_id = js.ids.p + ne;
+    a.free_of = js.ids.p + 2 * ne;
+    a.free_ids = a.free_of + js.n_clouds;
+    a.L = js.A.p;
+    a.Z = js.Z.p;
+    a.ss = js.cov.p;
+    a.s0sq = a.ss + ne;
+    a.cov_f = a.s0sq + 1;
+    a.cov_e = a.cov_f + 36 * (size_t)F;
+    a.bar = js.bar.p;
+    a.F = F;
+    a.n_edges = ne;
+    a.npad = js.npad;
+    for (int k = 0; k < 3; ++k) a.cw[k] = js.cw[k];
+    joint_cov_launch(c, a);
+    std::vector<double> h(1 + 36 * ((size_t)F + ne));
+    SICP_CUDA(cudaMemcpyAsync(h.data(), a.s0sq, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, c.stream));
+    SICP_CUDA(cudaStreamSynchronize(c.stream));
+    const double nan = std::nan(""), s0sq = h[0];
+    js.s0 = std::sqrt(s0sq);
+    // a fixed cloud some edge references: 0 (NaN with s0); one no edge references: NaN
+    js.cov_cloud.assign(36 * (size_t)js.n_clouds, std::isnan(s0sq) ? nan : 0.0);
+    for (int i = 0, f = 0; i < js.n_clouds; ++i) {
+      double* dst = js.cov_cloud.data() + 36 * (size_t)i;
+      if (js.role[(size_t)i] == 2) std::memcpy(dst, h.data() + 1 + 36 * (size_t)f++, sizeof(double) * 36);
+      else if (js.role[(size_t)i] == 0) std::fill(dst, dst + 36, nan);
+    }
+    js.cov_edge.assign(h.begin() + 1 + 36 * (size_t)F, h.end());
+    js.cov_done = true;
+  }
+  if (cloud_cov) std::memcpy(cloud_cov, js.cov_cloud.data(), sizeof(double) * js.cov_cloud.size());
+  if (edge_cov) std::memcpy(edge_cov, js.cov_edge.data(), sizeof(double) * js.cov_edge.size());
+  if (s0) *s0 = js.s0;
 }
 
 // sicp_get_batch_outputs: everything is read from the buffers the last run_pairs left behind.
@@ -1495,5 +1566,12 @@ extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double
                                           double* const* residuals, sicp_iter_record* log, double* T) {
   API_BEGIN(ctx)
   get_batch_outputs(c, n_pairs, mov_xyz_out, residuals, log, T);
+  API_END
+}
+
+extern "C" int32_t sicp_get_joint_covariances(sicp_ctx* ctx, int32_t n_clouds, double* cloud_cov, int32_t n_edges,
+                                              double* edge_cov, double* s0) {
+  API_BEGIN(ctx)
+  get_joint_covariances(c, n_clouds, cloud_cov, n_edges, edge_cov, s0);
   API_END
 }

@@ -275,6 +275,32 @@ struct JointArgs {
   double cw[3];            // the common world centre of the increments
   double min_planarity, min_change;
 };
+// sicp_get_joint_covariances (joint.cu: joint_cov_launch), from what the final iteration of the
+// last sicp_register_joint left: the factor L of its joint matrix (upper-left n x n of A), the
+// edges' final kept rows and residuals, and the returned poses.
+struct JointCovArgs {
+  const PairDev* pairs;
+  const DevState* state;
+  const uint8_t* keep;
+  const double* m_xyz;
+  const double* q_xyz;
+  const float4* q_nrm;
+  const JointEdge* edges;
+  const Rigid* pose;
+  const int* fix_id;
+  const int* mov_id;
+  const int* free_of;
+  const int* free_ids;
+  const double* L;    // npad x npad, row-major, lower triangle
+  double* Z;          // npad x npad: L^-1 in the lower triangle of the first n rows and columns
+  double* ss;         // per edge: sum of squared final residuals (0 for an edge that took no part)
+  double* s0sq;       // [1]: s0^2 (NaN when the redundancy is <= 0)
+  double* cov_f;      // per free cloud: C_c, row-major 6 x 6
+  double* cov_e;      // per edge: C_e
+  unsigned int* bar;  // grid barrier of k_joint_inv, {0, any} between launches
+  int F, n_edges, npad;
+  double cw[3];
+};
 struct JointStore {
   DevBuf<JointEdge> edges;
   DevBuf<JointFlags> flags;
@@ -283,12 +309,24 @@ struct JointStore {
   DevBuf<double> A;
   DevBuf<unsigned int> bar;
   JointFlags* flags_host = nullptr;  // pinned
+  // what sicp_get_joint_covariances needs of the last call (set by joint_loop), and its cache:
+  // per cloud and per edge row-major 6 x 6 blocks and s0, computed by the first get after the call
+  int n_clouds = 0, n_edges = 0, F = 0, npad = 0;
+  double cw[3] = {0, 0, 0};
+  std::vector<char> role;  // per cloud: 0 no edge references it, 1 fixed, 2 free
+  DevBuf<double> Z, cov;   // cov: ss (n_edges), s0^2 (1), C_c (F x 36), C_e (n_edges x 36)
+  bool cov_done = false;
+  std::vector<double> cov_cloud, cov_edge;
+  double s0 = 0.0;
   ~JointStore() {
     if (flags_host) cudaFreeHost(flags_host);
   }
 };
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges);
 void joint_solve_launch(Ctx& c, const JointArgs& a);
+// k_joint_cov_ss, k_joint_inv, k_joint_cov_cloud, k_joint_cov_edge: the covariances of the last
+// sicp_register_joint into a.cov_f / a.cov_e and s0^2 into a.s0sq (DESIGN.md §6.9)
+void joint_cov_launch(Ctx& c, const JointCovArgs& a);
 
 struct Batch {
   int n_pairs = 0;
@@ -337,6 +375,7 @@ struct Batch {
   // replace the map, and set only when one of the three returns successfully; the vectors are per
   // pair of that call.
   bool out_valid = false;
+  bool out_joint = false;  // that call was a sicp_register_joint (sicp_get_joint_covariances)
   int out_n_pairs = 0, out_max_iterations = 0;
   std::vector<long long> out_n_mov, out_n_kept;  // movable points, kept residuals
   std::vector<int> out_status, out_iterations; // sicp_status (SICP_ERR_NO_OVERLAP included), iterations run

@@ -13,6 +13,14 @@
 //                    back substitution; the pose update of every free cloud, each edge's new
 //                    relative transform, increment, residual statistics, record and stop rule
 //
+// and, on the first sicp_get_joint_covariances after a call, from what its final iteration left:
+//
+//   k_joint_cov_ss     one block per edge: the sum of the squared final residuals of its kept rows
+//   k_joint_inv        one cooperative launch: Z = L^-1 of the final factor, by 32 x 32 tiles
+//   k_joint_cov_cloud  one block per free cloud: s0^2, the block (N^-1)_cc = sum_k Z_kc^T Z_kc and
+//                      C_c = s0^2 J_c (N^-1)_cc J_c^T
+//   k_joint_cov_edge   one block per edge: the cross block of two free clouds and C_e
+//
 // DESIGN.md §6.9 gives the rule, the Ad mapping and the centring.  Every sum runs in a fixed
 // order (no atomics), so repeated calls give the same bits.
 #include "ctx.cuh"
@@ -438,6 +446,281 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
   }
 }
 
+// ---- sicp_get_joint_covariances: Cov(y) = s0^2 N^-1 = s0^2 Z^T Z with Z = L^-1 -------------------
+
+constexpr int JC_THREADS = 256;
+constexpr int JC_WARPS = JC_THREADS / 32;
+
+// k_joint_cov_ss, one block per edge: ss[e] = the sum of the squared final residuals of the kept
+// rows (final_residual: the values sicp_get_batch_outputs returns) of an edge that took part in the
+// final iteration, else 0.
+__global__ void __launch_bounds__(JC_THREADS) k_joint_cov_ss(const JointCovArgs a) {
+  __shared__ double red[JC_WARPS];
+  const int e = blockIdx.x, tid = threadIdx.x;
+  double acc = 0.0;
+  if (a.edges[e].part) {
+    const PairDev& pd = a.pairs[e];
+    const Rigid Tn = a.state[e].T_res;
+    for (long long i = tid; i < pd.K; i += JC_THREADS)
+      if (a.keep[pd.q_off + i]) {
+        const double r = final_residual(Tn, a.m_xyz, a.q_xyz, a.q_nrm, pd.q_off + i);
+        acc = fma(r, r, acc);
+      }
+  }
+  acc = warp_sum(acc);
+  if ((tid & 31) == 0) red[tid >> 5] = acc;
+  __syncthreads();
+  if (tid == 0) {
+    double v = 0.0;
+    for (int w = 0; w < JC_WARPS; ++w) v += red[w];
+    a.ss[e] = v;
+  }
+}
+
+// tile (ti, tj) of the factor of N: the rows and columns from n on are the identity's
+__device__ void load_l_tile(double (&t)[TS][TS + 1], const double* L, int npad, int n, int ti, int tj) {
+  for (int e = threadIdx.x; e < TS * TS; e += JS_THREADS) {
+    const int r = ti * TS + e / TS, c = tj * TS + e % TS;
+    t[e / TS][e % TS] = (r < n && c < n) ? L[(size_t)r * npad + c] : (r == c ? 1.0 : 0.0);
+  }
+}
+
+// p[q] = (X Y)[r][c] for the element e = tid + q JS_THREADS, r = e / TS, c = e % TS
+constexpr int TQ = TS * TS / JS_THREADS;
+__device__ __forceinline__ void tile_mul(const double (&X)[TS][TS + 1], const double (&Y)[TS][TS + 1], double (&p)[TQ]) {
+#pragma unroll
+  for (int q = 0; q < TQ; ++q) {
+    const int e = threadIdx.x + q * JS_THREADS, r = e / TS, c = e % TS;
+    double s = 0.0;
+#pragma unroll 8
+    for (int m = 0; m < TS; ++m) s = fma(X[r][m], Y[m][c], s);
+    p[q] = s;
+  }
+}
+
+// k_joint_inv, one cooperative launch: Z = L^-1 by tiles.  First every diagonal tile Z_kk = L_kk^-1
+// (forward substitution, one column per thread); then, for k = 0, 1, .., the right-looking update of
+// the block rows below k: B_ij -= L_ik Z_kj for i > k, j <= k (B_ij starts at 0, so its first update,
+// at k = j, is a store), and the tiles of row k + 1, whose sum is then complete, become
+// Z_(k+1)j = Z_(k+1)(k+1) B_(k+1)j.  One grid barrier per k; each B_ij takes its updates in
+// ascending k.  Only tiles on or below the diagonal are written.
+__global__ void __launch_bounds__(JS_THREADS) k_joint_inv(const JointCovArgs a) {
+  __shared__ double t0[TS][TS + 1];
+  __shared__ double t1[TS][TS + 1];
+  const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
+  const int n = 6 * a.F, npad = a.npad, KN = (n + TS - 1) / TS;
+  for (int k = bid; k < KN; k += G) {
+    load_l_tile(t0, a.L, npad, n, k, k);
+    __syncthreads();
+    if (tid < TS) {
+      const int c = tid;
+      for (int r = 0; r < TS; ++r) {
+        double v = 0.0;
+        if (r >= c) {
+          v = (r == c) ? 1.0 : 0.0;
+          for (int m = c; m < r; ++m) v = fma(-t0[r][m], t1[m][c], v);
+          v /= t0[r][r];
+        }
+        t1[r][c] = v;
+      }
+    }
+    __syncthreads();
+    store_tile(t1, a.Z, npad, k, k);
+    __syncthreads();
+  }
+  joint_grid_sync(a.bar);
+  for (int k = 0; k + 1 < KN; ++k) {
+    const int w = k + 1, cnt = (KN - 1 - k) * w;
+    for (int t = bid; t < cnt; t += G) {
+      const int i = k + 1 + t / w, j = t % w;
+      load_l_tile(t0, a.L, npad, n, i, k);
+      load_tile(t1, a.Z, npad, k, j);
+      __syncthreads();
+      double p[TQ], bv[TQ];
+      tile_mul(t0, t1, p);
+#pragma unroll
+      for (int q = 0; q < TQ; ++q) {
+        const int e = tid + q * JS_THREADS;
+        const size_t at = (size_t)(i * TS + e / TS) * npad + j * TS + e % TS;
+        bv[q] = (j == k) ? -p[q] : __ldcg(&a.Z[at]) - p[q];
+      }
+      if (i == k + 1) {
+        __syncthreads();
+        load_tile(t0, a.Z, npad, i, i);
+#pragma unroll
+        for (int q = 0; q < TQ; ++q) {
+          const int e = tid + q * JS_THREADS;
+          t1[e / TS][e % TS] = bv[q];
+        }
+        __syncthreads();
+        tile_mul(t0, t1, bv);
+      }
+#pragma unroll
+      for (int q = 0; q < TQ; ++q) {
+        const int e = tid + q * JS_THREADS;
+        __stcg(&a.Z[(size_t)(i * TS + e / TS) * npad + j * TS + e % TS], bv[q]);
+      }
+      __syncthreads();
+    }
+    joint_grid_sync(a.bar);
+  }
+}
+
+// g[6 i + j] = sum over k >= max(c0, c1) of Z[k][c0 + i] Z[k][c1 + j] (a 6 x 6 block of Z^T Z), by
+// the whole block: rows strided over the threads, then the warps' sums in warp order.  Z is lower
+// triangular: an entry above the diagonal counts as 0 and is not read.
+__device__ void gram6(const double* Z, int npad, int n, int c0, int c1, double (&red)[JC_WARPS][36], double* g) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double acc[36];
+#pragma unroll
+  for (int j = 0; j < 36; ++j) acc[j] = 0.0;
+  for (int k = max(c0, c1) + tid; k < n; k += JC_THREADS) {
+    const double* row = Z + (size_t)k * npad;
+    double x[6], y[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+      x[i] = (k >= c0 + i) ? row[c0 + i] : 0.0;
+      y[i] = (k >= c1 + i) ? row[c1 + i] : 0.0;
+    }
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) acc[6 * i + j] = fma(x[i], y[j], acc[6 * i + j]);
+  }
+#pragma unroll
+  for (int j = 0; j < 36; ++j) {
+    const double v = warp_sum(acc[j]);
+    if (lane == 0) red[warp][j] = v;
+  }
+  __syncthreads();
+  if (tid < 36) {
+    double v = 0.0;
+    for (int w = 0; w < JC_WARPS; ++w) v += red[w][tid];
+    g[tid] = v;
+  }
+  __syncthreads();
+}
+
+// out = A M B^T, 6 x 6 row-major
+__device__ void abt6(const double* A, const double* M, const double* B, double* out) {
+  double AM[36];
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) {
+      double v = 0.0;
+      for (int m = 0; m < 6; ++m) v = fma(A[6 * r + m], M[6 * m + c], v);
+      AM[6 * r + c] = v;
+    }
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) {
+      double v = 0.0;
+      for (int m = 0; m < 6; ++m) v = fma(AM[6 * r + m], B[6 * c + m], v);
+      out[6 * r + c] = v;
+    }
+}
+
+// [[P, 0], [-P [d]x, P]] with P = I (Q null) or Q^T (Q a row-major rotation): J_c for d = o_c - c_w,
+// G_a for Q = R_a, d = o_b - o_a
+__device__ void lever6(const double* Q, const double* d, double* out) {
+  double P[9];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) P[3 * r + c] = Q ? Q[3 * c + r] : (r == c ? 1.0 : 0.0);
+  const double S[9] = {0.0, -d[2], d[1], d[2], 0.0, -d[0], -d[1], d[0], 0.0};
+  for (int j = 0; j < 36; ++j) out[j] = 0.0;
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) {
+      double ps = 0.0;
+      for (int m = 0; m < 3; ++m) ps = fma(P[3 * r + m], S[3 * m + c], ps);
+      out[6 * r + c] = P[3 * r + c];
+      out[6 * (r + 3) + c + 3] = P[3 * r + c];
+      out[6 * (r + 3) + c] = -ps;
+    }
+}
+
+// the lower triangle of C mirrored, NaN everywhere when s0^2 is
+__device__ void store_sym6(const double* C, double s0sq, double* out) {
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c <= r; ++c) {
+      const double v = (s0sq == s0sq) ? C[6 * r + c] : s0sq;
+      out[6 * r + c] = v;
+      out[6 * c + r] = v;
+    }
+}
+
+// k_joint_cov_cloud, one block per free cloud p: s0^2 from the edges' sums (warp 0, fixed order;
+// block 0 stores it), the diagonal block (N^-1)_pp and C_c = s0^2 J_c (N^-1)_pp J_c^T
+__global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovArgs a) {
+  __shared__ double red[JC_WARPS][36];
+  __shared__ double g[36];
+  __shared__ double s0sq_s;
+  const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int n = 6 * a.F;
+  if (tid < 32) {
+    double ss = 0.0, m = 0.0;
+    for (int e = lane; e < a.n_edges; e += 32)
+      if (a.edges[e].part) {
+        ss += a.ss[e];
+        m += (double)a.edges[e].n;
+      }
+    ss = warp_sum(ss);
+    m = warp_sum(m);
+    if (lane == 0) {
+      const double dof = m - (double)n;
+      s0sq_s = dof > 0.0 ? ss / dof : nan("");
+      if (p == 0) *a.s0sq = s0sq_s;
+    }
+  }
+  gram6(a.Z, a.npad, n, 6 * p, 6 * p, red, g);
+  if (tid != 0) return;
+  const Rigid& T = a.pose[a.free_ids[p]];
+  const double d[3] = {T.t[0] - a.cw[0], T.t[1] - a.cw[1], T.t[2] - a.cw[2]};
+  double Jc[36], C[36], M[36];
+  lever6(nullptr, d, Jc);
+  for (int j = 0; j < 36; ++j) M[j] = s0sq_s * g[j];
+  abt6(Jc, M, Jc, C);
+  store_sym6(C, s0sq_s, a.cov_f + 36 * (size_t)p);
+}
+
+// k_joint_cov_edge, one block per edge e = (a, b): with both clouds free the cross block
+// (N^-1)_ab and C_ab = s0^2 J_a (N^-1)_ab J_b^T; then C_e = G_b C_b G_b^T + G_a C_a G_a^T - M - M^T,
+// M = G_a C_ab G_b^T, at the returned poses (a fixed cloud's blocks are 0)
+__global__ void __launch_bounds__(JC_THREADS) k_joint_cov_edge(const JointCovArgs a) {
+  __shared__ double red[JC_WARPS][36];
+  __shared__ double g[36];
+  const int e = blockIdx.x, tid = threadIdx.x;
+  const int ca = a.fix_id[e], cb = a.mov_id[e], fa = a.free_of[ca], fb = a.free_of[cb];
+  if (fa >= 0 && fb >= 0) gram6(a.Z, a.npad, 6 * a.F, 6 * fa, 6 * fb, red, g);
+  if (tid != 0) return;
+  const double s0sq = *a.s0sq;
+  const Rigid &Ta = a.pose[ca], &Tb = a.pose[cb];
+  const double dba[3] = {Tb.t[0] - Ta.t[0], Tb.t[1] - Ta.t[1], Tb.t[2] - Ta.t[2]}, zero[3] = {0.0, 0.0, 0.0};
+  double Ga[36], Gb[36], C[36], X[36];
+  lever6(Ta.r, dba, Ga);
+  lever6(Ta.r, zero, Gb);
+  for (int j = 0; j < 36; ++j) C[j] = 0.0;
+  if (fb >= 0) {
+    abt6(Gb, a.cov_f + 36 * (size_t)fb, Gb, X);
+    for (int j = 0; j < 36; ++j) C[j] += X[j];
+  }
+  if (fa >= 0) {
+    abt6(Ga, a.cov_f + 36 * (size_t)fa, Ga, X);
+    for (int j = 0; j < 36; ++j) C[j] += X[j];
+  }
+  if (fa >= 0 && fb >= 0) {
+    const Rigid &Pa = a.pose[ca], &Pb = a.pose[cb];
+    const double da[3] = {Pa.t[0] - a.cw[0], Pa.t[1] - a.cw[1], Pa.t[2] - a.cw[2]},
+                 db[3] = {Pb.t[0] - a.cw[0], Pb.t[1] - a.cw[1], Pb.t[2] - a.cw[2]};
+    double Ja[36], Jb[36], Cab[36], M[36];
+    lever6(nullptr, da, Ja);
+    lever6(nullptr, db, Jb);
+    for (int j = 0; j < 36; ++j) M[j] = s0sq * g[j];
+    abt6(Ja, M, Jb, Cab);
+    abt6(Ga, Cab, Gb, M);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) C[6 * r + c] -= M[6 * r + c] + M[6 * c + r];
+  }
+  store_sym6(C, s0sq, a.cov_e + 36 * (size_t)e);
+}
+
 }  // namespace
 
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges) {
@@ -451,6 +734,19 @@ void joint_solve_launch(Ctx& c, const JointArgs& a) {
   void* p[] = {&args};
   SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_solve, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
   c.tm.kernel_launches += 1;
+}
+
+// sicp_timings describe the last registration call: these launches do not count in it
+void joint_cov_launch(Ctx& c, const JointCovArgs& a) {
+  k_joint_cov_ss<<<a.n_edges, JC_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+  JointCovArgs args = a;
+  void* p[] = {&args};
+  SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_inv, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
+  k_joint_cov_cloud<<<a.F, JC_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+  k_joint_cov_edge<<<a.n_edges, JC_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
 }
 
 }  // namespace sicp

@@ -151,6 +151,19 @@ __device__ __forceinline__ unsigned long long global_timer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+
+// Residual of query i at the final transform Tn, in the reference's operation order
+// (optimization.py:117-124): the matched movable point moved by Tn, minus the fixed point, dotted
+// with the fixed normal.  The only definition: k_finish_batch takes its statistics from it,
+// k_final_residuals and k_batch_residuals return it, k_joint_cov_ss sums its squares.
+__device__ __forceinline__ double final_residual(const Rigid& Tn, const double* m_xyz, const double* q_xyz,
+                                                 const float4* q_nrm, long long i) {
+  double tx, ty, tz;
+  rigid_apply(Tn, m_xyz[3 * i + 0], m_xyz[3 * i + 1], m_xyz[3 * i + 2], tx, ty, tz);
+  const float4 nr = q_nrm[i];
+  const double dx = tx - q_xyz[3 * i + 0], dy = ty - q_xyz[3 * i + 1], dz = tz - q_xyz[3 * i + 2];
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, (double)nr.x), __dmul_rn(dy, (double)nr.y)), __dmul_rn(dz, (double)nr.z));
+}
 #endif
 
 }  // namespace sicp
