@@ -667,6 +667,14 @@ int32_t sicp_debug_seed_predictor(sicp_ctx* ctx, double med, double mad, double 
  * distance).                                                                                    */
 int32_t sicp_debug_match_counts(sicp_ctx* ctx, int64_t* n_certified /*[h]*/);
 
+/* Diagnostics: %globaltimer stamps (us, from the first block's entry) of the last one-pair grid
+ * match run with the option "match_stamps" set.  Thread 0 of the first block writes slots 0-6,
+ * thread 0 of the last block slots 8-14: kernel entry, dependent-launch wait released, state and
+ * certificate loaded, certified decision made, normal loaded, histogram atomic returned, exit.
+ * Slots 2-5 are only written for a query answered from its certificate; -1 marks a slot not
+ * written.                                                                                      */
+int32_t sicp_get_match_phase_times(sicp_ctx* ctx, double us[16] /*[h]*/);
+
 /* Test-only: the uniform grid the searches run on.  side 0 = the fixed cloud's grid (k-NN of the
  * normals; built by sicp_estimate_normals), 1 = the movable cloud's grid (correspondences; built
  * by sicp_set_clouds).  o = origin (the cloud's bounding-box minimum), h = cell size, dims = cells

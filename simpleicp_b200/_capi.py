@@ -43,7 +43,7 @@ SYMBOLS = (
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_register_joint", "sicp_get_batch_outputs",
     "sicp_get_joint_covariances",
-    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times",
+    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times", "sicp_get_match_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -184,6 +184,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
+        "sicp_get_match_phase_times": [vp, C.POINTER(dbl)],
         "sicp_debug_seed_predictor": [vp, dbl, dbl, dbl],
         "sicp_debug_match_counts": [vp, C.POINTER(i64)],
         "sicp_debug_grid_params": [vp, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(i32)],
@@ -814,6 +815,13 @@ class Engine:
         """Diagnostics: block-0 phase stamps (us) of the last reject+solve kernel."""
         us = (C.c_double * 32)()
         self._check(self._lib.sicp_get_phase_times(self._h, us))
+        return list(us)
+
+    def match_phase_times(self) -> list:
+        """Diagnostics: first- and last-block phase stamps (us) of the last one-pair grid match run
+        with the option match_stamps (sicp_get_match_phase_times)."""
+        us = (C.c_double * 16)()
+        self._check(self._lib.sicp_get_match_phase_times(self._h, us))
         return list(us)
 
     def selection(self) -> dict:

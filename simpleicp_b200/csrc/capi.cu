@@ -346,6 +346,8 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.warm_start = (value != 0) ? 1 : 0;
   } else if (k == "fused") {
     c.fused = (value != 0) ? 1 : 0;
+  } else if (k == "match_stamps") {
+    c.match_stamps = (value != 0) ? 1 : 0;
   } else if (k == "match_group") {
     SICP_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4 || value == 8 || value == 16, SICP_ERR_BAD_ARG,
                  "match_group must be 0 (auto), 1, 2, 4, 8 or 16");
@@ -1097,6 +1099,19 @@ int32_t sicp_get_phase_times(sicp_ctx* ctx, double us[32]) {
     us[i] = (i >= 24) ? (double)t[i]
             : (i == 23 || (t[28] == 2 && (i == 1 || i == 5 || i == 6))) ? (double)(long long)(t[i] - t[0]) * 1e-3
                         : ((t[i] >= t[0]) ? (double)(t[i] - t[0]) * 1e-3 : -1.0);
+  API_END
+}
+
+int32_t sicp_get_match_phase_times(sicp_ctx* ctx, double us[16]) {
+  API_BEGIN(ctx)
+  SICP_REQUIRE(us != nullptr, SICP_ERR_BAD_ARG, "us is NULL");
+  SICP_REQUIRE(c.match_t.p != nullptr, SICP_ERR_STATE, "no match has run with the option match_stamps");
+  unsigned long long t[16];
+  SICP_CUDA(cudaMemcpyAsync(t, c.match_t.p, sizeof(t), cudaMemcpyDeviceToHost, c.stream));
+  sync(c);
+  // first block's stamps in 0-6, the last block's in 8-14, both from the first block's entry; a
+  // point its thread did not pass (a searched query) reads -1
+  for (int i = 0; i < 16; ++i) us[i] = (t[i] != 0 && t[0] != 0) ? (double)(long long)(t[i] - t[0]) * 1e-3 : -1.0;
   API_END
 }
 

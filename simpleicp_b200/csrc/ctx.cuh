@@ -141,6 +141,8 @@ struct Ctx {
   DevBuf<unsigned int> cert_count;   // 2: queries answered from a certificate, by launch parity
   int cert_next = 0;                 // counter of the next certifying launch
   int cert_slot = -1;                // counter of the last match; -1: it could not certify
+  DevBuf<unsigned long long> match_t;  // 16 %globaltimer stamps of the one-pair match (MatchCert::stamps)
+  int match_stamps = 0;              // option "match_stamps": the one-pair match writes match_t
   int warm_start = 1;                // option "warm_start"
   int sphere_scan = 1;               // option "sphere_scan"
   int pdl = 1;                       // option "pdl": programmatic dependent launch between the two kernels of an iteration

@@ -174,15 +174,30 @@ __device__ __forceinline__ double plane_distance_rec(const Rigid& T, const Rec& 
 // slot of a per-bin store of the members' order-preserving distance keys (f64_to_key), so that
 // the reject/solve kernel reads the members of the few bins that hold its order statistics with
 // one load each (no scan, no gather pass, no barrier, no index chase).
-__device__ __forceinline__ void lin_hist_add(const DevState* st, unsigned int* lin_hist,
-                                             float planarity, double d, unsigned long long* binstore,
-                                             int bin_cap, long long qi) {
-  if (lin_hist != nullptr && st->pred_valid && (double)planarity >= st->pred_minpl) {
-    const int b = lh_bin(d, st->pred_med, st->pred_mad);
+struct Pred {
+  double med, mad, minpl;
+  int valid;
+};
+__device__ __forceinline__ Pred load_pred(const DevState* st) {
+  return Pred{st->pred_med, st->pred_mad, st->pred_minpl, st->pred_valid};
+}
+// Returns the slot (0 when the correspondence is not a member), for the diagnostics stamp that
+// marks the atomic's return.
+__device__ __forceinline__ unsigned int lin_hist_add(const Pred& p, unsigned int* lin_hist, float planarity, double d,
+                                                     unsigned long long* binstore, int bin_cap, long long qi) {
+  if (lin_hist != nullptr && p.valid && (double)planarity >= p.minpl) {
+    const int b = lh_bin(d, p.med, p.mad);
     const unsigned int slot = atomicAdd(&lin_hist[b], 1u);
     if (binstore != nullptr && b < LH_BINS && slot < (unsigned int)bin_cap)
       binstore[(size_t)b * bin_cap + slot] = f64_to_key(d);
+    return slot;
   }
+  return 0u;
+}
+__device__ __forceinline__ void lin_hist_add(const DevState* st, unsigned int* lin_hist,
+                                             float planarity, double d, unsigned long long* binstore,
+                                             int bin_cap, long long qi) {
+  lin_hist_add(load_pred(st), lin_hist, planarity, d, binstore, bin_cap, qi);
 }
 
 // Epilogue data of one correspondence for the fused reject/solve kernel: the matched movable
@@ -247,7 +262,31 @@ struct MatchCert {
   float* rho;             // K: radius of the certified ball, rounded down; <= 0: no certificate
   unsigned int* n_cert;   // queries of this launch answered from their certificate
   unsigned int* n_clear;  // the next launch's counter: zeroed here (ctx.cuh: cert_count)
+  unsigned long long* stamps;  // diagnostics, may be null: 16 phase stamps (sicp_get_match_phase_times)
 };
+
+// %globaltimer once `dep` has arrived: the timer read is predicated on a test of dep, so it cannot
+// issue before the loads dep is made of (a plain read would not wait for them).  0 in the
+// (diagnostics-only) case dep == ~0u.
+__device__ __forceinline__ unsigned long long global_timer_after(unsigned int dep) {
+  unsigned long long t;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0xffffffff;\n\tmov.u64 %0, 0;\n\t@p mov.u64 %0, %%globaltimer;\n\t}"
+      : "=l"(t)
+      : "r"(dep));
+  return t;
+}
+// A load the compiler keeps where it is written: it is not merged with a plain load of the same
+// address, and it stays ahead of the dependent-launch wait that follows it in the source (SASS:
+// LDG.STRONG.GPU before ACQBULK).  ptxas moves weak loads, .nc ones included, below the wait.
+__device__ __forceinline__ double ld_early(const double* p) {
+  double v;
+  asm volatile("ld.relaxed.gpu.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ unsigned int dep_bits(double v) {
+  return (unsigned int)__double2hiint(v) ^ (unsigned int)__double2loint(v);
+}
 
 __device__ __forceinline__ void store_matched(const CorrOut& co, long long qi, double x, double y, double z) {
   if (co.m_xyz) {
@@ -299,8 +338,9 @@ __global__ void __launch_bounds__(128)
 // squared distance, keep[qi] = (d2 < cap2), the comparison of k_range_keep (capi.cu).
 // CERT (one-pair match only): read and write the certificates of `cert` (MatchCert above);
 // cert.rho is null when the launch keeps none (with_distance = 0).
+// Returns true on the one lane of a group that answered its query from the certificate.
 template <int MG, bool KEEP = false, bool CERT = false>
-__device__ __forceinline__ void match_coop_body(
+__device__ __forceinline__ bool match_coop_body(
     const GridView& g, const DevState* __restrict__ st, const double* __restrict__ q_xyz,
     const float4* __restrict__ q_nrm, const double* __restrict__ mov_xyz, long long K, int rmax,
     int with_distance, long long* __restrict__ nn_idx, double* __restrict__ out,
@@ -309,41 +349,84 @@ __device__ __forceinline__ void match_coop_body(
     const MatchCert& cert = MatchCert{}) {
   const long long qi = gt / MG;
   const int sub = threadIdx.x & (MG - 1);
+  // diagnostics: thread 0 of the first and of the last block stamps its phases
+  unsigned long long* const stamp =
+      (CERT && cert.stamps != nullptr && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1))
+          ? cert.stamps + ((blockIdx.x == 0) ? 0 : 8)
+          : nullptr;
+  if (stamp) {
+    stamp[0] = global_timer_ns();
+    for (int i = 1; i < 7; ++i) stamp[i] = 0ull;  // a phase this launch does not reach reads -1
+  }
   pdl_launch_dependents();
-  if (qi >= K) return;  // a whole group leaves together
-  // the query's coordinates do not depend on the previous kernel: on their way before the wait
-  const double px = q_xyz[3 * qi + 0], py = q_xyz[3 * qi + 1], pz = q_xyz[3 * qi + 2];
+  if (qi >= K) return false;  // a whole group leaves together
+  // The query's coordinates do not depend on the previous kernel: on their way before the wait.
+  // The certified path takes its own copy through ld_early (below): a plain load is one value
+  // with the search's copy, which lives through the whole search, so at the register bound the
+  // compiler spilled it at once (waiting for the cold line before the wait) or sank the load
+  // below the wait.  The search reads q_xyz again after the decision (an L1/L2 hit).
+  double px, py, pz;
+  if constexpr (!CERT) {
+    px = q_xyz[3 * qi + 0];
+    py = q_xyz[3 * qi + 1];
+    pz = q_xyz[3 * qi + 2];
+  }
+  double epx = 0.0, epy = 0.0, epz = 0.0;
+  if constexpr (CERT) {
+    if (co.warm) {
+      epx = ld_early(q_xyz + 3 * qi + 0);
+      epy = ld_early(q_xyz + 3 * qi + 1);
+      epz = ld_early(q_xyz + 3 * qi + 2);
+    }
+  }
   pdl_wait();
+  if (stamp) stamp[1] = global_timer_ns();
   if constexpr (CERT) {
     if (gt == 0 && cert.n_clear) *cert.n_clear = 0u;
+    // Fast path: |q - c| < rho (computed norm times 1 + 1e-12, an upper bound) proves that the
+    // full search would return the record at nn_pos[qi] again, as the strict winner (DESIGN §3.2).
+    // nn_idx, nn_pos, m_xyz and the certificate keep their values; only the epilogue runs.  A
+    // non-finite q fails the comparison.  Every line the decision and the answer need
+    // (certificate, matched point, normal, stop flag, Tinv) is requested in one round: the stop
+    // flag is part of the decision instead of a branch before it, since the compiler sinks loads
+    // below such a branch.  T and the predictor are read after the decision: the state's lines
+    // are shared by every query, so that read hits L1 or L2.
+    if (co.warm) {
+      const double cx = cert.c[3 * qi + 0], cy = cert.c[3 * qi + 1], cz = cert.c[3 * qi + 2];
+      const float rho = cert.rho[qi];
+      const double mx = co.m_xyz[3 * qi + 0], my = co.m_xyz[3 * qi + 1], mz = co.m_xyz[3 * qi + 2];
+      const int stop = st->stop;
+      const Rigid Tinv = st->Tinv;
+      const long long midx = co.mov_nrm ? nn_idx[qi] : -1;
+      const float4 nr = q_nrm[qi];
+      double qx, qy, qz;
+      rigid_apply(Tinv, epx, epy, epz, qx, qy, qz);
+      const double ex = qx - cx, ey = qy - cy, ez = qz - cz;
+      if (stamp) stamp[2] = global_timer_after(dep_bits(ex + ey + ez) ^ __float_as_uint(rho));
+      if (stop == 0 && sqrt(ex * ex + ey * ey + ez * ez) * (1.0 + 1e-12) < (double)rho) {
+        if (sub != 0) return false;
+        if (stamp) stamp[3] = global_timer_ns();
+        const Rigid T = st->T;
+        const Pred pred = load_pred(st);
+        const Rec m{mx, my, mz, midx};
+        const double d = plane_distance_rec(T, m, epx, epy, epz, nr);
+        if (stamp) stamp[4] = global_timer_after(dep_bits(d));
+        out[qi] = d;
+        const unsigned int slot =
+            lin_hist_add(pred, lin_hist, effective_planarity(co, T, qi, m.idx, nr), d, co.binstore, co.bin_cap, qi);
+        if (stamp) stamp[5] = global_timer_after(slot ^ 0x80000000u);
+        return true;
+      }
+    }
+    px = q_xyz[3 * qi + 0];
+    py = q_xyz[3 * qi + 1];
+    pz = q_xyz[3 * qi + 2];
   }
-  if (st->stop) return;
+  if (st->stop) return false;
   const unsigned int gmask = (MG == 32) ? 0xffffffffu : (((1u << MG) - 1u) << ((threadIdx.x & 31) & ~(MG - 1)));
   const Rigid Tinv = st->Tinv;
   double qx, qy, qz;
   rigid_apply(Tinv, px, py, pz, qx, qy, qz);
-  if constexpr (CERT) {
-    // Fast path: |q - c| < rho (computed norm times 1 + 1e-12, an upper bound) proves that the
-    // full search would return the record at nn_pos[qi] again, as the strict winner (DESIGN §3.2).
-    // nn_idx, nn_pos, m_xyz and the certificate keep their values; only the epilogue runs.  A
-    // non-finite q fails the comparison.  The matched point is requested with the certificate.
-    if (co.warm) {
-      const double ex = qx - cert.c[3 * qi + 0], ey = qy - cert.c[3 * qi + 1], ez = qz - cert.c[3 * qi + 2];
-      const float rho = cert.rho[qi];
-      const double mx = co.m_xyz[3 * qi + 0], my = co.m_xyz[3 * qi + 1], mz = co.m_xyz[3 * qi + 2];
-      if (sqrt(ex * ex + ey * ey + ez * ez) * (1.0 + 1e-12) < (double)rho) {
-        if (sub != 0) return;
-        const unsigned int am = __activemask();
-        if ((threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(cert.n_cert, (unsigned int)__popc(am));
-        const float4 nr = q_nrm[qi];
-        const Rec m{mx, my, mz, co.mov_nrm ? nn_idx[qi] : -1};
-        const double d = plane_distance_rec(st->T, m, px, py, pz, nr);
-        out[qi] = d;
-        lin_hist_add(st, lin_hist, effective_planarity(co, st->T, qi, m.idx, nr), d, co.binstore, co.bin_cap, qi);
-        return;
-      }
-    }
-  }
   const int cx = cell_coord(qx, g.ox, g.inv_h, g.nx);
   const int cy = cell_coord(qy, g.oy, g.inv_h, g.ny);
   const int cz = cell_coord(qz, g.oz, g.inv_h, g.nz);
@@ -647,12 +730,12 @@ __device__ __forceinline__ void match_coop_body(
     }
     if (r >= rmax) break;
   }
-  if (sub != 0) return;
+  if (sub != 0) return false;
   if constexpr (KEEP) {
     // with cap2 the search stops once the side of the bound is decided (see grid_nn), so `best`
     // is then an upper bound below cap2 or a value at or above it: the comparison is exact
     keep[qi] = (best < cap2) ? 1u : 0u;  // strict: cKDTree distance_upper_bound semantics
-    return;
+    return false;
   }
   if (co.nn_pos) co.nn_pos[qi] = resolved ? bpos : 0xffffffffu;
   if constexpr (CERT) {
@@ -668,7 +751,7 @@ __device__ __forceinline__ void match_coop_body(
   if (!resolved) {
     const unsigned int slot = atomicAdd(&unresolved[K], 1u);
     unresolved[slot] = (unsigned int)qi;
-    return;
+    return false;
   }
   nn_idx[qi] = bidx;
   if (with_distance) {
@@ -683,17 +766,30 @@ __device__ __forceinline__ void match_coop_body(
   } else {
     out[qi] = best;
   }
+  return false;
 }
 
+// 6 blocks per SM (80 registers): the certified steady state is a few dependent round trips per
+// query, so its time is set by the number of waves; the compiler's own choice, 96, fits 5.
 template <int MG>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(128, 6)
     k_match_grid_coop(GridView g, const DevState* __restrict__ st, const double* __restrict__ q_xyz,
                       const float4* __restrict__ q_nrm, const double* __restrict__ mov_xyz,
                       long long K, int rmax, int with_distance, long long* __restrict__ nn_idx,
                       double* __restrict__ out, unsigned int* __restrict__ unresolved,
                       unsigned int* __restrict__ lin_hist, double cap2, CorrOut co, MatchCert cert) {
-  match_coop_body<MG, false, true>(g, st, q_xyz, q_nrm, mov_xyz, K, rmax, with_distance, nn_idx, out, unresolved,
-                                   lin_hist, cap2, co, blockIdx.x * (long long)blockDim.x + threadIdx.x, nullptr, cert);
+  const bool certified =
+      match_coop_body<MG, false, true>(g, st, q_xyz, q_nrm, mov_xyz, K, rmax, with_distance, nn_idx, out, unresolved,
+                                       lin_hist, cap2, co, blockIdx.x * (long long)blockDim.x + threadIdx.x, nullptr, cert);
+  // One atomic per block on the certified counter instead of one per warp (a single address:
+  // ~12 500 same-address atomics per launch at K = 100 000).  Every thread comes here, and a warp
+  // that is done holds nothing while it waits: the block retires with its slowest warp either way.
+  if (cert.n_cert) {
+    const int n = __syncthreads_count(certified);
+    if (threadIdx.x == 0 && n > 0) atomicAdd(cert.n_cert, (unsigned int)n);
+  }
+  if (cert.stamps && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1))
+    cert.stamps[((blockIdx.x == 0) ? 0 : 8) + 6] = global_timer_ns();
 }
 
 // Batched form: blockIdx.y is the pair, everything else comes from its descriptor.  The ring
@@ -1647,6 +1743,15 @@ void match_launch(Ctx& c, bool with_distance, double* out_d2, cudaEvent_t mid, b
       c.cert_slot = c.cert_next;
       c.cert_next ^= 1;
       cert = MatchCert{c.cert_c.p, c.cert_rho.p, c.cert_count.p + c.cert_slot, c.cert_count.p + (c.cert_slot ^ 1)};
+    }
+    if (c.match_stamps) {
+      // zeroed once, at allocation: a memset before every launch would end the programmatic
+      // dependence on the previous reject/solve kernel (the kernel clears its own slots)
+      if (c.match_t.p == nullptr) {
+        c.match_t.reserve(16);
+        SICP_CUDA(cudaMemsetAsync(c.match_t.p, 0, 16 * sizeof(unsigned long long), c.stream));
+      }
+      cert.stamps = c.match_t.p;
     }
     const int mg = match_lanes(c, K, 2);
     with_lanes<2, 4, 8, 16>(mg, [&](auto L) {
