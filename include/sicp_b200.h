@@ -550,6 +550,49 @@ int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const double* const*
                            float* const* planarity    /*[h|d] per cloud n[i], or NULL*/,
                            int64_t* n_within          /*[h] n_clouds, or NULL*/);
 
+/* ---- which clouds overlap: the overlap graph of many posed clouds --------------------------------
+ * sicp_overlap_graph answers, before any registration, which pairs of n_clouds clouds overlap
+ * under approximate poses and by how much: the edges of sicp_register_pairs / sicp_register_joint.
+ *  - Rule: H[16 c ..] is cloud c's pose (row-major 4 x 4, world <- cloud), or with H NULL every
+ *    cloud is in one frame.  For an ordered pair (a, b), a != b, T_ab = H_a^-1 H_b is formed as
+ *    sicp_register_joint forms its priors (the transposed rotation, then the product; exactly the
+ *    identity with H NULL), and the sample of a is S_a = {0, s, 2 s, ...} < n[a] (X_a[::s] for
+ *    s = stride).  count_ab = the points i of S_a whose overlap filter flag is set for the pair
+ *    (fixed a, movable b) under T_ab and max_distance r: the n_kept of sicp_set_clouds(X_a, X_b),
+ *    sicp_set_selected(S_a), sicp_select_in_range(T_ab, r), bit for bit (the same device search,
+ *    d2 < fl(r^2)).
+ *  - Output: one row per unordered pair a < b with count_ab + count_ba > 0, ascending in (a, b):
+ *    (pair_a, pair_b, count_ab, count_ba).  A pair whose counts are both 0 is never reported.
+ *    Empty clouds (n[c] = 0) take part in no pair.  *n_pairs = the number of rows; the first
+ *    min(*n_pairs, cap) are written to every output array that is not NULL.  A caller whose cap was
+ *    too small calls again with a larger one: the second call recomputes everything.
+ *  - Culls: the world boxes of two clouds' grids, grown by r, that do not meet, and a direction
+ *    (a, b) whose box (b's grid box mapped by T_ab, grown by r) holds no cell of a's grid, hold no
+ *    point within r, up to a proven rounding margin: they are not searched, and nothing they hold
+ *    could have been counted.  So the culls never change a count.
+ *  - Cost: the clouds' upload and grids (as for sicp_register_pairs), a host sweep of N log N plus
+ *    the candidate pairs, and bounded searches: about the sum over the candidate directions (a, b)
+ *    of the sampled points of a inside b's cull box.
+ *  - SICP_ERR_BAD_ARG, before any device work: n_clouds < 1, a negative n[i], a NULL xyz[i] with
+ *    n[i] > 0, a non-finite H entry, an H whose bottom row is not (0, 0, 0, 1) or whose rotation
+ *    part R has an entry of R^T R - I above 1e-6, a max_distance that is not finite and > 0,
+ *    stride < 1, cap < 0, sum n[i] >= 2^32, or n_pairs NULL.  A cloud with a non-finite coordinate
+ *    is refused by the grid builder, as sicp_register_pairs refuses it.
+ *  - Nothing else changes: the map, the batch outputs (sicp_get_batch_outputs,
+ *    sicp_get_joint_covariances) and the one-pair state.  sicp_timings: upload_ms and grid_fix_ms
+ *    are this call's upload and grid build, overlap_ms the rest (culls, count, read-back).
+ *  - Limits: the clouds share one grid build, so together they must fit its 2^31 cells (as for
+ *    sicp_register_pairs; SICP_ERR_BAD_ARG "batch needs too many grid cells" otherwise).
+ *  - Device memory: the clouds once (24 B per point) and their grid (32 B per point of records, the
+ *    build's scratch and the cell tables), 4 B per candidate pair and direction counter, and up to
+ *    about 72 MB of direction descriptors; all stay on the context for the next call.            */
+int32_t sicp_overlap_graph(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                           const int64_t* n /*[h]*/, const double* H /*[h] n_clouds x 16, or NULL*/,
+                           double max_distance, int64_t stride,
+                           int32_t* pair_a, int32_t* pair_b /*[h] cap each, or NULL*/,
+                           int64_t* count_ab, int64_t* count_ba /*[h] cap each, or NULL*/,
+                           int64_t cap, int64_t* n_pairs /*[h]*/);
+
 /* ---- the rest of SimpleICP.run's return value (simpleicp.py:316-324) for a batch ----------------
  * sicp_register_batch, sicp_register_to_map, sicp_register_pairs and sicp_register_joint report per pair only the
  * record above.  This call returns what else sicp_register returns, for every pair of the LAST

@@ -43,7 +43,7 @@ SYMBOLS = (
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_register_joint", "sicp_get_batch_outputs",
     "sicp_get_joint_covariances",
-    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times", "sicp_get_match_phase_times",
+    "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_overlap_graph", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times", "sicp_get_match_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
 )
@@ -181,6 +181,8 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_map_carve": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, vp, dbl, dbl, i32, vp, C.POINTER(i64)],
         "sicp_map_distances": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, i32, C.POINTER(vp), C.POINTER(vp),
                                C.POINTER(vp), C.POINTER(vp), vp],
+        "sicp_overlap_graph": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, i64, vp, vp, vp, vp, i64,
+                               C.POINTER(i64)],
         "sicp_get_timings": [vp, C.POINTER(Timings)],
         "sicp_time_stages": [vp, C.POINTER(RunParams), i32, i32, C.POINTER(dbl)],
         "sicp_get_phase_times": [vp, C.POINTER(dbl)],
@@ -709,6 +711,24 @@ class Engine:
         self._check(self._lib.sicp_map_distances(self._h, n, ptrs, counts, _ptr(H), float(max_distance), k, arr(idx),
                                                  arr(d2), arr(pd), arr(pl), _ptr(n_within)))
         return idx, d2, pd, pl, n_within
+
+    def overlap_graph(self, clouds, H=None, *, max_distance: float, stride: int = 1, cap: int = 0):
+        """sicp_overlap_graph: the overlapping pairs of `clouds` under the poses `H` ((n_clouds, 4,
+        4) world <- cloud, or None: one frame).  Returns (total, pairs, counts): the number of
+        pairs the rule reports, and the first min(total, cap) of them, pairs (m, 2) int64 (a < b,
+        ascending) and counts (m, 2) int64 [count_ab, count_ba]."""
+        keep, ptrs, counts = _clouds_arg(clouds)
+        n = len(counts)
+        H = _shaped_arg(H, "H", (n, 4, 4))
+        cap = max(int(cap), 0)
+        a, b = np.empty(cap, dtype=np.int32), np.empty(cap, dtype=np.int32)
+        cab, cba = np.empty(cap, dtype=np.int64), np.empty(cap, dtype=np.int64)
+        total = C.c_int64(0)
+        self._check(self._lib.sicp_overlap_graph(self._h, n, ptrs, counts, _ptr(H), float(max_distance), int(stride),
+                                                 _ptr(a), _ptr(b), _ptr(cab), _ptr(cba), cap, C.byref(total)))
+        m = min(int(total.value), cap)
+        return (int(total.value), np.column_stack((a[:m], b[:m])).astype(np.int64),
+                np.column_stack((cab[:m], cba[:m])))
 
     def get_map(self) -> np.ndarray:
         """sicp_get_map: the resident map, (n_map, 3) float64 in map order."""

@@ -602,6 +602,66 @@ def _map_clouds(method: str, clouds, H):
     return clouds, None if H is None else _finite_array(H, "H", (len(clouds), 4, 4))
 
 
+def _check_rigid(H: np.ndarray) -> None:
+    """ValueError unless every H[i] has the bottom row (0, 0, 0, 1) and an orthonormal rotation
+    part (|R^T R - I| <= 1e-6 entrywise), as sicp_overlap_graph requires."""
+    if np.any(H[:, 3, :] != np.array([0.0, 0.0, 0.0, 1.0])):
+        raise ValueError("H must have the bottom row (0, 0, 0, 1)")
+    R = H[:, :3, :3]
+    if np.abs(np.einsum("nji,njk->nik", R, R) - np.eye(3)).max(initial=0.0) > 1e-6:
+        raise ValueError("the rotation part of H must be orthonormal (to 1e-6)")
+
+
+@dataclass
+class OverlapGraph:
+    """overlap_graph's result: one row per pair (a, b), a < b, of clouds that overlap under the
+    poses, ascending.  ``pairs`` (m, 2) int64; ``counts`` (m, 2) int64 [count_ab, count_ba], the
+    sampled points of a within max_distance of b and the other way round; ``sampled`` (n_clouds,)
+    int64 the points each cloud samples, ceil(n_c / stride); ``fraction`` (m, 2) float64 each count
+    over the sampled points of its source cloud (a for count_ab, b for count_ba)."""
+
+    pairs: np.ndarray
+    counts: np.ndarray
+    sampled: np.ndarray
+    fraction: np.ndarray
+
+
+def overlap_graph(clouds: Sequence, H=None, *, max_distance: float, stride: int = 1, device: int = 0) -> OverlapGraph:
+    """Which pairs of these clouds overlap under these poses, and by how much (sicp_overlap_graph).
+
+    ``clouds`` is a sequence of (n_i, 3) NumPy arrays or CUDA tensors (empty clouds take part in
+    no pair); ``H`` is None (every cloud already in one frame) or (n_clouds, 4, 4) rigid poses,
+    world <- cloud, e.g. GNSS/INS or odometry priors.  For every ordered pair (a, b), count_ab is
+    the number of points of ``X_a[::stride]`` whose squared distance to the nearest point of b,
+    under T_ab = H_a^-1 H_b, is below max_distance^2: the ``n_kept`` of the pair's overlap filter
+    (fixed a, movable b, prior T_ab).  A pair is reported when count_ab + count_ba > 0.  The rows
+    make the edges of ``simpleicp_joint`` or ``simpleicp_edges``, e.g.
+    ``g.pairs[g.fraction.min(axis=1) > 0.2]``.  One library call on one device."""
+    r = float(max_distance)
+    if not (np.isfinite(r) and r > 0):
+        raise ValueError(f"max_distance must be finite and > 0, got {max_distance}")
+    if isinstance(stride, (bool, np.bool_)) or int(stride) != stride or not 1 <= int(stride) < (1 << 63):
+        raise ValueError(f"stride must be an integer >= 1, got {stride}")
+    s = int(stride)
+    clouds, H = _map_clouds("overlap_graph", clouds, H)
+    if H is not None:
+        _check_rigid(H)
+    n = np.array([int(X.shape[0]) for X in clouds], dtype=np.int64)
+    if int(n.sum()) >= 1 << 32:
+        raise ValueError("the points of the clouds must be below 2^32")
+    sampled = (n + s - 1) // s
+    import torch
+
+    with torch.cuda.device(device):
+        eng = _batch_engine(device)
+        cap = 8 * len(clouds)
+        total, pairs, counts = eng.overlap_graph(clouds, H, max_distance=r, stride=s, cap=cap)
+        if total > cap:  # the second call recomputes everything, with room for every row
+            total, pairs, counts = eng.overlap_graph(clouds, H, max_distance=r, stride=s, cap=total)
+    # a reported pair's clouds are not empty: every divisor is >= 1
+    return OverlapGraph(pairs, counts, sampled, counts / sampled[pairs])
+
+
 class Map:
     """A fixed cloud (a map) held on one GPU, against which many scans are registered.
 

@@ -334,7 +334,9 @@ void batch_filter(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, long lon
 // grown by r + 1e-12 (M + r), ten times more (5e-6 m at UTM coordinates).  The cells are the map
 // grid's own cell_coord of the box faces: floor((v - o) / h) is monotone in v, so every point in the
 // box lies in a cell between those of its faces, and the kernel tests each candidate against the
-// box itself.
+// box itself.  The proof covers two callers: sicp_register_to_map (map grid, scan i's movable grid,
+// its prior) and sicp_overlap_graph's direction cull (a's grid as the map, b's grid as the scan,
+// T_ab), whose count runs the same search under the same bound.
 static MapCull map_cull_box(const GridView& map, const GridView& g, const Rigid& T, double r) {
   MapCull cu;
   std::memset(&cu, 0, sizeof(cu));
@@ -1474,6 +1476,208 @@ static void map_distances(Ctx& c, int n_clouds, const double* const* xyz, const 
     for (int i = 0; i < n_clouds; ++i) n_within[i] = (int64_t)bounds[i + 1] - (int64_t)bounds[i];
 }
 
+// sicp_overlap_graph (DESIGN.md §6.10).  Every non-empty cloud is staged once and gridded once
+// under the batch cell policy, as sicp_register_pairs does it.  Two culls on the host leave the
+// directions whose count can be nonzero:
+//  - pair cull: the world box of each cloud's grid box under its pose, grown by half the bound
+//    (plus the rounding margin of map_cull_box); a sort-and-sweep along the axis with the widest
+//    spread of box centres gives the pairs whose grown boxes meet.  Two clouds whose grown boxes
+//    are disjoint hold no points within r of each other: both counts are 0.
+//  - direction cull: map_cull_box(a's grid, b's grid, T_ab, r) bounds the points of a that can
+//    pass; rows == 0 means count_ab = 0 with no search.
+// k_overlap_count (nn.cu) then runs the overlap filter's search for the sampled points of a in the
+// box, 65535 directions per launch, and one read-back brings the two counters of every candidate.
+// With poses that are not rigid to the last bits (the call accepts |R^T R - I| <= 1e-6), the
+// inverse of T_ab is off by up to about 3 eps times the coordinates' magnitude M; both culls grow
+// by 16 eps (M + r) more for that.
+static void overlap_graph(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, const double* H,
+                          double r, int64_t stride, int32_t* pair_a, int32_t* pair_b, int64_t* count_ab,
+                          int64_t* count_ba, int64_t cap, int64_t* n_pairs) {
+  SICP_REQUIRE(n_pairs, SICP_ERR_BAD_ARG, "n_pairs is NULL");
+  const std::vector<long long> off = check_clouds(n_clouds, xyz, n, H);
+  double eps = 0.0;  // the largest entry of |R^T R - I| over the poses
+  for (int i = 0; H && i < n_clouds; ++i) {
+    const double* h = H + 16 * (size_t)i;
+    SICP_REQUIRE(h[12] == 0.0 && h[13] == 0.0 && h[14] == 0.0 && h[15] == 1.0, SICP_ERR_BAD_ARG,
+                 "H[" + std::to_string(i) + "] does not have the bottom row (0, 0, 0, 1)");
+    for (int p = 0; p < 3; ++p)
+      for (int q = 0; q < 3; ++q) {
+        const double d = h[p] * h[q] + h[4 + p] * h[4 + q] + h[8 + p] * h[8 + q] - (p == q ? 1.0 : 0.0);
+        SICP_REQUIRE(std::fabs(d) <= 1e-6, SICP_ERR_BAD_ARG,
+                     "the rotation part of H[" + std::to_string(i) + "] is not orthonormal (to 1e-6)");
+        eps = std::max(eps, std::fabs(d));
+      }
+  }
+  SICP_REQUIRE(std::isfinite(r) && r > 0, SICP_ERR_BAD_ARG, "max_distance must be finite and > 0");
+  SICP_REQUIRE(stride >= 1, SICP_ERR_BAD_ARG, "stride must be >= 1");
+  SICP_REQUIRE(cap >= 0, SICP_ERR_BAD_ARG, "cap must be >= 0");
+  SICP_REQUIRE(off[(size_t)n_clouds] < (1ll << 32), SICP_ERR_BAD_ARG,
+               "the points of the clouds must be below 2^32 (32-bit offsets)");
+  *n_pairs = 0;
+  c.tm.upload_ms = c.tm.grid_fix_ms = c.tm.overlap_ms = 0;
+  std::vector<int> ids;  // the non-empty clouds; k-th grid = cloud ids[k]
+  for (int i = 0; i < n_clouds; ++i)
+    if (n[i] > 0) ids.push_back(i);
+  if (ids.size() < 2) return;
+  if (!c.ovl) c.ovl = new OverlapStore();
+  OverlapStore& o = *c.ovl;
+  cudaStream_t st = c.stream;
+  const int K = (int)ids.size();
+
+  // ---- every non-empty cloud once, and its grid
+  o.xyz.reserve(3 * (size_t)off[(size_t)n_clouds]);
+  {
+    StageTimer t(c, &c.tm.upload_ms);
+    for (int i : ids) upload_to_device(c, o.xyz.p + 3 * off[(size_t)i], xyz[i], sizeof(double) * 3 * (size_t)n[i]);
+    t.stop();
+  }
+  std::vector<HostCloud> clouds;
+  for (int i : ids) clouds.push_back(HostCloud{o.xyz.p + 3 * off[(size_t)i], n[i], off[(size_t)i]});
+  std::vector<GridView> views;
+  std::vector<double> centres;
+  {
+    StageTimer t(c, &c.tm.grid_fix_ms);
+    grid_build(c, o.grid, clouds, batch_policy(c), views, centres);
+    t.stop();
+  }
+  StageTimer timer(c, &c.tm.overlap_ms);
+
+  // ---- pair cull: world boxes, grown, swept along one axis
+  Rigid I;
+  std::memset(&I, 0, sizeof(I));
+  I.r[0] = I.r[4] = I.r[8] = 1.0;
+  std::vector<Rigid> T((size_t)K, I);
+  if (H)
+    for (int k = 0; k < K; ++k) T[(size_t)k] = rigid_from_H(H + 16 * (size_t)ids[(size_t)k]);
+  std::vector<double> wlo(3 * (size_t)K, kInf), whi(3 * (size_t)K, -kInf);
+  double mag = 0.0;
+  for (int k = 0; k < K; ++k) {
+    const GridView& g = views[(size_t)k];
+    const double lo[3] = {g.ox, g.oy, g.oz}, hi[3] = {g.ox + g.nx * g.h, g.oy + g.ny * g.h, g.oz + g.nz * g.h};
+    for (int a = 0; a < 3; ++a)
+      mag = std::max(mag, std::max(std::max(std::fabs(lo[a]), std::fabs(hi[a])), std::fabs(T[(size_t)k].t[a])));
+    for (int q = 0; q < 8; ++q) {
+      double v[3];
+      rigid_apply(T[(size_t)k], (q & 1) ? hi[0] : lo[0], (q & 2) ? hi[1] : lo[1], (q & 4) ? hi[2] : lo[2], v[0], v[1],
+                  v[2]);
+      for (int a = 0; a < 3; ++a) {
+        wlo[3 * (size_t)k + a] = std::min(wlo[3 * (size_t)k + a], v[a]);
+        whi[3 * (size_t)k + a] = std::max(whi[3 * (size_t)k + a], v[a]);
+        mag = std::max(mag, std::fabs(v[a]));
+      }
+    }
+  }
+  const double r_cull = r + 16.0 * eps * (mag + r);  // the bound the culls are proven for
+  const double half = 0.5 * (r_cull + 1e-12 * (mag + r_cull));
+  for (double& v : wlo) v -= half;
+  for (double& v : whi) v += half;
+  int ax = 0;
+  double best_spread = -1.0;
+  for (int a = 0; a < 3; ++a) {
+    double cmin = kInf, cmax = -kInf;
+    for (int k = 0; k < K; ++k) {
+      const double cen = 0.5 * (wlo[3 * (size_t)k + a] + whi[3 * (size_t)k + a]);
+      cmin = std::min(cmin, cen);
+      cmax = std::max(cmax, cen);
+    }
+    if (cmax - cmin > best_spread) {
+      best_spread = cmax - cmin;
+      ax = a;
+    }
+  }
+  std::vector<int> order((size_t)K);
+  for (int k = 0; k < K; ++k) order[(size_t)k] = k;
+  std::sort(order.begin(), order.end(), [&](int p, int q) { return wlo[3 * (size_t)p + ax] < wlo[3 * (size_t)q + ax]; });
+  std::vector<std::pair<int, int>> cand;  // (k, l), k < l: grid slots, ascending like the cloud ids
+  std::vector<int> active;
+  for (int k : order) {
+    size_t keep = 0;
+    for (int l : active) {
+      if (whi[3 * (size_t)l + ax] < wlo[3 * (size_t)k + ax]) continue;  // ends before every later box starts
+      active[keep++] = l;
+      bool meet = true;
+      for (int a = 0; a < 3; ++a)
+        meet = meet && wlo[3 * (size_t)k + a] <= whi[3 * (size_t)l + a] && wlo[3 * (size_t)l + a] <= whi[3 * (size_t)k + a];
+      if (meet) cand.emplace_back(std::min(k, l), std::max(k, l));
+    }
+    active.resize(keep);
+    active.push_back(k);
+  }
+  std::sort(cand.begin(), cand.end());
+  const long long n_cand = (long long)cand.size();
+
+  // ---- direction cull and count, 65535 directions per launch
+  o.views.reserve(K);
+  SICP_CUDA(cudaMemcpyAsync(o.views.p, views.data(), sizeof(GridView) * (size_t)K, cudaMemcpyHostToDevice, st));
+  o.counts.reserve(std::max<long long>(2 * n_cand, 1));
+  SICP_CUDA(cudaMemsetAsync(o.counts.p, 0, sizeof(uint32_t) * (size_t)std::max<long long>(2 * n_cand, 1), st));
+  constexpr int kChunk = 65535;  // blockIdx.y is the direction
+  const size_t ds = sizeof(DevState) * kChunk;
+  o.dirs.reserve(ds + sizeof(OverlapDir) * kChunk);
+  std::vector<DevState> hs;
+  std::vector<OverlapDir> hd;
+  long long max_rows = 0, n_q = 0;
+  auto flush = [&]() {
+    if (hd.empty()) return;
+    const int nd = (int)hd.size();
+    // the previous launch has read its directions before this copy lands (stream order); a
+    // pageable source is staged by the runtime before the call returns
+    SICP_CUDA(cudaMemcpyAsync(o.dirs.p, hs.data(), sizeof(DevState) * (size_t)nd, cudaMemcpyHostToDevice, st));
+    SICP_CUDA(cudaMemcpyAsync(o.dirs.p + ds, hd.data(), sizeof(OverlapDir) * (size_t)nd, cudaMemcpyHostToDevice, st));
+    // r2 as sicp_select_in_range computes it
+    overlap_count_launch(c, o.views.p, reinterpret_cast<const DevState*>(o.dirs.p),
+                         reinterpret_cast<const OverlapDir*>(o.dirs.p + ds), nd, max_rows, stride, r * r, o.counts.p,
+                         n_q);
+    hs.clear();
+    hd.clear();
+    max_rows = n_q = 0;
+  };
+  for (long long p = 0; p < n_cand; ++p) {
+    const int k = cand[(size_t)p].first, l = cand[(size_t)p].second;
+    for (int side = 0; side < 2; ++side) {
+      const int a = side ? l : k, b = side ? k : l;
+      // T_ab = T_a^-1 T_b as sicp_register_joint forms its priors; exactly I without poses
+      const Rigid Tab = H ? rigid_compose(rigid_inverse(T[(size_t)a]), T[(size_t)b]) : I;
+      OverlapDir d;
+      std::memset(&d, 0, sizeof(d));
+      d.cu = map_cull_box(views[(size_t)a], views[(size_t)b], Tab, r_cull);
+      if (d.cu.rows == 0) continue;
+      d.a = a;
+      d.b = b;
+      d.slot = (int)(2 * p + side);
+      DevState s;
+      std::memset(&s, 0, sizeof(s));
+      s.T = Tab;
+      s.Tinv = rigid_inverse(Tab);
+      hs.push_back(s);
+      hd.push_back(d);
+      max_rows = std::max(max_rows, d.cu.rows);
+      n_q += (long long)(d.cu.rows * (d.cu.c1[0] - d.cu.c0[0] + 1) * c.grid_target_occ) / stride;
+      if ((int)hd.size() == kChunk) flush();
+    }
+  }
+  flush();
+
+  // ---- one read-back: the rows with a nonzero total, in candidate order (ascending (a, b))
+  pinned_reserve(o.counts_host, o.counts_cap, (size_t)std::max<long long>(2 * n_cand, 1));
+  SICP_CUDA(cudaMemcpyAsync(o.counts_host, o.counts.p, sizeof(uint32_t) * 2 * (size_t)n_cand, cudaMemcpyDeviceToHost, st));
+  SICP_CUDA(cudaStreamSynchronize(st));
+  timer.stop();
+  long long total = 0;
+  for (long long p = 0; p < n_cand; ++p) {
+    const uint32_t cab = o.counts_host[2 * p], cba = o.counts_host[2 * p + 1];
+    if (cab == 0 && cba == 0) continue;
+    if (total < cap) {
+      if (pair_a) pair_a[total] = ids[(size_t)cand[(size_t)p].first];
+      if (pair_b) pair_b[total] = ids[(size_t)cand[(size_t)p].second];
+      if (count_ab) count_ab[total] = cab;
+      if (count_ba) count_ba[total] = cba;
+    }
+    ++total;
+  }
+  *n_pairs = total;
+}
+
 }  // namespace sicp
 
 using namespace sicp;
@@ -1559,6 +1763,15 @@ extern "C" int32_t sicp_map_distances(sicp_ctx* ctx, int32_t n_clouds, const dou
                                       int64_t* n_within) {
   API_BEGIN(ctx)
   map_distances(c, n_clouds, xyz, n, H, max_distance, neighbors, idx, dist2, plane_dist, planarity, n_within);
+  API_END
+}
+
+extern "C" int32_t sicp_overlap_graph(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
+                                      const double* H, double max_distance, int64_t stride, int32_t* pair_a,
+                                      int32_t* pair_b, int64_t* count_ab, int64_t* count_ba, int64_t cap,
+                                      int64_t* n_pairs) {
+  API_BEGIN(ctx)
+  overlap_graph(c, n_clouds, xyz, n, H, max_distance, stride, pair_a, pair_b, count_ab, count_ba, cap, n_pairs);
   API_END
 }
 

@@ -286,6 +286,8 @@ int32_t sicp_destroy(sicp_ctx* ctx) {
   c.batch = nullptr;
   delete c.map;
   c.map = nullptr;
+  delete c.ovl;
+  c.ovl = nullptr;
   if (c.rec_host) cudaFreeHost(c.rec_host);
   if (c.scal_host) cudaFreeHost(c.scal_host);
   if (c.grid_host) cudaFreeHost(c.grid_host);

@@ -75,6 +75,7 @@ struct CompactScratch {
 
 struct Batch;
 struct MapStore;
+struct OverlapStore;
 
 struct Ctx {
   int device = 0;
@@ -200,6 +201,7 @@ struct Ctx {
 
   Batch* batch = nullptr;  // created by the first sicp_register_batch
   MapStore* map = nullptr; // sicp_set_map: the resident fixed cloud of sicp_register_to_map
+  OverlapStore* ovl = nullptr;  // created by the first sicp_overlap_graph
 };
 // what the match kernels / reject kernels see of the movable-side attributes
 inline const float4* mov_attr_nrm(Ctx& c) { return c.mov_attr ? c.mov_nrm.p : nullptr; }
@@ -456,6 +458,32 @@ struct MapStore {
   DevBuf<uint32_t> carve_passes;
 };
 
+// One direction (a, b) of sicp_overlap_graph that survived the culls (batch.cu: overlap_graph):
+// the rows of a's grid inside cull, searched in b's grid under the DevState of the same index
+// (T = T_ab); the survivors are counted into counts[slot].
+struct OverlapDir {
+  MapCull cu;
+  int a, b;  // indices into the call's grid views
+  int slot;  // 2 p (count_ab) or 2 p + 1 (count_ba) of candidate pair p
+  int pad;
+};
+
+// sicp_overlap_graph's buffers, kept on the context like sicp_map_distances' staging: every
+// non-empty cloud once (24 B per point) and its grid, the grid views, the directions' states and
+// descriptors, and two 32-bit counters per candidate pair.  Nothing in them outlives the call.
+struct OverlapStore {
+  DevBuf<double> xyz;
+  GridBufs grid;
+  DevBuf<GridView> views;
+  DevBuf<unsigned char> dirs;  // n_dirs DevState, then n_dirs OverlapDir: one upload
+  DevBuf<uint32_t> counts;
+  uint32_t* counts_host = nullptr;  // pinned
+  size_t counts_cap = 0;
+  ~OverlapStore() {
+    if (counts_host) cudaFreeHost(counts_host);
+  }
+};
+
 // ---- stage entry points (each implemented in its own translation unit) ---------------------
 struct HostCloud {
   const double* xyz_dev;
@@ -547,6 +575,13 @@ void batch_overlap_launch(Ctx& c, Batch& b, const double* fix_xyz, long long max
 // survivors set bit i of the scan's row of MapStore::bits (cleared by the caller).
 void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev, long long max_rows, double r2,
                         long long n_candidates_hint);
+// sicp_overlap_graph's count (nn.cu: k_overlap_count), one launch for n_dirs <= 65535 directions:
+// for each direction d, the records of dirs[d].a's grid inside its MapCull (at most max_rows rows)
+// with idx % stride == 0 get the bounded search of batch_overlap_launch in dirs[d].b's grid under
+// state[d] (same device code, same flag); the survivors are added to counts[dirs[d].slot] (zeroed
+// by the caller).  n_candidates (records in the culls) picks the lanes per search.
+void overlap_count_launch(Ctx& c, const GridView* views, const DevState* state, const OverlapDir* dirs, int n_dirs,
+                          long long max_rows, long long stride, double r2, uint32_t* counts, long long n_candidates);
 // popcounts of MapStore::bits words (n_words of them) -> popc, and the ordered compaction of the
 // set bits into list (scan[w] = exclusive prefix sum of the popcounts): ascending map indices
 void map_bits_popc_launch(Ctx& c, const uint32_t* bits, long long n_words, uint32_t* popc);

@@ -905,6 +905,49 @@ __global__ void __launch_bounds__(128)
   if ((threadIdx.x & 31) == 0 && searched) atomicAdd(n_searched, (unsigned long long)searched);
 }
 
+// Count of sicp_overlap_graph, k_map_overlap's walk for many directions: blockIdx.y is the
+// direction (a, b), blockIdx.x one x-row of a's grid inside the direction's MapCull cells.  A
+// record inside the box whose index is a multiple of `stride` gets k_overlap_batch's bounded
+// search in b's grid under the direction's state (prior T_ab), so its flag is that of the pair's
+// overlap filter bit for bit.  The survivors are counted per warp and added with one atomic per
+// warp to the direction's 32-bit counter (a cloud has fewer than 2^32 points); integer sums, so
+// the count does not depend on the order.
+template <int MG>
+__global__ void __launch_bounds__(128)
+    k_overlap_count(const GridView* __restrict__ views, const DevState* __restrict__ state,
+                    const OverlapDir* __restrict__ dirs, uint32_t stride, double r2, uint32_t* __restrict__ counts) {
+  const OverlapDir& dr = dirs[blockIdx.y];
+  const MapCull& cu = dr.cu;
+  if ((long long)blockIdx.x >= cu.rows) return;
+  const GridView& ga = views[dr.a];
+  const int ny = cu.c1[1] - cu.c0[1] + 1;
+  const int y = cu.c0[1] + (int)(blockIdx.x % (unsigned)ny), z = cu.c0[2] + (int)(blockIdx.x / (unsigned)ny);
+  const long long row = ((long long)z * ga.ny + y) * ga.nx;
+  // the row's end lives in shared memory, as in k_map_overlap
+  __shared__ uint32_t row_end;
+  const uint32_t s = ga.cell_start[row + cu.c0[0]];
+  if (threadIdx.x == 0) row_end = ga.cell_start[row + cu.c1[0] + 1];
+  __syncthreads();
+  const Rec* __restrict__ recs = ga.recs;
+  const CorrOut co{nullptr, 0, nullptr, nullptr, 0, 0, nullptr, nullptr, -1.0};
+  const int sub = threadIdx.x & (MG - 1);
+  __shared__ uint32_t flags[128 / MG];
+  uint32_t* flag = flags + threadIdx.x / MG;
+  unsigned int kept = 0;
+  for (uint32_t p = s + threadIdx.x / MG; p < *(volatile uint32_t*)&row_end; p += 128 / MG) {
+    const Rec r = recs[p];  // the whole group reads the same record and takes the same branch
+    if (r.x < cu.lo[0] || r.x > cu.hi[0] || r.y < cu.lo[1] || r.y > cu.hi[1] || r.z < cu.lo[2] || r.z > cu.hi[2])
+      continue;
+    if (stride > 1 && (uint32_t)r.idx % stride != 0) continue;  // idx < 2^32 - 1
+    const double q[3] = {r.x, r.y, r.z};
+    match_coop_body<MG, true>(views[dr.b], state + blockIdx.y, q, nullptr, nullptr, 1, 1 << 30, 0, nullptr, nullptr,
+                              nullptr, nullptr, r2, co, sub, flag);
+    if (sub == 0) kept += *flag;  // the lane that wrote the flag
+  }
+  kept = __reduce_add_sync(0xffffffffu, kept);
+  if ((threadIdx.x & 31) == 0 && kept) atomicAdd(&counts[dr.slot], kept);
+}
+
 __global__ void __launch_bounds__(256) k_map_popc(const uint32_t* __restrict__ bits, long long n, uint32_t* __restrict__ popc) {
   const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (w < n) popc[w] = (uint32_t)__popc(bits[w]);
@@ -1594,6 +1637,17 @@ void map_overlap_launch(Ctx& c, Batch& b, MapStore& m, const MapCull* culls_dev,
   with_lanes<4, 8, 16>(match_lanes(c, n_candidates_hint, 4), [&](auto L) {
     k_map_overlap<decltype(L)::value>
         <<<grid, 128, 0, c.stream>>>(b.pairs.p, b.state.p, culls_dev, m.view, r2, words, m.bits.p, m.n_searched.p);
+  });
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void overlap_count_launch(Ctx& c, const GridView* views, const DevState* state, const OverlapDir* dirs, int n_dirs,
+                          long long max_rows, long long stride, double r2, uint32_t* counts, long long n_candidates) {
+  const uint32_t s32 = (uint32_t)std::min<long long>(stride, 0xffffffffll);
+  with_lanes<8, 16>(match_lanes(c, n_candidates, 8), [&](auto L) {
+    k_overlap_count<decltype(L)::value><<<dim3((unsigned)max_rows, (unsigned)n_dirs), 128, 0, c.stream>>>(
+        views, state, dirs, s32, r2, counts);
   });
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
