@@ -106,8 +106,9 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value);
  *        the driver stages on the calling thread; pinned and device sources never use them),
  *        "upload_chunk_kb" (slice size of that staging, default 2048), "normals_scratch_mb"
  *        (bound of the movable-normals estimate's neighbour scratch, default 64: it runs in
- *        launches of 2^20 x normals_scratch_mb / (4 k) queries), "defaults" (any value: every option back to its
- *        default)                                                       */
+ *        launches of 2^20 x normals_scratch_mb / (4 k) queries), "joint_solver" (the solve of
+ *        sicp_register_joint: 0 dense, the default; 1 sparse, see there), "defaults" (any value:
+ *        every option back to its default)                                */
 
 /* ---- clouds: SimpleICP.add_point_clouds (simpleicp.py:58-73) + PointCloud.X ---------------- */
 int32_t sicp_set_clouds(sicp_ctx* ctx, const double* fix_xyz /*[h|d] n_fix x 3*/, int64_t n_fix,
@@ -378,8 +379,8 @@ int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const
  *  - SICP_ERR_BAD_ARG, before any device work: every check of sicp_register_pairs under a
  *    linearised variant (n_edges in [1, 65535], correspondences <= 4096, zero observation weights,
  *    ...), mov_neighbors != 0, a self edge, a non-finite H0 entry, no free cloud or more than 256
- *    free clouds among the referenced ones, or a free cloud whose component of the edge graph holds
- *    no fixed cloud.  A cloud no edge references is not read (its pointer may be NULL).
+ *    free clouds among the referenced ones (16 384 under option "joint_solver" 1), or a free cloud
+ *    whose component of the edge graph holds no fixed cloud.  A cloud no edge references is not read (its pointer may be NULL).
  *  - Outputs: H_out[c] = the final T_c; fixed and unreferenced clouds get H0 (identity for a NULL
  *    H0) bit for bit.  out[e]: status, the call's iterations and convergence, the edge's last
  *    n_kept, H = final T_a^-1 T_b, x = the edge's last increment in frame a, mean_res / std_res of
@@ -395,7 +396,14 @@ int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const
  *    final T_a^-1 T_b, the final linear-model residuals in kept order, the log and T = that
  *    transform.  The map and the one-pair state are not touched.  sicp_timings: match_ms,
  *    reject_solve_ms and transform_ms are the loop's match, reject-and-blocks and joint solve +
- *    update times (device events, summed over the iterations run).                             */
+ *    update times (device events, summed over the iterations run).
+ *  - Option "joint_solver" (sicp_set_option), read by each call: 0 (the default) solves the joint
+ *    system by a dense Cholesky, at most 256 free clouds.  1 solves the same system, with the same
+ *    rule and outputs up to rounding, by a supernodal Cholesky over a nested-dissection ordering of
+ *    the edge graph (DESIGN.md §6.11): at most 16 384 free clouds (more is SICP_ERR_BAD_ARG), and a
+ *    factor of at most 4 GiB, computed from the edges before any upload (more is SICP_ERR_BAD_ARG,
+ *    with the bytes in the message).  After a call under 1, sicp_get_joint_covariances returns
+ *    SICP_ERR_STATE; sicp_get_batch_outputs works as after 0.                                   */
 int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
                             const int64_t* n /*[h]*/, int32_t n_edges,
                             const int32_t* fix_id, const int32_t* mov_id /*[h] n_edges*/,
@@ -646,7 +654,8 @@ int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
  *  - The first request after the call computes them on the device (sicp_register_joint itself does
  *    no extra work and its timings do not include it); every later one returns the same bits.
  *  - SICP_ERR_STATE whenever sicp_get_batch_outputs would return it, and when the last batched
- *    call was not a sicp_register_joint.  SICP_ERR_BAD_ARG: n_clouds or n_edges differs from that
+ *    call was not a sicp_register_joint or ran under option "joint_solver" 1 ("covariances need
+ *    joint_solver 0").  SICP_ERR_BAD_ARG: n_clouds or n_edges differs from that
  *    call's.  A NULL output is skipped.  Nothing else changes: the batch outputs, the map and the
  *    one-pair state.                                                                             */
 int32_t sicp_get_joint_covariances(sicp_ctx* ctx, int32_t n_clouds,

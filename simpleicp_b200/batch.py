@@ -305,6 +305,9 @@ def simpleicp_edges(clouds: Sequence, edges, *, rank: int = 0, world_size: int =
     return _gather_share(local, found, mine, n, rank, world_size, dist, device, on_error, full_output, messages)
 
 
+# simpleicp_joint's solvers and the free clouds each takes (option joint_solver 0 and 1)
+_JOINT_SOLVERS = {"dense": 256, "sparse": 16384}
+
 # run() arguments simpleicp_joint serves (sicp_register_joint, always the linearised rules)
 _JOINT_KEYS = {"correspondences", "neighbors", "min_planarity", "min_change", "max_iterations", "max_overlap_distance"}
 
@@ -322,7 +325,8 @@ class JointResult:
 
 
 def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
-                    full_output: bool = False, covariances: bool = False, **run_kwargs) -> JointResult:
+                    full_output: bool = False, covariances: bool = False, solver: str = "dense",
+                    **run_kwargs) -> JointResult:
     """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
     (a, b) of `edges` -- scan-to-scan pairs such as (i, i + 1), (i, i + 2) and loop closures -- is
     registered consistently.  Each iteration matches every edge as simpleicp_edges would under the
@@ -334,19 +338,29 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     The run() arguments served are correspondences (<= 4096), neighbors, min_planarity,
     min_change, max_iterations and max_overlap_distance; anything else is a TypeError.  Every free
     cloud an edge references must be connected to a fixed cloud through the edges, and there may be
-    at most 256 of them.  A cloud no edge references may be None; it keeps its H0.  One library call
-    on one device (sicp_register_joint).  `on_error` and `full_output` are as in simpleicp_edges:
-    an edge that failed (no overlap, too few correspondences) has its status in the table and raises
-    BatchError under "raise"; a failure of the whole call (SICP_ERR_SINGULAR, or a free cloud left
-    without a path to a fixed one by the edges without overlap) raises SicpError.
+    at most 256 of them (16 384 with solver="sparse").  A cloud no edge references may be None; it
+    keeps its H0.  One library call on one device (sicp_register_joint).  `on_error` and
+    `full_output` are as in simpleicp_edges: an edge that failed (no overlap, too few
+    correspondences) has its status in the table and raises BatchError under "raise"; a failure of
+    the whole call (SICP_ERR_SINGULAR, or a free cloud left without a path to a fixed one by the
+    edges without overlap) raises SicpError.
 
     `covariances=True` also returns the a-posteriori covariances of the final iteration
     (sicp_get_joint_covariances, DESIGN.md §6.9): cov[c] of cloud c's (rotation increment, origin
     displacement) in the world frame, zeros for a fixed cloud and NaN for a cloud no edge
     references; edge_cov[e] of edge (a, b)'s (rotation increment, displacement of b's origin) in
-    frame a; s0 the a-posteriori standard deviation of unit weight."""
+    frame a; s0 the a-posteriori standard deviation of unit weight.
+
+    `solver` picks the solve of the joint system (option joint_solver): "dense" (the default: the
+    dense Cholesky of DESIGN.md §6.9, at most 256 free clouds, the only one with covariances) or
+    "sparse" (a supernodal Cholesky over a nested-dissection ordering of the edge graph, DESIGN.md
+    §6.11: the same system and rule, up to rounding, for up to 16 384 free clouds)."""
     if not isinstance(covariances, (bool, np.bool_)):
         raise TypeError(f"covariances must be True or False, got {covariances!r}")
+    if not isinstance(solver, str) or solver not in _JOINT_SOLVERS:
+        raise ValueError(f"solver must be 'dense' or 'sparse', got {solver!r}")
+    if covariances and solver == "sparse":
+        raise ValueError("covariances=True needs solver='dense': the sparse solve has no covariances")
     _check_run_keys(run_kwargs, _JOINT_KEYS, "simpleicp_joint", "edge")
     n_clouds = len(clouds)
     e = _check_edges(edges, n_clouds)
@@ -366,8 +380,10 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     used = np.zeros(n_clouds, dtype=bool)
     used[e.ravel()] = True
     free = used & ~is_fixed
-    if not 1 <= int(free.sum()) <= 256:
-        raise ValueError(f"the edges must reference between 1 and 256 free clouds, got {int(free.sum())}")
+    cap = _JOINT_SOLVERS[solver]
+    if not 1 <= int(free.sum()) <= cap:
+        raise ValueError(f"the edges must reference between 1 and {cap} free clouds"
+                         f"{' under solver=sparse' if solver == 'sparse' else ''}, got {int(free.sum())}")
     up = list(range(n_clouds))
 
     def root(i):
@@ -393,6 +409,8 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         params = eng.run_params(run_kwargs.get("min_planarity", 0.3), run_kwargs.get("min_change", 1.0),
                                 run_kwargs.get("max_iterations", 100), lsq)
         mod = float(run_kwargs.get("max_overlap_distance", np.inf))
+        # every call sets the option: the engine is shared by the calls on this device
+        eng.set_option("joint_solver", 1 if solver == "sparse" else 0)
         H, res = eng.register_joint(list(clouds), e, is_fixed, H0, run_kwargs.get("correspondences", 1000),
                                     run_kwargs.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0)
         n = e.shape[0]

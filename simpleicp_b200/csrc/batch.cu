@@ -38,9 +38,11 @@
 #include <cstddef>
 #include <cmath>
 #include <cstring>
+#include <unordered_map>
 #include <vector>
 
 #include "ctx.cuh"
+#include "joint_plan.h"
 
 namespace sicp {
 
@@ -451,8 +453,102 @@ static void check_anchored(const JointRun& j, const std::vector<char>& use, int 
     }
 }
 
+// The sparse solve's plan (joint_plan.h) over the free-free pairs of the edges with use[e] != 0;
+// SICP_ERR_BAD_ARG when its panels would exceed JOINT_SPARSE_MAX_BYTES.
+static JointPlan joint_sparse_plan(const JointRun& j, const std::vector<char>& use) {
+  std::vector<std::pair<int, int>> pairs;
+  for (int e = 0; e < j.n_edges; ++e) {
+    const int fa = j.free_of[(size_t)j.fix_id[e]], fb = j.free_of[(size_t)j.mov_id[e]];
+    if (use[(size_t)e] && fa >= 0 && fb >= 0) pairs.emplace_back(fa, fb);
+  }
+  JointPlan pl = make_joint_plan(j.F, pairs);
+  SICP_REQUIRE(pl.factor_bytes() <= JOINT_SPARSE_MAX_BYTES, SICP_ERR_BAD_ARG,
+               "joint_solver 1: the factor of this edge graph needs " + std::to_string(pl.factor_bytes()) +
+                   " bytes, more than the limit of " + std::to_string(JOINT_SPARSE_MAX_BYTES));
+  return pl;
+}
+
+// What k_joint_sparse_solve reads of the plan, appended to ids (offsets into it in o): the
+// supernodes, structs, updates, maps, levels, the order, and every panel block's list of live edges
+// in ascending order (2 e + (1: the block's cloud is the edge's a) on a diagonal block).
+struct SparseIds {
+  size_t sn, st, up, map, lv_off, lv, perm, blk, lst_off, lst_edge;
+};
+static SparseIds joint_sparse_ids(const JointRun& j, const std::vector<char>& live, const JointPlan& pl,
+                                  std::vector<int>& ids) {
+  // the lists of the blocks the live edges touch, keyed by (free cloud, free cloud), smaller first
+  std::unordered_map<long long, int> key_of;
+  std::vector<std::vector<int>> lists;
+  auto add = [&](int p, int q, int v) {
+    const long long key = (long long)std::min(p, q) * j.F + std::max(p, q);
+    auto it = key_of.emplace(key, (int)lists.size()).first;
+    if (it->second == (int)lists.size()) lists.emplace_back();
+    lists[(size_t)it->second].push_back(v);
+  };
+  for (int e = 0; e < j.n_edges; ++e) {
+    if (!live[(size_t)e]) continue;
+    const int fa = j.free_of[(size_t)j.fix_id[e]], fb = j.free_of[(size_t)j.mov_id[e]];
+    if (fa >= 0) add(fa, fa, 2 * e + 1);
+    if (fb >= 0) add(fb, fb, 2 * e);
+    if (fa >= 0 && fb >= 0) add(fa, fb, 2 * e);
+  }
+  static_assert(sizeof(JointSuper) == 8 * sizeof(int), "JointSuper travels as 8 ints");
+  SparseIds o{};
+  o.sn = ids.size();
+  int table = 0;
+  for (int s = 0; s < pl.n_super; ++s) {
+    const int v[8] = {pl.first[(size_t)s], pl.ns(s), pl.nt(s), pl.st_off[(size_t)s], pl.up_off[(size_t)s],
+                      pl.up_off[(size_t)s + 1], table, 0};  // JointSuper
+    ids.insert(ids.end(), v, v + 8);
+    table += (pl.ns(s) + pl.nt(s)) * pl.ns(s);
+  }
+  o.st = ids.size();
+  ids.insert(ids.end(), pl.st.begin(), pl.st.end());
+  o.up = ids.size();
+  for (size_t u = 0; u < pl.up.size(); ++u) {
+    const int v[4] = {pl.up[u], pl.up_i0[u], pl.up_nj[u], pl.up_map[u]};
+    ids.insert(ids.end(), v, v + 4);
+  }
+  o.map = ids.size();
+  ids.insert(ids.end(), pl.map.begin(), pl.map.end());
+  o.lv_off = ids.size();
+  ids.insert(ids.end(), pl.lv_off.begin(), pl.lv_off.end());
+  o.lv = ids.size();
+  ids.insert(ids.end(), pl.lv.begin(), pl.lv.end());
+  o.perm = ids.size();
+  ids.insert(ids.end(), pl.perm.begin(), pl.perm.end());
+  o.blk = ids.size();
+  for (int s = 0; s < pl.n_super; ++s) {
+    const int ns = pl.ns(s), f0 = pl.first[(size_t)s];
+    for (int ri = 0; ri < ns + pl.nt(s); ++ri) {
+      const int pr = ri < ns ? f0 + ri : pl.st[(size_t)(pl.st_off[(size_t)s] + ri - ns)];
+      for (int cj = 0; cj < ns; ++cj) {
+        const int pc = f0 + cj;
+        int l = -1;
+        if (pr >= pc) {
+          const int a = pl.perm[(size_t)pr], b = pl.perm[(size_t)pc];
+          auto it = key_of.find((long long)std::min(a, b) * j.F + std::max(a, b));
+          if (it != key_of.end()) l = it->second;
+        }
+        ids.push_back(l);
+      }
+    }
+  }
+  o.lst_off = ids.size();
+  int at = 0;
+  for (const auto& l : lists) {
+    ids.push_back(at);
+    at += (int)l.size();
+  }
+  ids.push_back(at);
+  o.lst_edge = ids.size();
+  for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+  return o;
+}
+
 // The loop of sicp_register_joint, in place of run_pairs' per-pair loop: per iteration the match of
-// every edge, k_joint_reject and k_joint_solve (joint.cu), and the read of the stop flag every
+// every edge, k_joint_reject and k_joint_solve or, under option "joint_solver" 1,
+// k_joint_sparse_solve (joint.cu), and the read of the stop flag every
 // host_sync_every iterations.  The edges without overlap (parked by the filter) take no part.
 static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   JointRun& j = *r.joint;
@@ -467,10 +563,13 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   double cw[3];
   const double* cm = r.pd[(size_t)e0].cm;
   rigid_apply(j.pose[(size_t)j.mov_id[e0]], cm[0], cm[1], cm[2], cw[0], cw[1], cw[2]);
-  // the lower blocks every live edge touches, its edges in ascending order
+  // the lower blocks every live edge touches, its edges in ascending order (dense), or the plan
   const int F = j.F;
+  const bool sparse = c.joint_solver == 1;
+  JointPlan plan;
+  if (sparse) plan = joint_sparse_plan(j, live);
   std::vector<std::vector<int>> lists;
-  std::vector<int> blk_of((size_t)F * F, -1);
+  std::vector<int> blk_of(sparse ? 0 : (size_t)F * F, -1);
   auto add = [&](int p, int q, int v) {
     int& bi = blk_of[(size_t)p * F + q];
     if (bi < 0) {
@@ -479,7 +578,7 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     }
     lists[(size_t)bi].push_back(v);
   };
-  for (int e = 0; e < n_edges; ++e) {
+  for (int e = 0; e < n_edges && !sparse; ++e) {
     if (!live[(size_t)e]) continue;
     const int fa = j.free_of[(size_t)j.fix_id[e]], fb = j.free_of[(size_t)j.mov_id[e]];
     if (fa >= 0) add(fa, fa, 2 * e + 1);
@@ -501,6 +600,7 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   ids.push_back(at);
   const size_t o_edge = ids.size();
   for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+  const SparseIds so = sparse ? joint_sparse_ids(j, live, plan, ids) : SparseIds{};
 
   JointStore& js = b.joint;
   const int npad = (6 * F + 1 + 31) / 32 * 32;
@@ -513,12 +613,27 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   for (int e = 0; e < n_edges; ++e)
     for (int cl : {j.fix_id[e], j.mov_id[e]}) js.role[(size_t)cl] = j.free_of[(size_t)cl] >= 0 ? 2 : 1;
   js.cov_done = false;
+  js.sparse = sparse;
   js.edges.reserve(n_edges);
   js.flags.reserve(1);
   js.pose.reserve(j.n_clouds);
   js.ids.reserve(ids.size());
-  js.A.reserve((size_t)npad * npad);
+  if (!sparse) js.A.reserve((size_t)npad * npad);
   js.bar.reserve(2);
+  if (sparse) {
+    js.sp_panel.reserve(plan.panel.size());
+    js.sp_L.reserve((size_t)plan.panel.back());
+    js.sp_x.reserve(15 * (size_t)F);
+    js.sp_flags.reserve(1 + (size_t)c.num_sms);
+    SICP_CUDA(cudaMemcpyAsync(js.sp_panel.p, plan.panel.data(), sizeof(long long) * plan.panel.size(),
+                              cudaMemcpyHostToDevice, st));
+    SICP_CUDA(cudaMemsetAsync(js.sp_flags.p, 0, sizeof(int), st));
+    std::vector<double> dc(3 * (size_t)F);
+    for (int f = 0; f < F; ++f)
+      for (int k = 0; k < 3; ++k) dc[3 * (size_t)f + k] = j.pose[(size_t)j.free_ids[(size_t)f]].t[k] - cw[k];
+    SICP_CUDA(cudaMemcpyAsync(js.sp_x.p + 12 * (size_t)F, dc.data(), sizeof(double) * dc.size(),
+                              cudaMemcpyHostToDevice, st));
+  }
   if (!js.flags_host) SICP_CUDA(cudaMallocHost(&js.flags_host, sizeof(JointFlags)));
   SICP_CUDA(cudaMemsetAsync(js.edges.p, 0, sizeof(JointEdge) * (size_t)n_edges, st));
   SICP_CUDA(cudaMemsetAsync(js.flags.p, 0, sizeof(JointFlags), st));
@@ -554,6 +669,28 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   for (int k = 0; k < 3; ++k) a.cw[k] = cw[k];
   a.min_planarity = p.min_planarity;
   a.min_change = p.min_change;
+  JointSparseArgs sa{};
+  if (sparse) {
+    sa.j = a;
+    sa.sn = reinterpret_cast<const JointSuper*>(js.ids.p + so.sn);
+    sa.panel = js.sp_panel.p;
+    sa.st = js.ids.p + so.st;
+    sa.up = js.ids.p + so.up;
+    sa.map = js.ids.p + so.map;
+    sa.lv_off = js.ids.p + so.lv_off;
+    sa.lv = js.ids.p + so.lv;
+    sa.perm = js.ids.p + so.perm;
+    sa.blk = js.ids.p + so.blk;
+    sa.lst_off = js.ids.p + so.lst_off;
+    sa.lst_edge = js.ids.p + so.lst_edge;
+    sa.depth = plan.depth;
+    sa.L = js.sp_L.p;
+    sa.x = js.sp_x.p;
+    sa.xf = js.sp_x.p + 6 * (size_t)F;
+    sa.dc = js.sp_x.p + 12 * (size_t)F;
+    sa.bad = js.sp_flags.p;
+    sa.conv = js.sp_flags.p + 1;
+  }
 
   // device events around the three stages of the iterations queued since the last host read (match,
   // reject + blocks, solve + update: sicp_timings), read at each host read.  The host reads at
@@ -581,7 +718,13 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     SICP_CUDA(cudaEventRecord(e[1], st));
     joint_reject_launch(c, a, n_edges);
     SICP_CUDA(cudaEventRecord(e[2], st));
-    joint_solve_launch(c, a);
+    if (sparse) {
+      sa.j.it = it;
+      sa.j.last = a.last;
+      joint_sparse_solve_launch(c, sa);
+    } else {
+      joint_solve_launch(c, a);
+    }
     SICP_CUDA(cudaEventRecord(e[3], st));
     if (it >= next_sync || a.last) {
       next_sync = it + every;
@@ -759,6 +902,7 @@ static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n
                "sicp_register_joint, or a later call cleared its outputs");
   Batch& b = *c.batch;
   JointStore& js = b.joint;
+  SICP_REQUIRE(!js.sparse, SICP_ERR_STATE, "covariances need joint_solver 0");
   SICP_REQUIRE(n_clouds == js.n_clouds && n_edges == js.n_edges, SICP_ERR_BAD_ARG,
                "n_clouds and n_edges must equal the last sicp_register_joint's (" + std::to_string(js.n_clouds) +
                    ", " + std::to_string(js.n_edges) + ")");
@@ -1134,10 +1278,18 @@ static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const
     }
   }
   j.F = (int)j.free_ids.size();
-  SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_MAX_FREE, SICP_ERR_BAD_ARG,
-               "the edges must reference between 1 and 256 free clouds (got " + std::to_string(j.F) + ")");
-  check_anchored(j, std::vector<char>((size_t)n_edges, 1), SICP_ERR_BAD_ARG,
-                 "a free cloud is in a component of the edge graph without a fixed cloud");
+  if (c.joint_solver == 1)
+    SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_SPARSE_MAX_FREE, SICP_ERR_BAD_ARG,
+                 "the edges must reference between 1 and " + std::to_string(JOINT_SPARSE_MAX_FREE) +
+                     " free clouds under joint_solver 1 (got " + std::to_string(j.F) + ")");
+  else
+    SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_MAX_FREE, SICP_ERR_BAD_ARG,
+                 "the edges must reference between 1 and 256 free clouds (got " + std::to_string(j.F) + ")");
+  const std::vector<char> every((size_t)n_edges, 1);
+  check_anchored(j, every, SICP_ERR_BAD_ARG, "a free cloud is in a component of the edge graph without a fixed cloud");
+  // the sparse factor's size over every edge, before any upload (joint_loop checks it again over the
+  // edges that keep their overlap, whose plan it runs)
+  if (c.joint_solver == 1) joint_sparse_plan(j, every);
   j.prior.resize((size_t)n_edges);
   for (int e = 0; e < n_edges; ++e)
     j.prior[(size_t)e] = rigid_compose(rigid_inverse(j.pose[(size_t)fix_id[e]]), j.pose[(size_t)mov_id[e]]);

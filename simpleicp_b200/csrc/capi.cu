@@ -309,6 +309,7 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     c.grid_max_rings = d.grid_max_rings;
     c.grid_sort_cells = d.grid_sort_cells;
     c.match_group = d.match_group;
+    c.joint_solver = d.joint_solver;
     c.host_sync_every = d.host_sync_every;
     c.upload_threads = d.upload_threads;
     c.up.chunk = d.up.chunk;
@@ -354,6 +355,9 @@ int32_t sicp_set_option(sicp_ctx* ctx, const char* key, double value) {
     SICP_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4 || value == 8 || value == 16, SICP_ERR_BAD_ARG,
                  "match_group must be 0 (auto), 1, 2, 4, 8 or 16");
     c.match_group = (int)value;
+  } else if (k == "joint_solver") {
+    SICP_REQUIRE(value == 0 || value == 1, SICP_ERR_BAD_ARG, "joint_solver must be 0 (dense) or 1 (sparse)");
+    c.joint_solver = (int)value;
   } else if (k == "upload_threads") {
     SICP_REQUIRE(value >= 0 && value <= PageableUploader::kMaxThreads, SICP_ERR_BAD_ARG,
                  "upload_threads must be within [0, 8]");

@@ -92,6 +92,7 @@ struct Ctx {
   int host_sync_every = 4;
   int grid_sort_cells = 0;  // 1: sort the records inside each cell by index (layout only)
   int match_group = 0;   // lanes cooperating on one grid query: 0 = by K, else 1, 4, 8 or 16
+  int joint_solver = 0;  // sicp_register_joint's solve: 0 dense (k_joint_solve), 1 sparse (k_joint_sparse_solve)
 
   // clouds
   DevBuf<double> fix_xyz, mov_xyz;
@@ -279,6 +280,40 @@ struct JointArgs {
   double cw[3];            // the common world centre of the increments
   double min_planarity, min_change;
 };
+// One supernode of the sparse solve's plan (joint_plan.h): its clouds at positions first ..
+// first + ns - 1, its struct st[st_off .. st_off + nt), its updates [u0, u1) and the offset of its
+// panel block table.
+struct JointSuper {
+  int first, ns, nt, st_off, u0, u1, table, pad;
+};
+// k_joint_sparse_solve (option "joint_solver" 1): the plan of joint_plan.h on the device.  j is read
+// as k_joint_solve reads it, except blk_of / blk_off / blk_edge, npad and A.
+struct JointSparseArgs {
+  JointArgs j;
+  const JointSuper* sn;
+  const long long* panel;  // per supernode: offset of its column-major panel in L, in doubles
+  const int* st;           // the structs (positions)
+  const int* up;           // per update, 4 ints: descendant, first struct entry used, entries inside s, map offset
+  const int* map;          // the row maps of the updates: panel cloud rows of s
+  const int* lv_off;       // depth + 1
+  const int* lv;           // the supernodes by level
+  const int* perm;         // position -> free cloud
+  // panel block (cloud row ri, cloud column cj) of supernode s: list blk[table + ri ns + cj] of
+  // lst_edge[lst_off[list] ..] (2 e + (1: the cloud is the edge's a)), -1 for none or above the diagonal
+  const int* blk;
+  const int* lst_off;
+  const int* lst_edge;
+  // per free cloud, 3 doubles: the origin of its start pose minus c_w.  The system is solved for
+  // each cloud's increment about that origin, assembled from the edges' sums with levers of metres
+  // (the same solution as about c_w, DESIGN.md §6.11), and carried back to c_w for the update
+  const double* dc;
+  int depth;
+  double* L;               // the panels
+  double* x;               // 6 F: L^T x = y by positions, the working values of the back substitution
+  double* xf;              // 6 F: the solution in free-cloud order
+  int* bad;                // [1] a non-positive or non-finite pivot (0 between calls)
+  int* conv;               // per block: its edges met the stop rule
+};
 // sicp_get_joint_covariances (joint.cu: joint_cov_launch), from what the final iteration of the
 // last sicp_register_joint left: the factor L of its joint matrix (upper-left n x n of A), the
 // edges' final kept rows and residuals, and the returned poses.
@@ -312,6 +347,11 @@ struct JointStore {
   DevBuf<int> ids;  // fix_id, mov_id, free_of, free_ids, blk_of, blk_off, blk_edge
   DevBuf<double> A;
   DevBuf<unsigned int> bar;
+  // the sparse solve (joint_solver 1): its panels, x, xf and dc (15 F), bad + one flag per block
+  bool sparse = false;  // the last call used it (no covariances)
+  DevBuf<long long> sp_panel;
+  DevBuf<double> sp_L, sp_x;
+  DevBuf<int> sp_flags;
   JointFlags* flags_host = nullptr;  // pinned
   // what sicp_get_joint_covariances needs of the last call (set by joint_loop), and its cache:
   // per cloud and per edge row-major 6 x 6 blocks and s0, computed by the first get after the call
@@ -328,6 +368,7 @@ struct JointStore {
 };
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges);
 void joint_solve_launch(Ctx& c, const JointArgs& a);
+void joint_sparse_solve_launch(Ctx& c, const JointSparseArgs& a);
 // k_joint_cov_ss, k_joint_inv, k_joint_cov_cloud, k_joint_cov_edge: the covariances of the last
 // sicp_register_joint into a.cov_f / a.cov_e and s0^2 into a.s0sq (DESIGN.md §6.9)
 void joint_cov_launch(Ctx& c, const JointCovArgs& a);

@@ -12,6 +12,9 @@
 //                    order; right-looking tiled Cholesky (the augmented row leaves L^-1 b behind);
 //                    back substitution; the pose update of every free cloud, each edge's new
 //                    relative transform, increment, residual statistics, record and stop rule
+//   k_joint_sparse_solve  in its place under option "joint_solver" 1: the same system by the
+//                    supernodal Cholesky of joint_plan.h's nested-dissection plan, level by level,
+//                    and the same tail spread over the grid (DESIGN.md §6.11)
 //
 // and, on the first sicp_get_joint_covariances after a call, from what its final iteration left:
 //
@@ -233,6 +236,85 @@ __device__ __forceinline__ double change_pct(double v, double v0) {
   return (v0 == 0.0) ? ((v == 0.0) ? 0.0 : kInf) : fabs((v - v0) / v0 * 100.0);
 }
 
+// ---- the tail of an iteration, shared by k_joint_solve and k_joint_sparse_solve --------------------
+
+// poses: T_c <- dH(x_c) T_c for free cloud f, x_c = (omega, t' - omega x c_w), y = (omega, t')
+__device__ __forceinline__ void joint_pose_update(const JointArgs& a, int f, const double* y) {
+  const double x[6] = {y[0], y[1], y[2], y[3] - (y[1] * a.cw[2] - y[2] * a.cw[1]),
+                       y[4] - (y[2] * a.cw[0] - y[0] * a.cw[2]), y[5] - (y[0] * a.cw[1] - y[1] * a.cw[0])};
+  Rigid& T = a.pose[a.free_ids[f]];
+  T = rigid_compose(rigid_from_x(x), T);
+}
+
+// edge e after the pose update, as the body of a loop over the edges: new relative transform,
+// increment, residual statistics, record, stop rule, from xs (6 per free cloud, in free-cloud order);
+// conv is cleared when the edge takes part and does not meet the stop rule.  A macro rather than a
+// function, so that k_joint_solve compiles to the instructions it had before it shared this code.
+#define JOINT_EDGE_UPDATE(a, e, xs, conv)                                                                                \
+  {                                                                                                                      \
+    DevState& st = a.state[e];                                                                                           \
+    if (st.stop) continue;                                                                                               \
+    const JointEdge& je = a.edges[e];                                                                                    \
+    const int ca = a.fix_id[e], cb = a.mov_id[e];                                                                        \
+    const Rigid Rold = st.T;                                                                                             \
+    const Rigid Rn = rigid_compose(rigid_inverse(a.pose[ca]), a.pose[cb]);                                               \
+    st.T = Rn;                                                                                                           \
+    st.Tinv = rigid_inverse(Rn);                                                                                         \
+    st.H_rep = Rn;                                                                                                       \
+    st.T_new = Rn;                                                                                                       \
+    st.T_res = Rn;                                                                                                       \
+    st.n_kept = je.n;                                                                                                    \
+    st.iterations_done = a.it + 1;                                                                                       \
+    st.lm_ok = 1;                                                                                                        \
+    for (int j = 0; j < 6; ++j) st.sigma[j] = nan("");                                                                   \
+    if (!je.part) continue;                                                                                              \
+    const int fa = a.free_of[ca], fb = a.free_of[cb];                                                                    \
+    double y[6], xi[6];                                                                                                  \
+    for (int j = 0; j < 6; ++j) y[j] = (fb >= 0 ? xs[6 * fb + j] : 0.0) - (fa >= 0 ? xs[6 * fa + j] : 0.0);              \
+    ad_apply(je.Ra, je.v, y, xi);                                                                                        \
+    /* residuals a . xi + d of the kept rows: their sum and sum of squares from the sums */                           \
+    double sr = je.sd, quad = 0.0, lin = 0.0;                                                                            \
+    for (int r = 0; r < 6; ++r) {                                                                                        \
+      sr = fma(je.s[r], xi[r], sr);                                                                                      \
+      lin = fma(je.h[r], xi[r], lin);                                                                                    \
+      double row = 0.0;                                                                                                  \
+      for (int c = 0; c < 6; ++c) row = fma(je.N[r >= c ? tri(r, c) : tri(c, r)], xi[c], row);                           \
+      quad = fma(row, xi[r], quad);                                                                                      \
+    }                                                                                                                    \
+    const double nn = (double)je.n;                                                                                      \
+    const double mean = sr / nn;                                                                                         \
+    const double sr2 = quad + 2.0 * lin + je.sd2;                                                                        \
+    const double sd = sqrt(fmax(sr2 - nn * mean * mean, 0.0) / (nn - 1.0));                                              \
+    /* the origin-based increment of frame a: t = t_c - alpha x c_f */                                                \
+    const double ex[6] = {xi[0], xi[1], xi[2], xi[3] - (xi[1] * je.cf[2] - xi[2] * je.cf[1]),                            \
+                          xi[4] - (xi[2] * je.cf[0] - xi[0] * je.cf[2]), xi[5] - (xi[0] * je.cf[1] - xi[1] * je.cf[0])}; \
+    Rigid L;                                                                                                             \
+    L.r[0] = 1.0; L.r[1] = -ex[2]; L.r[2] = ex[1];                                                                       \
+    L.r[3] = ex[2]; L.r[4] = 1.0; L.r[5] = -ex[0];                                                                       \
+    L.r[6] = -ex[1]; L.r[7] = ex[0]; L.r[8] = 1.0;                                                                       \
+    L.t[0] = ex[3]; L.t[1] = ex[4]; L.t[2] = ex[5];                                                                      \
+    st.T_res = rigid_compose(L, Rold);                                                                                   \
+    sicp_iter_record* rec = a.rec + (size_t)e * a.rec_stride + a.it;                                                     \
+    for (int j = 0; j < 6; ++j) {                                                                                        \
+      rec->x[j] = ex[j];                                                                                                 \
+      st.x_new[j] = ex[j];                                                                                               \
+    }                                                                                                                    \
+    rec->mean_res = mean;                                                                                                \
+    rec->std_res = sd;                                                                                                   \
+    const bool stop = change_pct(mean, st.prev_mean) < a.min_change && change_pct(sd, st.prev_std) < a.min_change;       \
+    if (!stop) conv = 0;                                                                                                 \
+    st.prev_mean = mean;                                                                                                 \
+    st.prev_std = sd;                                                                                                    \
+  }
+
+// edge e when the call ends at this iteration (conv: every edge met the stop rule)
+__device__ __forceinline__ void joint_edge_finish(const JointArgs& a, int e, int conv) {
+  DevState& st = a.state[e];
+  if (st.stop) return;
+  st.converged = conv;
+  st.stop = a.edges[e].part ? (conv ? 1 : 0) : 2;
+}
+
 __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
   __shared__ SolveSmem sm;
   const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
@@ -364,83 +446,195 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
     __syncthreads();
   }
 
-  // ---- poses: T_c <- dH(x_c) T_c, x_c = (omega, t' - omega x c_w)
-  for (int f = tid; f < a.F; f += JS_THREADS) {
-    const double* y = sm.xs + 6 * f;
-    const double x[6] = {y[0], y[1], y[2], y[3] - (y[1] * a.cw[2] - y[2] * a.cw[1]),
-                         y[4] - (y[2] * a.cw[0] - y[0] * a.cw[2]), y[5] - (y[0] * a.cw[1] - y[1] * a.cw[0])};
-    Rigid& T = a.pose[a.free_ids[f]];
-    T = rigid_compose(rigid_from_x(x), T);
-  }
+  // ---- poses, then the edges' new relative transforms, records and stop rule
+  for (int f = tid; f < a.F; f += JS_THREADS) joint_pose_update(a, f, sm.xs + 6 * f);
   __syncthreads();
-
-  // ---- edges: new relative transform, increment, residual statistics, record, stop rule
   int conv = a.it > 0 ? 1 : 0;
-  for (int e = tid; e < a.n_edges; e += JS_THREADS) {
-    DevState& st = a.state[e];
-    if (st.stop) continue;
-    const JointEdge& je = a.edges[e];
-    const int ca = a.fix_id[e], cb = a.mov_id[e];
-    const Rigid Rold = st.T;
-    const Rigid Rn = rigid_compose(rigid_inverse(a.pose[ca]), a.pose[cb]);
-    st.T = Rn;
-    st.Tinv = rigid_inverse(Rn);
-    st.H_rep = Rn;
-    st.T_new = Rn;
-    st.T_res = Rn;
-    st.n_kept = je.n;
-    st.iterations_done = a.it + 1;
-    st.lm_ok = 1;
-    for (int j = 0; j < 6; ++j) st.sigma[j] = nan("");
-    if (!je.part) continue;
-    const int fa = a.free_of[ca], fb = a.free_of[cb];
-    double y[6], xi[6];
-    for (int j = 0; j < 6; ++j) y[j] = (fb >= 0 ? sm.xs[6 * fb + j] : 0.0) - (fa >= 0 ? sm.xs[6 * fa + j] : 0.0);
-    ad_apply(je.Ra, je.v, y, xi);
-    // residuals a . xi + d of the kept rows: their sum and sum of squares from the sums
-    double sr = je.sd, quad = 0.0, lin = 0.0;
-    for (int r = 0; r < 6; ++r) {
-      sr = fma(je.s[r], xi[r], sr);
-      lin = fma(je.h[r], xi[r], lin);
-      double row = 0.0;
-      for (int c = 0; c < 6; ++c) row = fma(je.N[r >= c ? tri(r, c) : tri(c, r)], xi[c], row);
-      quad = fma(row, xi[r], quad);
-    }
-    const double nn = (double)je.n;
-    const double mean = sr / nn;
-    const double sr2 = quad + 2.0 * lin + je.sd2;
-    const double sd = sqrt(fmax(sr2 - nn * mean * mean, 0.0) / (nn - 1.0));
-    // the origin-based increment of frame a: t = t_c - alpha x c_f
-    const double ex[6] = {xi[0], xi[1], xi[2], xi[3] - (xi[1] * je.cf[2] - xi[2] * je.cf[1]),
-                          xi[4] - (xi[2] * je.cf[0] - xi[0] * je.cf[2]), xi[5] - (xi[0] * je.cf[1] - xi[1] * je.cf[0])};
-    Rigid L;
-    L.r[0] = 1.0; L.r[1] = -ex[2]; L.r[2] = ex[1];
-    L.r[3] = ex[2]; L.r[4] = 1.0; L.r[5] = -ex[0];
-    L.r[6] = -ex[1]; L.r[7] = ex[0]; L.r[8] = 1.0;
-    L.t[0] = ex[3]; L.t[1] = ex[4]; L.t[2] = ex[5];
-    st.T_res = rigid_compose(L, Rold);
-    sicp_iter_record* rec = a.rec + (size_t)e * a.rec_stride + a.it;
-    for (int j = 0; j < 6; ++j) {
-      rec->x[j] = ex[j];
-      st.x_new[j] = ex[j];
-    }
-    rec->mean_res = mean;
-    rec->std_res = sd;
-    const bool stop = change_pct(mean, st.prev_mean) < a.min_change && change_pct(sd, st.prev_std) < a.min_change;
-    if (!stop) conv = 0;
-    st.prev_mean = mean;
-    st.prev_std = sd;
-  }
+  for (int e = tid; e < a.n_edges; e += JS_THREADS) JOINT_EDGE_UPDATE(a, e, sm.xs, conv)
   conv = __syncthreads_and(conv);
   const bool finish = conv || a.last;
   if (finish)
-    for (int e = tid; e < a.n_edges; e += JS_THREADS) {
-      DevState& st = a.state[e];
-      if (st.stop) continue;
-      st.converged = conv;
-      st.stop = a.edges[e].part ? (conv ? 1 : 0) : 2;
-    }
+    for (int e = tid; e < a.n_edges; e += JS_THREADS) joint_edge_finish(a, e, conv);
   if (tid == 0) {
+    a.flags->converged = conv;
+    a.flags->done = finish ? 1 : 0;
+  }
+}
+// ---- k_joint_sparse_solve: the supernodal Cholesky of joint_plan.h (DESIGN.md §6.11) -----------------
+
+// Column k of edge e's Ad for a cloud whose increment (omega, u) is taken about its own origin o:
+// Ad with the lever v - d = T_a c_f - o (d = o - c_w), metres where v itself can be kilometres.
+__device__ __forceinline__ void ad_column(const JointEdge& je, const double* d, int k, double (&col)[6]) {
+  const double lever[3] = {je.v[0] - d[0], je.v[1] - d[1], je.v[2] - d[2]};
+  double y[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  y[k] = 1.0;
+  ad_apply(je.Ra, lever, y, col);
+}
+
+// Supernode k by the whole block: assembly of its panel P (column-major, R = 6 (ns + nt) + 1 rows,
+// C = 6 ns columns, the right-hand side as row R - 1) from the edges in ascending edge order, each
+// cloud's unknowns taken about its own origin: Ad_r^T N Ad_c and -Ad_c^T h from the edge's sums in
+// frame a (ad_column), never from Nw / gw, whose kilometre levers about c_w cost precision that a
+// change of variables after the fact cannot recover; the left-looking updates from its descendants
+// in ascending order; the right-looking Cholesky of the diagonal block, whose column steps also
+// divide the rows below it (the right-hand side's row is left holding L^-1 b).  A non-positive or
+// non-finite pivot sets *bad.
+__device__ void sparse_factor(const JointSparseArgs& s, int k) {
+  const JointArgs& a = s.j;
+  const int tid = threadIdx.x;
+  const JointSuper& m = s.sn[k];
+  const int ns = m.ns, C = 6 * ns, R = 6 * (ns + m.nt) + 1;
+  double* P = s.L + s.panel[k];
+  for (int idx = tid; idx < R * C; idx += JS_THREADS) {
+    const int c = idx / R, r = idx % R, cj = c / 6;
+    const double* dcol = s.dc + 3 * s.perm[m.first + cj];
+    double v = 0.0;
+    if (r < R - 1) {
+      const int ri = r / 6, l = s.blk[m.table + ri * ns + cj];
+      const int pr = ri < ns ? m.first + ri : s.st[m.st_off + ri - ns];
+      const double* drow = s.dc + 3 * s.perm[pr];
+      if (l >= 0)
+        for (int q = s.lst_off[l]; q < s.lst_off[l + 1]; ++q) {
+          const JointEdge& je = a.edges[s.lst_edge[q] >> 1];
+          if (!je.part) continue;
+          double ar[6], ac[6];
+          ad_column(je, drow, r % 6, ar);
+          ad_column(je, dcol, c % 6, ac);
+          double w = 0.0;
+          for (int x = 0; x < 6; ++x) {
+            double row = 0.0;
+            for (int y = 0; y < 6; ++y) row = fma(je.N[x >= y ? tri(x, y) : tri(y, x)], ac[y], row);
+            w = fma(ar[x], row, w);
+          }
+          v += (ri == cj) ? w : -w;
+        }
+    } else {
+      const int l = s.blk[m.table + cj * ns + cj];
+      if (l >= 0)
+        for (int q = s.lst_off[l]; q < s.lst_off[l + 1]; ++q) {
+          const JointEdge& je = a.edges[s.lst_edge[q] >> 1];
+          if (!je.part) continue;
+          double ac[6];
+          ad_column(je, dcol, c % 6, ac);
+          double w = 0.0;
+          for (int y = 0; y < 6; ++y) w = fma(ac[y], -je.h[y], w);
+          v += (s.lst_edge[q] & 1) ? -w : w;
+        }
+    }
+    P[(size_t)c * R + r] = v;
+  }
+  __syncthreads();
+  // P[map(i), map(j)] -= sum_k Ld[i][k] Ld[j][k] over the rows i of descendant d from its first
+  // struct entry in s on (and its right-hand side's row), the columns j of those inside s
+  for (int u = m.u0; u < m.u1; ++u) {
+    const int* up = s.up + 4 * u;
+    const JointSuper& dm = s.sn[up[0]];
+    const int Cd = 6 * dm.ns, Rd = 6 * (dm.ns + dm.nt) + 1, r0 = Cd + 6 * up[1];
+    const int nr = Rd - r0, nj = 6 * up[2];
+    const int* map = s.map + up[3];
+    const double* Pd = s.L + s.panel[up[0]];
+    for (int idx = tid; idx < nr * nj; idx += JS_THREADS) {
+      const int i = idx % nr, j = idx / nr;
+      const int ti = (i < nr - 1) ? 6 * map[i / 6] + i % 6 : R - 1, tj = 6 * map[j / 6] + j % 6;
+      if (ti < tj) continue;  // above the diagonal
+      double v = 0.0;
+      for (int q = 0; q < Cd; ++q) v = fma(__ldcg(&Pd[(size_t)q * Rd + r0 + i]), __ldcg(&Pd[(size_t)q * Rd + r0 + j]), v);
+      P[(size_t)tj * R + ti] -= v;
+    }
+    __syncthreads();
+  }
+  for (int j = 0; j < C; ++j) {
+    const double d = P[(size_t)j * R + j];
+    if (tid == 0 && (!(d > 0.0) || !isfinite(d))) *s.bad = 1;
+    const double piv = sqrt(d);
+    for (int r = j + 1 + tid; r < R; r += JS_THREADS) P[(size_t)j * R + r] /= piv;
+    __syncthreads();
+    if (tid == 0) P[(size_t)j * R + j] = piv;
+    for (int r = j + 1 + tid; r < R; r += JS_THREADS) {
+      const double lr = P[(size_t)j * R + r];
+      const int ce = min(r, C - 1);
+      for (int c = j + 1; c <= ce; ++c) P[(size_t)c * R + r] = fma(-lr, P[(size_t)j * R + c], P[(size_t)c * R + r]);
+    }
+    __syncthreads();
+  }
+}
+
+// Supernode k by the whole block, after every ancestor: x_s = L_ss^-T (y_s - L_ts^T x_t), y_s its
+// right-hand side's row, t its struct; the solution goes to xf in free-cloud order.
+__device__ void sparse_back(const JointSparseArgs& s, int k) {
+  const int tid = threadIdx.x;
+  const JointSuper& m = s.sn[k];
+  const int nt = m.nt, C = 6 * m.ns, R = 6 * (m.ns + nt) + 1;
+  const double* P = s.L + s.panel[k];
+  double* x = s.x + 6 * m.first;
+  for (int c = tid; c < C; c += JS_THREADS) {
+    double v = P[(size_t)c * R + R - 1];
+    for (int r = 0; r < 6 * nt; ++r)
+      v = fma(-P[(size_t)c * R + C + r], __ldcg(&s.xf[6 * s.perm[s.st[m.st_off + r / 6]] + r % 6]), v);
+    x[c] = v;
+  }
+  __syncthreads();
+  for (int c = C - 1; c >= 0; --c) {
+    const double xc = x[c] / P[(size_t)c * R + c];
+    for (int i = tid; i < c; i += JS_THREADS) x[i] = fma(-P[(size_t)i * R + c], xc, x[i]);
+    if (tid == 0) s.xf[6 * s.perm[m.first + c / 6] + c % 6] = xc;
+    __syncthreads();
+  }
+}
+
+// One cooperative launch per iteration in place of k_joint_solve: the factor bottom-up by level and
+// the back substitution top-down (one supernode per block, one grid barrier per level), then the
+// tail of k_joint_solve spread over the grid.
+__global__ void __launch_bounds__(JS_THREADS) k_joint_sparse_solve(const JointSparseArgs s) {
+  __shared__ int conv_s;
+  const JointArgs& a = s.j;
+  const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
+  if (a.flags->done) return;  // uniform: only block 0 writes it, at the very end of this launch
+  for (int l = 0; l < s.depth; ++l) {
+    for (int i = s.lv_off[l] + bid; i < s.lv_off[l + 1]; i += G) sparse_factor(s, s.lv[i]);
+    joint_grid_sync(a.bar);
+  }
+  if (__ldcg(s.bad)) {
+    if (bid == 0 && tid == 0) {
+      a.flags->singular = 1;
+      a.flags->done = 1;
+    }
+    return;
+  }
+  for (int l = s.depth - 1; l >= 0; --l) {
+    for (int i = s.lv_off[l] + bid; i < s.lv_off[l + 1]; i += G) sparse_back(s, s.lv[i]);
+    joint_grid_sync(a.bar);
+  }
+  const int gt = bid * JS_THREADS + tid, GT = G * JS_THREADS;
+  // (omega, u) about each cloud's centre -> (omega, t') about c_w, in place for the edges
+  for (int f = gt; f < a.F; f += GT) {
+    double y[6];
+    for (int q = 0; q < 6; ++q) y[q] = __ldcg(&s.xf[6 * f + q]);
+    const double* d = s.dc + 3 * f;
+    y[3] += d[1] * y[2] - d[2] * y[1];
+    y[4] += d[2] * y[0] - d[0] * y[2];
+    y[5] += d[0] * y[1] - d[1] * y[0];
+    for (int q = 3; q < 6; ++q) s.xf[6 * f + q] = y[q];
+    joint_pose_update(a, f, y);
+  }
+  joint_grid_sync(a.bar);
+  const double* xs = s.xf;
+  int conv = a.it > 0 ? 1 : 0;
+  for (int e = gt; e < a.n_edges; e += GT) JOINT_EDGE_UPDATE(a, e, xs, conv)
+  conv = __syncthreads_and(conv);
+  if (tid == 0) s.conv[bid] = conv;
+  joint_grid_sync(a.bar);
+  if (tid == 0) {
+    int v = 1;
+    for (int b = 0; b < G; ++b) v &= __ldcg(&s.conv[b]);
+    conv_s = v;
+  }
+  __syncthreads();
+  conv = conv_s;
+  const bool finish = conv || a.last;
+  if (finish)
+    for (int e = gt; e < a.n_edges; e += GT) joint_edge_finish(a, e, conv);
+  if (bid == 0 && tid == 0) {
     a.flags->converged = conv;
     a.flags->done = finish ? 1 : 0;
   }
@@ -733,6 +927,14 @@ void joint_solve_launch(Ctx& c, const JointArgs& a) {
   JointArgs args = a;
   void* p[] = {&args};
   SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_solve, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
+  c.tm.kernel_launches += 1;
+}
+
+void joint_sparse_solve_launch(Ctx& c, const JointSparseArgs& a) {
+  JointSparseArgs args = a;
+  void* p[] = {&args};
+  SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_sparse_solve, dim3(c.num_sms), dim3(JS_THREADS), p, 0,
+                                        c.stream));
   c.tm.kernel_launches += 1;
 }
 
