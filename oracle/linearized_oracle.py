@@ -76,10 +76,11 @@ def euler_angles_to_rotation_matrix(a1: float, a2: float, a3: float) -> np.ndarr
     )
 
 
-def select_in_range(X_fix: np.ndarray, X_mov: np.ndarray, max_range: float) -> np.ndarray:
+def select_in_range(X_fix: np.ndarray, X_mov: np.ndarray, max_range: float, workers: int = -1) -> np.ndarray:
     """pointcloud.cpp:33-76 -- keep fixed points whose nearest movable point is within range
-    (deselect when dist > max_range, i.e. keep dist <= max_range)."""
-    d, _ = spatial.cKDTree(X_mov).query(X_fix, k=1, workers=-1)
+    (deselect when dist > max_range, i.e. keep dist <= max_range).  `workers` only splits the
+    exact query over threads (1 for small clouds, where starting threads costs more than it saves)."""
+    d, _ = spatial.cKDTree(X_mov).query(X_fix, k=1, workers=workers)
     return np.flatnonzero(d <= max_range)
 
 

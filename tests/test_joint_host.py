@@ -82,6 +82,73 @@ def test_ring_joint_beats_chained_pairs_and_closes_the_loop():
     assert pose_error(res.H, truth) < 1e-2
 
 
+def test_oracle_sparse_solve_equals_its_dense_solve_on_the_ring():
+    """solver="sparse" (scipy.sparse.linalg.spsolve of the same blocks) against the dense path:
+    the same iterations and kept counts, the poses within 1e-12 (measured 3.0e-15)."""
+    scans, truth, H0, edges = ring()
+    kw = dict(fixed=(0,), H0=H0, max_iterations=30, max_overlap_distance=1.0)
+    dense = J.simpleicp_joint(scans, edges, **kw)
+    sparse = J.simpleicp_joint(scans, edges, solver="sparse", **kw)
+    assert [[e.n_kept for e in r] for r in dense.log] == [[e.n_kept for e in r] for r in sparse.log]
+    assert sparse.converged == dense.converged
+    assert np.abs(sparse.H - dense.H).max() < 1e-12
+
+
+def test_oracle_sparse_solve_equals_its_dense_solve_on_the_128_cloud_strip():
+    """The strip of tests/test_gpu_joint.py, 128 clouds of 5 000 points, 400 edges, three
+    iterations.  The oracle's unknowns are about the world origin, so its matrix is ill-conditioned
+    on a 270 m strip and the two solves of the first iteration part by 8.4e-9 in the poses; the
+    iterations pull both to the same poses, 3.3e-11 apart after three (bound 1e-10).  Every kept
+    count exact."""
+    from test_gpu_joint import strip
+
+    scans, truth, H0, edges = strip(128, 5_000, 400)
+    kw = dict(fixed=(0,), H0=H0, max_iterations=3, max_overlap_distance=1.0)
+    dense = J.simpleicp_joint(scans, edges, **kw)
+    sparse = J.simpleicp_joint(scans, edges, solver="sparse", **kw)
+    assert [[e.n_kept for e in r] for r in dense.log] == [[e.n_kept for e in r] for r in sparse.log]
+    assert np.abs(sparse.H - dense.H).max() < 1e-10
+
+
+def test_first_iteration_sums_are_the_first_iterations_rows():
+    """first_iteration_sums against the rows simpleicp_joint solves: the kept counts of its first
+    iteration, and the first increments from a dense solve assembled from the sums."""
+    scans, truth, H0, edges = ring()
+    ref = J.simpleicp_joint(scans, edges, fixed=(0,), H0=H0, max_iterations=1, max_overlap_distance=1.0)
+    s = J.first_iteration_sums(scans, edges, fixed=(0,), H0=H0, max_overlap_distance=1.0)
+    assert list(s.n_kept) == [e.n_kept for e in ref.log[0]] and s.free == list(range(1, 8))
+    F = len(s.free)
+    M, g = np.zeros((6 * F, 6 * F)), np.zeros(6 * F)
+    for (a, b), N, h, Ta in zip(edges, s.N, s.g, s.T_a):
+        Ad = J.ad_world_to_frame(Ta)
+        for c, sgn in ((a, -1.0), (b, 1.0)):
+            if c > 0:
+                i = 6 * (c - 1)
+                g[i:i + 6] += sgn * Ad.T @ h
+                for d, sgn2 in ((a, -1.0), (b, 1.0)):
+                    if d > 0:
+                        j = 6 * (d - 1)
+                        M[i:i + 6, j:j + 6] += sgn * sgn2 * Ad.T @ N @ Ad
+    x = np.linalg.solve(M, g)
+    for c in range(1, 8):
+        assert np.abs(J.rigid_from_x(x[6 * (c - 1):6 * c]) @ H0[c] - ref.H[c]).max() < 1e-12
+
+
+def test_an_edge_without_overlap_has_no_rows_and_takes_no_part():
+    """Edge (1, 2) to a fixed cloud 1 km away has an empty selection under max_overlap_distance:
+    kept count 0 in every iteration and in first_iteration_sums, and the poses are those of the
+    same problem without that edge, bit for bit."""
+    scans, truth, H0, edges = ring()
+    clouds = [scans[0], scans[1], scans[2] + 1000.0]
+    kw = dict(fixed=(0, 2), H0=H0[:3], max_iterations=30, max_overlap_distance=1.0)
+    res = J.simpleicp_joint(clouds, [(0, 1), (1, 2)], **kw)
+    alone = J.simpleicp_joint(clouds, [(0, 1)], **kw)
+    assert all(r[1].n_kept == 0 and r[1].xi is None for r in res.log)
+    assert len(res.log) == len(alone.log) and np.array_equal(res.H, alone.H)
+    s = J.first_iteration_sums(clouds, [(0, 1), (1, 2)], fixed=(0, 2), H0=H0[:3], max_overlap_distance=1.0)
+    assert s.n_kept[1] == 0 and not s.N[1].any() and not s.g[1].any()
+
+
 def _clouds(n=3, m=200):
     rng = np.random.default_rng(1)
     return [rng.normal(size=(m, 3)) for _ in range(n)]

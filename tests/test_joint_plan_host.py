@@ -182,10 +182,13 @@ def test_cholesky_stays_inside_the_symbolic_pattern(lib, name):
     assert not np.any(nz & ~allowed), np.argwhere(nz & ~allowed)[:5]
 
 
-def supernodal_solve(pl, N, b):
+def supernodal_solve(pl, N, b, fault=None):
     """k_joint_sparse_solve's arithmetic on the plan: the panels assembled from N (free-cloud order)
     and b as their last row, the descendants' updates, the column Cholesky, and the back
-    substitution from the top level down.  Returns x in free-cloud order."""
+    substitution from the top level down.  Returns x in free-cloud order.  `fault` = (kind, s, u)
+    makes one deliberate mistake in supernode s, as a wrong kernel would: "drop" skips update u,
+    "flip" negates the off-diagonal 6 x 6 block u = (row block, column block) of its panel,
+    "stale" sends the last row of update u's map to the panel row block that precedes it."""
     perm, S = pl["perm"], pl["n_super"]
     panels = []
     for s in range(S):
@@ -195,11 +198,19 @@ def supernodal_solve(pl, N, b):
         P = np.zeros((R, Cn))
         P[:R - 1] = N[np.ix_(expand(perm[rows]), expand(perm[cols]))]
         P[R - 1] = b[expand(perm[cols])]
+        if fault and fault[0] == "flip" and fault[1] == s:
+            i, j = fault[2]
+            P[6 * i:6 * i + 6, 6 * j:6 * j + 6] *= -1.0
         for u in range(pl["up_off"][s], pl["up_off"][s + 1]):
+            if fault and fault[0] == "drop" and fault[1:] == (s, u):
+                continue
             d, i0, nj, mo = (int(pl[f][u]) for f in ("up", "up_i0", "up_nj", "up_map"))
             Pd = panels[d]
             r0 = 6 * (pl["first"][d + 1] - pl["first"][d]) + 6 * i0
             m = pl["map"][mo:mo + (Pd.shape[0] - 1 - r0) // 6]
+            if fault and fault[0] == "stale" and fault[1:] == (s, u):
+                m = m.copy()
+                m[-1] -= 1
             ti = np.concatenate((expand(m), [R - 1]))
             tj = expand(m[:nj])
             P[np.ix_(ti, tj)] -= Pd[r0:] @ Pd[r0:r0 + 6 * nj].T
@@ -229,6 +240,42 @@ def test_supernodal_solve_equals_the_dense_solve(lib, name):
     x = supernodal_solve(pl, N, b)
     ref = np.linalg.solve(N, b)
     assert np.abs(x - ref).max() <= 1e-11 * np.abs(ref).max()
+
+
+def backward_error(N, b, x):
+    """eta = |b - N x|_inf / (|N|_inf |x|_inf + |b|_inf), the residual in extended precision: the
+    normwise backward error of x as a solution of N x = b (DESIGN.md §6.11)."""
+    r = np.asarray(b, dtype=np.longdouble) - np.asarray(N, dtype=np.longdouble) @ np.asarray(x, dtype=np.longdouble)
+    return float(np.abs(r).max() / (np.abs(N).sum(1).max() * np.abs(x).max() + np.abs(b).max()))
+
+
+def test_backward_error_catches_a_wrong_update_sign_or_row_map(lib):
+    """The metric of the GPU backward-error tests (tests/test_gpu_joint_graphs.py) on the 2-D grid,
+    against the restatement above with one mistake at a time: the last update of the supernode
+    with the most updates dropped, the sign of one off-diagonal block, one stale row of a
+    map.  The correct solve is at rounding level (measured 1.6e-16); each mistake is at least 1e-8."""
+    F, pairs = graph("grid_2d")
+    pl = make_plan(lib, F, pairs)
+    N = spd_matrix(F, pairs, seed=1)
+    b = np.random.default_rng(2).normal(size=6 * F)
+    assert backward_error(N, b, supernodal_solve(pl, N, b)) <= 1e-14
+    n_up = np.diff(pl["up_off"])
+    s = int(np.argmax(n_up))
+    assert n_up[s] >= 2
+    u_last = int(pl["up_off"][s + 1]) - 1
+    # the first supernode with an off-diagonal block that N holds; the first update whose map has
+    # rows below the columns it updates
+    def rows(t):
+        return pl["perm"][np.concatenate((np.arange(pl["first"][t], pl["first"][t + 1]), struct(pl, t)))]
+
+    s_fl, flip = next((t, (i, j)) for t in range(pl["n_super"]) for j in range(pl["first"][t + 1] - pl["first"][t])
+                      for i in range(j + 1, rows(t).size)
+                      if np.any(N[6 * rows(t)[i]:6 * rows(t)[i] + 6, 6 * rows(t)[j]:6 * rows(t)[j] + 6]))
+    s_st, stale = next((t, u) for t in range(pl["n_super"]) for u in range(pl["up_off"][t], pl["up_off"][t + 1])
+                       if struct(pl, int(pl["up"][u])).size - int(pl["up_i0"][u]) > int(pl["up_nj"][u]))
+    for fault in (("drop", s, u_last), ("flip", s_fl, flip), ("stale", s_st, stale)):
+        eta = backward_error(N, b, supernodal_solve(pl, N, b, fault))
+        assert eta >= 1e-8, (fault, eta)
 
 
 def test_strip_of_4096_clouds_has_a_shallow_tree(lib):
