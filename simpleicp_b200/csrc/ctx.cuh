@@ -182,6 +182,7 @@ struct Ctx {
   bool lin_hist_pending = false;          // filled by a match, not yet consumed by a reject
   bool lin_hist_init = false;
   bool rsb_attr_set = false;
+  bool rs_attr_set = false;               // k_reject_solve's dynamic shared memory limit raised on this device
   bool rsf_attr_set = false;              // k_rs_fused's dynamic shared memory limit raised on this device
   DevBuf<RsSelect> rs_sel;                // k_rs_fused -> k_rs_solve
   DevBuf<RsScratch> rs_scratch;           // stores of k_rs_solve's rehearsal

@@ -471,7 +471,8 @@ __device__ __forceinline__ Rigid rigid_from_x_warp(const double* x, int lane) {
 // order, so the results are those of the dense products bit for bit.
 __device__ __forceinline__ void moment_products(Shared& s, int lane) {
   // B[r][c] for the columns c = 0, 1, 2 (rotation) and 6 (theta): 52 dot products, two per lane
-#pragma unroll
+  // (one copy of the product's code, run twice)
+#pragma unroll 1
   for (int h = 0; h < 2; ++h) {
     const int e = lane + 32 * h;
     if (e < 52) {
@@ -600,17 +601,21 @@ __device__ __forceinline__ void tri_coords(int lane, int& ri, int& cj) {
 }
 
 // In: val = this lane's entry of the augmented matrix.  Out: its entry of the factor L (the
-// diagonal holds sqrt(d_j)); inv[j] = 1 / sqrt(d_j) in every lane; returns false when a pivot is
-// not positive (uniform across the warp).
-__device__ __forceinline__ bool warp_chol7_factor(double& val, int ri, int cj, double (&inv)[6]) {
+// diagonal holds sqrt(d_j)); inv = 1 / sqrt(d_cj), the inverse pivot of this lane's column (cj < 6);
+// returns false when a pivot is not positive (uniform across the warp).  The loops here stay
+// rolled: each pivot depends on the last, so unrolling gains no overlap, only code to fetch.
+__device__ __forceinline__ bool warp_chol7_factor(double& val, int ri, int cj, double& inv) {
   bool ok = true;
-#pragma unroll
+  inv = 0.0;
+#pragma unroll 1
   for (int j = 0; j < 6; ++j) {
     const double d = __shfl_sync(0xffffffffu, val, j * (j + 1) / 2 + j);
     ok = ok && (d > 0.0) && isfinite(d);
     const double r = rsqrt(d);
-    inv[j] = r;
-    if (cj == j) val *= r;
+    if (cj == j) {
+      inv = r;
+      val *= r;
+    }
     const double lij = __shfl_sync(0xffffffffu, val, ri * (ri + 1) / 2 + j);
     const double lkj = __shfl_sync(0xffffffffu, val, cj * (cj + 1) / 2 + j);
     if (cj > j) val = fma(-lij, lkj, val);
@@ -619,11 +624,10 @@ __device__ __forceinline__ bool warp_chol7_factor(double& val, int ri, int cj, d
 }
 
 // Back substitution L^T x = y on the factored lanes; returns x[lane] in lanes 0..5.
-__device__ __forceinline__ double warp_chol7_backsolve(double val, int lane, int ri, int cj,
-                                                       const double (&inv)[6]) {
-#pragma unroll
+__device__ __forceinline__ double warp_chol7_backsolve(double val, int lane, int ri, int cj, const double inv) {
+#pragma unroll 1
   for (int i = 5; i >= 0; --i) {
-    if (ri == 6 && cj == i) val *= inv[i];
+    if (ri == 6 && cj == i) val *= inv;
     const double xi = __shfl_sync(0xffffffffu, val, 21 + i);
     const double lik = __shfl_sync(0xffffffffu, val, i * (i + 1) / 2 + min(cj, i));
     if (ri == 6 && cj < i) val = fma(-lik, xi, val);
@@ -709,7 +713,7 @@ __device__ void lm_solve(Shared& s, const RSArgs& a, double w, const double* x0,
       } else {
         val = 1.0;
       }
-      double inv[6];
+      double inv;
       const bool spd = warp_chol7_factor(val, ri, cj, inv);
       const double sol = warp_chol7_backsolve(val, lane, ri, cj, inv);
       if (lane < 6) s.delta[lane] = sol;
@@ -814,7 +818,7 @@ __device__ void lin_solve(Shared& s, const Rigid& Tc, const double* cf, int lane
   double val = 1.0;
   if (ri < 6) val = s.A[ri * 6 + cj];
   else if (cj < 6) val = -s.g[cj];
-  double inv[6];
+  double inv;
   const bool spd = warp_chol7_factor(val, ri, cj, inv);
   const double sol = warp_chol7_backsolve(val, lane, ri, cj, inv);
   if (lane < 6) s.delta[lane] = sol;
@@ -850,8 +854,10 @@ __device__ void uncertainties(Shared& s, const RSArgs& a, const double* An, doub
   } else if (ri == 6 && cj < 6) {
     val = 0.0;
   }
-  double inv[6];
-  const bool ok = warp_chol7_factor(val, ri, cj, inv);
+  double inv_c, inv[6];
+  const bool ok = warp_chol7_factor(val, ri, cj, inv_c);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) inv[i] = __shfl_sync(0xffffffffu, inv_c, i * (i + 1) / 2 + i);
   // (N^-1)_jj = |L^-1 e_j|^2: lane j forward-substitutes its own unit vector against the factor,
   // which the owning lanes publish through shared memory.
   double* L = s.cholL;
@@ -923,16 +929,36 @@ __device__ __forceinline__ void accumulate_moments(double (&acc)[N], const int r
   }
 }
 
+// Sum of x[0..31] paired as warp_sum() pairs the lanes (l with l + 16, then at distance 8, 4, 2,
+// 1): the bits lane 0 of warp_sum() returns for a warp whose lane l holds x[l].  One thread per
+// sum, on values a warp left in shared memory, instead of a shuffle butterfly per value: the code
+// runs once per launch, and its size, not its arithmetic, is what the first pass pays for.
+constexpr int TREE_STRIDE = 33;  // doubles between the 32 values of two sums (conflict-free reads)
+__device__ __forceinline__ double tree_sum32(const double* x) {
+  double t[16];
+#pragma unroll
+  for (int l = 0; l < 16; ++l) t[l] = x[l] + x[l + 16];
+#pragma unroll
+  for (int l = 0; l < 8; ++l) t[l] += t[l + 8];
+#pragma unroll
+  for (int l = 0; l < 4; ++l) t[l] += t[l + 4];
+  t[0] += t[2];
+  t[1] += t[3];
+  return t[0] + t[1];
+}
+
 // The block's partial sums: every accumulator summed over its warp, then over the four warps of
 // its role in warp order.  Thread t < 3 NACC returns value t (role t / NACC, accumulator t % NACC).
+// buf: RS_WARPS * NACC * TREE_STRIDE doubles of shared memory.
 template <int NACC>
-__device__ __forceinline__ double block_partial(const double (&acc)[NACC], double (&red)[RS_WARPS][NACC]) {
+__device__ __forceinline__ double block_partial(const double (&acc)[NACC], double* buf,
+                                                double (&red)[RS_WARPS][NACC]) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double* mine = buf + warp * NACC * TREE_STRIDE + lane;
 #pragma unroll
-  for (int j = 0; j < NACC; ++j) {
-    const double v = warp_sum(acc[j]);
-    if (lane == 0) red[warp][j] = v;
-  }
+  for (int j = 0; j < NACC; ++j) mine[j * TREE_STRIDE] = acc[j];
+  __syncthreads();
+  if (tid < RS_WARPS * NACC) red[tid / NACC][tid % NACC] = tree_sum32(buf + tid * TREE_STRIDE);
   __syncthreads();
   double v = 0.0;
   if (tid < 3 * NACC) {
@@ -944,10 +970,11 @@ __device__ __forceinline__ double block_partial(const double (&acc)[NACC], doubl
 
 // Fixed-order sum of the per-block partials, stored value-major ([value][block], G <=
 // RSF_MAX_BLOCKS): each warp owns a few values, issues the loads of all their block entries before
-// the first use (one L2 round trip, not one per value) and finishes with a shuffle tree.
-// Deterministic: the order depends on G only.
+// the first use (one L2 round trip, not one per value) and finishes with warp_sum's tree, one
+// thread per value (tree_sum32).  Deterministic: the order depends on G only.  Called by the whole
+// block; buf: NPART * TREE_STRIDE doubles of shared memory.  tot is complete after a barrier.
 template <int NPART>
-__device__ __forceinline__ void reduce_partials(const double* partials, const int G, double* tot) {
+__device__ __forceinline__ void reduce_partials(const double* partials, const int G, double* buf, double* tot) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NO = (NPART + RS_WARPS - 1) / RS_WARPS;  // values per warp
   constexpr int NB = RSF_MAX_BLOCKS / 32;
@@ -967,9 +994,10 @@ __device__ __forceinline__ void reduce_partials(const double* partials, const in
     double v = 0.0;
 #pragma unroll
     for (int u = 0; u < NB; ++u) v += r[q][u];
-    v = warp_sum(v);
-    if (lane == 0 && o < NPART) tot[o] = v;
+    if (o < NPART) buf[o * TREE_STRIDE + lane] = v;
   }
+  __syncthreads();
+  if (threadIdx.x < NPART) tot[threadIdx.x] = tree_sum32(buf + threadIdx.x * TREE_STRIDE);
 }
 
 // Entry (r, c) of M from the reduced sums: the 6 x 10 normal-product sums, the 3 x 4 d n (x) (u, 1)
@@ -1107,9 +1135,11 @@ __device__ __forceinline__ void store_iteration_end(const RSArgs& a, DevState* s
   sto->converged = stop;
 }
 
+constexpr size_t RS_TREEBUF = sizeof(double) * RS_WARPS * RS_NACC * TREE_STRIDE;  // >= RS_NPART sums
 template <bool MULTI>
 __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork wk) {
   __shared__ Shared s;
+  extern __shared__ double rs_treebuf[];  // RS_TREEBUF bytes: block_partial, reduce_partials
   DevState* st = a.state;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const long long K = a.K;
@@ -1198,7 +1228,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
         if (hb) a.keep[ib] = kB ? 1 : 0;
       }
     }
-    const double v = block_partial(acc, s.red);
+    const double v = block_partial(acc, rs_treebuf, s.red);
     if (tid < RS_NPART) {
       if (MULTI)
         wk.partials[(size_t)tid * G + blockIdx.x] = v;
@@ -1212,7 +1242,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) k_reject_solve(RSArgs a, RSWork
 
   // ---- D: block 0 reduces the partials and solves
   if (blockIdx.x == 0) {
-    if (MULTI) reduce_partials<RS_NPART>(wk.partials, G, s.tot);
+    if (MULTI) reduce_partials<RS_NPART>(wk.partials, G, rs_treebuf, s.tot);
     __syncthreads();
     RS_STAMP(17);
     for (int e = tid; e < 169; e += RS_THREADS) s.M[e / 13][e % 13] = moment_entry<RS_NACC>(s.tot, e / 13, e % 13);
@@ -1385,6 +1415,7 @@ struct SharedTail {
   Shared s;
   double totf[RSF_NPART];
   double m1[13];  // sum phi
+  double sumbuf[RSF_NPART * TREE_STRIDE];  // reduce_partials
 };
 
 struct SharedF : SharedTail {
@@ -1397,7 +1428,9 @@ struct SharedF : SharedTail {
   unsigned long long edgebuf[RS_CAP];  // MAD candidates (the median candidates go to s.sortbuf)
   alignas(8) uint64_t t_bar;
   double redf[RS_WARPS][RSF_NACC];
+  double partbuf[RS_WARPS * RSF_NACC * TREE_STRIDE];  // block_partial
 };
+static_assert(sizeof(SharedF) <= 227 * 1024, "k_rs_fused: more shared memory than an H100 SM has");
 
 // k-th smallest (0-based) and its successor among n <= RS_THREADS keys in shared memory by direct
 // ranking — three block barriers instead of the eight radix passes block_select() needs when the
@@ -1679,7 +1712,7 @@ __device__ void rs_fused_body(const RSArgs& a, const RSWork& wk, const int G, co
         if (tid == 0) issue_tile(t0 + RSF_TILE);
       }
     }
-    const double vv = block_partial(acc, sf.redf);
+    const double vv = block_partial(acc, sf.partbuf, sf.redf);
     if (tid < RSF_NPART) wk.partials[(size_t)tid * G + bid] = vv;
   } else if (have_tile) {
     mbar_wait(&sf.t_bar, tile_phase);  // never leave with a bulk copy into this block's shared memory in flight
@@ -1748,7 +1781,7 @@ __device__ __forceinline__ void rs_tail_body(SharedTail& sf, const RSArgs& a, co
     }
     return;
   }
-  reduce_partials<RSF_NPART>(partials, G, sf.totf);
+  reduce_partials<RSF_NPART>(partials, G, sf.sumbuf, sf.totf);
   __syncthreads();
   if (tid == 0) pt[17] = global_timer_ns();
   for (int e = tid; e < 169 + 13; e += RS_THREADS) {
@@ -2162,12 +2195,17 @@ void reject_solve_launch(Ctx& c, const sicp_run_params& p, int it, bool do_solve
   wk.barrier = c.grid_bar.p;
   wk.lin_hist = c.lin_hist.p;
 
+  if (!c.rs_attr_set) {
+    SICP_CUDA(cudaFuncSetAttribute(k_reject_solve<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_TREEBUF));
+    SICP_CUDA(cudaFuncSetAttribute(k_reject_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_TREEBUF));
+    c.rs_attr_set = true;
+  }
   if (multi) {
     void* args[] = {&a, &wk};
     SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_reject_solve<true>, dim3(G), dim3(RS_THREADS),
-                                          args, 0, c.stream));
+                                          args, RS_TREEBUF, c.stream));
   } else {
-    k_reject_solve<false><<<1, RS_THREADS, 0, c.stream>>>(a, wk);
+    k_reject_solve<false><<<1, RS_THREADS, RS_TREEBUF, c.stream>>>(a, wk);
     SICP_CUDA(cudaGetLastError());
   }
   c.tm.kernel_launches += 1;
