@@ -413,6 +413,44 @@ int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const
                             double* H_out /*[h] n_clouds x 16*/,
                             sicp_pair_result* out /*[h] n_edges*/, int64_t* n_selected /*[h] or NULL*/);
 
+/* ---- joint registration with POSE PRIORS (DESIGN.md §6.12) ---------------------------------------
+ * sicp_register_joint_priors is sicp_register_joint with a weighted observation of each cloud's
+ * absolute pose (GNSS/INS, odometry); sicp_register_joint is this call with both NULL.
+ *  - Rule: cloud c's prior is an observed rigid pose P_c = prior_H[c] (world <- cloud) and six
+ *    weights w_c = prior_w[c] = (w_wx, w_wy, w_wz, w_x, w_y, w_z) >= 0 in world axes, 1/rad^2 and
+ *    1/m^2, relative to the unit weight of a point-to-plane row in metres (w = (sigma_row /
+ *    sigma_prior)^2); 0: that component is not observed.  At every iteration, at the current pose
+ *    T_c = (R_c, o_c), the prior observes u_c = (omega_c, do_c), the world rotation increment and
+ *    the displacement of the cloud's origin, with l_c = (rotvec(R_P R_c^T), o_P - o_c); the joint
+ *    minimisation adds sum_c (u_c - l_c)^T diag(w_c) (u_c - l_c).  The pose update, the per-edge
+ *    records and the stop rule (every live edge's, priors take no part) are sicp_register_joint's.
+ *  - Read: the prior of a free cloud some edge references with at least one non-zero weight.  The
+ *    pose of any other prior (fixed, unreferenced, all weights 0) is not read and may be NaN.  A
+ *    call that reads no prior runs exactly as sicp_register_joint: same launches, same bits.
+ *  - Anchoring: a component of the edge graph is anchored by a fixed cloud or by a free cloud whose
+ *    six weights are all > 0, both in the check before any device work (SICP_ERR_BAD_ARG) and over
+ *    the edges that keep their overlap (SICP_ERR_NO_OVERLAP); so no fixed cloud at all is legal when
+ *    priors anchor every component.  Priors on fewer components (e.g. position only) count in the
+ *    system but not as an anchor; a system they leave indefinite is SICP_ERR_SINGULAR.
+ *  - SICP_ERR_BAD_ARG, before any device work, besides sicp_register_joint's checks: exactly one of
+ *    prior_H and prior_w NULL; any weight of prior_w negative or not finite (use is_fixed for an
+ *    exact pose); a read prior pose with a non-finite entry, a bottom row other than (0, 0, 0, 1)
+ *    or a rotation part with |R^T R - I| > 1e-6.
+ *  - sicp_get_joint_covariances after this call: N includes the priors' blocks, and s0^2 =
+ *    (sum_e sum_i r_ei^2 + sum_c v_c^T W_c v_c) / (sum_e n_e + sum_c m_c - 6 F), v_c = u_c - l_c the
+ *    prior's linear-model residual of the final iteration (l_c at the poses that iteration started
+ *    from) and m_c the number of non-zero weights of each read prior.                           */
+int32_t sicp_register_joint_priors(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                                   const int64_t* n /*[h]*/, int32_t n_edges,
+                                   const int32_t* fix_id, const int32_t* mov_id /*[h] n_edges*/,
+                                   const int32_t* is_fixed /*[h] n_clouds, nonzero: pose held*/,
+                                   const double* H0 /*[h] n_clouds x 16 row-major, or NULL: identity*/,
+                                   const double* prior_H /*[h] n_clouds x 16 row-major, or NULL*/,
+                                   const double* prior_w /*[h] n_clouds x 6, or NULL*/,
+                                   const sicp_register_params* p,
+                                   double* H_out /*[h] n_clouds x 16*/,
+                                   sicp_pair_result* out /*[h] n_edges*/, int64_t* n_selected /*[h] or NULL*/);
+
 /* ---- growing the map and reading it back -------------------------------------------------------
  * sicp_map_insert appends to the map, for every voxel of size voxel_size it does not occupy, the
  * first new point that falls into it.  C is the concatenation of the n_clouds clouds in call
@@ -636,7 +674,8 @@ int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
  * sicp_get_joint_covariances returns, for the LAST sicp_register_joint on this context, the
  * covariance of every cloud's pose and of every edge's relative pose, all from its final iteration
  * (the last one whose solve ran; its increments gave the returned poses):
- *  - N is that iteration's joint normal matrix over the edges with >= 6 kept rows, unweighted.
+ *  - N is that iteration's joint normal matrix over the edges with >= 6 kept rows, unweighted
+ *    (after sicp_register_joint_priors also the priors' blocks, and s0 counts their residuals).
  *    s0^2 = sum_e sum_i r_ei^2 / (sum_e n_e - 6 F) over those edges, r_ei the final residuals that
  *    sicp_get_batch_outputs returns and n_e = out[e].n_kept; a denominator <= 0 makes s0 and every
  *    covariance NaN.

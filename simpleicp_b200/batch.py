@@ -326,14 +326,14 @@ class JointResult:
 
 def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
                     full_output: bool = False, covariances: bool = False, solver: str = "dense",
-                    **run_kwargs) -> JointResult:
+                    prior_poses=None, prior_weights=None, **run_kwargs) -> JointResult:
     """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
     (a, b) of `edges` -- scan-to-scan pairs such as (i, i + 1), (i, i + 2) and loop closures -- is
     registered consistently.  Each iteration matches every edge as simpleicp_edges would under the
     linearised rules (median / MAD of all distances, sigma = 1.4826 MAD, point-to-plane rows of the
     C++ driver) and solves ONE least-squares problem for the increments of all free clouds; the
-    clouds listed in `fixed` (indices, at least one) hold their pose.  `H0` (n_clouds, 4, 4) are
-    the start poses (None: identity), world <- cloud.
+    clouds listed in `fixed` (indices, at least one unless pose priors anchor every component) hold
+    their pose.  `H0` (n_clouds, 4, 4) are the start poses (None: identity), world <- cloud.
 
     The run() arguments served are correspondences (<= 4096), neighbors, min_planarity,
     min_change, max_iterations and max_overlap_distance; anything else is a TypeError.  Every free
@@ -354,7 +354,17 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     `solver` picks the solve of the joint system (option joint_solver): "dense" (the default: the
     dense Cholesky of DESIGN.md §6.9, at most 256 free clouds, the only one with covariances) or
     "sparse" (a supernodal Cholesky over a nested-dissection ordering of the edge graph, DESIGN.md
-    §6.11: the same system and rule, up to rounding, for up to 16 384 free clouds)."""
+    §6.11: the same system and rule, up to rounding, for up to 16 384 free clouds).
+
+    `prior_poses` (n_clouds, 4, 4) and `prior_weights` (n_clouds, 6), given together, are weighted
+    observations of each cloud's pose (DESIGN.md §6.12), e.g. GNSS/INS poses: cloud c's rotation
+    and origin are pulled towards prior_poses[c] with the weights (w_wx, w_wy, w_wz, w_x, w_y, w_z)
+    in world axes, 1/rad^2 and 1/m^2 relative to a point-to-plane row in metres, i.e.
+    (sigma_row / sigma_prior)^2; 0 leaves a component unobserved.  Only the priors of free clouds
+    with a non-zero weight are read (any other pose may be NaN); weights must be finite and >= 0
+    and a read pose finite and rigid (to 1e-6).  A free cloud whose six weights are all > 0
+    anchors its component of the edge graph as a fixed cloud does, so with priors `fixed` may be
+    empty.  Both solvers take priors; covariances=True includes them."""
     if not isinstance(covariances, (bool, np.bool_)):
         raise TypeError(f"covariances must be True or False, got {covariances!r}")
     if not isinstance(solver, str) or solver not in _JOINT_SOLVERS:
@@ -368,10 +378,16 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         raise ValueError("simpleicp_joint needs at least one edge")
     if np.any(e[:, 0] == e[:, 1]):
         raise ValueError(f"edges must not be self edges: edge {int(np.flatnonzero(e[:, 0] == e[:, 1])[0])}")
+    priors = prior_poses is not None or prior_weights is not None
+    if priors and (prior_poses is None or prior_weights is None):
+        raise ValueError("prior_poses and prior_weights must be given together")
     fx = np.asarray(fixed)
-    if fx.ndim != 1 or fx.size < 1 or not np.issubdtype(fx.dtype, np.integer):
-        raise ValueError("fixed must be a sequence of at least one integer cloud index")
-    if fx.min() < 0 or fx.max() >= n_clouds:
+    if priors and fx.size == 0:  # priors may anchor every component
+        fx = fx.astype(np.int64).reshape(0)
+    if fx.ndim != 1 or (fx.size < 1 and not priors) or not np.issubdtype(fx.dtype, np.integer):
+        raise ValueError("fixed must be a sequence of at least one integer cloud index"
+                         f"{' (or none, with priors)' if priors else ''}")
+    if fx.size and (fx.min() < 0 or fx.max() >= n_clouds):
         raise ValueError(f"fixed must index the {n_clouds} clouds")
     is_fixed = np.zeros(n_clouds, dtype=bool)
     is_fixed[fx] = True
@@ -384,6 +400,9 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     if not 1 <= int(free.sum()) <= cap:
         raise ValueError(f"the edges must reference between 1 and {cap} free clouds"
                          f"{' under solver=sparse' if solver == 'sparse' else ''}, got {int(free.sum())}")
+    full = np.zeros(n_clouds, dtype=bool)
+    if priors:
+        prior_poses, prior_weights, full = _joint_priors(prior_poses, prior_weights, free)
     up = list(range(n_clouds))
 
     def root(i):
@@ -394,10 +413,11 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
 
     for a, b in e:
         up[root(int(a))] = root(int(b))
-    anchored = {root(i) for i in np.flatnonzero(is_fixed)}
+    anchored = {root(i) for i in np.flatnonzero(is_fixed | full)}
     lost = [i for i in np.flatnonzero(free) if root(int(i)) not in anchored]
     if lost:
-        raise ValueError(f"free cloud {int(lost[0])} has no path to a fixed cloud over the edges")
+        raise ValueError(f"free cloud {int(lost[0])} has no path to a fixed cloud over the edges"
+                         f"{' and no pose prior with six non-zero weights in its component' if priors else ''}")
     for i in np.flatnonzero(used):
         if clouds[i] is None:
             raise ValueError(f"cloud {int(i)} is referenced by an edge but is None")
@@ -412,7 +432,8 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         # every call sets the option: the engine is shared by the calls on this device
         eng.set_option("joint_solver", 1 if solver == "sparse" else 0)
         H, res = eng.register_joint(list(clouds), e, is_fixed, H0, run_kwargs.get("correspondences", 1000),
-                                    run_kwargs.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0)
+                                    run_kwargs.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0,
+                                    prior_poses, prior_weights)
         n = e.shape[0]
         table = np.zeros((n, RECORD_LEN))
         messages: List[str] = []
@@ -428,6 +449,31 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
                       bool(ok) and all(bool(r.converged) for r in ok), results, *cov)
     _raise_failed(table, on_error, messages, results)
     return out
+
+
+def _joint_priors(prior_poses, prior_weights, free: np.ndarray):
+    """simpleicp_joint's pose priors checked: (poses, weights, full) as float64 arrays of shapes
+    (n_clouds, 4, 4) and (n_clouds, 6), and the mask of the free clouds whose six weights are all
+    > 0.  Every weight must be finite and >= 0; the pose of a read prior (a free cloud with a
+    non-zero weight) finite and rigid to 1e-6.  Else ValueError."""
+    n_clouds = free.shape[0]
+    W = np.ascontiguousarray(prior_weights, dtype=np.float64)
+    if W.shape != (n_clouds, 6):
+        raise ValueError(f"prior_weights must have shape ({n_clouds}, 6), got {W.shape}")
+    if not np.isfinite(W).all() or (W < 0).any():
+        raise ValueError("prior_weights must be finite and >= 0 (a cloud whose pose is exact belongs in fixed)")
+    P = np.ascontiguousarray(prior_poses, dtype=np.float64)
+    if P.shape != (n_clouds, 4, 4):
+        raise ValueError(f"prior_poses must have shape ({n_clouds}, 4, 4), got {P.shape}")
+    read = free & (W != 0).any(axis=1)
+    bad = read & ~np.isfinite(P).all(axis=(1, 2))
+    if bad.any():
+        raise ValueError(f"prior_poses[{int(np.flatnonzero(bad)[0])}] has non-finite entries")
+    try:
+        _check_rigid(P[read])
+    except ValueError as ex:
+        raise ValueError(f"prior_poses: {ex}") from None
+    return P, W, read & (W > 0).all(axis=1)
 
 
 def _check_edges(edges, n_clouds: int) -> np.ndarray:

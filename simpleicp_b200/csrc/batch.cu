@@ -430,10 +430,16 @@ struct JointRun {
   std::vector<Rigid> pose;      // per cloud, world <- cloud
   std::vector<Rigid> prior;     // per edge: T_a^-1 T_b
   std::vector<int> free_of, free_ids;
+  // the pose priors the call reads (DESIGN.md §6.12): per cloud, a prior with six non-zero weights
+  // (an anchor like a fixed cloud); the priors in free-cloud order, and per free cloud its prior or -1
+  std::vector<char> full_prior;
+  std::vector<JointPrior> poses;
+  std::vector<int> prior_of;
 };
 
 // Union-find of the clouds over the edges with use[e] != 0; SICP_REQUIRE fails with `code` when a
-// cloud some edge references shares its component with no fixed cloud.
+// cloud some edge references shares its component with no fixed cloud and no free cloud whose pose
+// prior has six non-zero weights.
 static void check_anchored(const JointRun& j, const std::vector<char>& use, int code, const char* msg) {
   std::vector<int> up((size_t)j.n_clouds);
   for (int i = 0; i < j.n_clouds; ++i) up[(size_t)i] = i;
@@ -445,7 +451,7 @@ static void check_anchored(const JointRun& j, const std::vector<char>& use, int 
     if (use[(size_t)e]) up[(size_t)root(j.fix_id[e])] = root(j.mov_id[e]);
   std::vector<char> anchored((size_t)j.n_clouds, 0);
   for (int i = 0; i < j.n_clouds; ++i)
-    if (j.fixed[(size_t)i]) anchored[(size_t)root(i)] = 1;
+    if (j.fixed[(size_t)i] || j.full_prior[(size_t)i]) anchored[(size_t)root(i)] = 1;
   for (int e = 0; e < j.n_edges; ++e)
     for (int k = 0; k < 2; ++k) {
       const int cl = k ? j.mov_id[e] : j.fix_id[e];
@@ -557,9 +563,10 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   std::vector<char> live((size_t)n_edges);
   for (int e = 0; e < n_edges; ++e) live[(size_t)e] = !r.no_overlap[(size_t)e];
   check_anchored(j, live, SICP_ERR_NO_OVERLAP, "a free cloud has no path to a fixed cloud over edges with overlap");
-  // the common centre: the box centre of the first live edge's movable cloud, in the world
+  // the common centre: the box centre of the first live edge's movable cloud, in the world (of the
+  // last edge when none is live: then priors hold every free cloud)
   int e0 = 0;
-  while (!live[(size_t)e0]) ++e0;
+  while (e0 + 1 < n_edges && !live[(size_t)e0]) ++e0;
   double cw[3];
   const double* cm = r.pd[(size_t)e0].cm;
   rigid_apply(j.pose[(size_t)j.mov_id[e0]], cm[0], cm[1], cm[2], cw[0], cw[1], cw[2]);
@@ -601,6 +608,9 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   const size_t o_edge = ids.size();
   for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
   const SparseIds so = sparse ? joint_sparse_ids(j, live, plan, ids) : SparseIds{};
+  const int n_prior = (int)j.poses.size();
+  const size_t o_prior = ids.size();
+  if (n_prior > 0) ids.insert(ids.end(), j.prior_of.begin(), j.prior_of.end());
 
   JointStore& js = b.joint;
   const int npad = (6 * F + 1 + 31) / 32 * 32;
@@ -614,6 +624,12 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     for (int cl : {j.fix_id[e], j.mov_id[e]}) js.role[(size_t)cl] = j.free_of[(size_t)cl] >= 0 ? 2 : 1;
   js.cov_done = false;
   js.sparse = sparse;
+  js.n_prior = n_prior;
+  if (n_prior > 0) {
+    js.prior.reserve(n_prior);
+    SICP_CUDA(cudaMemcpyAsync(js.prior.p, j.poses.data(), sizeof(JointPrior) * (size_t)n_prior,
+                              cudaMemcpyHostToDevice, st));
+  }
   js.edges.reserve(n_edges);
   js.flags.reserve(1);
   js.pose.reserve(j.n_clouds);
@@ -669,6 +685,11 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
   for (int k = 0; k < 3; ++k) a.cw[k] = cw[k];
   a.min_planarity = p.min_planarity;
   a.min_change = p.min_change;
+  if (n_prior > 0) {
+    a.prior = js.prior.p;
+    a.prior_of = js.ids.p + o_prior;
+    a.n_prior = n_prior;
+  }
   JointSparseArgs sa{};
   if (sparse) {
     sa.j = a;
@@ -717,6 +738,7 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     batch_match_launch(c, b, c.warm_start && it > 0);
     SICP_CUDA(cudaEventRecord(e[1], st));
     joint_reject_launch(c, a, n_edges);
+    if (n_prior > 0) joint_prior_launch(c, a, sparse ? sa.dc : nullptr);
     SICP_CUDA(cudaEventRecord(e[2], st));
     if (sparse) {
       sa.j.it = it;
@@ -934,6 +956,8 @@ static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n
     a.n_edges = ne;
     a.npad = js.npad;
     for (int k = 0; k < 3; ++k) a.cw[k] = js.cw[k];
+    a.prior = js.prior.p;
+    a.n_prior = js.n_prior;
     joint_cov_launch(c, a);
     std::vector<double> h(1 + 36 * ((size_t)F + ne));
     SICP_CUDA(cudaMemcpyAsync(h.data(), a.s0sq, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, c.stream));
@@ -1239,12 +1263,51 @@ struct VariantScope {
   ~VariantScope() { c.variant = saved; }
 };
 
+// The pose priors of sicp_register_joint_priors (DESIGN.md §6.12), checked and kept in j: a prior is
+// read for a free cloud with a non-zero weight; its pose must then be finite and rigid (to 1e-6, as
+// sicp_overlap_graph's poses).  Every weight must be finite and >= 0.
+static void check_joint_priors(JointRun& j, const double* prior_H, const double* prior_w) {
+  j.full_prior.assign((size_t)j.n_clouds, 0);
+  SICP_REQUIRE((prior_H == nullptr) == (prior_w == nullptr), SICP_ERR_BAD_ARG,
+               "prior_H and prior_w must both be given or both be NULL");
+  if (!prior_w) return;
+  for (long long k = 0; k < 6ll * j.n_clouds; ++k)
+    SICP_REQUIRE(std::isfinite(prior_w[k]) && prior_w[k] >= 0.0, SICP_ERR_BAD_ARG,
+                 "prior_w[" + std::to_string(k / 6) + "] has a weight that is negative or not finite");
+  j.prior_of.assign((size_t)j.F, -1);
+  for (int f = 0; f < j.F; ++f) {
+    const int i = j.free_ids[(size_t)f];
+    const double* w = prior_w + 6 * (size_t)i;
+    int nz = 0;
+    for (int q = 0; q < 6; ++q) nz += w[q] != 0.0;
+    if (nz == 0) continue;
+    const double* h = prior_H + 16 * (size_t)i;
+    for (int q = 0; q < 16; ++q)
+      SICP_REQUIRE(std::isfinite(h[q]), SICP_ERR_BAD_ARG, "prior_H[" + std::to_string(i) + "] has non-finite entries");
+    SICP_REQUIRE(h[12] == 0.0 && h[13] == 0.0 && h[14] == 0.0 && h[15] == 1.0, SICP_ERR_BAD_ARG,
+                 "prior_H[" + std::to_string(i) + "] does not have the bottom row (0, 0, 0, 1)");
+    for (int p = 0; p < 3; ++p)
+      for (int q = 0; q < 3; ++q) {
+        const double d = h[p] * h[q] + h[4 + p] * h[4 + q] + h[8 + p] * h[8 + q] - (p == q ? 1.0 : 0.0);
+        SICP_REQUIRE(std::fabs(d) <= 1e-6, SICP_ERR_BAD_ARG,
+                     "the rotation part of prior_H[" + std::to_string(i) + "] is not orthonormal (to 1e-6)");
+      }
+    JointPrior pr{};
+    pr.P = rigid_from_H(h);
+    for (int q = 0; q < 6; ++q) pr.w[q] = w[q];
+    pr.f = f;
+    j.prior_of[(size_t)f] = (int)j.poses.size();
+    j.poses.push_back(pr);
+    j.full_prior[(size_t)i] = nz == 6;
+  }
+}
+
 // sicp_register_joint: sicp_register_pairs' stages under the linearised rules, edge e = pair
 // (fix_id[e], mov_id[e]) starting from T_a^-1 T_b, with joint_loop in place of the per-pair loop.
 static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_edges,
                            const int32_t* fix_id, const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
-                           const sicp_register_params* rp, double* H_out, sicp_pair_result* out,
-                           int64_t* n_selected) {
+                           const double* prior_H, const double* prior_w, const sicp_register_params* rp,
+                           double* H_out, sicp_pair_result* out, int64_t* n_selected) {
   if (c.batch) c.batch->out_valid = false;
   VariantScope linearised(c, SICP_VARIANT_LINEARIZED);
   check_pairs_params(c, n_edges, xyz && n && fix_id && mov_id && is_fixed && H_out && out, rp);
@@ -1278,6 +1341,7 @@ static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const
     }
   }
   j.F = (int)j.free_ids.size();
+  check_joint_priors(j, prior_H, prior_w);
   if (c.joint_solver == 1)
     SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_SPARSE_MAX_FREE, SICP_ERR_BAD_ARG,
                  "the edges must reference between 1 and " + std::to_string(JOINT_SPARSE_MAX_FREE) +
@@ -1866,13 +1930,24 @@ extern "C" int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const do
   API_END
 }
 
+extern "C" int32_t sicp_register_joint_priors(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz,
+                                              const int64_t* n, int32_t n_edges, const int32_t* fix_id,
+                                              const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
+                                              const double* prior_H, const double* prior_w,
+                                              const sicp_register_params* p, double* H_out, sicp_pair_result* out,
+                                              int64_t* n_selected) {
+  API_BEGIN(ctx)
+  register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, prior_H, prior_w, p, H_out, out,
+                 n_selected);
+  API_END
+}
+
 extern "C" int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,
                                        int32_t n_edges, const int32_t* fix_id, const int32_t* mov_id,
                                        const int32_t* is_fixed, const double* H0, const sicp_register_params* p,
                                        double* H_out, sicp_pair_result* out, int64_t* n_selected) {
-  API_BEGIN(ctx)
-  register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, p, H_out, out, n_selected);
-  API_END
+  return sicp_register_joint_priors(ctx, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, nullptr, nullptr,
+                                    p, H_out, out, n_selected);
 }
 
 extern "C" int32_t sicp_map_insert(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

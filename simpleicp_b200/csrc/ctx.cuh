@@ -247,6 +247,18 @@ struct JointEdge {
   int part;  // >= 6 kept rows this iteration: the edge enters the joint system
   int pad;
 };
+// A pose prior of free cloud f that the call reads (DESIGN.md §6.12): the observed pose P and the
+// weights w in world axes; per iteration k_joint_prior leaves the observation l = (rotvec(R_P R_c^T),
+// o_P - o_c), the lever d of J_c = [[I, 0], [-[d]x, I]] in the unknowns of the solve in use, and the
+// cloud's block Nw = J^T W J and right-hand side gw = J^T W l; k_joint_solve leaves the cloud's
+// unknowns y (the covariances' residual v = J y - l).
+struct JointPrior {
+  Rigid P;
+  double w[6];
+  double Nw[36], gw[6];
+  double l[6], lev[3], y[6];
+  int f, pad;
+};
 struct JointFlags {
   int done;       // converged, last iteration or singular: every later queued kernel returns
   int converged;
@@ -280,6 +292,11 @@ struct JointArgs {
   unsigned int* bar;       // grid barrier of k_joint_solve, {0, any} between launches
   double cw[3];            // the common world centre of the increments
   double min_planarity, min_change;
+  // the pose priors the call reads (DESIGN.md §6.12), and per free cloud its prior or -1; both null
+  // without priors
+  JointPrior* prior;
+  const int* prior_of;
+  int n_prior;
 };
 // One supernode of the sparse solve's plan (joint_plan.h): its clouds at positions first ..
 // first + ns - 1, its struct st[st_off .. st_off + nt), its updates [u0, u1) and the offset of its
@@ -340,6 +357,8 @@ struct JointCovArgs {
   unsigned int* bar;  // grid barrier of k_joint_inv, {0, any} between launches
   int F, n_edges, npad;
   double cw[3];
+  const JointPrior* prior;  // the pose priors of the call (their v^T W v and count enter s0^2)
+  int n_prior;
 };
 struct JointStore {
   DevBuf<JointEdge> edges;
@@ -348,6 +367,8 @@ struct JointStore {
   DevBuf<int> ids;  // fix_id, mov_id, free_of, free_ids, blk_of, blk_off, blk_edge
   DevBuf<double> A;
   DevBuf<unsigned int> bar;
+  DevBuf<JointPrior> prior;
+  int n_prior = 0;  // the pose priors of the last call
   // the sparse solve (joint_solver 1): its panels, x, xf and dc (15 F), bad + one flag per block
   bool sparse = false;  // the last call used it (no covariances)
   DevBuf<long long> sp_panel;
@@ -370,6 +391,9 @@ struct JointStore {
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges);
 void joint_solve_launch(Ctx& c, const JointArgs& a);
 void joint_sparse_solve_launch(Ctx& c, const JointSparseArgs& a);
+// k_joint_prior: the blocks of a.n_prior pose priors at the current poses, in the unknowns of the
+// dense solve (dc null) or of the sparse solve (dc: its per-free-cloud start origins minus c_w)
+void joint_prior_launch(Ctx& c, const JointArgs& a, const double* dc);
 // k_joint_cov_ss, k_joint_inv, k_joint_cov_cloud, k_joint_cov_edge: the covariances of the last
 // sicp_register_joint into a.cov_f / a.cov_e and s0^2 into a.s0sq (DESIGN.md §6.9)
 void joint_cov_launch(Ctx& c, const JointCovArgs& a);

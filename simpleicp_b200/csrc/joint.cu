@@ -7,6 +7,8 @@
 //                    kept rows a = [w x n, n] with w = R_e (p - c_m) (centred about the edge's movable
 //                    centre c_f = R_e c_m in frame a), and the edge's 6 x 6 block Ad^T N Ad and
 //                    right-hand side -Ad^T h in the common world parameterisation
+//   k_joint_prior    with pose priors only (DESIGN.md §6.12): one thread per prior, its observation
+//                    at the current pose and the cloud's block and right-hand side
 //   k_joint_solve    one cooperative launch: assembly of the dense 6F x 6F normal matrix, augmented
 //                    by the right-hand side as one more row, from the edge blocks in ascending edge
 //                    order; right-looking tiled Cholesky (the augmented row leaves L^-1 b behind);
@@ -336,12 +338,15 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
           const JointEdge& je = a.edges[a.blk_edge[l] >> 1];
           if (je.part) v += (p == qq) ? je.Nw[ri * 6 + cj] : -je.Nw[ri * 6 + cj];
         }
+      if (p == qq && a.prior_of && a.prior_of[p] >= 0) v += a.prior[a.prior_of[p]].Nw[ri * 6 + cj];
     } else if (i == n && j < n) {
       const int p = j / 6, b = a.blk_of[p * a.F + p];
-      for (int l = a.blk_off[b]; l < a.blk_off[b + 1]; ++l) {
-        const JointEdge& je = a.edges[a.blk_edge[l] >> 1];
-        if (je.part) v += (a.blk_edge[l] & 1) ? -je.gw[j % 6] : je.gw[j % 6];
-      }
+      if (b >= 0)  // none: a cloud whose edges all lost their overlap, held by its prior
+        for (int l = a.blk_off[b]; l < a.blk_off[b + 1]; ++l) {
+          const JointEdge& je = a.edges[a.blk_edge[l] >> 1];
+          if (je.part) v += (a.blk_edge[l] & 1) ? -je.gw[j % 6] : je.gw[j % 6];
+        }
+      if (a.prior_of && a.prior_of[p] >= 0) v += a.prior[a.prior_of[p]].gw[j % 6];
     } else if (i == j) {
       v = 1.0;
     }
@@ -447,7 +452,11 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
   }
 
   // ---- poses, then the edges' new relative transforms, records and stop rule
-  for (int f = tid; f < a.F; f += JS_THREADS) joint_pose_update(a, f, sm.xs + 6 * f);
+  for (int f = tid; f < a.F; f += JS_THREADS) {
+    joint_pose_update(a, f, sm.xs + 6 * f);
+    if (a.prior_of && a.prior_of[f] >= 0)
+      for (int q = 0; q < 6; ++q) a.prior[a.prior_of[f]].y[q] = sm.xs[6 * f + q];
+  }
   __syncthreads();
   int conv = a.it > 0 ? 1 : 0;
   for (int e = tid; e < a.n_edges; e += JS_THREADS) JOINT_EDGE_UPDATE(a, e, sm.xs, conv)
@@ -472,7 +481,8 @@ __device__ __forceinline__ void ad_column(const JointEdge& je, const double* d, 
 }
 
 // Supernode k by the whole block: assembly of its panel P (column-major, R = 6 (ns + nt) + 1 rows,
-// C = 6 ns columns, the right-hand side as row R - 1) from the edges in ascending edge order, each
+// C = 6 ns columns, the right-hand side as row R - 1) from the edges in ascending edge order, then
+// each cloud's pose prior on its diagonal block and right-hand side (k_joint_prior), each
 // cloud's unknowns taken about its own origin: Ad_r^T N Ad_c and -Ad_c^T h from the edge's sums in
 // frame a (ad_column), never from Nw / gw, whose kilometre levers about c_w cost precision that a
 // change of variables after the fact cannot recover; the left-looking updates from its descendants
@@ -524,6 +534,16 @@ __device__ void sparse_factor(const JointSparseArgs& s, int k) {
     P[(size_t)c * R + r] = v;
   }
   __syncthreads();
+  if (a.prior_of) {  // each cloud's prior on its diagonal block and right-hand side
+    for (int idx = tid; idx < 42 * ns; idx += JS_THREADS) {
+      const int cj = idx / 42, q = idx % 42, pk = a.prior_of[s.perm[m.first + cj]];
+      if (pk < 0) continue;
+      const JointPrior& pr = a.prior[pk];
+      if (q < 36) P[(size_t)(6 * cj + q % 6) * R + 6 * cj + q / 6] += pr.Nw[q];
+      else P[(size_t)(6 * cj + q - 36) * R + R - 1] += pr.gw[q - 36];
+    }
+    __syncthreads();
+  }
   // P[map(i), map(j)] -= sum_k Ld[i][k] Ld[j][k] over the rows i of descendant d from its first
   // struct entry in s on (and its right-hand side's row), the columns j of those inside s
   for (int u = m.u0; u < m.u1; ++u) {
@@ -830,6 +850,66 @@ __device__ void lever6(const double* Q, const double* d, double* out) {
     }
 }
 
+// ---- k_joint_prior: the pose priors (DESIGN.md §6.12) -------------------------------------------------
+
+// w = rotvec(M) for a rotation M (row-major): the angle in [0, pi] from atan2(|s|, (tr M - 1) / 2),
+// s = vee(M - M^T) / 2 = sin(angle) n; the axis from s while the angle is below 2 pi / 3, else from
+// the symmetric part (M + M^T) / 2 - cos I = (1 - cos) n n^T, turned to the side of s
+__device__ void rotvec(const double* M, double* w) {
+  const double s[3] = {0.5 * (M[7] - M[5]), 0.5 * (M[2] - M[6]), 0.5 * (M[3] - M[1])};
+  const double sn = sqrt(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
+  const double cs = 0.5 * (M[0] + M[4] + M[8] - 1.0);
+  const double th = atan2(sn, cs);
+  if (cs > -0.5) {
+    const double k = sn > 0.0 ? th / sn : 1.0;
+    for (int q = 0; q < 3; ++q) w[q] = k * s[q];
+    return;
+  }
+  int kk = 0;
+  for (int q = 1; q < 3; ++q)
+    if (M[4 * q] > M[4 * kk]) kk = q;
+  const double bkk = M[4 * kk] - cs;
+  double n[3];
+  for (int q = 0; q < 3; ++q) n[q] = (q == kk) ? bkk : 0.5 * (M[3 * q + kk] + M[3 * kk + q]);
+  const double sc = 1.0 / sqrt(bkk * (1.0 - cs));
+  const double sg = (n[0] * s[0] + n[1] * s[1] + n[2] * s[2]) < 0.0 ? -sc : sc;
+  for (int q = 0; q < 3; ++q) w[q] = th * sg * n[q];
+}
+
+// one thread per prior k of free cloud f, at its current pose T_c: l = (rotvec(R_P R_c^T), o_P - o_c),
+// the lever d = o_c - c_w - dc_f of J_c (dc null: the dense solve's unknowns about c_w; else the
+// sparse solve's about each cloud's start origin), Nw = J^T W J and gw = J^T W l
+__global__ void __launch_bounds__(128) k_joint_prior(const JointArgs a, const double* dc) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a.flags->done || k >= a.n_prior) return;
+  JointPrior& pr = a.prior[k];
+  const int f = pr.f;
+  const Rigid T = a.pose[a.free_ids[f]];
+  double M[9], l[6], d[3], Jc[36];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      M[3 * r + c] = pr.P.r[3 * r + 0] * T.r[3 * c + 0] + pr.P.r[3 * r + 1] * T.r[3 * c + 1] +
+                     pr.P.r[3 * r + 2] * T.r[3 * c + 2];
+  rotvec(M, l);
+  for (int q = 0; q < 3; ++q) {
+    l[3 + q] = pr.P.t[q] - T.t[q];
+    d[q] = (T.t[q] - a.cw[q]) - (dc ? dc[3 * f + q] : 0.0);
+  }
+  lever6(nullptr, d, Jc);
+  for (int r = 0; r < 6; ++r) {
+    for (int c = 0; c < 6; ++c) {
+      double v = 0.0;
+      for (int q = 0; q < 6; ++q) v = fma(Jc[6 * q + r] * pr.w[q], Jc[6 * q + c], v);
+      pr.Nw[6 * r + c] = v;
+    }
+    double g = 0.0;
+    for (int q = 0; q < 6; ++q) g = fma(Jc[6 * q + r] * pr.w[q], l[q], g);
+    pr.gw[r] = g;
+    pr.l[r] = l[r];
+  }
+  for (int q = 0; q < 3; ++q) pr.lev[q] = d[q];
+}
+
 // the lower triangle of C mirrored, NaN everywhere when s0^2 is
 __device__ void store_sym6(const double* C, double s0sq, double* out) {
   for (int r = 0; r < 6; ++r)
@@ -855,6 +935,20 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovAr
         ss += a.ss[e];
         m += (double)a.edges[e].n;
       }
+    // the pose priors: v^T W v with v = J y - l, and their non-zero weights (DESIGN.md §6.12)
+    for (int k = lane; k < a.n_prior; k += 32) {
+      const JointPrior& pr = a.prior[k];
+      const double* y = pr.y;
+      const double* d = pr.lev;
+      const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),
+                           y[5] - (d[0] * y[1] - d[1] * y[0])};
+      for (int q = 0; q < 6; ++q)
+        if (pr.w[q] != 0.0) {
+          const double v = u[q] - pr.l[q];
+          ss = fma(pr.w[q] * v, v, ss);
+          m += 1.0;
+        }
+    }
     ss = warp_sum(ss);
     m = warp_sum(m);
     if (lane == 0) {
@@ -919,6 +1013,12 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_edge(const JointCovArg
 
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges) {
   k_joint_reject<<<n_edges, JR_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void joint_prior_launch(Ctx& c, const JointArgs& a, const double* dc) {
+  k_joint_prior<<<(a.n_prior + 127) / 128, 128, 0, c.stream>>>(a, dc);
   SICP_CUDA(cudaGetLastError());
   c.tm.kernel_launches += 1;
 }
