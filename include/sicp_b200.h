@@ -451,6 +451,45 @@ int32_t sicp_register_joint_priors(sicp_ctx* ctx, int32_t n_clouds, const double
                                    double* H_out /*[h] n_clouds x 16*/,
                                    sicp_pair_result* out /*[h] n_edges*/, int64_t* n_selected /*[h] or NULL*/);
 
+/* ---- joint registration with RELATIVE POSE OBSERVATIONS (DESIGN.md §6.13) -----------------------
+ * sicp_register_joint_relative is sicp_register_joint_priors with weighted observations of the
+ * relative pose of two clouds (wheel or visual odometry, the INS trajectory between two scans, an
+ * earlier pairwise result); sicp_register_joint_priors is this call with n_rel = 0.
+ *  - Rule: observation k joins clouds a = rel_a[k] != b = rel_b[k] with an observed rigid transform
+ *    Z_k = rel_H[k] of T_a^-1 T_b (cloud b in frame a) and six weights w_k = rel_w[k] = (w_ax, w_ay,
+ *    w_az, w_x, w_y, w_z) >= 0 in frame-a axes, 1/rad^2 and 1/m^2, relative to the unit weight of a
+ *    point-to-plane row in metres (w = (sigma_row / sigma_odo)^2); 0: that component is not
+ *    observed.  At every iteration, at the current poses, it observes u_k = (alpha, dq), the
+ *    rotation increment of T_a^-1 T_b in frame-a axes and the displacement of o_b in frame a, with
+ *    l_k = (rotvec(R_Z R_ab^T), t_Z - t_ab), R_ab = R_a^T R_b, t_ab = R_a^T (o_b - o_a); the joint
+ *    minimisation adds sum_k (u_k - l_k)^T diag(w_k) (u_k - l_k), linearised as the edge
+ *    covariances' u_e below.  Pose update, per-edge records and stop rule are unchanged.
+ *  - Read: an observation with a non-zero weight and at least one free end.  The Z of any other is
+ *    not read and may be NaN.  A call that reads none runs exactly as sicp_register_joint_priors.
+ *  - Anchoring: a read observation whose six weights are all > 0 joins its two clouds' components
+ *    of the edge graph, in both anchoring checks of sicp_register_joint_priors; weaker ones count in
+ *    the system only.
+ *  - SICP_ERR_BAD_ARG, before any device work, besides sicp_register_joint_priors' checks: n_rel
+ *    outside [0, 65535]; a NULL array with n_rel > 0; a cloud id outside [0, n_clouds), a = b, or a
+ *    cloud that no edge references; a weight negative or not finite; a read Z with a non-finite
+ *    entry, a bottom row other than (0, 0, 0, 1) or |R^T R - I| > 1e-6.
+ *  - sicp_get_joint_covariances after this call: N includes the observations' blocks, and s0^2
+ *    adds sum_k v_k^T W_k v_k to the numerator and sum_k m_k to the denominator (v_k the linear-model
+ *    residual of the final iteration, m_k the non-zero weights of each read observation).        */
+int32_t sicp_register_joint_relative(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
+                                     const int64_t* n /*[h]*/, int32_t n_edges,
+                                     const int32_t* fix_id, const int32_t* mov_id /*[h] n_edges*/,
+                                     const int32_t* is_fixed /*[h] n_clouds, nonzero: pose held*/,
+                                     const double* H0 /*[h] n_clouds x 16 row-major, or NULL: identity*/,
+                                     const double* prior_H /*[h] n_clouds x 16 row-major, or NULL*/,
+                                     const double* prior_w /*[h] n_clouds x 6, or NULL*/,
+                                     int32_t n_rel, const int32_t* rel_a, const int32_t* rel_b /*[h] n_rel*/,
+                                     const double* rel_H /*[h] n_rel x 16 row-major*/,
+                                     const double* rel_w /*[h] n_rel x 6*/,
+                                     const sicp_register_params* p,
+                                     double* H_out /*[h] n_clouds x 16*/,
+                                     sicp_pair_result* out /*[h] n_edges*/, int64_t* n_selected /*[h] or NULL*/);
+
 /* ---- growing the map and reading it back -------------------------------------------------------
  * sicp_map_insert appends to the map, for every voxel of size voxel_size it does not occupy, the
  * first new point that falls into it.  C is the concatenation of the n_clouds clouds in call
@@ -675,7 +714,8 @@ int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
  * covariance of every cloud's pose and of every edge's relative pose, all from its final iteration
  * (the last one whose solve ran; its increments gave the returned poses):
  *  - N is that iteration's joint normal matrix over the edges with >= 6 kept rows, unweighted
- *    (after sicp_register_joint_priors also the priors' blocks, and s0 counts their residuals).
+ *    (after sicp_register_joint_priors also the priors' blocks, and s0 counts their residuals;
+ *    after sicp_register_joint_relative also the relative observations', likewise).
  *    s0^2 = sum_e sum_i r_ei^2 / (sum_e n_e - 6 F) over those edges, r_ei the final residuals that
  *    sicp_get_batch_outputs returns and n_e = out[e].n_kept; a denominator <= 0 makes s0 and every
  *    covariance NaN.

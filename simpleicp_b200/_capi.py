@@ -42,7 +42,7 @@ SYMBOLS = (
     "sicp_uncertainties", "sicp_run", "sicp_get_transform", "sicp_get_residuals", "sicp_iterate", "sicp_transform",
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_register_joint", "sicp_get_batch_outputs",
-    "sicp_register_joint_priors", "sicp_get_joint_covariances",
+    "sicp_register_joint_priors", "sicp_register_joint_relative", "sicp_get_joint_covariances",
     "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_overlap_graph", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times", "sicp_get_match_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
@@ -175,6 +175,10 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
         "sicp_register_joint_priors": [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i32), C.POINTER(i32),
                                        C.POINTER(i32), vp, vp, vp, C.POINTER(RegisterParams), vp,
                                        C.POINTER(PairResult), vp],
+        "sicp_register_joint_relative": [vp, i32, C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i32),
+                                         C.POINTER(i32), C.POINTER(i32), vp, vp, vp, i32, C.POINTER(i32),
+                                         C.POINTER(i32), vp, vp, C.POINTER(RegisterParams), vp,
+                                         C.POINTER(PairResult), vp],
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_get_joint_covariances": [vp, i32, vp, i32, vp, C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
@@ -629,15 +633,18 @@ class Engine:
                              fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p), C.byref(rp), _ptr(observed))
 
     def register_joint(self, clouds, edges, fixed, H0, correspondences, neighbors, params: RunParams,
-                       max_overlap_distance: float = -1.0, prior_H=None, prior_w=None):
-        """sicp_register_joint_priors: one pose per cloud from the edges (n_edges, 2) of (fixed
+                       max_overlap_distance: float = -1.0, prior_H=None, prior_w=None, rel_pairs=None,
+                       rel_H=None, rel_w=None):
+        """sicp_register_joint_relative: one pose per cloud from the edges (n_edges, 2) of (fixed
         side, movable side) indices into `clouds` (NumPy arrays or CUDA tensors, None for a cloud no
         edge uses), `fixed` a boolean mask of the clouds whose pose is held, `H0` (n_clouds, 4, 4)
-        or None (identity) the start poses, world <- cloud, and the pose priors `prior_H`
+        or None (identity) the start poses, world <- cloud, the pose priors `prior_H`
         (n_clouds, 4, 4) and `prior_w` (n_clouds, 6) or None (DESIGN.md §6.12; both None is
-        sicp_register_joint).  Always the linearised rules; the lsq part of `params` is not read
-        beyond its checks.  Returns (H, out): the final poses (n_clouds, 4, 4) and the PairResult
-        array per edge (H = final T_a^-1 T_b), which batch_outputs reads."""
+        sicp_register_joint), and the relative observations `rel_pairs` (n_rel, 2) of clouds (a,
+        b), `rel_H` (n_rel, 4, 4) and `rel_w` (n_rel, 6) or None (DESIGN.md §6.13; None is
+        sicp_register_joint_priors).  Always the linearised rules; the lsq part of `params` is not
+        read beyond its checks.  Returns (H, out): the final poses (n_clouds, 4, 4) and the
+        PairResult array per edge (H = final T_a^-1 T_b), which batch_outputs reads."""
         fix, mov = _ids_arg(edges, "edges")
         keep, ptrs, counts = _clouds_arg(clouds, allow_none=True)
         n, m = len(fix), len(counts)
@@ -645,12 +652,19 @@ class Engine:
         H0 = _shaped_arg(H0, "H0", (m, 4, 4))
         prior_H = _shaped_arg(prior_H, "prior_H", (m, 4, 4))
         prior_w = _shaped_arg(prior_w, "prior_w", (m, 6))
+        ra = rb = np.zeros(0, dtype=np.int32)
+        if rel_pairs is not None:
+            ra, rb = _ids_arg(rel_pairs, "rel_pairs")
+        k = len(ra)
+        rel_H = _shaped_arg(rel_H, "rel_H", (k, 4, 4))
+        rel_w = _shaped_arg(rel_w, "rel_w", (k, 6))
         rp = self._register_params(correspondences, neighbors, params, max_overlap_distance, 0, -1.0)
         H = np.zeros((m, 4, 4))
         i32p = C.POINTER(C.c_int32)
-        out = self._batched(self._lib.sicp_register_joint_priors, params, counts, mov, m, ptrs, counts, n,
+        out = self._batched(self._lib.sicp_register_joint_relative, params, counts, mov, m, ptrs, counts, n,
                             fix.ctypes.data_as(i32p), mov.ctypes.data_as(i32p), is_fixed.ctypes.data_as(i32p),
-                            _ptr(H0), _ptr(prior_H), _ptr(prior_w), C.byref(rp), _ptr(H))
+                            _ptr(H0), _ptr(prior_H), _ptr(prior_w), k, ra.ctypes.data_as(i32p),
+                            rb.ctypes.data_as(i32p), _ptr(rel_H), _ptr(rel_w), C.byref(rp), _ptr(H))
         return H, out
 
     def joint_covariances(self, n_clouds: int, n_edges: int):

@@ -317,16 +317,21 @@ class JointResult:
     (n_edges, 20) record table of simpleicp_edges with H = the final T_a^-1 T_b of each edge;
     iterations and converged of the call; results (full_output) the per-edge result objects; with
     covariances=True cov (n_clouds, 6, 6), edge_cov (n_edges, 6, 6) and s0, the a-posteriori
-    covariances of sicp_get_joint_covariances (else None)."""
+    covariances of sicp_get_joint_covariances (else None); with relative observations
+    relative_misclosure (n_rel, 6), each observation's (rotvec(R_Z R_ab^T), t_Z - t_ab) at the
+    returned poses (else None)."""
 
-    def __init__(self, H, table, iterations, converged, results=None, cov=None, edge_cov=None, s0=None):
+    def __init__(self, H, table, iterations, converged, results=None, cov=None, edge_cov=None, s0=None,
+                 relative_misclosure=None):
         self.H, self.table, self.iterations, self.converged, self.results = H, table, iterations, converged, results
         self.cov, self.edge_cov, self.s0 = cov, edge_cov, s0
+        self.relative_misclosure = relative_misclosure
 
 
 def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
                     full_output: bool = False, covariances: bool = False, solver: str = "dense",
-                    prior_poses=None, prior_weights=None, **run_kwargs) -> JointResult:
+                    prior_poses=None, prior_weights=None, relative_pairs=None, relative_poses=None,
+                    relative_weights=None, **run_kwargs) -> JointResult:
     """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
     (a, b) of `edges` -- scan-to-scan pairs such as (i, i + 1), (i, i + 2) and loop closures -- is
     registered consistently.  Each iteration matches every edge as simpleicp_edges would under the
@@ -364,7 +369,18 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     with a non-zero weight are read (any other pose may be NaN); weights must be finite and >= 0
     and a read pose finite and rigid (to 1e-6).  A free cloud whose six weights are all > 0
     anchors its component of the edge graph as a fixed cloud does, so with priors `fixed` may be
-    empty.  Both solvers take priors; covariances=True includes them."""
+    empty.  Both solvers take priors; covariances=True includes them.
+
+    `relative_pairs` (n_rel, 2), `relative_poses` (n_rel, 4, 4) and `relative_weights` (n_rel, 6),
+    given together, are weighted observations of the relative pose of two clouds (DESIGN.md
+    §6.13), e.g. odometry between consecutive scans: observation k pulls T_a^-1 T_b of its clouds
+    (a, b) towards relative_poses[k] (cloud b in frame a) with the weights (w_ax, w_ay, w_az, w_x,
+    w_y, w_z) in frame-a axes, in the units of the prior weights.  Both clouds must be referenced
+    by an edge.  Only observations with a non-zero weight and a free cloud are read (any other pose
+    may be NaN); weights must be finite and >= 0 and a read pose finite and rigid (to 1e-6).  An
+    observation whose six weights are all > 0 links its two clouds' components of the edge graph,
+    e.g. across a stretch without overlap.  Both solvers take them; covariances=True includes them;
+    the result's relative_misclosure shows how far each is from the returned poses."""
     if not isinstance(covariances, (bool, np.bool_)):
         raise TypeError(f"covariances must be True or False, got {covariances!r}")
     if not isinstance(solver, str) or solver not in _JOINT_SOLVERS:
@@ -381,12 +397,15 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     priors = prior_poses is not None or prior_weights is not None
     if priors and (prior_poses is None or prior_weights is None):
         raise ValueError("prior_poses and prior_weights must be given together")
+    rel = relative_pairs is not None or relative_poses is not None or relative_weights is not None
+    if rel and (relative_pairs is None or relative_poses is None or relative_weights is None):
+        raise ValueError("relative_pairs, relative_poses and relative_weights must be given together")
     fx = np.asarray(fixed)
-    if priors and fx.size == 0:  # priors may anchor every component
+    if (priors or rel) and fx.size == 0:  # priors (linked by observations) may anchor every component
         fx = fx.astype(np.int64).reshape(0)
-    if fx.ndim != 1 or (fx.size < 1 and not priors) or not np.issubdtype(fx.dtype, np.integer):
+    if fx.ndim != 1 or (fx.size < 1 and not (priors or rel)) or not np.issubdtype(fx.dtype, np.integer):
         raise ValueError("fixed must be a sequence of at least one integer cloud index"
-                         f"{' (or none, with priors)' if priors else ''}")
+                         f"{' (or none, with priors)' if priors or rel else ''}")
     if fx.size and (fx.min() < 0 or fx.max() >= n_clouds):
         raise ValueError(f"fixed must index the {n_clouds} clouds")
     is_fixed = np.zeros(n_clouds, dtype=bool)
@@ -403,6 +422,11 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     full = np.zeros(n_clouds, dtype=bool)
     if priors:
         prior_poses, prior_weights, full = _joint_priors(prior_poses, prior_weights, free)
+    links = np.zeros((0, 2), dtype=np.int64)
+    if rel:
+        relative_pairs, relative_poses, relative_weights, link = _joint_relative(
+            relative_pairs, relative_poses, relative_weights, used, free)
+        links = relative_pairs[link]
     up = list(range(n_clouds))
 
     def root(i):
@@ -411,12 +435,13 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
             i = up[i]
         return i
 
-    for a, b in e:
+    for a, b in np.concatenate((e, links)):
         up[root(int(a))] = root(int(b))
     anchored = {root(i) for i in np.flatnonzero(is_fixed | full)}
     lost = [i for i in np.flatnonzero(free) if root(int(i)) not in anchored]
     if lost:
         raise ValueError(f"free cloud {int(lost[0])} has no path to a fixed cloud over the edges"
+                         f"{' and the relative observations with six non-zero weights' if rel else ''}"
                          f"{' and no pose prior with six non-zero weights in its component' if priors else ''}")
     for i in np.flatnonzero(used):
         if clouds[i] is None:
@@ -433,7 +458,8 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         eng.set_option("joint_solver", 1 if solver == "sparse" else 0)
         H, res = eng.register_joint(list(clouds), e, is_fixed, H0, run_kwargs.get("correspondences", 1000),
                                     run_kwargs.get("neighbors", 10), params, mod if np.isfinite(mod) else -1.0,
-                                    prior_poses, prior_weights)
+                                    prior_poses, prior_weights, *((relative_pairs, relative_poses, relative_weights)
+                                                                  if rel and len(relative_pairs) else ()))
         n = e.shape[0]
         table = np.zeros((n, RECORD_LEN))
         messages: List[str] = []
@@ -446,7 +472,8 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         cov = eng.joint_covariances(n_clouds, n) if covariances else (None, None, None)
     ok = [r for r in res if r.status == 0]
     out = JointResult(H, table, max((int(r.iterations) for r in ok), default=0),
-                      bool(ok) and all(bool(r.converged) for r in ok), results, *cov)
+                      bool(ok) and all(bool(r.converged) for r in ok), results, *cov,
+                      relative_misclosure(H, relative_pairs, relative_poses) if rel else None)
     _raise_failed(table, on_error, messages, results)
     return out
 
@@ -474,6 +501,77 @@ def _joint_priors(prior_poses, prior_weights, free: np.ndarray):
     except ValueError as ex:
         raise ValueError(f"prior_poses: {ex}") from None
     return P, W, read & (W > 0).all(axis=1)
+
+
+def _joint_relative(pairs, poses, weights, used: np.ndarray, free: np.ndarray):
+    """simpleicp_joint's relative observations checked: (pairs, poses, weights, link) as an int64
+    (n_rel, 2) array and float64 arrays of shapes (n_rel, 4, 4) and (n_rel, 6), and the mask of the
+    observations whose six weights are all > 0 and that are read.  At most 65 535 observations, each
+    of two different clouds that edges reference; every weight finite and >= 0; the pose of a read
+    observation (a non-zero weight, a free cloud) finite and rigid to 1e-6.  Else ValueError."""
+    n_clouds = free.shape[0]
+    p = np.asarray(pairs)
+    if p.ndim != 2 or p.shape[1] != 2 or not np.issubdtype(p.dtype, np.integer):
+        raise ValueError(f"relative_pairs must be integers of shape (n_rel, 2), got {p.dtype} of shape {p.shape}")
+    p = p.astype(np.int64)
+    n = p.shape[0]
+    if n > 65535:
+        raise ValueError(f"at most 65535 relative observations, got {n}")
+    if n and (p.min() < 0 or p.max() >= n_clouds):
+        raise ValueError(f"relative_pairs must index the {n_clouds} clouds")
+    if np.any(p[:, 0] == p[:, 1]):
+        k = int(np.flatnonzero(p[:, 0] == p[:, 1])[0])
+        raise ValueError(f"relative_pairs must join two clouds: observation {k}")
+    bad = ~(used[p[:, 0]] & used[p[:, 1]])
+    if bad.any():
+        raise ValueError(f"relative observation {int(np.flatnonzero(bad)[0])} joins a cloud that no edge references")
+    W = np.ascontiguousarray(weights, dtype=np.float64)
+    if W.shape != (n, 6):
+        raise ValueError(f"relative_weights must have shape ({n}, 6), got {W.shape}")
+    if not np.isfinite(W).all() or (W < 0).any():
+        raise ValueError("relative_weights must be finite and >= 0")
+    Z = np.ascontiguousarray(poses, dtype=np.float64)
+    if Z.shape != (n, 4, 4):
+        raise ValueError(f"relative_poses must have shape ({n}, 4, 4), got {Z.shape}")
+    read = (W != 0).any(axis=1) & (free[p[:, 0]] | free[p[:, 1]])
+    bad = read & ~np.isfinite(Z).all(axis=(1, 2))
+    if bad.any():
+        raise ValueError(f"relative_poses[{int(np.flatnonzero(bad)[0])}] has non-finite entries")
+    try:
+        _check_rigid(Z[read])
+    except ValueError as ex:
+        raise ValueError(f"relative_poses: {ex}") from None
+    return p, Z, W, read & (W > 0).all(axis=1)
+
+
+def _rotvec(M: np.ndarray) -> np.ndarray:
+    """The rotation vectors (n, 3) of rotations M (n, 3, 3), angles in [0, pi]: the axis from the
+    skew part below 2 pi / 3, else from the symmetric part, as the device's rotvec."""
+    s = 0.5 * np.stack((M[:, 2, 1] - M[:, 1, 2], M[:, 0, 2] - M[:, 2, 0], M[:, 1, 0] - M[:, 0, 1]), axis=1)
+    sn = np.linalg.norm(s, axis=1)
+    cs = 0.5 * (np.trace(M, axis1=1, axis2=2) - 1.0)
+    th = np.arctan2(sn, cs)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        w = s * np.where(sn > 0.0, th / sn, 1.0)[:, None]
+    for i in np.flatnonzero(cs <= -0.5):
+        k = int(np.argmax(np.diagonal(M[i])))
+        n = 0.5 * (M[i][:, k] + M[i][k, :])
+        n[k] = M[i][k, k] - cs[i]
+        n *= np.copysign(1.0, n @ s[i]) / np.sqrt(n[k] * (1.0 - cs[i]))
+        w[i] = th[i] * n
+    return w
+
+
+def relative_misclosure(H, pairs, Z) -> np.ndarray:
+    """(n_rel, 6): each relative observation's (rotvec(R_Z R_ab^T), t_Z - t_ab) at the poses H
+    (n_clouds, 4, 4), R_ab = R_a^T R_b and t_ab = R_a^T (o_b - o_a) (DESIGN.md §6.13)."""
+    H = np.asarray(H, dtype=np.float64)
+    Z = np.asarray(Z, dtype=np.float64).reshape(-1, 4, 4)
+    pairs = np.asarray(pairs, dtype=np.int64).reshape(-1, 2)
+    Ra, Rb = H[pairs[:, 0], :3, :3], H[pairs[:, 1], :3, :3]
+    Rab = np.transpose(Ra, (0, 2, 1)) @ Rb
+    tab = np.einsum("nji,nj->ni", Ra, H[pairs[:, 1], :3, 3] - H[pairs[:, 0], :3, 3])
+    return np.concatenate((_rotvec(Z[:, :3, :3] @ np.transpose(Rab, (0, 2, 1))), Z[:, :3, 3] - tab), axis=1)
 
 
 def _check_edges(edges, n_clouds: int) -> np.ndarray:

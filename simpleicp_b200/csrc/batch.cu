@@ -38,7 +38,9 @@
 #include <cstddef>
 #include <cmath>
 #include <cstring>
+#include <tuple>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "ctx.cuh"
@@ -435,7 +437,42 @@ struct JointRun {
   std::vector<char> full_prior;
   std::vector<JointPrior> poses;
   std::vector<int> prior_of;
+  // the relative observations the call reads (DESIGN.md §6.13), in call order
+  std::vector<JointRel> rels;
 };
+
+// Every read relative observation k, ascending, in the list of each block of the joint matrix it
+// touches: the diagonal blocks of its free ends and, with both ends free, their lower off-diagonal
+// block; block(p, q), p >= q, gives (and creates, as an empty edge list) the block's index.
+template <class Block>
+static std::vector<std::vector<int>> joint_rel_lists(const JointRun& j, Block block) {
+  std::vector<std::vector<int>> rl;
+  auto add = [&](int bi, int k) {
+    if (bi >= (int)rl.size()) rl.resize((size_t)bi + 1);
+    rl[(size_t)bi].push_back(k);
+  };
+  for (int k = 0; k < (int)j.rels.size(); ++k) {
+    const int fa = j.rels[(size_t)k].fa, fb = j.rels[(size_t)k].fb;
+    if (fa >= 0) add(block(fa, fa), k);
+    if (fb >= 0) add(block(fb, fb), k);
+    if (fa >= 0 && fb >= 0) add(block(std::max(fa, fb), std::min(fa, fb)), k);
+  }
+  return rl;
+}
+
+// lists appended to ids as offsets (lists.size() + 1), then entries; returns where each starts
+static std::pair<size_t, size_t> append_lists(std::vector<int>& ids, const std::vector<std::vector<int>>& lists) {
+  const size_t o = ids.size();
+  int at = 0;
+  for (const auto& l : lists) {
+    ids.push_back(at);
+    at += (int)l.size();
+  }
+  ids.push_back(at);
+  const size_t k = ids.size();
+  for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+  return {o, k};
+}
 
 // Union-find of the clouds over the edges with use[e] != 0; SICP_REQUIRE fails with `code` when a
 // cloud some edge references shares its component with no fixed cloud and no free cloud whose pose
@@ -450,6 +487,9 @@ static void check_anchored(const JointRun& j, const std::vector<char>& use, int 
   for (int e = 0; e < j.n_edges; ++e)
     if (use[(size_t)e]) up[(size_t)root(j.fix_id[e])] = root(j.mov_id[e]);
   std::vector<char> anchored((size_t)j.n_clouds, 0);
+  for (const JointRel& o : j.rels)  // an observation with six non-zero weights joins its clouds
+    if (o.w[0] > 0.0 && o.w[1] > 0.0 && o.w[2] > 0.0 && o.w[3] > 0.0 && o.w[4] > 0.0 && o.w[5] > 0.0)
+      up[(size_t)root(o.ca)] = root(o.cb);
   for (int i = 0; i < j.n_clouds; ++i)
     if (j.fixed[(size_t)i] || j.full_prior[(size_t)i]) anchored[(size_t)root(i)] = 1;
   for (int e = 0; e < j.n_edges; ++e)
@@ -459,14 +499,16 @@ static void check_anchored(const JointRun& j, const std::vector<char>& use, int 
     }
 }
 
-// The sparse solve's plan (joint_plan.h) over the free-free pairs of the edges with use[e] != 0;
-// SICP_ERR_BAD_ARG when its panels would exceed JOINT_SPARSE_MAX_BYTES.
+// The sparse solve's plan (joint_plan.h) over the free-free pairs of the edges with use[e] != 0 and
+// of the relative observations; SICP_ERR_BAD_ARG when its panels would exceed JOINT_SPARSE_MAX_BYTES.
 static JointPlan joint_sparse_plan(const JointRun& j, const std::vector<char>& use) {
   std::vector<std::pair<int, int>> pairs;
   for (int e = 0; e < j.n_edges; ++e) {
     const int fa = j.free_of[(size_t)j.fix_id[e]], fb = j.free_of[(size_t)j.mov_id[e]];
     if (use[(size_t)e] && fa >= 0 && fb >= 0) pairs.emplace_back(fa, fb);
   }
+  for (const JointRel& o : j.rels)
+    if (o.fa >= 0 && o.fb >= 0) pairs.emplace_back(o.fa, o.fb);
   JointPlan pl = make_joint_plan(j.F, pairs);
   SICP_REQUIRE(pl.factor_bytes() <= JOINT_SPARSE_MAX_BYTES, SICP_ERR_BAD_ARG,
                "joint_solver 1: the factor of this edge graph needs " + std::to_string(pl.factor_bytes()) +
@@ -476,9 +518,11 @@ static JointPlan joint_sparse_plan(const JointRun& j, const std::vector<char>& u
 
 // What k_joint_sparse_solve reads of the plan, appended to ids (offsets into it in o): the
 // supernodes, structs, updates, maps, levels, the order, and every panel block's list of live edges
-// in ascending order (2 e + (1: the block's cloud is the edge's a) on a diagonal block).
+// in ascending order (2 e + (1: the block's cloud is the edge's a) on a diagonal block); with
+// relative observations also each list's observations (rel: offsets, then entries).
 struct SparseIds {
   size_t sn, st, up, map, lv_off, lv, perm, blk, lst_off, lst_edge;
+  std::pair<size_t, size_t> rel;
 };
 static SparseIds joint_sparse_ids(const JointRun& j, const std::vector<char>& live, const JointPlan& pl,
                                   std::vector<int>& ids) {
@@ -498,6 +542,12 @@ static SparseIds joint_sparse_ids(const JointRun& j, const std::vector<char>& li
     if (fb >= 0) add(fb, fb, 2 * e);
     if (fa >= 0 && fb >= 0) add(fa, fb, 2 * e);
   }
+  std::vector<std::vector<int>> rel = joint_rel_lists(j, [&](int p, int q) {
+    auto it = key_of.emplace((long long)std::min(p, q) * j.F + std::max(p, q), (int)lists.size()).first;
+    if (it->second == (int)lists.size()) lists.emplace_back();
+    return it->second;
+  });
+  rel.resize(lists.size());
   static_assert(sizeof(JointSuper) == 8 * sizeof(int), "JointSuper travels as 8 ints");
   SparseIds o{};
   o.sn = ids.size();
@@ -540,15 +590,8 @@ static SparseIds joint_sparse_ids(const JointRun& j, const std::vector<char>& li
       }
     }
   }
-  o.lst_off = ids.size();
-  int at = 0;
-  for (const auto& l : lists) {
-    ids.push_back(at);
-    at += (int)l.size();
-  }
-  ids.push_back(at);
-  o.lst_edge = ids.size();
-  for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+  std::tie(o.lst_off, o.lst_edge) = append_lists(ids, lists);
+  if (!j.rels.empty()) o.rel = append_lists(ids, rel);
   return o;
 }
 
@@ -592,25 +635,32 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     if (fb >= 0) add(fb, fb, 2 * e);
     if (fa >= 0 && fb >= 0) add(std::max(fa, fb), std::min(fa, fb), 2 * e);
   }
+  // the relative observations' blocks, after the edges' (a block only they touch has no edges)
+  std::vector<std::vector<int>> rel;
+  if (!sparse) {
+    rel = joint_rel_lists(j, [&](int p, int q) {
+      int& bi = blk_of[(size_t)p * F + q];
+      if (bi < 0) {
+        bi = (int)lists.size();
+        lists.emplace_back();
+      }
+      return bi;
+    });
+    rel.resize(lists.size());
+  }
   std::vector<int> ids;
   ids.insert(ids.end(), j.fix_id, j.fix_id + n_edges);
   ids.insert(ids.end(), j.mov_id, j.mov_id + n_edges);
   ids.insert(ids.end(), j.free_of.begin(), j.free_of.end());
   ids.insert(ids.end(), j.free_ids.begin(), j.free_ids.end());
   ids.insert(ids.end(), blk_of.begin(), blk_of.end());
-  const size_t o_off = ids.size();
-  int at = 0;
-  for (const auto& l : lists) {
-    ids.push_back(at);
-    at += (int)l.size();
-  }
-  ids.push_back(at);
-  const size_t o_edge = ids.size();
-  for (const auto& l : lists) ids.insert(ids.end(), l.begin(), l.end());
+  const auto [o_off, o_edge] = append_lists(ids, lists);
   const SparseIds so = sparse ? joint_sparse_ids(j, live, plan, ids) : SparseIds{};
   const int n_prior = (int)j.poses.size();
   const size_t o_prior = ids.size();
   if (n_prior > 0) ids.insert(ids.end(), j.prior_of.begin(), j.prior_of.end());
+  const int n_rel = (int)j.rels.size();
+  const std::pair<size_t, size_t> o_rel = sparse ? so.rel : n_rel > 0 ? append_lists(ids, rel) : so.rel;
 
   JointStore& js = b.joint;
   const int npad = (6 * F + 1 + 31) / 32 * 32;
@@ -629,6 +679,12 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     js.prior.reserve(n_prior);
     SICP_CUDA(cudaMemcpyAsync(js.prior.p, j.poses.data(), sizeof(JointPrior) * (size_t)n_prior,
                               cudaMemcpyHostToDevice, st));
+  }
+  js.n_rel = n_rel;
+  if (n_rel > 0) {
+    js.rel.reserve(n_rel);
+    SICP_CUDA(cudaMemcpyAsync(js.rel.p, j.rels.data(), sizeof(JointRel) * (size_t)n_rel, cudaMemcpyHostToDevice, st));
+    if (!sparse) js.rel_y.reserve(6 * (size_t)F);
   }
   js.edges.reserve(n_edges);
   js.flags.reserve(1);
@@ -690,9 +746,18 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     a.prior_of = js.ids.p + o_prior;
     a.n_prior = n_prior;
   }
+  JointRelArgs ra{};
+  if (n_rel > 0) {
+    ra.rel = js.rel.p;
+    ra.off = js.ids.p + o_rel.first;
+    ra.k = js.ids.p + o_rel.second;
+    ra.y = sparse ? nullptr : js.rel_y.p;
+    ra.n = n_rel;
+  }
   JointSparseArgs sa{};
   if (sparse) {
     sa.j = a;
+    sa.r = ra;
     sa.sn = reinterpret_cast<const JointSuper*>(js.ids.p + so.sn);
     sa.panel = js.sp_panel.p;
     sa.st = js.ids.p + so.st;
@@ -739,13 +804,14 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     SICP_CUDA(cudaEventRecord(e[1], st));
     joint_reject_launch(c, a, n_edges);
     if (n_prior > 0) joint_prior_launch(c, a, sparse ? sa.dc : nullptr);
+    if (n_rel > 0) joint_relative_launch(c, a, ra, sparse ? sa.dc : nullptr);
     SICP_CUDA(cudaEventRecord(e[2], st));
     if (sparse) {
       sa.j.it = it;
       sa.j.last = a.last;
       joint_sparse_solve_launch(c, sa);
     } else {
-      joint_solve_launch(c, a);
+      joint_solve_launch(c, a, ra);
     }
     SICP_CUDA(cudaEventRecord(e[3], st));
     if (it >= next_sync || a.last) {
@@ -958,6 +1024,9 @@ static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n
     for (int k = 0; k < 3; ++k) a.cw[k] = js.cw[k];
     a.prior = js.prior.p;
     a.n_prior = js.n_prior;
+    a.rel = js.rel.p;
+    a.rel_y = js.rel_y.p;
+    a.n_rel = js.n_rel;
     joint_cov_launch(c, a);
     std::vector<double> h(1 + 36 * ((size_t)F + ne));
     SICP_CUDA(cudaMemcpyAsync(h.data(), a.s0sq, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, c.stream));
@@ -1302,12 +1371,64 @@ static void check_joint_priors(JointRun& j, const double* prior_H, const double*
   }
 }
 
+// The relative observations of sicp_register_joint_relative (DESIGN.md §6.13), checked and kept in
+// j: observation k is read when a weight is non-zero and an end is free; its Z must then be finite and
+// rigid (to 1e-6).  Every observation must join two different clouds that some edge references, and
+// every weight must be finite and >= 0.
+static void check_joint_relative(JointRun& j, int n_rel, const int32_t* rel_a, const int32_t* rel_b,
+                                 const double* rel_H, const double* rel_w) {
+  SICP_REQUIRE(n_rel >= 0 && n_rel <= 65535, SICP_ERR_BAD_ARG, "n_rel must be in [0, 65535]");
+  if (n_rel == 0) return;
+  SICP_REQUIRE(rel_a && rel_b && rel_H && rel_w, SICP_ERR_BAD_ARG,
+               "rel_a, rel_b, rel_H and rel_w must not be NULL when n_rel > 0");
+  std::vector<char> used((size_t)j.n_clouds, 0);
+  for (int e = 0; e < j.n_edges; ++e) used[(size_t)j.fix_id[e]] = used[(size_t)j.mov_id[e]] = 1;
+  for (int k = 0; k < n_rel; ++k) {
+    const std::string at = "relative observation " + std::to_string(k);
+    const int a = rel_a[k], b = rel_b[k];
+    SICP_REQUIRE(a >= 0 && a < j.n_clouds && b >= 0 && b < j.n_clouds, SICP_ERR_BAD_ARG,
+                 at + ": cloud ids must be in [0, n_clouds)");
+    SICP_REQUIRE(a != b, SICP_ERR_BAD_ARG, at + " joins a cloud to itself");
+    SICP_REQUIRE(used[(size_t)a] && used[(size_t)b], SICP_ERR_BAD_ARG,
+                 at + ": both clouds must be referenced by an edge");
+    const double* w = rel_w + 6 * (size_t)k;
+    int nz = 0;
+    for (int q = 0; q < 6; ++q) {
+      SICP_REQUIRE(std::isfinite(w[q]) && w[q] >= 0.0, SICP_ERR_BAD_ARG,
+                   at + " has a weight that is negative or not finite");
+      nz += w[q] != 0.0;
+    }
+    if (nz == 0 || (j.fixed[(size_t)a] && j.fixed[(size_t)b])) continue;
+    const double* h = rel_H + 16 * (size_t)k;
+    for (int q = 0; q < 16; ++q)
+      SICP_REQUIRE(std::isfinite(h[q]), SICP_ERR_BAD_ARG, "rel_H[" + std::to_string(k) + "] has non-finite entries");
+    SICP_REQUIRE(h[12] == 0.0 && h[13] == 0.0 && h[14] == 0.0 && h[15] == 1.0, SICP_ERR_BAD_ARG,
+                 "rel_H[" + std::to_string(k) + "] does not have the bottom row (0, 0, 0, 1)");
+    for (int p = 0; p < 3; ++p)
+      for (int q = 0; q < 3; ++q) {
+        const double d = h[p] * h[q] + h[4 + p] * h[4 + q] + h[8 + p] * h[8 + q] - (p == q ? 1.0 : 0.0);
+        SICP_REQUIRE(std::fabs(d) <= 1e-6, SICP_ERR_BAD_ARG,
+                     "the rotation part of rel_H[" + std::to_string(k) + "] is not orthonormal (to 1e-6)");
+      }
+    JointRel o{};
+    o.Z = rigid_from_H(h);
+    for (int q = 0; q < 6; ++q) o.w[q] = w[q];
+    o.ca = a;
+    o.cb = b;
+    o.fa = j.free_of[(size_t)a];
+    o.fb = j.free_of[(size_t)b];
+    j.rels.push_back(o);
+  }
+}
+
 // sicp_register_joint: sicp_register_pairs' stages under the linearised rules, edge e = pair
 // (fix_id[e], mov_id[e]) starting from T_a^-1 T_b, with joint_loop in place of the per-pair loop.
 static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const int64_t* n, int n_edges,
                            const int32_t* fix_id, const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
-                           const double* prior_H, const double* prior_w, const sicp_register_params* rp,
-                           double* H_out, sicp_pair_result* out, int64_t* n_selected) {
+                           const double* prior_H, const double* prior_w, int n_rel, const int32_t* rel_a,
+                           const int32_t* rel_b, const double* rel_H, const double* rel_w,
+                           const sicp_register_params* rp, double* H_out, sicp_pair_result* out,
+                           int64_t* n_selected) {
   if (c.batch) c.batch->out_valid = false;
   VariantScope linearised(c, SICP_VARIANT_LINEARIZED);
   check_pairs_params(c, n_edges, xyz && n && fix_id && mov_id && is_fixed && H_out && out, rp);
@@ -1342,6 +1463,7 @@ static void register_joint(Ctx& c, int n_clouds, const double* const* xyz, const
   }
   j.F = (int)j.free_ids.size();
   check_joint_priors(j, prior_H, prior_w);
+  check_joint_relative(j, n_rel, rel_a, rel_b, rel_H, rel_w);
   if (c.joint_solver == 1)
     SICP_REQUIRE(j.F >= 1 && j.F <= JOINT_SPARSE_MAX_FREE, SICP_ERR_BAD_ARG,
                  "the edges must reference between 1 and " + std::to_string(JOINT_SPARSE_MAX_FREE) +
@@ -1930,16 +2052,27 @@ extern "C" int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const do
   API_END
 }
 
+extern "C" int32_t sicp_register_joint_relative(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz,
+                                                const int64_t* n, int32_t n_edges, const int32_t* fix_id,
+                                                const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
+                                                const double* prior_H, const double* prior_w, int32_t n_rel,
+                                                const int32_t* rel_a, const int32_t* rel_b, const double* rel_H,
+                                                const double* rel_w, const sicp_register_params* p, double* H_out,
+                                                sicp_pair_result* out, int64_t* n_selected) {
+  API_BEGIN(ctx)
+  register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, prior_H, prior_w, n_rel, rel_a, rel_b,
+                 rel_H, rel_w, p, H_out, out, n_selected);
+  API_END
+}
+
 extern "C" int32_t sicp_register_joint_priors(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz,
                                               const int64_t* n, int32_t n_edges, const int32_t* fix_id,
                                               const int32_t* mov_id, const int32_t* is_fixed, const double* H0,
                                               const double* prior_H, const double* prior_w,
                                               const sicp_register_params* p, double* H_out, sicp_pair_result* out,
                                               int64_t* n_selected) {
-  API_BEGIN(ctx)
-  register_joint(c, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, prior_H, prior_w, p, H_out, out,
-                 n_selected);
-  API_END
+  return sicp_register_joint_relative(ctx, n_clouds, xyz, n, n_edges, fix_id, mov_id, is_fixed, H0, prior_H, prior_w, 0,
+                                      nullptr, nullptr, nullptr, nullptr, p, H_out, out, n_selected);
 }
 
 extern "C" int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz, const int64_t* n,

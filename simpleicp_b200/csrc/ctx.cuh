@@ -259,6 +259,31 @@ struct JointPrior {
   double l[6], lev[3], y[6];
   int f, pad;
 };
+// A relative pose observation the call reads (DESIGN.md §6.13): clouds ca and cb (free indices fa,
+// fb; -1 for a fixed end), the observed Z of T_a^-1 T_b and the weights w in frame-a axes.  Per
+// iteration k_joint_relative leaves the observation l = (rotvec(R_Z R_ab^T), t_Z - t_ab) and, with
+// B_c = G_c J_c in the unknowns of the solve in use, the blocks N[0] = B_a^T W B_a, N[1] = B_b^T W B_b,
+// N[2] = -B_b^T W B_a (rows b, columns a) and right-hand sides g[0] = -B_a^T W l, g[1] = B_b^T W l
+// (a fixed end's left unset), and for the covariances' residual v = B_b y_b - B_a y_a - l the levers
+// of J_a and J_b, o_b - o_a and R_a.
+struct JointRel {
+  Rigid Z;
+  double w[6];
+  double N[3][36], g[2][6];
+  double l[6], lev[2][3], dba[3], Ra[9];
+  int ca, cb, fa, fb;
+};
+// The relative observations of a call for the solves (all null / 0 without them): per block of the
+// solve in use (the dense solve's blk_of blocks, the sparse solve's panel lists) its observations
+// k[off[b] ..] in ascending order; y: per free cloud, 6 doubles, the dense solve's unknowns of the
+// iteration (for the covariances)
+struct JointRelArgs {
+  JointRel* rel;
+  const int* off;
+  const int* k;
+  double* y;
+  int n;
+};
 struct JointFlags {
   int done;       // converged, last iteration or singular: every later queued kernel returns
   int converged;
@@ -331,6 +356,7 @@ struct JointSparseArgs {
   double* xf;              // 6 F: the solution in free-cloud order
   int* bad;                // [1] a non-positive or non-finite pivot (0 between calls)
   int* conv;               // per block: its edges met the stop rule
+  JointRelArgs r;          // off / k by the lists of lst_off; y unused
 };
 // sicp_get_joint_covariances (joint.cu: joint_cov_launch), from what the final iteration of the
 // last sicp_register_joint left: the factor L of its joint matrix (upper-left n x n of A), the
@@ -359,6 +385,9 @@ struct JointCovArgs {
   double cw[3];
   const JointPrior* prior;  // the pose priors of the call (their v^T W v and count enter s0^2)
   int n_prior;
+  const JointRel* rel;      // the relative observations of the call and the final unknowns y (the
+  const double* rel_y;      // same for them, DESIGN.md §6.13)
+  int n_rel;
 };
 struct JointStore {
   DevBuf<JointEdge> edges;
@@ -369,6 +398,9 @@ struct JointStore {
   DevBuf<unsigned int> bar;
   DevBuf<JointPrior> prior;
   int n_prior = 0;  // the pose priors of the last call
+  DevBuf<JointRel> rel;
+  DevBuf<double> rel_y;
+  int n_rel = 0;    // the relative observations of the last call
   // the sparse solve (joint_solver 1): its panels, x, xf and dc (15 F), bad + one flag per block
   bool sparse = false;  // the last call used it (no covariances)
   DevBuf<long long> sp_panel;
@@ -389,11 +421,14 @@ struct JointStore {
   }
 };
 void joint_reject_launch(Ctx& c, const JointArgs& a, int n_edges);
-void joint_solve_launch(Ctx& c, const JointArgs& a);
+void joint_solve_launch(Ctx& c, const JointArgs& a, const JointRelArgs& r);
 void joint_sparse_solve_launch(Ctx& c, const JointSparseArgs& a);
 // k_joint_prior: the blocks of a.n_prior pose priors at the current poses, in the unknowns of the
 // dense solve (dc null) or of the sparse solve (dc: its per-free-cloud start origins minus c_w)
 void joint_prior_launch(Ctx& c, const JointArgs& a, const double* dc);
+// k_joint_relative: the blocks of r.n relative observations at the current poses, in the unknowns of
+// the dense solve (dc null) or of the sparse solve
+void joint_relative_launch(Ctx& c, const JointArgs& a, const JointRelArgs& r, const double* dc);
 // k_joint_cov_ss, k_joint_inv, k_joint_cov_cloud, k_joint_cov_edge: the covariances of the last
 // sicp_register_joint into a.cov_f / a.cov_e and s0^2 into a.s0sq (DESIGN.md §6.9)
 void joint_cov_launch(Ctx& c, const JointCovArgs& a);

@@ -9,6 +9,8 @@
 //                    right-hand side -Ad^T h in the common world parameterisation
 //   k_joint_prior    with pose priors only (DESIGN.md §6.12): one thread per prior, its observation
 //                    at the current pose and the cloud's block and right-hand side
+//   k_joint_relative with relative observations only (DESIGN.md §6.13): one thread per observation,
+//                    its value at the current poses and the blocks and right-hand sides of its clouds
 //   k_joint_solve    one cooperative launch: assembly of the dense 6F x 6F normal matrix, augmented
 //                    by the right-hand side as one more row, from the edge blocks in ascending edge
 //                    order; right-looking tiled Cholesky (the augmented row leaves L^-1 b behind);
@@ -317,15 +319,21 @@ __device__ __forceinline__ void joint_edge_finish(const JointArgs& a, int e, int
   st.stop = a.edges[e].part ? (conv ? 1 : 0) : 2;
 }
 
-__global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
+// relative observation o's term of the block of free clouds (fr row, fc column), entry (ri, cj)
+__device__ __forceinline__ double rel_entry(const JointRel& o, int fr, int fc, int ri, int cj) {
+  if (fr == fc) return o.N[fr == o.fa ? 0 : 1][6 * ri + cj];
+  return fr == o.fb ? o.N[2][6 * ri + cj] : o.N[2][6 * cj + ri];
+}
+
+__global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a, const JointRelArgs ro) {
   __shared__ SolveSmem sm;
   const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
   if (a.flags->done) return;  // uniform: only block 0 writes it, at the very end of this launch
   const int n = 6 * a.F, npad = a.npad, KT = npad / TS;
   double* A = a.A;
 
-  // ---- assembly of the lower triangle: edge blocks in ascending edge order, the right-hand side
-  // as row n, identity padding
+  // ---- assembly of the lower triangle: edge blocks in ascending edge order, then the prior, then
+  // the relative observations in ascending order; the right-hand side as row n, identity padding
   for (long long idx = (long long)bid * JS_THREADS + tid; idx < (long long)npad * npad; idx += (long long)G * JS_THREADS) {
     const int i = (int)(idx / npad), j = (int)(idx % npad);
     if (j > i) continue;
@@ -339,6 +347,9 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
           if (je.part) v += (p == qq) ? je.Nw[ri * 6 + cj] : -je.Nw[ri * 6 + cj];
         }
       if (p == qq && a.prior_of && a.prior_of[p] >= 0) v += a.prior[a.prior_of[p]].Nw[ri * 6 + cj];
+      if (ro.off && b >= 0)
+#pragma unroll 1
+        for (int l = ro.off[b]; l < ro.off[b + 1]; ++l) v += rel_entry(ro.rel[ro.k[l]], p, qq, ri, cj);
     } else if (i == n && j < n) {
       const int p = j / 6, b = a.blk_of[p * a.F + p];
       if (b >= 0)  // none: a cloud whose edges all lost their overlap, held by its prior
@@ -347,6 +358,11 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
           if (je.part) v += (a.blk_edge[l] & 1) ? -je.gw[j % 6] : je.gw[j % 6];
         }
       if (a.prior_of && a.prior_of[p] >= 0) v += a.prior[a.prior_of[p]].gw[j % 6];
+      if (ro.off && b >= 0)  // none: a cloud held by its prior alone
+        for (int l = ro.off[b]; l < ro.off[b + 1]; ++l) {
+          const JointRel& o = ro.rel[ro.k[l]];
+          v += o.g[p == o.fa ? 0 : 1][j % 6];
+        }
     } else if (i == j) {
       v = 1.0;
     }
@@ -456,6 +472,8 @@ __global__ void __launch_bounds__(JS_THREADS) k_joint_solve(const JointArgs a) {
     joint_pose_update(a, f, sm.xs + 6 * f);
     if (a.prior_of && a.prior_of[f] >= 0)
       for (int q = 0; q < 6; ++q) a.prior[a.prior_of[f]].y[q] = sm.xs[6 * f + q];
+    if (ro.y)
+      for (int q = 0; q < 6; ++q) ro.y[6 * f + q] = sm.xs[6 * f + q];
   }
   __syncthreads();
   int conv = a.it > 0 ? 1 : 0;
@@ -482,7 +500,8 @@ __device__ __forceinline__ void ad_column(const JointEdge& je, const double* d, 
 
 // Supernode k by the whole block: assembly of its panel P (column-major, R = 6 (ns + nt) + 1 rows,
 // C = 6 ns columns, the right-hand side as row R - 1) from the edges in ascending edge order, then
-// each cloud's pose prior on its diagonal block and right-hand side (k_joint_prior), each
+// each cloud's pose prior on its diagonal block and right-hand side (k_joint_prior), then each
+// block's relative observations in ascending order (k_joint_relative), each
 // cloud's unknowns taken about its own origin: Ad_r^T N Ad_c and -Ad_c^T h from the edge's sums in
 // frame a (ad_column), never from Nw / gw, whose kilometre levers about c_w cost precision that a
 // change of variables after the fact cannot recover; the left-looking updates from its descendants
@@ -541,6 +560,25 @@ __device__ void sparse_factor(const JointSparseArgs& s, int k) {
       const JointPrior& pr = a.prior[pk];
       if (q < 36) P[(size_t)(6 * cj + q % 6) * R + 6 * cj + q / 6] += pr.Nw[q];
       else P[(size_t)(6 * cj + q - 36) * R + R - 1] += pr.gw[q - 36];
+    }
+    __syncthreads();
+  }
+  if (s.r.off) {  // each block's relative observations in ascending order (rel_entry)
+    for (int idx = tid; idx < (ns + m.nt) * C * 6 + C; idx += JS_THREADS) {
+      const int bq = idx / 36, e = idx % 36, rhs = bq >= (ns + m.nt) * ns;
+      const int ri = rhs ? (idx - 36 * (ns + m.nt) * ns) / 6 : bq / ns, cj = rhs ? ri : bq % ns;
+      const int l = s.blk[m.table + ri * ns + cj];
+      if (l < 0) continue;
+      const int fc = s.perm[m.first + cj], r6 = rhs ? 0 : e / 6, c6 = rhs ? idx % 6 : e % 6;
+      const int fr = s.perm[ri < ns ? m.first + ri : s.st[m.st_off + ri - ns]];
+      double& x = P[(size_t)(6 * cj + c6) * R + (rhs ? R - 1 : 6 * ri + r6)];
+      double v = x;
+#pragma unroll 1
+      for (int q = s.r.off[l]; q < s.r.off[l + 1]; ++q) {
+        const JointRel& o = s.r.rel[s.r.k[q]];
+        v += rhs ? o.g[fc == o.fa ? 0 : 1][c6] : rel_entry(o, fr, fc, r6, c6);
+      }
+      x = v;
     }
     __syncthreads();
   }
@@ -910,6 +948,70 @@ __global__ void __launch_bounds__(128) k_joint_prior(const JointArgs a, const do
   for (int q = 0; q < 3; ++q) pr.lev[q] = d[q];
 }
 
+// ---- k_joint_relative: the relative observations (DESIGN.md §6.13) ---------------------------------
+
+// one thread per observation k of clouds a, b at their current poses: l = (rotvec(R_Z R_ab^T),
+// t_Z - t_ab) with R_ab = R_a^T R_b, t_ab = R_a^T (o_b - o_a); per free end c the lever d_c of J_c
+// (k_joint_prior's), B_c = G_c J_c with G_b = diag(R_a^T, R_a^T) and G_a = lever6(R_a, o_b - o_a);
+// then the blocks B_c^T W B_c, -B_b^T W B_a and the right-hand sides -B_a^T W l, B_b^T W l
+__global__ void __launch_bounds__(128) k_joint_relative(const JointArgs a, const JointRelArgs ro, const double* dc) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a.flags->done || k >= ro.n) return;
+  JointRel& o = ro.rel[k];
+  const Rigid Ta = a.pose[o.ca], Tb = a.pose[o.cb];
+  double Rab[9], M[9], l[6], dba[3];
+  for (int q = 0; q < 3; ++q) dba[q] = Tb.t[q] - Ta.t[q];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      Rab[3 * r + c] = Ta.r[r] * Tb.r[c] + Ta.r[3 + r] * Tb.r[3 + c] + Ta.r[6 + r] * Tb.r[6 + c];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      M[3 * r + c] = o.Z.r[3 * r + 0] * Rab[3 * c + 0] + o.Z.r[3 * r + 1] * Rab[3 * c + 1] +
+                     o.Z.r[3 * r + 2] * Rab[3 * c + 2];
+  rotvec(M, l);
+  for (int q = 0; q < 3; ++q) l[3 + q] = o.Z.t[q] - (Ta.r[q] * dba[0] + Ta.r[3 + q] * dba[1] + Ta.r[6 + q] * dba[2]);
+  double B[2][36];
+  for (int e = 0; e < 2; ++e) {
+    const int f = e ? o.fb : o.fa;
+    const Rigid& T = e ? Tb : Ta;
+    double d[3], Jc[36], G[36];
+    for (int q = 0; q < 3; ++q) {
+      d[q] = (T.t[q] - a.cw[q]) - (dc && f >= 0 ? dc[3 * f + q] : 0.0);
+      o.lev[e][q] = d[q];
+    }
+    if (f < 0) continue;
+    const double zero[3] = {0.0, 0.0, 0.0};
+    lever6(nullptr, d, Jc);
+    lever6(Ta.r, e ? zero : dba, G);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) {
+        double v = 0.0;
+        for (int m = 0; m < 6; ++m) v = fma(G[6 * r + m], Jc[6 * m + c], v);
+        B[e][6 * r + c] = v;
+      }
+    for (int r = 0; r < 6; ++r) {
+      for (int c = 0; c < 6; ++c) {
+        double v = 0.0;
+        for (int q = 0; q < 6; ++q) v = fma(B[e][6 * q + r] * o.w[q], B[e][6 * q + c], v);
+        o.N[e][6 * r + c] = v;
+      }
+      double g = 0.0;
+      for (int q = 0; q < 6; ++q) g = fma(B[e][6 * q + r] * o.w[q], l[q], g);
+      o.g[e][r] = e ? g : -g;
+    }
+  }
+  if (o.fa >= 0 && o.fb >= 0)
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) {
+        double v = 0.0;
+        for (int q = 0; q < 6; ++q) v = fma(B[1][6 * q + r] * o.w[q], B[0][6 * q + c], v);
+        o.N[2][6 * r + c] = -v;
+      }
+  for (int q = 0; q < 6; ++q) o.l[q] = l[q];
+  for (int q = 0; q < 3; ++q) o.dba[q] = dba[q];
+  for (int q = 0; q < 9; ++q) o.Ra[q] = Ta.r[q];
+}
+
 // the lower triangle of C mirrored, NaN everywhere when s0^2 is
 __device__ void store_sym6(const double* C, double s0sq, double* out) {
   for (int r = 0; r < 6; ++r)
@@ -946,6 +1048,31 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovAr
         if (pr.w[q] != 0.0) {
           const double v = u[q] - pr.l[q];
           ss = fma(pr.w[q] * v, v, ss);
+          m += 1.0;
+        }
+    }
+    // the relative observations: v = G_b J_b y_b - G_a J_a y_a - l, after the priors (DESIGN.md §6.13)
+    for (int k = lane; k < a.n_rel; k += 32) {
+      const JointRel& o = a.rel[k];
+      double pu[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // R_a u
+      for (int e = 1; e >= 0; --e) {
+        const int f = e ? o.fb : o.fa;
+        if (f < 0) continue;
+        const double* y = a.rel_y + 6 * f;
+        const double* d = o.lev[e];
+        const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),
+                             y[5] - (d[0] * y[1] - d[1] * y[0])};
+        const double* b = o.dba;
+        for (int q = 0; q < 3; ++q) {
+          pu[q] += e ? u[q] : -u[q];
+          pu[3 + q] += e ? u[3 + q] : -(u[3 + q] - (b[(q + 1) % 3] * u[(q + 2) % 3] - b[(q + 2) % 3] * u[(q + 1) % 3]));
+        }
+      }
+      for (int q = 0; q < 6; ++q)
+        if (o.w[q] != 0.0) {
+          const int h = q < 3 ? 0 : 3, r = q - h;
+          const double v = (o.Ra[r] * pu[h] + o.Ra[3 + r] * pu[h + 1] + o.Ra[6 + r] * pu[h + 2]) - o.l[q];
+          ss = fma(o.w[q] * v, v, ss);
           m += 1.0;
         }
     }
@@ -1023,9 +1150,16 @@ void joint_prior_launch(Ctx& c, const JointArgs& a, const double* dc) {
   c.tm.kernel_launches += 1;
 }
 
-void joint_solve_launch(Ctx& c, const JointArgs& a) {
+void joint_relative_launch(Ctx& c, const JointArgs& a, const JointRelArgs& r, const double* dc) {
+  k_joint_relative<<<(r.n + 127) / 128, 128, 0, c.stream>>>(a, r, dc);
+  SICP_CUDA(cudaGetLastError());
+  c.tm.kernel_launches += 1;
+}
+
+void joint_solve_launch(Ctx& c, const JointArgs& a, const JointRelArgs& r) {
   JointArgs args = a;
-  void* p[] = {&args};
+  JointRelArgs rel = r;
+  void* p[] = {&args, &rel};
   SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_solve, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
   c.tm.kernel_launches += 1;
 }
