@@ -403,7 +403,8 @@ int32_t sicp_register_pairs(sicp_ctx* ctx, int32_t n_clouds, const double* const
  *    the edge graph (DESIGN.md §6.11): at most 16 384 free clouds (more is SICP_ERR_BAD_ARG), and a
  *    factor of at most 4 GiB, computed from the edges before any upload (more is SICP_ERR_BAD_ARG,
  *    with the bytes in the message).  After a call under 1, sicp_get_joint_covariances returns
- *    SICP_ERR_STATE; sicp_get_batch_outputs works as after 0.                                   */
+ *    SICP_ERR_STATE (sicp_get_joint_selected_covariances serves both solvers);
+ *    sicp_get_batch_outputs works as after 0.                                                   */
 int32_t sicp_register_joint(sicp_ctx* ctx, int32_t n_clouds, const double* const* xyz /*[h|d]*/,
                             const int64_t* n /*[h]*/, int32_t n_edges,
                             const int32_t* fix_id, const int32_t* mov_id /*[h] n_edges*/,
@@ -740,6 +741,33 @@ int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs,
 int32_t sicp_get_joint_covariances(sicp_ctx* ctx, int32_t n_clouds,
                                    double* cloud_cov /*[h] n_clouds x 36, or NULL*/, int32_t n_edges,
                                    double* edge_cov /*[h] n_edges x 36, or NULL*/, double* s0 /*[h] or NULL*/);
+
+/* ---- the same covariances under either solver (DESIGN.md §6.14) --------------------------------
+ * sicp_get_joint_selected_covariances takes sicp_get_joint_covariances' arguments and returns its
+ * outputs under its rule (priors and relative observations included), after a call under either
+ * option "joint_solver":
+ *  - After a call under 0 it is sicp_get_joint_covariances: the same launches, the same cache and
+ *    the same bits, whichever of the two is asked first.
+ *  - After a call under 1 it computes the blocks from the sparse solve's factor L of the final
+ *    iteration's matrix N' in that solve's unknowns y'_c = (omega_c, u_c), each cloud's increment
+ *    about its start origin o_c^0: Z = N'^-1 by Takahashi's recurrence (selected inversion) on the
+ *    pattern of L, supernode by supernode from the roots down.  C_c = s0^2 J'_c Z_cc J'_c^T with
+ *    J'_c = [[I, 0], [-[o_c - o_c^0]x, I]], equal to the dense J_c (N^-1)_cc J_c^T since y = K y'.
+ *    The pattern holds every free cloud's diagonal block and the cross block of every two free
+ *    clouds joined by an edge with overlap or a read relative observation.  An edge of two free
+ *    clouds that the overlap filter parked before the first iteration may fall outside it: its
+ *    cross block is w_a^T w_b, w_c = L^-1 E_c (non-zero only on the elimination-tree path from c's
+ *    supernode to its root), exactly 0 for clouds in different components.  Equal to the dense
+ *    request up to rounding.
+ *  - Device memory after a call under 1: Z and y' together take the factor's bytes (the message of
+ *    sicp_register_joint's factor check), allocated on the first request; SICP_ERR_CUDA if that
+ *    fails.  SICP_ERR_BAD_ARG (before any launch) for an elimination tree more than 64 levels deep.
+ *  - SICP_ERR_STATE and SICP_ERR_BAD_ARG as sicp_get_joint_covariances, without its solver check.
+ *    sicp_get_joint_covariances keeps refusing after a call under 1, also after this request. */
+int32_t sicp_get_joint_selected_covariances(sicp_ctx* ctx, int32_t n_clouds,
+                                            double* cloud_cov /*[h] n_clouds x 36, or NULL*/, int32_t n_edges,
+                                            double* edge_cov /*[h] n_edges x 36, or NULL*/,
+                                            double* s0 /*[h] or NULL*/);
 
 /* ---- PointCloud.transform_by_H (pointcloud.py:205-217), final application simpleicp.py:316 -- */
 int32_t sicp_transform(sicp_ctx* ctx, const double H[16], double* mov_xyz_out /*[h|d] n_mov x 3*/);

@@ -43,6 +43,7 @@ SYMBOLS = (
     "sicp_select_n_points", "sicp_register",
     "sicp_register_batch", "sicp_set_map", "sicp_register_to_map", "sicp_register_pairs", "sicp_register_joint", "sicp_get_batch_outputs",
     "sicp_register_joint_priors", "sicp_register_joint_relative", "sicp_get_joint_covariances",
+    "sicp_get_joint_selected_covariances",
     "sicp_map_insert", "sicp_get_map", "sicp_map_crop", "sicp_map_thin", "sicp_map_carve", "sicp_map_distances", "sicp_overlap_graph", "sicp_get_timings", "sicp_time_stages", "sicp_get_phase_times", "sicp_get_match_phase_times",
     "sicp_debug_seed_predictor", "sicp_debug_match_counts", "sicp_debug_grid_params",
     "sicp_xyz_load", "sicp_xyz_free", "sicp_xyz_save", "sicp_io_last_error",
@@ -181,6 +182,7 @@ def load_library(build_if_missing: bool = True) -> C.CDLL:
                                          C.POINTER(PairResult), vp],
         "sicp_get_batch_outputs": [vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(IterRecord), C.POINTER(dbl)],
         "sicp_get_joint_covariances": [vp, i32, vp, i32, vp, C.POINTER(dbl)],
+        "sicp_get_joint_selected_covariances": [vp, i32, vp, i32, vp, C.POINTER(dbl)],
         "sicp_map_insert": [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, dbl, vp],
         "sicp_get_map": [vp, vp, i64, C.POINTER(i64)],
         "sicp_map_crop": [vp, i32, vp, dbl, C.POINTER(i64)],
@@ -671,11 +673,19 @@ class Engine:
         """sicp_get_joint_covariances for the last register_joint: (cov, edge_cov, s0) with cov
         (n_clouds, 6, 6) the covariance of each cloud's (omega, d origin), edge_cov (n_edges, 6, 6)
         that of each edge's (alpha, d q) in frame a, and s0 (DESIGN.md §6.9)."""
+        return self._joint_cov(self._lib.sicp_get_joint_covariances, n_clouds, n_edges)
+
+    def joint_selected_covariances(self, n_clouds: int, n_edges: int):
+        """sicp_get_joint_selected_covariances: joint_covariances' outputs after a register_joint
+        under either joint_solver; after a sparse call by selected inversion of its factor
+        (DESIGN.md §6.14)."""
+        return self._joint_cov(self._lib.sicp_get_joint_selected_covariances, n_clouds, n_edges)
+
+    def _joint_cov(self, fn, n_clouds: int, n_edges: int):
         cov = np.empty((int(n_clouds), 6, 6))
         edge_cov = np.empty((int(n_edges), 6, 6))
         s0 = C.c_double(0.0)
-        self._check(self._lib.sicp_get_joint_covariances(self._h, int(n_clouds), _ptr(cov), int(n_edges),
-                                                         _ptr(edge_cov), C.byref(s0)))
+        self._check(fn(self._h, int(n_clouds), _ptr(cov), int(n_edges), _ptr(edge_cov), C.byref(s0)))
         return cov, edge_cov, s0.value
 
     def _batched(self, fn, params: RunParams, counts, mov, *args):

@@ -316,8 +316,8 @@ class JointResult:
     """simpleicp_joint's return value: H (n_clouds, 4, 4) final poses, world <- cloud; table the
     (n_edges, 20) record table of simpleicp_edges with H = the final T_a^-1 T_b of each edge;
     iterations and converged of the call; results (full_output) the per-edge result objects; with
-    covariances=True cov (n_clouds, 6, 6), edge_cov (n_edges, 6, 6) and s0, the a-posteriori
-    covariances of sicp_get_joint_covariances (else None); with relative observations
+    covariances=True or "selected" cov (n_clouds, 6, 6), edge_cov (n_edges, 6, 6) and s0, the
+    a-posteriori covariances of sicp_get_joint_covariances (else None); with relative observations
     relative_misclosure (n_rel, 6), each observation's (rotvec(R_Z R_ab^T), t_Z - t_ab) at the
     returned poses (else None)."""
 
@@ -329,7 +329,7 @@ class JointResult:
 
 
 def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int = 0, on_error: str = "raise",
-                    full_output: bool = False, covariances: bool = False, solver: str = "dense",
+                    full_output: bool = False, covariances=False, solver: str = "dense",
                     prior_poses=None, prior_weights=None, relative_pairs=None, relative_poses=None,
                     relative_weights=None, **run_kwargs) -> JointResult:
     """Register many clouds jointly (multi-scan ICP): one pose per cloud such that every edge
@@ -354,10 +354,13 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     (sicp_get_joint_covariances, DESIGN.md §6.9): cov[c] of cloud c's (rotation increment, origin
     displacement) in the world frame, zeros for a fixed cloud and NaN for a cloud no edge
     references; edge_cov[e] of edge (a, b)'s (rotation increment, displacement of b's origin) in
-    frame a; s0 the a-posteriori standard deviation of unit weight.
+    frame a; s0 the a-posteriori standard deviation of unit weight.  `covariances="selected"`
+    returns the same under either solver (sicp_get_joint_selected_covariances, DESIGN.md §6.14):
+    under "dense" the bits of True, under "sparse" the blocks by selected inversion of the sparse
+    solve's factor.  True under "sparse" is a ValueError.
 
     `solver` picks the solve of the joint system (option joint_solver): "dense" (the default: the
-    dense Cholesky of DESIGN.md §6.9, at most 256 free clouds, the only one with covariances) or
+    dense Cholesky of DESIGN.md §6.9, at most 256 free clouds, the only one with covariances=True) or
     "sparse" (a supernodal Cholesky over a nested-dissection ordering of the edge graph, DESIGN.md
     §6.11: the same system and rule, up to rounding, for up to 16 384 free clouds).
 
@@ -381,12 +384,14 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
     observation whose six weights are all > 0 links its two clouds' components of the edge graph,
     e.g. across a stretch without overlap.  Both solvers take them; covariances=True includes them;
     the result's relative_misclosure shows how far each is from the returned poses."""
-    if not isinstance(covariances, (bool, np.bool_)):
-        raise TypeError(f"covariances must be True or False, got {covariances!r}")
+    selected = isinstance(covariances, str) and covariances == "selected"
+    if not selected and not isinstance(covariances, (bool, np.bool_)):
+        raise TypeError(f"covariances must be True, False or 'selected', got {covariances!r}")
     if not isinstance(solver, str) or solver not in _JOINT_SOLVERS:
         raise ValueError(f"solver must be 'dense' or 'sparse', got {solver!r}")
-    if covariances and solver == "sparse":
-        raise ValueError("covariances=True needs solver='dense': the sparse solve has no covariances")
+    if not selected and covariances and solver == "sparse":
+        raise ValueError("covariances=True needs solver='dense': the sparse solve has no covariances; "
+                         "covariances='selected' serves both solvers")
     _check_run_keys(run_kwargs, _JOINT_KEYS, "simpleicp_joint", "edge")
     n_clouds = len(clouds)
     e = _check_edges(edges, n_clouds)
@@ -469,7 +474,10 @@ def simpleicp_joint(clouds: Sequence, edges, *, fixed=(0,), H0=None, device: int
         if full_output:
             results = [None if o is None else _batch_result(r, o, np.zeros(6), (0.0,) * 6)
                        for r, o in zip(res, eng.batch_outputs(res))]
-        cov = eng.joint_covariances(n_clouds, n) if covariances else (None, None, None)
+        if selected:
+            cov = eng.joint_selected_covariances(n_clouds, n)
+        else:
+            cov = eng.joint_covariances(n_clouds, n) if covariances else (None, None, None)
     ok = [r for r in res if r.status == 0]
     out = JointResult(H, table, max((int(r.iterations) for r in ok), default=0),
                       bool(ok) and all(bool(r.converged) for r in ok), results, *cov,

@@ -776,6 +776,8 @@ static void joint_loop(Ctx& c, Batch& b, PairsRun& r) {
     sa.dc = js.sp_x.p + 12 * (size_t)F;
     sa.bad = js.sp_flags.p;
     sa.conv = js.sp_flags.p + 1;
+    js.sp_args = sa;
+    js.sp_plan = std::move(plan);
   }
 
   // device events around the three stages of the iterations queued since the last host read (match,
@@ -981,22 +983,79 @@ static void run_pairs(Ctx& c, Batch& b, PairsRun& r, const double* fix_xyz, MapS
   b.out_joint = r.joint != nullptr;
 }
 
-// sicp_get_joint_covariances: the first request after a sicp_register_joint runs joint_cov_launch
-// on what its final iteration left and keeps the result on the host; every later one copies it.
+// The selected inversion's device inputs after a sparse call (DESIGN.md §6.14), checked before any
+// launch: pos and the parked edges (both clouds free, their pair outside the pattern of L) into
+// js.sel_ids, Z and y' into js.Z (the factor's size), the blocks of k_joint_sel_parked in *blocks.
+static JointSelArgs joint_sel_args(Ctx& c, JointStore& js, int* blocks) {
+  const JointPlan& pl = js.sp_plan;
+  const int F = js.F;
+  SICP_REQUIRE(pl.depth <= JOINT_SEL_MAX_PATH, SICP_ERR_BAD_ARG,
+               "selected covariances: the elimination tree of this edge graph is " + std::to_string(pl.depth) +
+                   " levels deep, more than " + std::to_string(JOINT_SEL_MAX_PATH));
+  auto owner = [&](int p) { return (int)(std::upper_bound(pl.first.begin(), pl.first.end(), p) - pl.first.begin()) - 1; };
+  auto path_len = [&](int p) {  // the unknowns of the supernodes from p's to its root
+    long long n = 0;
+    for (int k = owner(p); k >= 0; k = pl.parent[(size_t)k]) n += 6 * pl.ns(k);
+    return n;
+  };
+  // the edges' clouds and the free index of every cloud, from the head of the call's ids
+  std::vector<int> h_ids(2 * (size_t)js.n_edges + js.n_clouds);
+  SICP_CUDA(cudaMemcpy(h_ids.data(), js.ids.p, sizeof(int) * h_ids.size(), cudaMemcpyDeviceToHost));
+  const int *fix_id = h_ids.data(), *mov_id = fix_id + js.n_edges, *free_of = mov_id + js.n_edges;
+  std::vector<int> ids(pl.pos.begin(), pl.pos.end());
+  long long need = 0;
+  for (int e = 0; e < js.n_edges; ++e) {
+    const int fa = free_of[fix_id[e]], fb = free_of[mov_id[e]];
+    if (fa < 0 || fb < 0) continue;
+    const int pa = pl.pos[(size_t)fa], pb = pl.pos[(size_t)fb], lo = std::min(pa, pb), hi = std::max(pa, pb);
+    const int k = owner(lo);
+    if (hi < pl.first[(size_t)k + 1] ||
+        std::binary_search(pl.st.begin() + pl.st_off[(size_t)k], pl.st.begin() + pl.st_off[(size_t)k + 1], hi))
+      continue;
+    ids.push_back(e);
+    need = std::max(need, 6 * (path_len(pa) + path_len(pb)));
+  }
+  const int n_parked = (int)ids.size() - F;
+  const long long zsize = pl.panel.back() - 6ll * F;
+  *blocks = n_parked > 0 ? (int)std::min<long long>({(long long)n_parked, (long long)c.num_sms, zsize / need}) : 0;
+  SICP_REQUIRE(n_parked == 0 || *blocks > 0, SICP_ERR_BAD_ARG,
+               "selected covariances: an edge outside the factor's pattern needs more scratch than the factor holds");
+  js.Z.reserve((size_t)pl.panel.back());
+  js.sel_ids.reserve(ids.size());
+  SICP_CUDA(cudaMemcpyAsync(js.sel_ids.p, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, c.stream));
+  JointSelArgs g{};
+  g.s = js.sp_args;
+  g.Z = js.Z.p;
+  g.y = js.Z.p + zsize;
+  g.pos = js.sel_ids.p;
+  g.parked = js.sel_ids.p + F;
+  g.n_parked = n_parked;
+  g.scratch = need;
+  return g;
+}
+
+// sicp_get_joint_covariances (selected false) and sicp_get_joint_selected_covariances (true): the
+// first request after a sicp_register_joint runs joint_cov_launch (a dense call) or joint_sel_launch
+// (a sparse one) on what its final iteration left and keeps the result on the host; every later one
+// copies it.
 static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n_edges, double* edge_cov,
-                                  double* s0) {
+                                  double* s0, bool selected) {
   SICP_REQUIRE(c.batch && c.batch->out_valid && c.batch->out_joint, SICP_ERR_STATE,
                "no joint covariances: the last batched call on this context was not a successful "
                "sicp_register_joint, or a later call cleared its outputs");
   Batch& b = *c.batch;
   JointStore& js = b.joint;
-  SICP_REQUIRE(!js.sparse, SICP_ERR_STATE, "covariances need joint_solver 0");
+  SICP_REQUIRE(selected || !js.sparse, SICP_ERR_STATE,
+               "covariances need joint_solver 0 (sicp_get_joint_selected_covariances serves both solvers)");
   SICP_REQUIRE(n_clouds == js.n_clouds && n_edges == js.n_edges, SICP_ERR_BAD_ARG,
                "n_clouds and n_edges must equal the last sicp_register_joint's (" + std::to_string(js.n_clouds) +
                    ", " + std::to_string(js.n_edges) + ")");
   if (!js.cov_done) {
     const int F = js.F, ne = js.n_edges;
-    js.Z.reserve((size_t)js.npad * js.npad);
+    JointSelArgs g{};
+    int parked_blocks = 0;
+    if (js.sparse) g = joint_sel_args(c, js, &parked_blocks);
+    else js.Z.reserve((size_t)js.npad * js.npad);
     js.cov.reserve((size_t)ne + 1 + 36 * ((size_t)F + ne));
     JointCovArgs a{};
     a.pairs = b.pairs.p;
@@ -1025,9 +1084,14 @@ static void get_joint_covariances(Ctx& c, int n_clouds, double* cloud_cov, int n
     a.prior = js.prior.p;
     a.n_prior = js.n_prior;
     a.rel = js.rel.p;
-    a.rel_y = js.rel_y.p;
+    a.rel_y = js.sparse ? g.y : js.rel_y.p;
     a.n_rel = js.n_rel;
-    joint_cov_launch(c, a);
+    if (js.sparse) {
+      g.c = a;
+      joint_sel_launch(c, g, parked_blocks);
+    } else {
+      joint_cov_launch(c, a);
+    }
     std::vector<double> h(1 + 36 * ((size_t)F + ne));
     SICP_CUDA(cudaMemcpyAsync(h.data(), a.s0sq, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, c.stream));
     SICP_CUDA(cudaStreamSynchronize(c.stream));
@@ -2145,6 +2209,13 @@ extern "C" int32_t sicp_get_batch_outputs(sicp_ctx* ctx, int32_t n_pairs, double
 extern "C" int32_t sicp_get_joint_covariances(sicp_ctx* ctx, int32_t n_clouds, double* cloud_cov, int32_t n_edges,
                                               double* edge_cov, double* s0) {
   API_BEGIN(ctx)
-  get_joint_covariances(c, n_clouds, cloud_cov, n_edges, edge_cov, s0);
+  get_joint_covariances(c, n_clouds, cloud_cov, n_edges, edge_cov, s0, false);
+  API_END
+}
+
+extern "C" int32_t sicp_get_joint_selected_covariances(sicp_ctx* ctx, int32_t n_clouds, double* cloud_cov,
+                                                       int32_t n_edges, double* edge_cov, double* s0) {
+  API_BEGIN(ctx)
+  get_joint_covariances(c, n_clouds, cloud_cov, n_edges, edge_cov, s0, true);
   API_END
 }

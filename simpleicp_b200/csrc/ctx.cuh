@@ -2,6 +2,7 @@
 #pragma once
 #include "common.cuh"
 #include "grid_plan.h"
+#include "joint_plan.h"
 #include "reject_solve.cuh"
 #include "upload.cuh"
 
@@ -235,6 +236,7 @@ struct PairDev {
 // ---- sicp_register_joint (joint.cu): one edge of the joint problem per pair of the batch ----
 constexpr int JE_NSUM = 36;  // N (21, packed lower), sum a d (6), sum a (6), sum d, sum d^2, count
 constexpr int JOINT_MAX_FREE = 256;
+constexpr int JOINT_SEL_MAX_PATH = 64;  // the selected inversion: elimination-tree depth, at most
 constexpr int JOINT_MAX_PAD = 1568;  // 6 JOINT_MAX_FREE + 1 rounded up to the 32-wide tiles
 // What k_joint_reject leaves of edge e = (a, b) for the solve and the update: the sums of its
 // kept rows a = [w x n, n] (centred about c_f in frame a), its world block Nw = Ad^T N Ad and
@@ -389,6 +391,18 @@ struct JointCovArgs {
   const double* rel_y;      // same for them, DESIGN.md §6.13)
   int n_rel;
 };
+// sicp_get_joint_selected_covariances after a call under joint_solver 1 (joint.cu: joint_sel_launch,
+// DESIGN.md §6.14): Z = N'^-1 on the pattern of the final iteration's factor s.L, by supernodes.
+struct JointSelArgs {
+  JointSparseArgs s;   // the plan, the factor, xf, dc and the grid barrier of the call
+  JointCovArgs c;      // ss, s0sq, cov_f, cov_e and what k_joint_cov_ss reads (L, Z, npad unused)
+  double* Z;           // supernode k's block of Z at panel[k] - 6 first[k]: 6 (ns + nt) x 6 ns, column-major
+  double* y;           // 6 F: the final iteration's unknowns y' = (omega, u) about each start origin
+  const int* pos;      // per free cloud: its position in the plan's order
+  const int* parked;   // the edges of two free clouds whose cross block lies outside the pattern
+  int n_parked;
+  long long scratch;   // doubles of Z per block of k_joint_sel_parked, before Z is formed
+};
 struct JointStore {
   DevBuf<JointEdge> edges;
   DevBuf<JointFlags> flags;
@@ -402,7 +416,10 @@ struct JointStore {
   DevBuf<double> rel_y;
   int n_rel = 0;    // the relative observations of the last call
   // the sparse solve (joint_solver 1): its panels, x, xf and dc (15 F), bad + one flag per block
-  bool sparse = false;  // the last call used it (no covariances)
+  bool sparse = false;  // the last call used it (covariances by sicp_get_joint_selected_covariances)
+  JointPlan sp_plan;           // its plan and solve arguments, for the selected inversion
+  JointSparseArgs sp_args{};
+  DevBuf<int> sel_ids;  // the selected inversion's pos and parked edges
   DevBuf<long long> sp_panel;
   DevBuf<double> sp_L, sp_x;
   DevBuf<int> sp_flags;
@@ -432,6 +449,10 @@ void joint_relative_launch(Ctx& c, const JointArgs& a, const JointRelArgs& r, co
 // k_joint_cov_ss, k_joint_inv, k_joint_cov_cloud, k_joint_cov_edge: the covariances of the last
 // sicp_register_joint into a.cov_f / a.cov_e and s0^2 into a.s0sq (DESIGN.md §6.9)
 void joint_cov_launch(Ctx& c, const JointCovArgs& a);
+// k_joint_cov_ss, k_joint_sel_parked (parked_blocks > 0), k_joint_selinv, k_joint_sel_s0,
+// k_joint_sel_cloud, k_joint_sel_edge: the covariances of the last sicp_register_joint under
+// joint_solver 1 into a.c.cov_f / a.c.cov_e and s0^2 into a.c.s0sq (DESIGN.md §6.14)
+void joint_sel_launch(Ctx& c, const JointSelArgs& a, int parked_blocks);
 
 struct Batch {
   int n_pairs = 0;

@@ -28,6 +28,16 @@
 //                      C_c = s0^2 J_c (N^-1)_cc J_c^T
 //   k_joint_cov_edge   one block per edge: the cross block of two free clouds and C_e
 //
+// and, on the first sicp_get_joint_selected_covariances after a call under joint_solver 1
+// (DESIGN.md §6.14), after k_joint_cov_ss:
+//
+//   k_joint_sel_parked  per edge whose cross block lies outside the pattern: w_a^T w_b, w_c = L^-1 E_c
+//   k_joint_selinv      one cooperative launch: Z = N'^-1 on the pattern of the sparse factor, by
+//                       Takahashi's recurrence from the roots down, one block per supernode
+//   k_joint_sel_s0      one warp: s0^2 (the statement k_joint_cov_cloud uses)
+//   k_joint_sel_cloud   one thread per free cloud: C_c = s0^2 J'_c (N'^-1)_cc J'_c^T
+//   k_joint_sel_edge    one thread per edge: the cross block and C_e
+//
 // DESIGN.md §6.9 gives the rule, the Ad mapping and the centring.  Every sum runs in a fixed
 // order (no atomics), so repeated calls give the same bits.
 #include "ctx.cuh"
@@ -1022,6 +1032,61 @@ __device__ void store_sym6(const double* C, double s0sq, double* out) {
     }
 }
 
+// s0^2's sums by warp 0 (lane: the thread's lane; every lane ends with the totals ss and m): over
+// the edges that took part, ss[e] and the kept counts; then the pose priors' v^T W v and non-zero
+// weights (DESIGN.md §6.12); then the relative observations' (§6.13).  Their residuals v use the
+// final unknowns (pr.y, rel_y) in the variables of the levers pr.lev, o.lev: the solve's.  A macro
+// rather than a function, so that k_joint_cov_cloud compiles to the instructions it had before it
+// shared this statement with k_joint_sel_s0.
+#define JOINT_S0_SUMS(a, lane, ss, m)                                                                                   \
+  double ss = 0.0, m = 0.0;                                                                                             \
+  for (int e = lane; e < a.n_edges; e += 32)                                                                            \
+    if (a.edges[e].part) {                                                                                              \
+      ss += a.ss[e];                                                                                                    \
+      m += (double)a.edges[e].n;                                                                                        \
+    }                                                                                                                   \
+  /* the pose priors: v^T W v with v = J y - l, and their non-zero weights (DESIGN.md §6.12) */                         \
+  for (int k = lane; k < a.n_prior; k += 32) {                                                                          \
+    const JointPrior& pr = a.prior[k];                                                                                  \
+    const double* y = pr.y;                                                                                             \
+    const double* d = pr.lev;                                                                                           \
+    const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),      \
+                         y[5] - (d[0] * y[1] - d[1] * y[0])};                                                           \
+    for (int q = 0; q < 6; ++q)                                                                                         \
+      if (pr.w[q] != 0.0) {                                                                                             \
+        const double v = u[q] - pr.l[q];                                                                                \
+        ss = fma(pr.w[q] * v, v, ss);                                                                                   \
+        m += 1.0;                                                                                                       \
+      }                                                                                                                 \
+  }                                                                                                                     \
+  /* the relative observations: v = G_b J_b y_b - G_a J_a y_a - l, after the priors (DESIGN.md §6.13) */                \
+  for (int k = lane; k < a.n_rel; k += 32) {                                                                            \
+    const JointRel& o = a.rel[k];                                                                                       \
+    double pu[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  /* R_a u */                                                         \
+    for (int e = 1; e >= 0; --e) {                                                                                      \
+      const int f = e ? o.fb : o.fa;                                                                                    \
+      if (f < 0) continue;                                                                                              \
+      const double* y = a.rel_y + 6 * f;                                                                                \
+      const double* d = o.lev[e];                                                                                       \
+      const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),    \
+                           y[5] - (d[0] * y[1] - d[1] * y[0])};                                                         \
+      const double* b = o.dba;                                                                                          \
+      for (int q = 0; q < 3; ++q) {                                                                                     \
+        pu[q] += e ? u[q] : -u[q];                                                                                      \
+        pu[3 + q] += e ? u[3 + q] : -(u[3 + q] - (b[(q + 1) % 3] * u[(q + 2) % 3] - b[(q + 2) % 3] * u[(q + 1) % 3]));  \
+      }                                                                                                                 \
+    }                                                                                                                   \
+    for (int q = 0; q < 6; ++q)                                                                                         \
+      if (o.w[q] != 0.0) {                                                                                              \
+        const int h = q < 3 ? 0 : 3, r = q - h;                                                                         \
+        const double v = (o.Ra[r] * pu[h] + o.Ra[3 + r] * pu[h + 1] + o.Ra[6 + r] * pu[h + 2]) - o.l[q];                \
+        ss = fma(o.w[q] * v, v, ss);                                                                                    \
+        m += 1.0;                                                                                                       \
+      }                                                                                                                 \
+  }                                                                                                                     \
+  ss = warp_sum(ss);                                                                                                    \
+  m = warp_sum(m);
+
 // k_joint_cov_cloud, one block per free cloud p: s0^2 from the edges' sums (warp 0, fixed order;
 // block 0 stores it), the diagonal block (N^-1)_pp and C_c = s0^2 J_c (N^-1)_pp J_c^T
 __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovArgs a) {
@@ -1031,53 +1096,7 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovAr
   const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
   const int n = 6 * a.F;
   if (tid < 32) {
-    double ss = 0.0, m = 0.0;
-    for (int e = lane; e < a.n_edges; e += 32)
-      if (a.edges[e].part) {
-        ss += a.ss[e];
-        m += (double)a.edges[e].n;
-      }
-    // the pose priors: v^T W v with v = J y - l, and their non-zero weights (DESIGN.md §6.12)
-    for (int k = lane; k < a.n_prior; k += 32) {
-      const JointPrior& pr = a.prior[k];
-      const double* y = pr.y;
-      const double* d = pr.lev;
-      const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),
-                           y[5] - (d[0] * y[1] - d[1] * y[0])};
-      for (int q = 0; q < 6; ++q)
-        if (pr.w[q] != 0.0) {
-          const double v = u[q] - pr.l[q];
-          ss = fma(pr.w[q] * v, v, ss);
-          m += 1.0;
-        }
-    }
-    // the relative observations: v = G_b J_b y_b - G_a J_a y_a - l, after the priors (DESIGN.md §6.13)
-    for (int k = lane; k < a.n_rel; k += 32) {
-      const JointRel& o = a.rel[k];
-      double pu[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // R_a u
-      for (int e = 1; e >= 0; --e) {
-        const int f = e ? o.fb : o.fa;
-        if (f < 0) continue;
-        const double* y = a.rel_y + 6 * f;
-        const double* d = o.lev[e];
-        const double u[6] = {y[0], y[1], y[2], y[3] - (d[1] * y[2] - d[2] * y[1]), y[4] - (d[2] * y[0] - d[0] * y[2]),
-                             y[5] - (d[0] * y[1] - d[1] * y[0])};
-        const double* b = o.dba;
-        for (int q = 0; q < 3; ++q) {
-          pu[q] += e ? u[q] : -u[q];
-          pu[3 + q] += e ? u[3 + q] : -(u[3 + q] - (b[(q + 1) % 3] * u[(q + 2) % 3] - b[(q + 2) % 3] * u[(q + 1) % 3]));
-        }
-      }
-      for (int q = 0; q < 6; ++q)
-        if (o.w[q] != 0.0) {
-          const int h = q < 3 ? 0 : 3, r = q - h;
-          const double v = (o.Ra[r] * pu[h] + o.Ra[3 + r] * pu[h + 1] + o.Ra[6 + r] * pu[h + 2]) - o.l[q];
-          ss = fma(o.w[q] * v, v, ss);
-          m += 1.0;
-        }
-    }
-    ss = warp_sum(ss);
-    m = warp_sum(m);
+    JOINT_S0_SUMS(a, lane, ss, m)
     if (lane == 0) {
       const double dof = m - (double)n;
       s0sq_s = dof > 0.0 ? ss / dof : nan("");
@@ -1095,9 +1114,51 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_cloud(const JointCovAr
   store_sym6(C, s0sq_s, a.cov_f + 36 * (size_t)p);
 }
 
+// C_e of edge e = (a, b) from g = (N^-1)_ab (read with both clouds free): C_ab = s0^2 J_a g J_b^T; then
+// C_e = G_b C_b G_b^T + G_a C_a G_a^T - M - M^T, M = G_a C_ab G_b^T, at the returned poses (a fixed
+// cloud's blocks are 0).  dc: nullptr for the dense solve's unknowns about c_w, else the sparse solve's
+// start origins minus c_w, whose J'_c take the lever o_c - o_c^0.  A macro rather than a function, so
+// that k_joint_cov_edge compiles to the instructions it had before it shared this statement.
+#define JOINT_EDGE_COV(a, e, ca, cb, fa, fb, g, dc)                                                                   \
+  {                                                                                                                   \
+  const double s0sq = *a.s0sq;                                                                                        \
+  const Rigid &Ta = a.pose[ca], &Tb = a.pose[cb];                                                                     \
+  const double dba[3] = {Tb.t[0] - Ta.t[0], Tb.t[1] - Ta.t[1], Tb.t[2] - Ta.t[2]}, zero[3] = {0.0, 0.0, 0.0};         \
+  double Ga[36], Gb[36], C[36], X[36];                                                                                \
+  lever6(Ta.r, dba, Ga);                                                                                              \
+  lever6(Ta.r, zero, Gb);                                                                                             \
+  for (int j = 0; j < 36; ++j) C[j] = 0.0;                                                                            \
+  if (fb >= 0) {                                                                                                      \
+    abt6(Gb, a.cov_f + 36 * (size_t)fb, Gb, X);                                                                       \
+    for (int j = 0; j < 36; ++j) C[j] += X[j];                                                                        \
+  }                                                                                                                   \
+  if (fa >= 0) {                                                                                                      \
+    abt6(Ga, a.cov_f + 36 * (size_t)fa, Ga, X);                                                                       \
+    for (int j = 0; j < 36; ++j) C[j] += X[j];                                                                        \
+  }                                                                                                                   \
+  if (fa >= 0 && fb >= 0) {                                                                                           \
+    const Rigid &Pa = a.pose[ca], &Pb = a.pose[cb];                                                                   \
+    double da[3] = {Pa.t[0] - a.cw[0], Pa.t[1] - a.cw[1], Pa.t[2] - a.cw[2]},                                         \
+           db[3] = {Pb.t[0] - a.cw[0], Pb.t[1] - a.cw[1], Pb.t[2] - a.cw[2]};                                         \
+    if (dc != nullptr)                                                                                                        \
+      for (int q = 0; q < 3; ++q) {                                                                                   \
+        da[q] -= (dc)[3 * fa + q];                                                                                      \
+        db[q] -= (dc)[3 * fb + q];                                                                                      \
+      }                                                                                                               \
+    double Ja[36], Jb[36], Cab[36], M[36];                                                                            \
+    lever6(nullptr, da, Ja);                                                                                          \
+    lever6(nullptr, db, Jb);                                                                                          \
+    for (int j = 0; j < 36; ++j) M[j] = s0sq * g[j];                                                                  \
+    abt6(Ja, M, Jb, Cab);                                                                                             \
+    abt6(Ga, Cab, Gb, M);                                                                                             \
+    for (int r = 0; r < 6; ++r)                                                                                       \
+      for (int c = 0; c < 6; ++c) C[6 * r + c] -= M[6 * r + c] + M[6 * c + r];                                        \
+  }                                                                                                                   \
+  store_sym6(C, s0sq, a.cov_e + 36 * (size_t)e);                                                                      \
+  }
+
 // k_joint_cov_edge, one block per edge e = (a, b): with both clouds free the cross block
-// (N^-1)_ab and C_ab = s0^2 J_a (N^-1)_ab J_b^T; then C_e = G_b C_b G_b^T + G_a C_a G_a^T - M - M^T,
-// M = G_a C_ab G_b^T, at the returned poses (a fixed cloud's blocks are 0)
+// (N^-1)_ab by gram6, then C_e (joint_edge_cov)
 __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_edge(const JointCovArgs a) {
   __shared__ double red[JC_WARPS][36];
   __shared__ double g[36];
@@ -1105,35 +1166,325 @@ __global__ void __launch_bounds__(JC_THREADS) k_joint_cov_edge(const JointCovArg
   const int ca = a.fix_id[e], cb = a.mov_id[e], fa = a.free_of[ca], fb = a.free_of[cb];
   if (fa >= 0 && fb >= 0) gram6(a.Z, a.npad, 6 * a.F, 6 * fa, 6 * fb, red, g);
   if (tid != 0) return;
+  JOINT_EDGE_COV(a, e, ca, cb, fa, fb, g, (const double*)nullptr)
+}
+
+// ---- sicp_get_joint_selected_covariances after a sparse call: Z = N'^-1 on the pattern of L ----------
+// (DESIGN.md §6.14).  Supernode k's block of Z has the rows of its factor panel without the right-hand
+// side's (Rz = 6 (ns + nt)) and the same columns: Z_JJ in full (both triangles), then Z_TJ.
+
+constexpr int SEL_MAX_PATH = JOINT_SEL_MAX_PATH;  // supernodes on a path to a root, at most
+
+// the supernode holding position p: the last k with first[k] <= p (supernodes in elimination order)
+__device__ int sel_owner(const JointSparseArgs& s, int p) {
+  int lo = 0, hi = s.lv_off[s.depth];
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (s.sn[mid].first <= p) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+// the parent of supernode k: the owner of its struct's first position, -1 for a root
+__device__ __forceinline__ int sel_parent(const JointSparseArgs& s, int k) {
+  return s.sn[k].nt > 0 ? sel_owner(s, s.st[s.sn[k].st_off]) : -1;
+}
+__device__ __forceinline__ double* sel_z(const JointSelArgs& g, int k) {
+  return g.Z + (g.s.panel[k] - 6ll * g.s.sn[k].first);
+}
+
+// struct(k) as runs of the ancestors t it falls in, ascending: run i holds the entries b0[i] ..
+// b0[i + 1] - 1, and map[mo[i] + b - b0[i]] is entry b's panel cloud row in t (the row map of the
+// update of t from k); z, rz: t's block of Z and its rows
+struct SelRuns {
+  double* z[SEL_MAX_PATH];
+  int rz[SEL_MAX_PATH], b0[SEL_MAX_PATH + 1], mo[SEL_MAX_PATH];
+  int n;
+};
+__device__ __forceinline__ int sel_run(const SelRuns& r, int b) {
+  int lo = 0, hi = r.n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (r.b0[mid] <= b) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Supernode k by the whole block, after every ancestor (Takahashi's recurrence; W = L_TJ L_JJ^-1):
+//   X = Z_TT L_TJ, gathered from the ancestors' blocks through the update row maps;
+//   Z_TJ = -X L_JJ^-1, row by row in place;
+//   Z_JJ from Z_JJ L_JJ = L_JJ^-T - Z_TJ^T L_TJ, column by column from the last, the off-diagonal
+//   entries of a column before its diagonal one, each mirrored above the diagonal.
+// Every sum runs in a fixed order (ascending index; the diagonal entries by warp_sum), no atomics.
+__device__ void sel_node(const JointSelArgs& g, int k, SelRuns& r) {
+  const JointSparseArgs& s = g.s;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const JointSuper& m = s.sn[k];
+  const int nt = m.nt, C = 6 * m.ns, T = 6 * nt, Rl = C + T + 1, Rz = C + T;
+  const double* L = s.L + s.panel[k];
+  double* Z = sel_z(g, k);
+  if (tid == 0) {
+    int n = 0;
+    for (int b = 0; b < nt; ++n) {
+      const int t = sel_owner(s, s.st[m.st_off + b]);
+      const JointSuper& tm = s.sn[t];
+      int lo = tm.u0, hi = tm.u1 - 1;  // the update of t from k: t's updates by ascending descendant
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (s.up[4 * mid] < k) lo = mid + 1;
+        else hi = mid;
+      }
+      r.z[n] = sel_z(g, t);
+      r.rz[n] = 6 * (tm.ns + tm.nt);
+      r.b0[n] = b;
+      r.mo[n] = s.up[4 * lo + 3];
+      b += s.up[4 * lo + 2];
+    }
+    r.n = n;
+    r.b0[n] = nt;
+  }
+  __syncthreads();
+  // X = Z_TT L_TJ into the rows of Z_TJ: Z_TT's block (ca, cb) lies in the column of the earlier of
+  // the two clouds, in the block of Z of its supernode, at the later one's row there
+  for (int idx = tid; idx < T * C; idx += JS_THREADS) {
+    const int row = idx % T, j = idx / T, ca = row / 6, qa = row % 6, ia = sel_run(r, ca);
+    const double* Lc = L + (size_t)j * Rl + C;
+    double v = 0.0;
+    for (int i = 0; i < r.n; ++i)
+      for (int cb = r.b0[i]; cb < r.b0[i + 1]; ++cb) {
+        const double* zc;
+        int rr;
+        if (cb <= ca) {  // Z(ca, cb) in cb's ancestor: column cb, row ca
+          zc = r.z[i] + (size_t)(6 * s.map[r.mo[i] + cb - r.b0[i]]) * r.rz[i];
+          rr = 6 * s.map[r.mo[i] + ca - r.b0[i]] + qa;
+          for (int qb = 0; qb < 6; ++qb) v = fma(zc[(size_t)qb * r.rz[i] + rr], Lc[6 * cb + qb], v);
+        } else {  // Z(cb, ca)^T in ca's ancestor: column ca, row cb
+          zc = r.z[ia] + (size_t)(6 * s.map[r.mo[ia] + ca - r.b0[ia]] + qa) * r.rz[ia];
+          rr = 6 * s.map[r.mo[ia] + cb - r.b0[ia]];
+          for (int qb = 0; qb < 6; ++qb) v = fma(zc[rr + qb], Lc[6 * cb + qb], v);
+        }
+      }
+    Z[(size_t)j * Rz + C + row] = v;
+  }
+  __syncthreads();
+  // Z_TJ L_JJ = -X: Z[t][j] = (-X[t][j] - sum_{c > j} Z[t][c] L[c][j]) / L[j][j]
+  for (int row = tid; row < T; row += JS_THREADS)
+    for (int j = C - 1; j >= 0; --j) {
+      double v = -Z[(size_t)j * Rz + C + row];
+      for (int c = j + 1; c < C; ++c) v = fma(-Z[(size_t)c * Rz + C + row], L[(size_t)j * Rl + c], v);
+      Z[(size_t)j * Rz + C + row] = v / L[(size_t)j * Rl + j];
+    }
+  __syncthreads();
+  // B = -Z_TJ^T L_TJ on and below the diagonal, into Z_JJ's slots
+  for (int idx = tid; idx < C * C; idx += JS_THREADS) {
+    const int i = idx % C, j = idx / C;
+    if (i < j) continue;
+    const double* zi = Z + (size_t)i * Rz + C;
+    const double* lj = L + (size_t)j * Rl + C;
+    double v = 0.0;
+    for (int t = 0; t < T; ++t) v = fma(-zi[t], lj[t], v);
+    Z[(size_t)j * Rz + i] = v;
+  }
+  __syncthreads();
+  for (int j = C - 1; j >= 0; --j) {
+    const double ljj = L[(size_t)j * Rl + j];
+    for (int i = j + 1 + tid; i < C; i += JS_THREADS) {
+      double v = Z[(size_t)j * Rz + i];
+      for (int c = j + 1; c < C; ++c) v = fma(-Z[(size_t)c * Rz + i], L[(size_t)j * Rl + c], v);
+      v /= ljj;
+      Z[(size_t)j * Rz + i] = v;
+      Z[(size_t)i * Rz + j] = v;
+    }
+    __syncthreads();
+    if (tid < 32) {
+      double v = 0.0;
+      for (int c = j + 1 + lane; c < C; c += 32) v = fma(Z[(size_t)j * Rz + c], L[(size_t)j * Rl + c], v);
+      v = warp_sum(v);
+      if (lane == 0) Z[(size_t)j * Rz + j] = (1.0 / ljj + Z[(size_t)j * Rz + j] - v) / ljj;
+    }
+    __syncthreads();
+  }
+}
+
+// k_joint_selinv, one cooperative launch: the final unknowns y' = (omega, u) about each start origin
+// from xf (u = t' - dc x omega) into y and every read prior's y, for k_joint_sel_s0; then the
+// supernodes by level from the roots down, one block per supernode, one grid barrier per level.
+__global__ void __launch_bounds__(JS_THREADS) k_joint_selinv(const JointSelArgs g) {
+  __shared__ SelRuns r;
+  const JointSparseArgs& s = g.s;
+  const JointArgs& a = s.j;
+  const int tid = threadIdx.x, bid = blockIdx.x, G = gridDim.x;
+  for (int f = bid * JS_THREADS + tid; f < a.F; f += G * JS_THREADS) {
+    double y[6];
+    for (int q = 0; q < 6; ++q) y[q] = s.xf[6 * f + q];
+    const double* d = s.dc + 3 * f;
+    y[3] -= d[1] * y[2] - d[2] * y[1];
+    y[4] -= d[2] * y[0] - d[0] * y[2];
+    y[5] -= d[0] * y[1] - d[1] * y[0];
+    for (int q = 0; q < 6; ++q) g.y[6 * f + q] = y[q];
+    if (a.prior_of && a.prior_of[f] >= 0)
+      for (int q = 0; q < 6; ++q) a.prior[a.prior_of[f]].y[q] = y[q];
+  }
+  for (int l = s.depth - 1; l >= 0; --l) {
+    for (int i = s.lv_off[l] + bid; i < s.lv_off[l + 1]; i += G) sel_node(g, s.lv[i], r);
+    joint_grid_sync(a.bar);
+  }
+}
+
+// k_joint_sel_parked, before k_joint_selinv (its scratch is Z's memory): for each parked edge, one
+// block at a time, (N'^-1)_ab = w_a^T w_b, w_c = L^-1 E_c by forward substitution along the path from
+// c's supernode to its root (the only supernodes where w_c is non-zero), into the edge's slot of
+// cov_e (k_joint_sel_edge reads it there).  Clouds in different trees: no common supernode, 0.
+__global__ void __launch_bounds__(JS_THREADS) k_joint_sel_parked(const JointSelArgs g) {
+  __shared__ int path[2][SEL_MAX_PATH], np[2];
+  __shared__ long long off[2][SEL_MAX_PATH + 1];
+  const JointSparseArgs& s = g.s;
+  const JointArgs& a = s.j;
+  const int tid = threadIdx.x;
+  double* W = g.Z + (size_t)blockIdx.x * g.scratch;
+  for (int i = blockIdx.x; i < g.n_parked; i += gridDim.x) {
+    const int e = g.parked[i];
+    const int f[2] = {a.free_of[a.fix_id[e]], a.free_of[a.mov_id[e]]};
+    if (tid < 2) {
+      int n = 0;
+      long long o = 0;
+      for (int k = sel_owner(s, g.pos[f[tid]]); k >= 0; k = sel_parent(s, k), ++n) {
+        path[tid][n] = k;
+        off[tid][n] = o;
+        o += 6 * s.sn[k].ns;
+      }
+      np[tid] = n;
+      off[tid][n] = o;
+    }
+    __syncthreads();
+    double* v[2] = {W, W + 6 * off[0][np[0]]};
+    for (int side = 0; side < 2; ++side) {
+      double* w = v[side];
+      const long long La = off[side][np[side]];
+      for (long long x = tid; x < 6 * La; x += JS_THREADS) w[x] = 0.0;
+      __syncthreads();
+      if (tid < 6) w[tid * La + 6 * (g.pos[f[side]] - s.sn[path[side][0]].first) + tid] = 1.0;
+      __syncthreads();
+      for (int h = 0; h < np[side]; ++h) {
+        const JointSuper& m = s.sn[path[side][h]];
+        const int C = 6 * m.ns, T = 6 * m.nt, Rl = C + T + 1;
+        const double* L = s.L + s.panel[path[side][h]];
+        const long long o = off[side][h];
+        for (int j = 0; j < C; ++j) {
+          const double ljj = L[(size_t)j * Rl + j];
+          for (int x = tid; x < 6 * (C - j - 1); x += JS_THREADS) {
+            const int q = x % 6, ii = j + 1 + x / 6;
+            const double xj = w[q * La + o + j] / ljj;
+            w[q * La + o + ii] = fma(-L[(size_t)j * Rl + ii], xj, w[q * La + o + ii]);
+          }
+          __syncthreads();
+          if (tid < 6) w[tid * La + o + j] /= ljj;
+          __syncthreads();
+        }
+        // the struct's rows: w_T -= L_TJ w_J, each on its ancestor's place in the path
+        for (int x = tid; x < 6 * T; x += JS_THREADS) {
+          const int q = x % 6, t = x / 6, p = s.st[m.st_off + t / 6];
+          int h2 = h + 1;
+          while (p >= s.sn[path[side][h2]].first + s.sn[path[side][h2]].ns) ++h2;
+          const long long at = q * La + off[side][h2] + 6 * (p - s.sn[path[side][h2]].first) + t % 6;
+          double acc = 0.0;
+          for (int c = 0; c < C; ++c) acc = fma(L[(size_t)c * Rl + C + t], w[q * La + o + c], acc);
+          w[at] -= acc;
+        }
+        __syncthreads();
+      }
+    }
+    // the common supernodes: from the first of a's path that b's path holds on, both paths agree
+    if (tid < 36) {
+      const int qa = tid / 6, qb = tid % 6;
+      const long long La = off[0][np[0]], Lb = off[1][np[1]];
+      int h0 = 0, h1 = -1;
+      for (; h0 < np[0]; ++h0) {
+        for (int x = 0; x < np[1]; ++x)
+          if (path[1][x] == path[0][h0]) h1 = x;
+        if (h1 >= 0) break;
+      }
+      double acc = 0.0;
+      if (h1 >= 0)
+        for (int h = h0; h < np[0]; ++h, ++h1)
+          for (long long x = 0; x < off[0][h + 1] - off[0][h]; ++x)
+            acc = fma(v[0][qa * La + off[0][h] + x], v[1][qb * Lb + off[1][h1] + x], acc);
+      g.c.cov_e[36 * (size_t)e + tid] = acc;
+    }
+    __syncthreads();
+  }
+}
+
+// k_joint_sel_s0, one warp: s0^2 of the call into *s0sq by JOINT_S0_SUMS, the statement
+// k_joint_cov_cloud uses, from the unknowns k_joint_selinv left in y and the priors' y
+__global__ void __launch_bounds__(32) k_joint_sel_s0(const JointCovArgs a) {
+  const int lane = threadIdx.x;
+  JOINT_S0_SUMS(a, lane, ss, m)
+  if (lane == 0) {
+    const double dof = m - (double)(6 * a.F);
+    *a.s0sq = dof > 0.0 ? ss / dof : nan("");
+  }
+}
+
+// k_joint_sel_cloud, one thread per position p of free cloud f: C_c = s0^2 J'_c (N'^-1)_cc J'_c^T,
+// with the lever o_c - o_c^0 of J'_c
+__global__ void __launch_bounds__(128) k_joint_sel_cloud(const JointSelArgs g) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const JointSparseArgs& s = g.s;
+  const JointCovArgs& a = g.c;
+  if (p >= a.F) return;
+  const int f = s.perm[p], k = sel_owner(s, p), cj = p - s.sn[k].first;
+  const int Rz = 6 * (s.sn[k].ns + s.sn[k].nt);
+  const double* Z = sel_z(g, k) + (size_t)(6 * cj) * Rz + 6 * cj;
   const double s0sq = *a.s0sq;
-  const Rigid &Ta = a.pose[ca], &Tb = a.pose[cb];
-  const double dba[3] = {Tb.t[0] - Ta.t[0], Tb.t[1] - Ta.t[1], Tb.t[2] - Ta.t[2]}, zero[3] = {0.0, 0.0, 0.0};
-  double Ga[36], Gb[36], C[36], X[36];
-  lever6(Ta.r, dba, Ga);
-  lever6(Ta.r, zero, Gb);
-  for (int j = 0; j < 36; ++j) C[j] = 0.0;
-  if (fb >= 0) {
-    abt6(Gb, a.cov_f + 36 * (size_t)fb, Gb, X);
-    for (int j = 0; j < 36; ++j) C[j] += X[j];
-  }
-  if (fa >= 0) {
-    abt6(Ga, a.cov_f + 36 * (size_t)fa, Ga, X);
-    for (int j = 0; j < 36; ++j) C[j] += X[j];
-  }
+  const Rigid& T = a.pose[a.free_ids[f]];
+  double d[3], Jc[36], C[36], M[36];
+  for (int q = 0; q < 3; ++q) d[q] = (T.t[q] - a.cw[q]) - s.dc[3 * f + q];
+  lever6(nullptr, d, Jc);
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) M[6 * r + c] = s0sq * Z[(size_t)c * Rz + r];
+  abt6(Jc, M, Jc, C);
+  store_sym6(C, s0sq, a.cov_f + 36 * (size_t)f);
+}
+
+// k_joint_sel_edge, one thread per edge e = (a, b): with both clouds free the cross block (N'^-1)_ab
+// from the block of Z of the earlier position's supernode, at the later one's row there, or, for a
+// pair outside the pattern, from k_joint_sel_parked's value in e's slot of cov_e; then C_e
+// (JOINT_EDGE_COV in the sparse unknowns)
+__global__ void __launch_bounds__(128) k_joint_sel_edge(const JointSelArgs g) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  const JointSparseArgs& s = g.s;
+  const JointCovArgs& a = g.c;
+  if (e >= a.n_edges) return;
+  const int ca = a.fix_id[e], cb = a.mov_id[e], fa = a.free_of[ca], fb = a.free_of[cb];
+  double gx[36];
   if (fa >= 0 && fb >= 0) {
-    const Rigid &Pa = a.pose[ca], &Pb = a.pose[cb];
-    const double da[3] = {Pa.t[0] - a.cw[0], Pa.t[1] - a.cw[1], Pa.t[2] - a.cw[2]},
-                 db[3] = {Pb.t[0] - a.cw[0], Pb.t[1] - a.cw[1], Pb.t[2] - a.cw[2]};
-    double Ja[36], Jb[36], Cab[36], M[36];
-    lever6(nullptr, da, Ja);
-    lever6(nullptr, db, Jb);
-    for (int j = 0; j < 36; ++j) M[j] = s0sq * g[j];
-    abt6(Ja, M, Jb, Cab);
-    abt6(Ga, Cab, Gb, M);
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) C[6 * r + c] -= M[6 * r + c] + M[6 * c + r];
+    const int pa = g.pos[fa], pb = g.pos[fb], lo = min(pa, pb), hi = max(pa, pb);
+    const int k = sel_owner(s, lo);
+    const JointSuper& m = s.sn[k];
+    int ri = -1;
+    if (hi < m.first + m.ns) {
+      ri = hi - m.first;
+    } else {
+      int l = 0, h = m.nt;  // struct(k) ascending
+      while (l < h) {
+        const int mid = (l + h) >> 1;
+        if (s.st[m.st_off + mid] < hi) l = mid + 1;
+        else h = mid;
+      }
+      if (l < m.nt && s.st[m.st_off + l] == hi) ri = m.ns + l;
+    }
+    if (ri >= 0) {
+      const int Rz = 6 * (m.ns + m.nt);
+      const double* Z = sel_z(g, k) + (size_t)(6 * (lo - m.first)) * Rz + 6 * ri;  // rows hi, columns lo
+      for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) gx[6 * r + c] = (pa == hi) ? Z[(size_t)c * Rz + r] : Z[(size_t)r * Rz + c];
+    } else {
+      for (int j = 0; j < 36; ++j) gx[j] = a.cov_e[36 * (size_t)e + j];
+    }
   }
-  store_sym6(C, s0sq, a.cov_e + 36 * (size_t)e);
+  JOINT_EDGE_COV(a, e, ca, cb, fa, fb, gx, s.dc)
 }
 
 }  // namespace
@@ -1182,6 +1533,24 @@ void joint_cov_launch(Ctx& c, const JointCovArgs& a) {
   k_joint_cov_cloud<<<a.F, JC_THREADS, 0, c.stream>>>(a);
   SICP_CUDA(cudaGetLastError());
   k_joint_cov_edge<<<a.n_edges, JC_THREADS, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+}
+
+void joint_sel_launch(Ctx& c, const JointSelArgs& a, int parked_blocks) {
+  k_joint_cov_ss<<<a.c.n_edges, JC_THREADS, 0, c.stream>>>(a.c);
+  SICP_CUDA(cudaGetLastError());
+  if (parked_blocks > 0) {
+    k_joint_sel_parked<<<parked_blocks, JS_THREADS, 0, c.stream>>>(a);
+    SICP_CUDA(cudaGetLastError());
+  }
+  JointSelArgs args = a;
+  void* p[] = {&args};
+  SICP_CUDA(cudaLaunchCooperativeKernel((void*)k_joint_selinv, dim3(c.num_sms), dim3(JS_THREADS), p, 0, c.stream));
+  k_joint_sel_s0<<<1, 32, 0, c.stream>>>(a.c);
+  SICP_CUDA(cudaGetLastError());
+  k_joint_sel_cloud<<<(a.c.F + 127) / 128, 128, 0, c.stream>>>(a);
+  SICP_CUDA(cudaGetLastError());
+  k_joint_sel_edge<<<(a.c.n_edges + 127) / 128, 128, 0, c.stream>>>(a);
   SICP_CUDA(cudaGetLastError());
 }
 
